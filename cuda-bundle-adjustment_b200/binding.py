@@ -51,7 +51,7 @@ _SYMBOLS = [
     "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
-    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_dropin_problem", "cuba_bench_stage",
+    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_bench_stage",
 ]
 
 
@@ -104,6 +104,7 @@ def load_library():
         "cuba_debug_build_structure_host": [C.POINTER(_Problem), i, i, C.POINTER(_Sizes), vp, vp, vp, vp, vp, vp, vp, vp],
         "cuba_debug_pcg_partition": [C.POINTER(_Problem), i, i, vp],
         "cuba_debug_pcg5_plan": [C.POINTER(_Problem), i, i, i, vp],
+        "cuba_debug_pcg5_plan_apc": [C.POINTER(_Problem), i, i, i, i, vp, C.POINTER(C.c_uint64)],
         "cuba_debug_dropin_problem": [vp, C.POINTER(_Problem)],
         "cuba_bench_stage": [vp, i, i, i, d, C.POINTER(d)],
     }
@@ -177,6 +178,19 @@ def pcg5_plan_host(prob, world=1, num_sms=148, max_aggregates=74):
     info = np.zeros(8, np.int32)
     _check(L.cuba_debug_pcg5_plan(C.byref(P), int(world), int(num_sms), int(max_aggregates), _p(info)))
     return dict(zip(("ok", "G", "gs", "A", "needMax", "maxRows", "maxNeedAgg", "halo_rows"), (int(v) for v in info)))
+
+
+def pcg5_plan_apc_host(prob, aggs_per_cta, world=1, num_sms=132, max_aggregates=148):
+    """pcg5_plan_host with `aggs_per_cta` aggregates per CTA (the one-GPU tuned kernel's coarse space); also returns "hash", an
+    FNV-1a hash over every array of the plan"""
+    L = load_library()
+    P, keep = _problem_struct(prob)
+    info = np.zeros(8, np.int32)
+    h = C.c_uint64(0)
+    _check(L.cuba_debug_pcg5_plan_apc(C.byref(P), int(world), int(num_sms), int(max_aggregates), int(aggs_per_cta), _p(info), C.byref(h)))
+    out = dict(zip(("ok", "G", "gs", "A", "needMax", "maxRows", "maxNeedAgg", "halo_rows"), (int(v) for v in info)))
+    out["hash"] = int(h.value)
+    return out
 
 
 class Engine:

@@ -1563,39 +1563,49 @@ struct Engine : EngineBase {
 		// rows over world x G virtual CTAs (about eight rows each, never more than 42: one thread per (row, component) pair in the
 		// row sums), rank-aligned aggregates, halo masks: cuba_structure.cpp (CPU-tested through cuba_debug_pcg5_plan)
 		const int maxAgg = (cfg.reserved[6] > 0 && cfg.reserved[6] < PCG5_MAXAGG) ? cfg.reserved[6] : PCG5_MAXAGG;
-		Pcg5Plan plan;
-		build_pcg5_plan(numP, S.nfull, S.fRowPtr, S.fColInd, W, numSMs, maxAgg, 2 * PCG5_BLOCK / 6, plan, &hostPP);
-		if (!plan.ok) return CUBA_OK;
-		const int G = plan.G, gs = plan.gs, A = plan.A;
-		const PcgPartition& PP = plan.P; const CoarsePartition& CP = plan.C;
-		const std::vector<unsigned char>& peers = plan.rowPeers;
-		const int Aloc = G / gs, NR = 3 + 6 * Aloc, nc = 6 * A;
-		Pcg5Dims d{};
-		d.needMax = PP.needMax; d.maxRows = PP.maxRows; d.nc = nc; d.maxNeedAgg = CP.maxNeedAgg;
-		d.npv = std::max(std::max(G * 9, W * NR), 6 * CP.maxNeedAgg); d.nls = NR;
-		d.sliceRows = (nc + G - 1) / G;
-		const size_t per = 36 * sizeof(T) + 4;
-		size_t wantCache = PP.blkMax > PCG5_REGBLK ? (size_t)(PP.blkMax - PCG5_REGBLK) : 0;
-		// the tuned shape (cuba_pcg5t.cuh): a solve on one GPU whose blocks fit registers + shared memory
+		// the tuned shape (cuba_pcg5t.cuh): a solve on one GPU whose blocks fit registers + shared memory, with apc aggregates per
+		// CTA -- the largest apc <= p5t::DEFAULT_APC (CUBA_PCG5_AGGS_PER_CTA: another bound, 1 = one aggregate per CTA group as
+		// k_pcg5) whose plan exists and whose shared memory fits; every other shape: one aggregate per group of gs CTAs
+		const bool tryTuned = W == 1 && !getenv("CUBA_PCG5_LEGACY");
+		int apcTop = p5t::DEFAULT_APC;
+		if (const char* e = getenv("CUBA_PCG5_AGGS_PER_CTA")) apcTop = std::min(3, std::max(1, atoi(e)));
 		p5Tuned = false;
-		if (W == 1 && !getenv("CUBA_PCG5_LEGACY")) {
+		Pcg5Plan plan;
+		Pcg5Dims d{};
+		int NR = 0;
+		const size_t per = 36 * sizeof(T) + 4;
+		size_t wantCache = 0;
+		for (int apc = tryTuned ? apcTop : 1; apc >= 1 && !p5Tuned; apc--) {
+			build_pcg5_plan(numP, S.nfull, S.fRowPtr, S.fColInd, W, numSMs, maxAgg, 2 * PCG5_BLOCK / 6, plan, &hostPP, apc);
+			if (!plan.ok) continue;
+			const int G = plan.G, nc = 6 * plan.A;
+			const PcgPartition& PP = plan.P; const CoarsePartition& CP = plan.C;
+			NR = 3 + 6 * (G / plan.gs);
+			d = Pcg5Dims{};
+			d.needMax = PP.needMax; d.maxRows = PP.maxRows; d.nc = nc; d.maxNeedAgg = CP.maxNeedAgg;
+			d.npv = std::max(std::max(G * p5t::pcg5t_np(apc), W * NR), 6 * CP.maxNeedAgg); d.nls = NR;
+			d.sliceRows = (nc + G - 1) / G;
+			wantCache = PP.blkMax > PCG5_REGBLK ? (size_t)(PP.blkMax - PCG5_REGBLK) : 0;
+			if (!tryTuned) break;
 			using TS = p5t::Pcg5Shape;
 			p5t::Pcg5Dims t{};
 			t.needMax = PP.needMax; t.maxRows = PP.maxRows; t.nc = nc; t.maxNeedAgg = CP.maxNeedAgg;
 			t.npv = d.npv; t.nls = NR; t.sliceRows = d.sliceRows;
 			t.ccCap = PP.blkMax >= TS::CHUNK ? TS::CHUNK : std::max((std::max(PP.blkMax, PP.needMax) + 31) / 32 * 32, 32);
-			t.sqWords = std::max(9 * PP.maxRows * 6, 9 * (TS::BLOCK / 32));
+			t.sqWords = p5t::pcg5t_np(apc) * (TS::BLOCK / 32);
 			t.capBlocks = 0; t.zhInSmem = 0;
 			const size_t base = p5t::Pcg5Layout<T>(t).total + 64;
 			const size_t zhBytes = (size_t)t.needMax * 36 * sizeof(T);
-			size_t used = base + wantCache * per;
+			size_t used = base + wantCache * per, cap = wantCache;
 			if (used + zhBytes <= budget) { t.zhInSmem = 1; used += zhBytes; }
+			// apc > 1: the larger slice of Ac^-1 may take the place of cached blocks (the rest is read from the global copy)
+			if (apc > 1 && used > budget && base <= budget) { cap = std::min(wantCache, (budget - base) / per); used = base + cap * per; }
 			if (PP.maxRows * 6 <= TS::BLOCK && used <= budget) {
-				t.capBlocks = (int)wantCache;
+				t.capBlocks = (int)cap;
 				p5tDims = t;
 				p5tDimsBJ = t; p5tDimsBJ.nc = 0; p5tDimsBJ.maxNeedAgg = 0; p5tDimsBJ.zhInSmem = 0; p5tDimsBJ.sliceRows = 0; p5tDimsBJ.nls = 3; p5tDimsBJ.npv = std::max(G * 3, W * 3);
 				const size_t smemT = std::max(p5t::Pcg5Layout<T>(p5tDims).total, p5t::Pcg5Layout<T>(p5tDimsBJ).total);
-				const void* fn = (const void*)p5t::k_pcg5t<T>;
+				const void* fn = apc == 3 ? (const void*)p5t::k_pcg5t<T, 3> : apc == 2 ? (const void*)p5t::k_pcg5t<T, 2> : (const void*)p5t::k_pcg5t<T, 1>;
 				int perSM = 0;
 				if (smemT <= (size_t)smemMax - 1024 && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemT) == cudaSuccess &&
 					cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fn, TS::BLOCK, smemT) == cudaSuccess && perSM >= 1) {
@@ -1604,7 +1614,14 @@ struct Engine : EngineBase {
 					d.capBlocks = t.capBlocks; d.zhInSmem = t.zhInSmem;
 				} else cudaGetLastError();
 			}
+			// the other shapes take one aggregate per CTA group
+			if (!p5Tuned && apc == 1) break;
 		}
+		if (!plan.ok) return CUBA_OK;
+		const int G = plan.G, gs = plan.gs, A = plan.A;
+		const PcgPartition& PP = plan.P; const CoarsePartition& CP = plan.C;
+		const std::vector<unsigned char>& peers = plan.rowPeers;
+		const int nc = 6 * A;
 		if (!p5Tuned) {
 		bool big = PP.maxRows * 6 > PCG5_BLOCK;
 		{
@@ -1634,14 +1651,16 @@ struct Engine : EngineBase {
 		else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_pcg5<T, false>, PCG5_BLOCK, p5Smem));
 		if (perSM < 1) return CUBA_OK;
 		}
-		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: world %d G %d gs %d A %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceRows %d cap %d smem %zu\n",
-			W, G, gs, A, d.needMax, d.maxRows, PP.blkMax, d.maxNeedAgg, d.zhInSmem, d.sliceRows, d.capBlocks, p5Smem);
+		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: world %d G %d gs %d A %d aggsPerCta %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceRows %d cap %d smem %zu\n",
+			W, G, gs, A, plan.apc, d.needMax, d.maxRows, PP.blkMax, d.maxNeedAgg, d.zhInSmem, d.sliceRows, d.capBlocks, p5Smem);
 		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: shape %s, %d threads\n", p5Big ? "big" : p5Tuned ? "tuned" : "legacy", p5Block);
-		// coarse inverse: packed block triangle in the shared memory of one CTA (A <= 37), of an 8-CTA cluster (A <= 74) or of a
-		// 16-CTA cluster (A <= 148; non-portable cluster size)
-		p5Cluster = A > PCG4_MAXAGG1 ? (A > PCG4_MAXAGG ? 16 : 8) : 0;
+		// coarse inverse: k_coarse_dense on the whole chip (A > 37; the only one past A = 148), or the packed block triangle in the
+		// shared memory of one CTA (A <= 37), of an 8-CTA cluster (A <= 74) or of a 16-CTA cluster (A <= 148; non-portable cluster size)
+		p5Dense = A > PCG4_MAXAGG1 && (A > PCG5_MAXAGG || !getenv("CUBA_COARSE_CLUSTER"));
+		p5Cluster = A > PCG5_MAXAGG ? 0 : A > PCG4_MAXAGG1 ? (A > PCG4_MAXAGG ? 16 : 8) : 0;
 		const size_t nblkPz = (size_t)A * (A + 1) / 2;
-		if (p5Cluster) {
+		if (A > PCG5_MAXAGG) p5InvSmem = 0;
+		else if (p5Cluster) {
 			const size_t nloc = (nblkPz + p5Cluster - 1) / p5Cluster;
 			p5InvSmem = nloc * 36 * sizeof(double) + 2 * nloc + 16;
 		} else p5InvSmem = (nblkPz + 2 * (size_t)A) * 36 * sizeof(double);
@@ -1650,8 +1669,8 @@ struct Engine : EngineBase {
 			CUDA_TRY(cudaFuncSetAttribute(k_coarse_chol_cluster2<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p5InvSmem));
 			CUDA_TRY(cudaFuncSetAttribute(k_coarse_chol_cluster2<16>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
 		} else if (p5Cluster == 8) CUDA_TRY(cudaFuncSetAttribute(k_coarse_chol_cluster2<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p5InvSmem));
-		else CUDA_TRY(cudaFuncSetAttribute(k_coarse_invert<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(p5InvSmem, (!pcg4Cluster && pcg4Ok) ? pcg4InvSmem : 0)));
-		if ((size_t)A * 36 * sizeof(double) > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(k_coarse_trinv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)A * 36 * sizeof(double))));
+		else if (!p5Dense) CUDA_TRY(cudaFuncSetAttribute(k_coarse_invert<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(p5InvSmem, (!pcg4Cluster && pcg4Ok) ? pcg4InvSmem : 0)));
+		if (p5Cluster && (size_t)A * 36 * sizeof(double) > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(k_coarse_trinv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)A * 36 * sizeof(double))));
 		CUDA_TRY(p5CtaRow.upload(PP.rows, stream, arena)); CUDA_TRY(p5NeedPtr.upload(PP.nptr, stream, arena)); CUDA_TRY(p5NeedCol.upload(PP.ncol, stream, arena));
 		CUDA_TRY(p5Local.upload(PP.local, stream, arena)); CUDA_TRY(p5RowPeers.upload(peers, stream, arena));
 		CUDA_TRY(p5AggRow.upload(CP.aggRow, stream, arena)); CUDA_TRY(p5NaPtr.upload(CP.naPtr, stream, arena)); CUDA_TRY(p5NaList.upload(CP.naList, stream, arena));
@@ -1662,14 +1681,13 @@ struct Engine : EngineBase {
 		CUDA_TRY(cZx.alloc(36 * nP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(cInfo.alloc(1));
 		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull));
 		CUDA_TRY(p5AcP.alloc(nblkPz * 36)); CUDA_TRY(p5AcInv.alloc((size_t)nc * nc)); CUDA_TRY(p5Lp.alloc(nblkPz * 36)); CUDA_TRY(p5Wp.alloc(nblkPz * 36)); CUDA_TRY(p5Ld.alloc((size_t)A * 36));
-		p5Dense = A > PCG4_MAXAGG1 && !getenv("CUBA_COARSE_CLUSTER");
 		if (p5Dense) {
 			const size_t ntd = ((size_t)nc + cdense::NB - 1) / cdense::NB, npd = ntd * cdense::NB;
 			CUDA_TRY(cdM.alloc(npd * npd)); CUDA_TRY(cdL.alloc(npd * npd)); CUDA_TRY(cdW.alloc(npd * npd)); CUDA_TRY(cdDinv.alloc(ntd * cdense::NB * cdense::NB));
 			CUDA_TRY(gridBar.alloc(1));
 		}
 		// boards (16-byte words): [2 solve halves][2 pass parities] of w, of the per-CTA partials and of the rank summaries, then the control block
-		const size_t wW = 4 * 6 * nP, pW = 4 * (size_t)PCG5_REPL * G * 9, rW = 4 * (size_t)PCG5_REPL * W * NR, cW = 4 * (size_t)PCG5_REPL * nc;
+		const size_t wW = 4 * 6 * nP, pW = 4 * (size_t)PCG5_REPL * G * p5t::pcg5t_np(plan.apc), rW = 4 * (size_t)PCG5_REPL * W * NR, cW = 4 * (size_t)PCG5_REPL * nc;
 		const size_t words2 = 2 * (wW + pW + rW + cW) + (sizeof(Pcg5Ctl) + 7) / 8 + 2;
 		const bool fresh = !p5Boards.p || words2 > p5Boards.cap || wW != p5WWords || pW != p5PWords || rW != p5RWords || cW != p5CWords;
 		if (fresh) {
@@ -1793,6 +1811,7 @@ struct Engine : EngineBase {
 		void* args[1];
 		if (p5Tuned) {
 			fill(at);
+			at.aggRow = p5AggRow;
 			at.dims = twoLevel ? p5tDims : p5tDimsBJ;
 			at.dims.capBlocks = p5tDims.capBlocks;
 #ifdef CUBA_PCG_TIMING
@@ -2185,6 +2204,10 @@ struct Engine : EngineBase {
 			case 4: curLambda = lambda; rc = launch_pcg(); break;
 			case 5: rc = launch_backsub(lam); if (!rc) rc = stage_update_nofetch(lam); break;
 			case 6: rc = launch_chi2(cur, 0); break;
+			case 7:   // one rebuild of the coarse inverse of k_pcg5 / k_pcg5t (projection, assembly, inverse) from the current system
+				if (!p5Ok || p5A < 1) rc = fail(CUBA_ERR_STATE, "bench_stage: no two-level k_pcg5 plan");
+				else rc = launch_coarse_setup(p5A, p5Cluster, p5InvSmem, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5Lp, p5Ld, p5Wp, p5Dense);
+				break;
 			default: rc = fail(CUBA_ERR_INVALID, "bench_stage: unknown stage");
 			}
 			if (rc) return rc;
@@ -2387,13 +2410,19 @@ int cuba_debug_pcg_partition(const cuba_problem* p, int nCtas, int maxAgg, int32
  * number of rows some other rank needs (halo rows) */
 int cuba_debug_pcg5_plan(const cuba_problem* p, int world, int numSMs, int maxAgg, int32_t* info)
 {
-	if (!p || world < 1 || world > 8 || numSMs < 1 || maxAgg < 1) return fail(CUBA_ERR_INVALID, "pcg5_plan: bad arguments");
+	return cuba_debug_pcg5_plan_apc(p, world, numSMs, maxAgg, 1, info, nullptr);
+}
+
+int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int maxAgg, int aggsPerCta, int32_t* info, uint64_t* hash)
+{
+	if (!p || world < 1 || world > 8 || numSMs < 1 || maxAgg < 1 || aggsPerCta < 1 || aggsPerCta > 3) return fail(CUBA_ERR_INVALID, "pcg5_plan: bad arguments");
 	Structure S;
 	const char* err = "";
 	if (!build_structure(p->Pall, p->numP, p->Lall, p->numL, p->E2, p->idx2, p->E3, p->idx3, 0, 1, TILE, S, &err)) return fail(CUBA_ERR_INVALID, err);
 	Pcg5Plan plan;
-	build_pcg5_plan(S.numP, S.nfull, S.fRowPtr, S.fColInd, world, numSMs, maxAgg, 2 * PCG5_BLOCK / 6, plan);
+	build_pcg5_plan(S.numP, S.nfull, S.fRowPtr, S.fColInd, world, numSMs, maxAgg, 2 * PCG5_BLOCK / 6, plan, nullptr, aggsPerCta);
 	if (info) for (int i = 0; i < 8; i++) info[i] = 0;
+	if (hash) *hash = 0;
 	if (!plan.ok) return CUBA_OK;
 	const char* bad = check_pcg5_plan(S.numP, S.nfull, S.fRowPtr, S.fColInd, plan);
 	if (bad) return fail(CUBA_ERR_INVALID, std::string("pcg5_plan self-check: ") + bad);
@@ -2401,6 +2430,20 @@ int cuba_debug_pcg5_plan(const cuba_problem* p, int world, int numSMs, int maxAg
 		int halo = 0;
 		for (unsigned char m : plan.rowPeers) if (m) halo++;
 		info[0] = 1; info[1] = plan.G; info[2] = plan.gs; info[3] = plan.A; info[4] = plan.P.needMax; info[5] = plan.P.maxRows; info[6] = plan.C.maxNeedAgg; info[7] = halo;
+	}
+	if (hash) {
+		uint64_t h = 1469598103934665603ull;
+		auto mix = [&h](const void* data, size_t bytes) {
+			const unsigned char* b = (const unsigned char*)data;
+			for (size_t i = 0; i < bytes; i++) { h ^= b[i]; h *= 1099511628211ull; }
+		};
+		auto vec = [&mix](const std::vector<int>& v) { const uint64_t n = v.size(); mix(&n, sizeof n); mix(v.data(), v.size() * sizeof(int)); };
+		const int scal[] = { plan.G, plan.gs, plan.A, plan.P.needMax, plan.P.blkMax, plan.P.maxRows, plan.C.maxNeedAgg };
+		mix(scal, sizeof scal);
+		for (const std::vector<int>* v : { &plan.P.rows, &plan.P.nptr, &plan.P.ncol, &plan.P.local, &plan.C.aggRow, &plan.C.rowAgg, &plan.C.naPtr,
+			&plan.C.naList, &plan.C.needAgg, &plan.C.rowOf, &plan.C.cbPtr, &plan.C.cbList }) vec(*v);
+		mix(plan.rowPeers.data(), plan.rowPeers.size());
+		*hash = h;
 	}
 	return CUBA_OK;
 }

@@ -4,8 +4,9 @@
 //     shared-memory and L2 latencies of the short phases between the exchanges;
 //   * the coarse residual is advanced first and this CTA's rows of c = Ac^-1 rc are published BEFORE r, s, p, y are advanced, so the
 //     words cross the L2 while the CTA still has work to do;
-//   * the three scalars are summed by three warps (one each) instead of by all sixteen; the nine partial products of the
+//   * the three scalars are summed by three warps (one each) instead of by all sixteen; the 3 + 6K partial products of the
 //     (row, component) threads are added by warp butterflies instead of through a shared-memory staging array;
+//   * K = 1, 2 or 3 aggregates per CTA on the coarse level (k_pcg5: one per group of gs CTAs);
 //   * up to two blocks per thread in one product round (register block, then one cached block), the staging sized by what a CTA owns.
 // cuba_pcg5.cuh keeps the multi-GPU and large-graph shape: the same source restructured to serve both shapes ran slower on the
 // streamed (BIG) path, so the shapes live in two files.
@@ -26,6 +27,12 @@ struct Pcg5Shape {
 	static constexpr int CHUNK = BLOCK * CPT;
 	static constexpr int PCH = 3;                      // polled words in flight per thread
 };
+
+// aggregates per CTA the engine tries first (then fewer, until the plan exists and the shared memory fits).  1: on ba_kitti_00
+// (one H100 80GB HBM3, 700 W) K = 2 cut the iterations per LM step from 1561 to 1250 but cost 18.1 instead of 11.2 us per
+// iteration (71 fewer cached blocks and Z^ from L2 to make room for the 76 KB slice of Ac^-1) and 4.2 instead of 1.5 ms per
+// coarse rebuild: 29.0 instead of 24.0 ms per step.  K = 3 does not fit in shared memory.
+constexpr int DEFAULT_APC = 1;
 
 struct Pcg5Dims {
 	int capBlocks, needMax, maxRows, nc, maxNeedAgg, zhInSmem;
@@ -88,6 +95,7 @@ struct Pcg5Args {
 	PcgStatus* status;
 	// coarse level (A == 0: off)
 	const float* AcInv; const int* naPtr; const int* naList; const int* needAgg;
+	const int* aggRow;      // [A+1] first row of every aggregate (read for the K > 1 aggregates of a CTA)
 	int A, gs;
 	// boards of THIS GPU, [2 solve parity][2 pass parity]...
 	unsigned long long* wBoard;      // ... [6 numP][2]
@@ -137,12 +145,20 @@ __device__ __forceinline__ bool ll_poll_many(int n, SlotOf slotOf, double* dst, 
 	return ll_poll_each<KB, KPCH>(n, slotOf, [dst](int i, double v) { dst[i] = v; }, tag, ctl);
 }
 
-template <typename T>
+// partial words of a CTA: gamma, delta, rho, then Z^^T w of each of its K aggregates
+__host__ __device__ constexpr int pcg5t_np(int K) { return 3 + 6 * K; }
+
+// K aggregates per CTA on the coarse level (one GPU; K > 1 needs gs == 1): aggregate K cta + j = the j-th of K contiguous groups
+// of the CTA's rows.  The coarse space grows K-fold (fewer iterations), a CTA publishes 3 + 6K partial words and multiplies 6K rows
+// of Ac^-1.
+template <typename T, int K>
 __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T> a)
 {
 	using Shape = Pcg5Shape;
 	// the names of cuba_pcg5.cuh's constants, bound to this shape
 	constexpr int PCG5_BLOCK = Shape::BLOCK, PCG5_BPT = Shape::BPT, PCG5_CPT = Shape::CPT, PCG5_CHUNK = Shape::CHUNK, PCG5_PCH = Shape::PCH;
+	constexpr int NPK = pcg5t_np(K);
+	constexpr int PPCH = K == 1 ? PCG5_PCH : 2 * K;        // polled partial words in flight per thread: G (3 + 6K) in one round on 132 CTAs
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const Pcg5Layout<T> lay(a.dims);
 	const int capBlocks = a.dims.capBlocks, nc = a.dims.nc, ccCap = a.dims.ccCap;
@@ -174,8 +190,12 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 	const int G = a.G, lc = blockIdx.x, cta = a.rank * G + lc, world = a.world;
 	const bool coarse = a.A > 0;
 	const int Aloc = coarse ? G / a.gs : 0;             // aggregates hosted by one rank (gs divides G)
-	const int NP = coarse ? 9 : 3, NR = 3 + 6 * Aloc;
+	const int NP = coarse ? NPK : 3, NR = 3 + 6 * Aloc;
 	const int row0 = a.ctaRow[cta], row1 = a.ctaRow[cta + 1], nrows = row1 - row0;
+	// first local row of this CTA's aggregates 1 .. K-1
+	int aggCut[K > 1 ? K - 1 : 1];
+#pragma unroll
+	for (int j = 0; j + 1 < K; j++) aggCut[j] = coarse ? a.aggRow[cta * K + j + 1] - row0 : nrows;
 	const int need0 = a.needPtr[cta], nneed = a.needPtr[cta + 1] - need0;
 	const int blk0 = a.fRowPtr[row0], nblkCta = a.fRowPtr[row1] - blk0;
 	constexpr int REGBLK = Shape::REGBLK;
@@ -322,7 +342,7 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 					// two lists, one after the other (one mixed list, the loads of both boards in flight together, was slower on
 					// ba_kitti_00 with 256 and with 512 threads)
 					bool ok = ll_poll_many<PCG5_BLOCK, PCG5_PCH>(nW, [&](int i) { return wB + 2 * (size_t)s_woff[i]; }, s_w, tag, a.ctl);
-					ok = ok && ll_poll_many<PCG5_BLOCK, PCG5_PCH>(nPl, [&](int i) { return pB + 2 * (size_t)i; }, s_pv, tag, a.ctl);
+					ok = ok && ll_poll_many<PCG5_BLOCK, PPCH>(nPl, [&](int i) { return pB + 2 * (size_t)i; }, s_pv, tag, a.ctl);
 					if (!ok) s_abort = 1;
 				}
 				__syncthreads();
@@ -403,9 +423,10 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 						double wcv;
 						if (world > 1) wcv = s_pv[(q / (6 * Aloc)) * NR + 3 + (q % (6 * Aloc))];
 						else {
-							const int al = q / 6, comp = q - 6 * al;
+							// aggregate ag: part j of the gs CTAs from c0 on (K == 1: j = 0; K > 1: gs = 1)
+							const int ag = q / 6, comp = q - 6 * ag, c0 = ag / K * a.gs, j = ag - ag / K * K;
 							wcv = 0;
-							for (int c = al * a.gs; c < (al + 1) * a.gs; c++) wcv += s_pv[c * NP + 3 + comp];
+							for (int c = c0; c < c0 + a.gs; c++) wcv += s_pv[c * NP + 3 + 6 * j + comp];
 						}
 						const T sc = (T)wcv + (T)beta * s_sc[q];
 						s_sc[q] = sc;
@@ -543,12 +564,12 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 #ifdef CUBA_PCG_TIMING
 			long long t7 = 0;
 #endif
-			// Every (row, component) thread keeps its nine products in registers; a butterfly adds them over the warp, lane 0 leaves the
-			// warp's sums in shared memory and 9 x REPL threads add the eight warps in a fixed order and publish the replicas.
-			double* s_q = reinterpret_cast<double*>(smem_raw + lay.sq);   // [warps][9]; rewritten only after the next pass's barriers
-			double q9[9];
+			// Every (row, component) thread keeps its NPK products in registers; a butterfly adds them over the warp, lane 0 leaves the
+			// warp's sums in shared memory and NP x REPL threads add the warps in a fixed order and publish the replicas.
+			double* s_q = reinterpret_cast<double*>(smem_raw + lay.sq);   // [warps][NPK]; rewritten only after the next pass's barriers
+			double q9[NPK];
 #pragma unroll
-			for (int w = 0; w < 9; w++) q9[w] = 0.0;
+			for (int w = 0; w < NPK; w++) q9[w] = 0.0;
 #pragma unroll
 			for (int pu = 0; pu < NPU; pu++) {
 				const int pair = tid / tpp + pu * PCG5_BLOCK;
@@ -573,15 +594,26 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 				q9[2] += (double)ri * (double)ri;
 				if (coarse) {
 					const T* Zh = a.dims.zhInSmem ? s_zh + 36 * (size_t)dl + comp : a.Zhat + 36 * (size_t)(row0 + li) + comp;
+					int ja = 0;                                                    // the row's aggregate within this CTA
 #pragma unroll
-					for (int q = 0; q < 6; q++) q9[3 + q] += (double)(Zh[6 * q] * wv1);   // (Z^^T w)(q) = sum_comp Z^(comp,q) w(comp)
+					for (int j = 0; j + 1 < K; j++) ja += li >= aggCut[j] ? 1 : 0;
+#pragma unroll
+					for (int q = 0; q < 6; q++) {
+						const double z = (double)(Zh[6 * q] * wv1);                  // (Z^^T w)(q) = sum_comp Z^(comp,q) w(comp)
+#pragma unroll
+						for (int j = 0; j < K; j++) if (ja == j) q9[3 + 6 * j + q] += z;
+					}
 				}
 			}
+			// only the lanes tid % tpp == 0 hold products: the butterfly starts at distance tpp (the shorter ones would add zeros)
 #pragma unroll
-			for (int w = 0; w < 9; w++) if (w < NP) q9[w] = warp_sum(q9[w]);
+			for (int w = 0; w < NPK; w++) if (w < NP) {
+#pragma unroll
+				for (int o = 16; o > 0; o >>= 1) if (o >= tpp) q9[w] += __shfl_xor_sync(0xffffffffu, q9[w], o);
+			}
 			if (lane == 0) {
 #pragma unroll
-				for (int w = 0; w < 9; w++) if (w < NP) s_q[wid * 9 + w] = q9[w];
+				for (int w = 0; w < NPK; w++) if (w < NP) s_q[wid * NPK + w] = q9[w];
 			}
 			__syncthreads();
 #ifdef CUBA_PCG_TIMING
@@ -591,7 +623,7 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 				const int word = tid / PCG5_REPL, rp = tid - word * PCG5_REPL;
 				double v = 0;
 #pragma unroll
-				for (int w8 = 0; w8 < PCG5_BLOCK / 32; w8++) v += s_q[w8 * 9 + word];
+				for (int w8 = 0; w8 < PCG5_BLOCK / 32; w8++) v += s_q[w8 * NPK + word];
 				ll_store(a.pBoard + 2 * (pHalf + (size_t)opar * pStride + ((size_t)rp * G + lc) * NP + word), v, otag);
 			}
 			PCG_T(t8);

@@ -254,14 +254,24 @@ void build_pcg_partition(int numP, int nfull, const std::vector<int>& fRowPtr, c
 	P.nptr[G] = (int)P.ncol.size();
 }
 
-void build_coarse_partition(int numP, const PcgPartition& P, int maxAgg, CoarsePartition& C)
+void build_coarse_partition(int numP, const PcgPartition& P, int maxAgg, CoarsePartition& C, int apc)
 {
 	C = CoarsePartition();
 	const int G = P.G;
-	const int gs = (G + maxAgg - 1) / maxAgg, A = (G + gs - 1) / gs;
-	C.gs = gs; C.A = A;
-	C.aggRow.assign(A + 1, numP);
-	for (int ag = 0; ag < A; ag++) C.aggRow[ag] = P.rows[std::min(ag * gs, G)];
+	if (apc > 1) {
+		// apc aggregates per CTA: the CTA's rows in apc contiguous groups balanced by row count (a CTA with fewer rows: no partition)
+		for (int c = 0; c < G; c++) if (P.rows[c + 1] - P.rows[c] < apc) return;
+		C.gs = 1; C.apc = apc; C.A = G * apc;
+		C.aggRow.assign(C.A + 1, numP);
+		for (int c = 0; c < G; c++)
+			for (int j = 0; j < apc; j++) C.aggRow[c * apc + j] = P.rows[c] + (P.rows[c + 1] - P.rows[c]) * j / apc;
+	} else {
+		const int gs = (G + maxAgg - 1) / maxAgg;
+		C.gs = gs; C.A = (G + gs - 1) / gs;
+		C.aggRow.assign(C.A + 1, numP);
+		for (int ag = 0; ag < C.A; ag++) C.aggRow[ag] = P.rows[std::min(ag * gs, G)];
+	}
+	const int A = C.A;
 	C.rowAgg.assign(numP, 0);
 	for (int ag = 0; ag < A; ag++) for (int r = C.aggRow[ag]; r < C.aggRow[ag + 1]; r++) C.rowAgg[r] = ag;
 	C.naPtr.assign(G + 1, 0);
@@ -334,11 +344,18 @@ const char* check_pcg_partition(int numP, int nfull, const std::vector<int>& fRo
 		if (nn > P.needMax || P.rows[c + 1] - P.rows[c] > P.maxRows || fRowPtr[P.rows[c + 1]] - fRowPtr[P.rows[c]] > P.blkMax) return "maxima too small";
 	}
 	// coarse level
-	const int A = C.A;
+	const int A = C.A, apc = C.apc;
 	if (A < 1 || (int)C.aggRow.size() != A + 1 || C.aggRow[0] != 0 || C.aggRow[A] != numP) return "aggregates do not cover [0, numP)";
+	if (apc < 1 || (apc > 1 && (C.gs != 1 || A != G * apc))) return "aggregates per CTA inconsistent";
 	for (int a = 0; a < A; a++) {
 		if (C.aggRow[a + 1] <= C.aggRow[a]) return "empty aggregate";
-		if (C.aggRow[a] != P.rows[std::min(a * C.gs, G)]) return "aggregate not aligned with a CTA boundary";
+		if (apc == 1 && C.aggRow[a] != P.rows[std::min(a * C.gs, G)]) return "aggregate not aligned with a CTA boundary";
+		if (apc > 1) {
+			// aggregate a is part j of CTA c: it starts at the CTA's first row when j == 0 and never leaves the CTA
+			const int c = a / apc, j = a - c * apc, n = P.rows[c + 1] - P.rows[c];
+			if ((j == 0 && C.aggRow[a] != P.rows[c]) || C.aggRow[a + 1] > P.rows[c + 1]) return "aggregate straddles two CTAs";
+			if (std::abs((C.aggRow[a + 1] - C.aggRow[a]) - n / apc) > 1) return "aggregates of a CTA not balanced by row count";
+		}
 		for (int r = C.aggRow[a]; r < C.aggRow[a + 1]; r++) if (C.rowAgg[r] != a) return "rowAgg inconsistent";
 	}
 	for (int c = 0; c < G; c++) {
@@ -350,7 +367,7 @@ const char* check_pcg_partition(int numP, int nfull, const std::vector<int>& fRo
 			const int pos = C.needAgg[k];
 			if (pos < 0 || pos >= na || al[pos] != C.rowAgg[P.ncol[k]]) return "needAgg does not point at the column's aggregate";
 		}
-		if (C.rowAgg[P.rows[c]] != c / C.gs) return "a CTA's rows are not in aggregate cta / gs";
+		if (C.rowAgg[P.rows[c]] != c / C.gs * apc) return "a CTA's first row is not in aggregate cta / gs * apc";
 	}
 	if (!C.cbPtr.empty()) {
 		const int nblkP = A * (A + 1) / 2;
@@ -372,24 +389,25 @@ const char* check_pcg_partition(int numP, int nfull, const std::vector<int>& fRo
 }
 
 void build_pcg5_plan(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, int world, int numSMs, int maxAgg,
-	int maxRowsPerCta, Pcg5Plan& plan, const PcgPartition* same)
+	int maxRowsPerCta, Pcg5Plan& plan, const PcgPartition* same, int apc)
 {
 	plan = Pcg5Plan();
 	plan.world = world;
-	if (numP < 1 || world < 1 || world > 8) return;
+	if (numP < 1 || world < 1 || world > 8 || apc < 1 || (apc > 1 && world > 1)) return;
 	// CTAs per GPU: about eight rows each
 	int G = std::max(1, std::min(numSMs, (numP / world + 7) / 8));
 	if (world * G > numP) G = std::max(1, numP / world);
-	const int gs = (world * G + maxAgg - 1) / maxAgg;
+	// one aggregate per group of gs CTAs (at most maxAgg of them), or apc aggregates per CTA (maxAgg does not apply)
+	const int gs = apc > 1 ? 1 : (world * G + maxAgg - 1) / maxAgg;
 	G = std::max(gs, G / gs * gs);
-	const int Gt = world * G, A = Gt / gs;
+	const int Gt = world * G, A = Gt / gs * apc;
 	if (Gt > numP || A < 1 || G > numSMs) return;
 	if (same && same->G == Gt && (int)same->rows.size() == Gt + 1 && same->rows[Gt] == numP && (int)same->local.size() == nfull) plan.P = *same;
 	else build_pcg_partition(numP, nfull, fRowPtr, fColInd, Gt, plan.P);
 	// balanced by blocks, a CTA may get more rows than the row sums can take (a large graph on a GPU with fewer SMs, e.g. 10 000 poses
 	// on an H100's 132): balance again with the row count capped
 	if (plan.P.maxRows > maxRowsPerCta) build_pcg_partition(numP, nfull, fRowPtr, fColInd, Gt, plan.P, maxRowsPerCta);
-	build_coarse_partition(numP, plan.P, A, plan.C);
+	build_coarse_partition(numP, plan.P, A, plan.C, apc);
 	if (plan.C.gs != gs || plan.C.A != A || plan.P.maxRows > maxRowsPerCta) return;
 	build_coarse_lists(numP, nfull, fRowPtr, fColInd, plan.C);
 	plan.rowPeers.assign(numP, 0);
@@ -402,21 +420,22 @@ void build_pcg5_plan(int numP, int nfull, const std::vector<int>& fRowPtr, const
 				if (rowRank[j] != c / G) plan.rowPeers[j] |= (unsigned char)(1u << (c / G));
 			}
 	}
-	plan.G = G; plan.gs = gs; plan.A = A;
+	plan.G = G; plan.gs = gs; plan.A = A; plan.apc = apc;
 	plan.ok = true;
 }
 
 const char* check_pcg5_plan(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, const Pcg5Plan& plan)
 {
 	if (!plan.ok) return "plan not ok";
-	const int G = plan.G, W = plan.world, Gt = G * W, gs = plan.gs;
+	const int G = plan.G, W = plan.world, Gt = G * W, gs = plan.gs, apc = plan.apc;
 	if (plan.P.G != Gt) return "virtual CTA count";
-	if (G % gs != 0 || plan.A * gs != Gt) return "aggregates do not tile the ranks";
+	if (apc != plan.C.apc || (apc > 1 && (gs != 1 || W != 1))) return "aggregates per CTA";
+	if (G % gs != 0 || plan.A * gs != Gt * apc) return "aggregates do not tile the ranks";
 	const char* bad = check_pcg_partition(numP, nfull, fRowPtr, fColInd, plan.P, plan.C);
 	if (bad) return bad;
 	// every aggregate lies inside one rank
 	for (int a = 0; a < plan.A; a++) {
-		const int c0 = a * gs, c1 = c0 + gs - 1;
+		const int c0 = a / apc * gs, c1 = c0 + gs - 1;
 		if (c0 / G != c1 / G) return "aggregate straddles two ranks";
 	}
 	// rowPeers: exactly the ranks (not the owner) with a CTA that needs the row

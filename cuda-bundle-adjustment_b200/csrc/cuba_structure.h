@@ -84,8 +84,10 @@ void build_pcg_partition(int numP, int nfull, const std::vector<int>& fRowPtr, c
 
 // Coarse level of the two-level PCG: aggregates = groups of gs consecutive CTAs (at most maxAgg of them), the aggregates every
 // CTA needs, and -- build_coarse_lists -- the fine blocks of every coarse block of the lower triangle in ascending order.
+// With apc > 1 aggregates per CTA instead (gs = 1, A = apc G): the CTA's rows cut into apc contiguous groups balanced by row count,
+// aggregate c apc + j = group j of CTA c; A = 0 when some CTA has fewer than apc rows.
 struct CoarsePartition {
-	int gs = 1, A = 0, maxNeedAgg = 1;
+	int gs = 1, apc = 1, A = 0, maxNeedAgg = 1;
 	std::vector<int> aggRow;   // [A+1] first row of every aggregate
 	std::vector<int> rowAgg;   // [numP]
 	std::vector<int> naPtr;    // [G+1]
@@ -95,7 +97,7 @@ struct CoarsePartition {
 	std::vector<int> cbPtr;    // [A(A+1)/2 + 1]
 	std::vector<int> cbList;   // fine blocks of coarse block (ib >= jb) at index ib (ib+1)/2 + jb
 };
-void build_coarse_partition(int numP, const PcgPartition& P, int maxAgg, CoarsePartition& C);
+void build_coarse_partition(int numP, const PcgPartition& P, int maxAgg, CoarsePartition& C, int apc = 1);
 void build_coarse_lists(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, CoarsePartition& C);
 // invariants of both (nullptr when everything holds)
 const char* check_pcg_partition(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd,
@@ -104,17 +106,17 @@ const char* check_pcg_partition(int numP, int nfull, const std::vector<int>& fRo
 // Plan of the row-distributed two-level PCG (k_pcg5): rows cut into world x G contiguous ranges ("virtual CTAs"), G per GPU;
 // aggregates = groups of gs consecutive virtual CTAs with gs | G, so that no aggregate straddles two ranks; rowPeers[j] = bit
 // mask of the ranks (other than the owner) whose CTAs need row j's w entries.  ok == false: the system is too small / the row
-// ranges too long for the kernel (the engine then keeps the older kernels).
+// ranges too long for the kernel (the engine then keeps the older kernels).  apc > 1 (one GPU only): apc aggregates per CTA.
 struct Pcg5Plan {
 	bool ok = false;
-	int world = 1, G = 0, gs = 1, A = 0;
+	int world = 1, G = 0, gs = 1, A = 0, apc = 1;
 	PcgPartition P;
 	CoarsePartition C;
 	std::vector<unsigned char> rowPeers;
 };
 // `same`: a partition of the same system the caller already has (k_pcg3's); copied instead of rebuilt when its CTA count fits.
 void build_pcg5_plan(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, int world, int numSMs, int maxAgg,
-	int maxRowsPerCta, Pcg5Plan& plan, const PcgPartition* same = nullptr);
+	int maxRowsPerCta, Pcg5Plan& plan, const PcgPartition* same = nullptr, int apc = 1);
 // invariants of a plan (nullptr when everything holds)
 const char* check_pcg5_plan(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, const Pcg5Plan& plan);
 

@@ -226,6 +226,9 @@ int cuba_debug_pcg_partition(const cuba_problem* p, int nCtas, int maxAgg, int32
  * CTAs, aggregates aligned with the ranks, halo masks.  info[8] = ok (0: system too small for this kernel), G, gs, A, needMax,
  * maxRows, maxNeedAgg, number of halo rows.  No device needed. */
 int cuba_debug_pcg5_plan(const cuba_problem* p, int world, int numSMs, int maxAgg, int32_t* info);
+/* The same with aggsPerCta aggregates per CTA (the one-GPU tuned kernel; 1: the plan of cuba_debug_pcg5_plan).  hash (may be null):
+ * FNV-1a over every array of the plan, to compare plans across builds. */
+int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int maxAgg, int aggsPerCta, int32_t* info, uint64_t* hash);
 /* The flat arrays the drop-in class (cuba::CudaBundleAdjustment, csrc/cuba_api.cpp) built in its last initialize(): what optimize()
  * hands to cuba_engine_set_problem.  `dropin` is the object's address; the pointers stay valid until the next initialize().
  * Needs no GPU (tests of the graph container: tombstones, re-added edges, fixed vertices, vertices without edges). */
