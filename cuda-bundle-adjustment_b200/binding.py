@@ -14,6 +14,14 @@ PROFILE_ITEMS = ("0: Initialize Optimizer", "1: Build Structure", "2: Compute Er
                  "4: Schur Complement", "5: Symbolic Decomposition", "6: Numerical Decomposition", "7: Update Solution")
 
 
+# cuba_debug_get_pcg_info (include/cuba_b200.h): info[] fields and the kernel names behind CUBA_PCG_KERNEL_* / CUBA_COARSE_KERNEL_*
+PCG_INFO_LEN = 16
+PCG_INFO_FIELDS = ("kernel", "two_level", "aggs_per_cta", "G", "gs", "A", "maxRows", "capBlocks", "zhInSmem", "coarse_kernel",
+                   "cinfo", "status", "iters", "coarse_rebuilds", "bj_retries", "bad_rebuilds")
+PCG_KERNELS = ("none", "k_pcg", "k_pcg2", "k_pcg3", "k_pcg4", "k_pcg5", "k_pcg5_big", "k_pcg5t")
+COARSE_KERNELS = ("none", "k_coarse_invert", "cluster2<8>", "cluster2<16>", "k_coarse_dense", "k_coarse_chol_cluster")
+
+
 class CubaError(RuntimeError):
     pass
 
@@ -51,7 +59,7 @@ _SYMBOLS = [
     "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
-    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_bench_stage",
+    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_bench_stage",
 ]
 
 
@@ -101,6 +109,8 @@ def load_library():
         "cuba_debug_get_system": [vp, vp, vp, vp, vp, vp],
         "cuba_debug_get_schur": [vp, vp, vp, vp],
         "cuba_debug_get_delta": [vp, vp, vp],
+        "cuba_debug_get_pcg_info": [vp, vp, C.POINTER(d)],
+        "cuba_debug_get_coarse": [vp, vp, vp, vp],
         "cuba_debug_build_structure_host": [C.POINTER(_Problem), i, i, C.POINTER(_Sizes), vp, vp, vp, vp, vp, vp, vp, vp],
         "cuba_debug_pcg_partition": [C.POINTER(_Problem), i, i, vp],
         "cuba_debug_pcg5_plan": [C.POINTER(_Problem), i, i, i, vp],
@@ -365,6 +375,26 @@ class Engine:
         xp = np.zeros((s["numP"], 6)); xl = np.zeros((s["numL"], 3))
         _check(self.L.cuba_debug_get_delta(self.h, _p(xp), _p(xl)))
         return xp, xl
+
+    def pcg_info(self):
+        """what the last solve ran (include/cuba_b200.h: cuba_debug_get_pcg_info), kernels by name"""
+        info = np.zeros(PCG_INFO_LEN, np.int32)
+        lam = C.c_double(0)
+        _check(self.L.cuba_debug_get_pcg_info(self.h, _p(info), C.byref(lam)))
+        out = dict(zip(PCG_INFO_FIELDS, (int(v) for v in info)))
+        out["kernel"] = PCG_KERNELS[out["kernel"]]
+        out["coarse_kernel"] = COARSE_KERNELS[out["coarse_kernel"]]
+        out["two_level"] = bool(out["two_level"])
+        out["coarse_lambda"] = lam.value
+        return out
+
+    def coarse(self):
+        """(aggregate of every free pose, packed lower blocks of Ac = Z^T S Z [A(A+1)/2][36] column-major, fp32 Ac^-1 [6A][6A]) of
+        the k_pcg5 coarse level the last two-level solve applied"""
+        A = self.pcg_info()["A"]
+        agg = np.zeros(self.sizes["numP"], np.int32); AcP = np.zeros((A * (A + 1) // 2, 36)); AcInv = np.zeros((6 * A, 6 * A), np.float32)
+        _check(self.L.cuba_debug_get_coarse(self.h, _p(agg), _p(AcP), _p(AcInv)))
+        return agg, AcP, AcInv
 
     def bench_stage(self, stage, reps=10, flush_l2=True, lam=1.0):
         ms = C.c_double(0)

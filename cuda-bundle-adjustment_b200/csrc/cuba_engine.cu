@@ -195,6 +195,8 @@ struct EngineBase {
 	virtual int dbg_delta(double* xp, double* xl) = 0;
 	virtual int bench_stage(int stage, int reps, int flush, double lambda, double* ms) = 0;
 	virtual int dbg_pcg_timing(long long* out, int maxCtas) = 0;
+	virtual int dbg_pcg_info(int32_t* info, double* coarseLambda) = 0;
+	virtual int dbg_coarse(int32_t* rowAgg, double* AcP, float* AcInv) = 0;
 };
 
 template <typename T>
@@ -396,6 +398,7 @@ struct Engine : EngineBase {
 			(p->E3 > 0 && (!p->idx3 || !p->meas3 || !p->omega3)))
 			return fail(CUBA_ERR_INVALID, "set_problem: null array with a non-zero count");
 		const auto t0 = std::chrono::steady_clock::now();
+		lastPcgKernel = CUBA_PCG_KERNEL_NONE; p5Rebuilds = 0; bjRetries = 0;
 		// Same topology as the problem this engine already holds (sizes, fixed/free split and every (iP, iL) pair identical): only the
 		// numbers changed -- the estimate after a previous optimize(), new measurements -- so every index structure, tile list,
 		// product list and PCG partition on the device stays valid.  Upload the values and re-run the three kernels that scatter them.
@@ -1398,6 +1401,7 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg4<T>, dim3(pcg2Grid), dim3(PCG4_BLOCK), args, pcg4Smem, stream));
 		launches++;
 		lastPcgTwoLevel = true;
+		lastPcgKernel = CUBA_PCG_KERNEL_PCG4;
 		return CUBA_OK;
 	}
 	bool lastPcgTwoLevel = false;
@@ -1434,11 +1438,13 @@ struct Engine : EngineBase {
 			void* args3[] = { (void*)&b };
 			CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg3<T>, dim3(pcg2Grid), dim3(PCG3_BLOCK), args3, pcg2Smem, stream));
 			launches++;
+			lastPcgKernel = CUBA_PCG_KERNEL_PCG3;
 			return CUBA_OK;
 		}
 		void* args[] = { (void*)&a };
 		CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg2<T>, dim3(pcg2Grid), dim3(PCG2_BLOCK), args, pcg2Smem, stream));
 		launches++;
+		lastPcgKernel = CUBA_PCG_KERNEL_PCG2;
 		return CUBA_OK;
 	}
 
@@ -1466,6 +1472,14 @@ struct Engine : EngineBase {
 	int p5Cluster = 0;                             // CTAs of the cluster that factors the coarse matrix (0: one CTA)
 	bool p5CoarseValid = false; int p5CoarseAge = 0; double p5CoarseLambda = 0;
 	size_t p5InvSmem = 0;
+	int p5Apc = 1;                                 // aggregates per CTA of the plan (k_pcg5t)
+	// read by cuba_debug_get_pcg_info only: the kernel of the last solve (CUBA_PCG_KERNEL_*), counters since set_problem, and a
+	// log of the cInfo flag of every k_pcg5 coarse rebuild -- rebuild n writes slot 1 + n % P5_INFO_LOG of cInfo (k_pcg4 keeps
+	// slot 0), so no rebuild's outcome is overwritten by the next one and nothing is copied on the solve's path
+	static constexpr int P5_INFO_LOG = 256;
+	int lastPcgKernel = CUBA_PCG_KERNEL_NONE;
+	long long p5Rebuilds = 0, bjRetries = 0;
+	int* p5InfoSlot() const { return cInfo.p + 1 + (int)(p5Rebuilds % P5_INFO_LOG); }
 	long long p5TagBound = 0;                      // conservative host-side bound on the device tag base
 
 	Pcg5Ctl* p5Ctl(void* base) const { return (Pcg5Ctl*)((unsigned long long*)base + 2 * (p5WWords + p5PWords + p5RWords + p5CWords)); }
@@ -1678,7 +1692,8 @@ struct Engine : EngineBase {
 		CUDA_TRY(cRowOf.upload(CP.rowOf, stream, arena));
 		const size_t nP = (size_t)numP;
 		CUDA_TRY(p5Linv.alloc(36 * nP)); CUDA_TRY(p5R0.alloc(6 * nP)); CUDA_TRY(p5Zhat.alloc(36 * nP)); CUDA_TRY(p5RcRow.alloc(6 * nP)); CUDA_TRY(p5Rc0.alloc(std::max(nc, 1)));
-		CUDA_TRY(cZx.alloc(36 * nP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(cInfo.alloc(1));
+		CUDA_TRY(cZx.alloc(36 * nP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(cInfo.alloc(1 + P5_INFO_LOG));
+		CUDA_TRY(cudaMemsetAsync(cInfo.p, 0, sizeof(int) * cInfo.n, stream));
 		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull));
 		CUDA_TRY(p5AcP.alloc(nblkPz * 36)); CUDA_TRY(p5AcInv.alloc((size_t)nc * nc)); CUDA_TRY(p5Lp.alloc(nblkPz * 36)); CUDA_TRY(p5Wp.alloc(nblkPz * 36)); CUDA_TRY(p5Ld.alloc((size_t)A * 36));
 		if (p5Dense) {
@@ -1698,7 +1713,7 @@ struct Engine : EngineBase {
 			p5WWords = wW; p5PWords = pW; p5RWords = rW; p5CWords = cW;
 			p5TagBound = 0;
 		}
-		p5G = G; p5W = W; p5A = A; p5Gs = gs;
+		p5G = G; p5W = W; p5A = A; p5Gs = gs; p5Apc = plan.apc;
 		if (W > 1) {
 			bool ok = false;
 			int rc = p5Exchange(ok); if (rc) return rc;
@@ -1716,13 +1731,14 @@ struct Engine : EngineBase {
 	int launch_coarse_setup(int A, int cluster, size_t invSmem, const int* cbPtr, const int* cbList, double* AcP, float* AcInv, double* Lp, double* Ld, double* Wp, bool dense = false)
 	{
 		const int nblkP = A * (A + 1) / 2;
+		int* infoP = p5InfoSlot();
 		KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, cRowOf.p, fColInd.p, S.nfull, cZx.p, cU.p);
 		KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, cbPtr, cbList, cU.p, nblkP, AcP);
 		if (dense) {
 			// dense tile Cholesky + inverse on the whole chip (cuba_coarse_dense.cuh): one persistent cooperative kernel
 			CUDA_TRY(cudaMemsetAsync(cdM.p, 0, sizeof(double) * cdM.n, stream));
 			cdense::Args da;
-			da.AcP = AcP; da.A = A; da.M = cdM; da.Lm = cdL; da.Dinv = cdDinv; da.W = cdW; da.AcInv = AcInv; da.info = cInfo; da.bar = gridBar;
+			da.AcP = AcP; da.A = A; da.M = cdM; da.Lm = cdL; da.Dinv = cdDinv; da.W = cdW; da.AcInv = AcInv; da.info = infoP; da.bar = gridBar;
 			void* dargs[] = { (void*)&da };
 			CUDA_TRY(cudaLaunchCooperativeKernel((void*)cdense::k_coarse_dense, dim3(numSMs), dim3(cdense::WARPS * 32), dargs, 0, stream));
 			launches++;
@@ -1735,14 +1751,13 @@ struct Engine : EngineBase {
 			cudaLaunchAttribute at[1];
 			at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
 			lc.attrs = at; lc.numAttrs = 1;
-			int* infoP = cInfo.p;
 			if (cluster == 16) CUDA_TRY(cudaLaunchKernelEx(&lc, k_coarse_chol_cluster2<16>, (const double*)AcP, A, Lp, Ld, AcInv, infoP));
 			else CUDA_TRY(cudaLaunchKernelEx(&lc, k_coarse_chol_cluster2<8>, (const double*)AcP, A, Lp, Ld, AcInv, infoP));
-			k_coarse_trinv<<<A, 256, (size_t)A * 36 * sizeof(double), stream>>>(Lp, Ld, A, Wp, cInfo.p);
-			k_coarse_wtw<<<(nblkP * 36 + 255) / 256, 256, 0, stream>>>(Wp, A, AcInv, cInfo.p);
+			k_coarse_trinv<<<A, 256, (size_t)A * 36 * sizeof(double), stream>>>(Lp, Ld, A, Wp, infoP);
+			k_coarse_wtw<<<(nblkP * 36 + 255) / 256, 256, 0, stream>>>(Wp, A, AcInv, infoP);
 			launches += 2;
 		}
-		else k_coarse_invert<T><<<1, 1024, invSmem, stream>>>(AcP, A, AcInv, cInfo.p);
+		else k_coarse_invert<T><<<1, 1024, invSmem, stream>>>(AcP, A, AcInv, infoP);
 		launches++;
 		CUDA_TRY(cudaGetLastError());
 		return CUBA_OK;
@@ -1775,7 +1790,7 @@ struct Engine : EngineBase {
 			const double lamRatio = (p5CoarseValid && p5CoarseLambda > 0 && curLambda > 0) ? std::max(curLambda / p5CoarseLambda, p5CoarseLambda / curLambda) : 1.0;
 			if (!p5CoarseValid || p5CoarseAge >= refreshEvery || lamRatio > 300.0) {
 				int rc = launch_coarse_setup(A, p5Cluster, p5InvSmem, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5Lp, p5Ld, p5Wp, p5Dense); if (rc) return rc;
-				p5CoarseValid = true; p5CoarseAge = 0; p5CoarseLambda = curLambda;
+				p5CoarseValid = true; p5CoarseAge = 0; p5CoarseLambda = curLambda; p5Rebuilds++;
 			}
 			p5CoarseAge++;
 		}
@@ -1833,6 +1848,7 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaGetLastError());
 		if (p5Dist) { int rc = allreduce(xp.p, 6 * (size_t)numP, true); if (rc) return rc; }
 		lastPcgTwoLevel = twoLevel;
+		lastPcgKernel = p5Tuned ? CUBA_PCG_KERNEL_PCG5T : p5Big ? CUBA_PCG_KERNEL_PCG5_BIG : CUBA_PCG_KERNEL_PCG5;
 		return CUBA_OK;
 	}
 
@@ -1864,6 +1880,7 @@ struct Engine : EngineBase {
 		void* args[] = { (void*)&a };
 		CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg<T>, dim3(pcgGrid), dim3(PCG_BLOCK), args, 0, stream));
 		launches++;
+		lastPcgKernel = CUBA_PCG_KERNEL_PCG;
 		return CUBA_OK;
 	}
 
@@ -1908,6 +1925,7 @@ struct Engine : EngineBase {
 			launches++;
 			CUDA_TRY(cudaGetLastError());
 			hScal->pcg.iters = 0; hScal->pcg.status = 0;
+			lastPcgKernel = CUBA_PCG_KERNEL_NONE;
 		} else if (S.numL > 0) {
 			nScaleL = (S.numL + RED_BLOCK - 1) / RED_BLOCK;
 			k_solve_landmarks_only<T><<<nScaleL, RED_BLOCK, 0, stream>>>(invHll, bl, S.numL, lam, Xw[cur], Xw[cur ^ 1], xl, scalePartialL);
@@ -2001,7 +2019,7 @@ struct Engine : EngineBase {
 					const double loose = sizeof(T) == 8 ? 1e-6 : 1e-3;
 					ok = ps.status == 0 || (ps.status == 1 && ps.rz0 > 0 && ps.rz <= loose * loose * ps.rz0);
 					if (ps.status == 2 && lastPcgTwoLevel && attempt == 0) {
-						forceBlockJacobi = true; coarseValid = false; p5CoarseValid = false;
+						forceBlockJacobi = true; coarseValid = false; p5CoarseValid = false; bjRetries++;
 						rc = stage_commit(0); if (rc) return rc;
 						continue;
 					}
@@ -2181,6 +2199,53 @@ struct Engine : EngineBase {
 		return n;
 	}
 
+	// include/cuba_b200.h: cuba_debug_get_pcg_info / cuba_debug_get_coarse (host copies; no engine state changes)
+	int dbg_pcg_info(int32_t* info, double* coarseLambda) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "no problem");
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		PcgStatus ps{};
+		CUDA_TRY(cudaMemcpy(&ps, &dScal.p->pcg, sizeof(ps), cudaMemcpyDeviceToHost));
+		int last = -1, bad = 0;
+		if (p5Ok && p5A > 0 && p5Rebuilds > 0) {
+			const int nlog = (int)std::min<long long>(p5Rebuilds, P5_INFO_LOG);
+			std::vector<int> log(nlog);
+			CUDA_TRY(cudaMemcpy(log.data(), cInfo.p + 1, sizeof(int) * nlog, cudaMemcpyDeviceToHost));
+			for (int v : log) if (v != 0) bad++;
+			last = log[(int)((p5Rebuilds - 1) % P5_INFO_LOG)];
+		}
+		int coarseKernel = CUBA_COARSE_KERNEL_NONE;
+		if (lastPcgTwoLevel && lastPcgKernel == CUBA_PCG_KERNEL_PCG4) coarseKernel = pcg4Cluster ? CUBA_COARSE_KERNEL_PCG4_CLUSTER : CUBA_COARSE_KERNEL_INVERT;
+		else if (lastPcgTwoLevel && p5Ok)
+			coarseKernel = p5Dense ? CUBA_COARSE_KERNEL_DENSE : p5Cluster == 16 ? CUBA_COARSE_KERNEL_CLUSTER16 : p5Cluster == 8 ? CUBA_COARSE_KERNEL_CLUSTER8 : CUBA_COARSE_KERNEL_INVERT;
+		const bool tuned = p5Ok && p5Tuned;
+		const int32_t v[CUBA_PCG_INFO_LEN] = {
+			lastPcgKernel, lastPcgKernel != CUBA_PCG_KERNEL_NONE && lastPcgTwoLevel ? 1 : 0,
+			p5Ok ? p5Apc : 0, p5Ok ? p5G : 0, p5Ok ? p5Gs : 0, p5Ok ? p5A : 0,
+			p5Ok ? (tuned ? p5tDims.maxRows : p5Dims.maxRows) : 0, p5Ok ? (tuned ? p5tDims.capBlocks : p5Dims.capBlocks) : 0,
+			p5Ok ? (tuned ? p5tDims.zhInSmem : p5Dims.zhInSmem) : 0,
+			coarseKernel, last, ps.status, ps.iters, (int32_t)p5Rebuilds, (int32_t)bjRetries, bad };
+		if (info) memcpy(info, v, sizeof(v));
+		if (coarseLambda) *coarseLambda = p5CoarseValid ? p5CoarseLambda : 0.0;
+		return CUBA_OK;
+	}
+	int dbg_coarse(int32_t* rowAgg, double* oAcP, float* oAcInv) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "no problem");
+		if (!p5Ok || p5A < 1 || !p5CoarseValid) return fail(CUBA_ERR_STATE, "debug_get_coarse: no coarse level of k_pcg5 has been built");
+		const int A = p5A, nc = 6 * A;
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		if (rowAgg) {
+			std::vector<int> ptr(A + 1);
+			CUDA_TRY(cudaMemcpy(ptr.data(), p5AggRow.p, sizeof(int) * (A + 1), cudaMemcpyDeviceToHost));
+			for (int i = 0; i < S.numP; i++) rowAgg[i] = -1;
+			for (int ag = 0; ag < A; ag++) for (int i = ptr[ag]; i < ptr[ag + 1] && i < S.numP; i++) rowAgg[i] = ag;
+		}
+		if (oAcP) CUDA_TRY(cudaMemcpy(oAcP, p5AcP.p, sizeof(double) * 36 * ((size_t)A * (A + 1) / 2), cudaMemcpyDeviceToHost));
+		if (oAcInv) CUDA_TRY(cudaMemcpy(oAcInv, p5AcInv.p, sizeof(float) * (size_t)nc * nc, cudaMemcpyDeviceToHost));
+		return CUBA_OK;
+	}
+
 	// ---- micro-benchmarks --------------------------------------------------------------------------------
 	int bench_stage(int stage, int reps, int flush, double lambda, double* ms) override
 	{
@@ -2352,6 +2417,8 @@ int cuba_debug_get_hsc_structure(cuba_engine* e, int32_t* rowPtr, int32_t* colIn
 int cuba_debug_get_system(cuba_engine* e, double* Hpp, double* bp, double* Hll, double* bl, double* Hpl) { ENGINE_OR_FAIL(e); return e->impl->dbg_system(Hpp, bp, Hll, bl, Hpl); }
 int cuba_debug_get_schur(cuba_engine* e, double* Hsc, double* bsc, double* invHll) { ENGINE_OR_FAIL(e); return e->impl->dbg_schur(Hsc, bsc, invHll); }
 int cuba_debug_get_delta(cuba_engine* e, double* xp, double* xl) { ENGINE_OR_FAIL(e); return e->impl->dbg_delta(xp, xl); }
+int cuba_debug_get_pcg_info(cuba_engine* e, int32_t* info, double* coarse_lambda) { ENGINE_OR_FAIL(e); return e->impl->dbg_pcg_info(info, coarse_lambda); }
+int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* AcInv) { ENGINE_OR_FAIL(e); return e->impl->dbg_coarse(aggRow, AcP, AcInv); }
 int cuba_debug_build_structure_host(const cuba_problem* p, int rank, int world, cuba_sizes* sizes,
 	int32_t* hplColPtr, int32_t* hplRowInd, int32_t* edge2Hpl, int32_t* hscRowPtr, int32_t* hscColInd,
 	int32_t* fullRowPtr, int32_t* fullColInd, int32_t* shard)

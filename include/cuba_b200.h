@@ -208,6 +208,39 @@ int cuba_debug_get_system(cuba_engine* e, double* Hpp /*36*numP*/, double* bp /*
 int cuba_debug_get_schur(cuba_engine* e, double* Hsc /*36*nblk, upper*/, double* bsc /*6*numP*/, double* invHll /*9*numL*/);
 int cuba_debug_get_delta(cuba_engine* e, double* xp /*6*numP*/, double* xl /*3*numL*/);
 
+/* What the last cuba_stage_solve (or the last trial of optimize) ran, for tests of the PCG and its two-level preconditioner.
+ * info[CUBA_PCG_INFO_LEN]:
+ *   0 kernel (CUBA_PCG_KERNEL_*)             1 two-level solve (0/1)
+ *   2..8 the k_pcg5 plan (zeros without one): aggregates per CTA, G (CTAs), gs (CTAs per aggregate), A (aggregates; nc = 6A),
+ *        maxRows (most rows of one CTA), capBlocks (blocks cached in shared memory per CTA), zhInSmem (Z^ rows in shared memory)
+ *   9 coarse-inverse kernel of the last solve (CUBA_COARSE_KERNEL_*; NONE for a block-Jacobi solve)
+ *  10 cInfo of the last k_pcg5 coarse rebuild (0 ok, 1 not positive definite; -1 none yet)
+ *  11 status of the last PCG (0 converged, 1 iteration cap, 2 breakdown)     12 its iterations
+ *  13 k_pcg5 coarse rebuilds since set_problem                                14 block-Jacobi retries of optimize() since set_problem
+ *  15 of the last 256 k_pcg5 coarse rebuilds, those whose cInfo was not 0
+ * coarse_lambda: the damping at which the current k_pcg5 coarse matrix was assembled (the inverse is reused across solves; 0 if
+ * there is none).  Either pointer may be NULL. */
+#define CUBA_PCG_INFO_LEN 16
+#define CUBA_PCG_KERNEL_NONE 0            /* no PCG: pose-only or landmark-only systems */
+#define CUBA_PCG_KERNEL_PCG 1
+#define CUBA_PCG_KERNEL_PCG2 2
+#define CUBA_PCG_KERNEL_PCG3 3
+#define CUBA_PCG_KERNEL_PCG4 4
+#define CUBA_PCG_KERNEL_PCG5 5            /* k_pcg5<T, false>: the legacy shape */
+#define CUBA_PCG_KERNEL_PCG5_BIG 6        /* k_pcg5<T, true> */
+#define CUBA_PCG_KERNEL_PCG5T 7           /* k_pcg5t<T, K>, K = info[2] */
+#define CUBA_COARSE_KERNEL_NONE 0
+#define CUBA_COARSE_KERNEL_INVERT 1       /* k_coarse_invert: one CTA */
+#define CUBA_COARSE_KERNEL_CLUSTER8 2     /* k_coarse_chol_cluster2<8> */
+#define CUBA_COARSE_KERNEL_CLUSTER16 3    /* k_coarse_chol_cluster2<16> */
+#define CUBA_COARSE_KERNEL_DENSE 4        /* cdense::k_coarse_dense: the whole chip */
+#define CUBA_COARSE_KERNEL_PCG4_CLUSTER 5 /* k_coarse_chol_cluster of k_pcg4 */
+int cuba_debug_get_pcg_info(cuba_engine* e, int32_t* info, double* coarse_lambda);
+/* The coarse level of k_pcg5 as the last two-level solve applied it: aggRow[numP] the aggregate of every free pose, AcP the packed
+ * lower block triangle of Ac = Z^T S Z (block (ib >= jb) at (ib (ib+1)/2 + jb) * 36, column-major 6x6; 36 A (A+1)/2 doubles) and
+ * AcInv its fp32 inverse [6A][6A].  Fails when no coarse level has been built.  Any pointer may be NULL. */
+int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* AcInv);
+
 /* Host-only (no CUDA call): builds the index structures from the (iP,iL) lists exactly as
  * cuba_engine_set_problem does and copies them out -- the not-gpu tests check them against the oracle.
  * Sizes are returned first with all array pointers NULL, then the arrays on a second call. */
