@@ -2060,9 +2060,10 @@ struct Engine : EngineBase {
 		std::vector<T> hp((size_t)S.Pall * 8), hx((size_t)S.Lall * 4);
 		g_d2hBytes += (long long)(sizeof(T) * (hp.size() + hx.size()));
 		CUDA_TRY(cudaMemcpyAsync(hp.data(), pose[cur].p, sizeof(T) * hp.size(), cudaMemcpyDeviceToHost, stream));
-		if (world > 1 && S.numL > 0) {
+		if (world > 1 && comm && S.numL > 0) {
 			// all-gather of the sharded landmarks: every rank broadcasts its own range in place (one grouped NCCL call).
 			// The trial buffer is free between LM iterations and serves as the gather target.
+			// (!comm: a CUBA_DRY_SHARD engine returns its own buffer -- its landmarks updated, the others as uploaded)
 			T* tmp = Xw[cur ^ 1].p;
 			trialValid = false;
 			CUDA_TRY(cudaMemcpyAsync(tmp, Xw[cur].p, sizeof(T) * 4 * (size_t)S.Lall, cudaMemcpyDeviceToDevice, stream));

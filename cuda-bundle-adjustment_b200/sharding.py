@@ -31,6 +31,16 @@ def shard_bounds(iL_of_edges, Lall, world):
     return b
 
 
+def sub_problem(prob, lo, hi):
+    """The problem made of the edges of the landmarks [lo, hi) only; every vertex is kept (the engine replicates the poses and
+    keeps the foreign landmarks as uploaded).  Rank 0's share of a sharded run is exactly the LM run of this problem."""
+    p = prob.copy()
+    m2 = (prob.idx2[:, 1] >= lo) & (prob.idx2[:, 1] < hi); m3 = (prob.idx3[:, 1] >= lo) & (prob.idx3[:, 1] < hi)
+    p.idx2, p.meas2, p.omega2 = prob.idx2[m2].copy(), prob.meas2[m2].copy(), prob.omega2[m2].copy()
+    p.idx3, p.meas3, p.omega3 = prob.idx3[m3].copy(), prob.meas3[m3].copy(), prob.omega3[m3].copy()
+    return p
+
+
 def allreduce_bytes_per_trial(numP, nblk_full, scalar_bytes=8):
     """bytes each rank contributes per LM trial / per linearisation (for DESIGN.md and the bench report)."""
     return {"per_linearize": (42 * numP + 1) * scalar_bytes, "per_trial": (36 * nblk_full + 6 * numP) * scalar_bytes + 16}

@@ -19,15 +19,6 @@ def _free_port():
     s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
 
 
-def _sub_problem(prob, lo, hi):
-    """the shard's edges only (vertices are replicated, like the engine's pose replicas)"""
-    p = prob.copy()
-    m2 = (prob.idx2[:, 1] >= lo) & (prob.idx2[:, 1] < hi); m3 = (prob.idx3[:, 1] >= lo) & (prob.idx3[:, 1] < hi)
-    p.idx2, p.meas2, p.omega2 = prob.idx2[m2].copy(), prob.meas2[m2].copy(), prob.omega2[m2].copy()
-    p.idx3, p.meas3, p.omega3 = prob.idx3[m3].copy(), prob.meas3[m3].copy(), prob.omega3[m3].copy()
-    return p
-
-
 def _worker(rank, world, port, q):
     sys.path.insert(0, ROOT)
     import __graft_entry__ as ge
@@ -39,7 +30,7 @@ def _worker(rank, world, port, q):
     b = pkg.sharding.shard_bounds(iL, prob.Lall, world)
     s = pkg.build_structure_host(prob, rank, world)
     assert (s["shard"][0], s["shard"][1]) == (b[rank], b[rank + 1])
-    o = oracle.Oracle(_sub_problem(prob, b[rank], b[rank + 1]), *HUBER)
+    o = oracle.Oracle(pkg.sharding.sub_problem(prob, b[rank], b[rank + 1]), *HUBER)
     chi = o.compute_errors(); o.build_system()
     Hpp, bp, Hll, bl, Hpl = o.system()
     t = torch.from_numpy(np.concatenate([Hpp.ravel(), bp.ravel(), [chi]]))
