@@ -59,7 +59,7 @@ _SYMBOLS = [
     "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
-    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_bench_stage",
+    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_bench_stage",
 ]
 
 
@@ -111,6 +111,7 @@ def load_library():
         "cuba_debug_get_delta": [vp, vp, vp],
         "cuba_debug_get_pcg_info": [vp, vp, C.POINTER(d)],
         "cuba_debug_get_coarse": [vp, vp, vp, vp],
+        "cuba_debug_coarse_inverse": [vp, vp, i, vp, vp],
         "cuba_debug_build_structure_host": [C.POINTER(_Problem), i, i, C.POINTER(_Sizes), vp, vp, vp, vp, vp, vp, vp, vp],
         "cuba_debug_pcg_partition": [C.POINTER(_Problem), i, i, vp],
         "cuba_debug_pcg5_plan": [C.POINTER(_Problem), i, i, i, vp],
@@ -395,6 +396,18 @@ class Engine:
         agg = np.zeros(self.sizes["numP"], np.int32); AcP = np.zeros((A * (A + 1) // 2, 36)); AcInv = np.zeros((6 * A, 6 * A), np.float32)
         _check(self.L.cuba_debug_get_coarse(self.h, _p(agg), _p(AcP), _p(AcInv)))
         return agg, AcP, AcInv
+
+    def coarse_inverse(self, AcP):
+        """(fp32 Ac^-1 [6A][6A], info) of k_coarse_dense run on the packed lower blocks AcP [A(A+1)/2][36] (column-major), as
+        coarse() returns them; info 1: not positive definite, Ac^-1 zeroed"""
+        AcP = np.ascontiguousarray(AcP, dtype=np.float64)
+        nb = AcP.shape[0]
+        A = int(round(((8 * nb + 1) ** 0.5 - 1) / 2))
+        assert A * (A + 1) // 2 == nb and AcP.shape[1:] == (36,), AcP.shape
+        AcInv = np.zeros((6 * A, 6 * A), np.float32)
+        info = C.c_int(-1)
+        _check(self.L.cuba_debug_coarse_inverse(self.h, _p(AcP), A, _p(AcInv), C.byref(info)))
+        return AcInv, info.value
 
     def bench_stage(self, stage, reps=10, flush_l2=True, lam=1.0):
         ms = C.c_double(0)

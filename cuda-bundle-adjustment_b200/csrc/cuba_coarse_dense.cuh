@@ -1,20 +1,28 @@
-// cuba_coarse_dense.cuh -- explicit inverse of the coarse matrix Ac = Z^T S Z of the two-level PCG (cuba_pcg5.cuh) by a dense,
-// tile-parallel Cholesky on the whole chip.
+// cuba_coarse_dense.cuh -- explicit inverse of the coarse matrix Ac = Z^T S Z of the two-level PCG (cuba_pcg5.cuh) by a blocked
+// symmetric sweep (block Gauss-Jordan on an SPD matrix, with every pivot applied through its Cholesky factor) on the whole chip.
 //
 // The cluster kernels of cuba_pcg4.cuh keep the packed 6x6-block triangle in the shared memory of 8 / 16 CTAs and walk it one
 // block column at a time: A aggregates = A x (diagonal factorisation by one warp + two cluster barriers), plus the triangular
 // inverse.  The matrix is tiny (at most 6A x 6A fp64, L2 resident) and the arithmetic is under a GFLOP: the time is all dependent
-// steps.  This kernel cuts the number of
-// dependent steps from A + A to 6A/16 + 6A/16 by working on plain 16 x 16 scalar tiles of the dense matrix, and spreads every
-// step over all SMs (one persistent cooperative kernel, the grid barrier of cuba_pcg2.cuh between steps):
-//   phase 0  packed blocks -> dense lower triangle M (padded to a multiple of 16 with a unit diagonal);
-//   phase 1  right-looking Cholesky: per step k every CTA factors the 16 x 16 diagonal tile itself (one warp, no
-//            barrier), then one WARP per trailing tile (i, j) forms the two panel tiles it needs on the fly
-//            (P_i = M_ik L_kk^-T: redundant across tiles, but it removes the panel barrier) and updates M_ij -= P_i P_j^T;
-//            the warp of tile (i, i) also stores P_i as the factor's tile L_ik;  ONE grid barrier per step;
-//   phase 2  W = L^-1, one CTA per tile column (columns are independent, a column is sequential in i);
-//   phase 3  Ac^-1 = W^T W, one warp per tile, written in fp32 to both triangles (the PCG applies it in fp32, see cuba_pcg4.cuh).
-// Fixed summation order everywhere: bit-reproducible.  On a non-positive pivot the inverse is zeroed (block-Jacobi alone).
+// steps.  A sweep does the work of the Cholesky factorisation, the triangular inverse and W^T W in one pass of 6A/32 steps over
+// 32 x 32 scalar tiles of the dense matrix, each step spread over all SMs (one persistent cooperative kernel, the grid barrier of
+// cuba_pcg2.cuh between steps).  For the pivot tile K, with A_KK = L L^T:
+//     Q_I   = A_IK L^-T                      every I != K
+//     A_IJ -= Q_I Q_J^T                      every lower tile I >= J, I, J != K
+//     A_IK  = Q_I L^-1,  A_KK = -L^-T L^-1
+// and after the last step A = -Ac^-1.  The update is applied as Q_I Q_J^T, never through the explicit P = A_KK^-1: on the
+// coarse matrix of rows_11k at lambda 0.1 (condition ~1e15, most of it scaling) A_IK P A_KJ loses the inverse to 4e-5 of its
+// largest entry, the factored form keeps it at 2e-8, as a Cholesky inverse does.  Only the lower tiles are kept (A_KJ = A_JK^T), so
+// the result is symmetric by construction; diagonal tiles are mirrored from their lower triangle whenever they are stored.
+//   phase 0  packed blocks -> lower tiles of copy 0 (padded to a multiple of 32 with a unit diagonal);
+//   step K   reads copy K & 1 and writes copy (K + 1) & 1, every lower tile, so that nothing is read after it is rewritten;
+//            every CTA factors the pivot tile itself in registers (warp 0: 32 scalar Cholesky steps, then L^-1 by forward
+//            substitution, no hop) while its warps stage their tiles; one WARP per trailing tile forms Q_I and Q_J on the fp64
+//            tensor pipe (redundant across the tiles of a row, but it removes the panel barrier) and updates its tile, and the warp
+//            of tile (I, I) also stores Q_I L^-1 as the new panel tile;  ONE grid barrier per step;  the last step writes -A in
+//            fp32 to both triangles of Ac^-1 (the PCG applies it in fp32, see cuba_pcg4.cuh) instead of a copy.
+// Fixed summation order everywhere, no atomics: bit-reproducible.  On a non-positive pivot the inverse is zeroed (block-Jacobi
+// alone).
 #pragma once
 
 #include "cuba_pcg4.cuh"
@@ -22,272 +30,279 @@
 namespace cuba_b200 {
 namespace cdense {
 
-constexpr int NB = 16;                 // tile edge
+constexpr int NB = 32;                 // tile edge
+constexpr int TT = NB * NB;            // doubles per stored tile (row-major)
 constexpr int WARPS = 8;
-constexpr int TS = NB + 1;             // padded row stride of a staged tile
+constexpr int TS = NB + 4;             // row stride of a staged tile: the fragment loads of both orientations hit 16 distinct banks
+constexpr size_t SMEM = ((size_t)(2 * WARPS + 2) * NB * TS + NB) * sizeof(double);
 
 struct Args {
 	const double* AcP;                 // packed lower block triangle, block (ib >= jb) at (ib (ib+1)/2 + jb) * 36, column-major 6x6
 	int A;                             // aggregates: n = 6 A
-	double* M;                         // [np][np] column-major work matrix (lower triangle), zeroed by the host before the launch
-	double* Lm;                        // [np][np] factor L (lower)
-	double* Dinv;                      // [np/16][256] inverses of the diagonal tiles of L, row-major 16x16
-	double* W;                         // [np][np] L^-1 (lower)
+	double* T;                         // [2][nt (nt+1) / 2][NB * NB] two copies of the lower tiles, tile (I >= J) at I (I+1)/2 + J
 	float* AcInv;                      // [n][n] out
 	int* info;                         // 0 ok, 1 not positive definite
 	GridBar* bar;
 };
 
-__device__ __forceinline__ double ldcg(const double* p) { return __ldcg(p); }
+__host__ __device__ constexpr size_t tiles(int nt) { return (size_t)nt * (nt + 1) / 2; }
+__device__ __forceinline__ const double* tile(const double* C, int I, int J) { return C + ((size_t)I * (I + 1) / 2 + J) * TT; }
+__device__ __forceinline__ double* tile(double* C, int I, int J) { return C + ((size_t)I * (I + 1) / 2 + J) * TT; }
 
-// lower Cholesky factor of the 16x16 tile in sD (row-major, stride TS) in place, its inverse (lower) into sLi; one warp.
-// Returns false on a non-positive pivot.
-__device__ __forceinline__ bool chol16(double* sD, double* sLi, int lane)
+// t -> (i, j), i >= j, of the lower triangle enumerated row by row
+__device__ __forceinline__ void tri_decode(int t, int& i, int& j)
 {
-	bool ok = true;
-	double rdiag = 0.0;                 // lane j ends up with 1 / L(j,j)
-	for (int j = 0; j < NB; j++) {
-		const double d = sD[j * TS + j];
-		if (!(d > 0)) { ok = false; break; }
-		const double sq = sqrt(d), rs = 1.0 / sq;            // one division per column, the scaling multiplies
-		__syncwarp();
-		if (lane == j) { sD[j * TS + j] = sq; rdiag = rs; }
-		else if (lane > j && lane < NB) sD[lane * TS + j] = sD[lane * TS + j] * rs;
-		__syncwarp();
-		if (lane > j && lane < NB) {
-			const double lrj = sD[lane * TS + j];
-			for (int c = j + 1; c <= lane; c++) sD[lane * TS + c] -= lrj * sD[c * TS + j];
+	i = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+	while ((i + 1) * (i + 2) / 2 <= t) i++;
+	while (i * (i + 1) / 2 > t) i--;
+	j = t - i * (i + 1) / 2;
+}
+
+// one warp copies a stored tile into shared memory (row stride TS) with 16-byte cp.async through L2
+__device__ __forceinline__ void stage(double* s, const double* g, int lane)
+{
+#pragma unroll
+	for (int e = lane; e < TT / 2; e += 32) {
+		const int r = e >> 4, c = (e & 15) * 2;
+		cp_async16(s + r * TS + c, g + r * NB + c);
+	}
+	asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// 32 x 32 x 32 product on the fp64 tensor pipe: D(8 bi + l/4, 8 bj + 2 (l%4) + h) += sum_m X(row, m) Y(m, col), with
+// X(r, m) = sX[r * xr + m * xc] and Y(m, c) = sY[m * yr + c * yc]; the k-steps in order
+__device__ __forceinline__ void mma32(double (&D)[4][4][2], const double* sX, int xr, int xc, const double* sY, int yr, int yc, int lane)
+{
+	const int r = lane >> 2, q = lane & 3;
+	const double* xb = sX + r * xr + q * xc;
+	const double* yb = sY + q * yr + r * yc;
+#pragma unroll
+	for (int s = 0; s < NB / 4; s++) {
+		double a[4], b[4];
+#pragma unroll
+		for (int u = 0; u < 4; u++) { a[u] = xb[8 * u * xr + 4 * s * xc]; b[u] = yb[4 * s * yr + 8 * u * yc]; }
+#pragma unroll
+		for (int bi = 0; bi < 4; bi++)
+#pragma unroll
+			for (int bj = 0; bj < 4; bj++) dmma884(D[bi][bj][0], D[bi][bj][1], a[bi], b[bj]);
+	}
+}
+
+// sgn x accumulator fragments -> shared memory (row-major, stride TS)
+__device__ __forceinline__ void frag_store(double* s, const double (&D)[4][4][2], double sgn, int lane)
+{
+	const int r = lane >> 2, c = 2 * (lane & 3);
+#pragma unroll
+	for (int bi = 0; bi < 4; bi++)
+#pragma unroll
+		for (int bj = 0; bj < 4; bj++) *reinterpret_cast<double2*>(s + (8 * bi + r) * TS + 8 * bj + c) = make_double2(sgn * D[bi][bj][0], sgn * D[bi][bj][1]);
+}
+
+// a finished tile in shared memory (element (r, c) = sgn s[r * sr + c * sc]; a diagonal tile mirrored from its lower triangle)
+// -> tile (I, J) of the next copy, or, at the last step, -value in fp32 to both triangles of Ac^-1
+__device__ __forceinline__ void tile_out(const double* s, int sr, int sc, double sgn, bool diag, int I, int J, double* dst, bool last,
+                                         float* AcInv, int n, int lane)
+{
+	auto at = [&](int r, int c) { if (diag && r < c) { const int t = r; r = c; c = t; } return sgn * s[r * sr + c * sc]; };
+	if (!last) {
+		for (int e = lane; e < TT / 2; e += 32) {
+			const int r = e >> 4, c = (e & 15) * 2;
+			__stcg(reinterpret_cast<double2*>(dst + r * NB + c), make_double2(at(r, c), at(r, c + 1)));
 		}
-		__syncwarp();
+		return;
 	}
-	if (!ok) return false;
-	// column q of the inverse by forward substitution (lane q); the reciprocals of the diagonal come by shuffle
-	double col[NB];
-#pragma unroll
-	for (int i = 0; i < NB; i++) col[i] = 0.0;
-	const int q = lane;
-#pragma unroll
-	for (int i = 0; i < NB; i++) {
-		const double ri = __shfl_sync(0xffffffffu, rdiag, i);
-		if (q < NB && i >= q) {
-			if (i == q) col[i] = ri;
-			else {
-				double s = 0;
-#pragma unroll
-				for (int k = 0; k < NB; k++) if (k >= q && k < i) s += sD[i * TS + k] * col[k];
-				col[i] = -s * ri;
-			}
-		}
+	for (int e = lane; e < TT; e += 32) {
+		const int r = e >> 5, c = e & 31;
+		const int row = NB * I + r, col = NB * J + c;
+		if (row < n && col < n) AcInv[(size_t)row * n + col] = (float)-at(r, c);
+		const int row2 = NB * J + r, col2 = NB * I + c;                  // mirror: element (c, r) of the tile
+		if (I != J && row2 < n && col2 < n) AcInv[(size_t)row2 * n + col2] = (float)-at(c, r);
 	}
-	if (q < NB) {
-#pragma unroll
-		for (int i = 0; i < NB; i++) sLi[i * TS + q] = i >= q ? col[i] : 0.0;
-	}
-	__syncwarp();
-	return true;
 }
 
 __global__ void __launch_bounds__(WARPS * 32, 1) k_coarse_dense(const Args a)
 {
-	__shared__ double sD[NB * TS], sLi[NB * TS];
-	__shared__ double sP[WARPS][2][NB * TS];         // per warp: two staged tiles (phase 2: [w][1] = partial sums of warp w)
+	extern __shared__ __align__(16) double smem[];
+	double* sN = smem;                                 // L^-1 of this step's pivot (lower), row-major, stride TS
+	double* sPv = sN + NB * TS;                        // warp 0: L, then -P of CTA 0
+	double* sRow = sPv + NB * TS;                      // warp 0: a column of L / the reciprocals of its diagonal
+	double* sW = sRow + NB;                            // [WARPS][2][NB * TS] per warp: two staged tiles
 	__shared__ int s_fail;
 	__shared__ unsigned int s_gen;
 	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
 	const int G = gridDim.x, cta = blockIdx.x;
-	const int n = 6 * a.A, nt = (n + NB - 1) / NB, np = nt * NB;
-	const int nwarps = G * WARPS, gw = cta * WARPS + wid;
+	const int n = 6 * a.A, nt = (n + NB - 1) / NB;
 	if (tid == 0) { s_gen = ld_acquire_u32(&a.bar->gen); s_fail = 0; }
 	__syncthreads();
 	unsigned int gen = s_gen;
-	// lane -> entries of a tile: row r = lane / 2, columns c0 .. c0 + 7
-	const int r = lane >> 1, c0 = (lane & 1) * 8;
 
-	// ---- phase 0: packed 6x6 blocks -> dense lower triangle; unit diagonal in the padding ----
+	// ---- phase 0: packed 6x6 blocks -> lower tiles of copy 0 (lower triangle of the diagonal blocks); unit diagonal in the padding ----
 	{
-		const int nblkP = a.A * (a.A + 1) / 2;
-		for (long long e = (long long)cta * blockDim.x + tid; e < (long long)nblkP * 36; e += (long long)G * blockDim.x) {
-			const int b = (int)(e / 36), rc = (int)(e - 36LL * b), c = rc / 6, rr = rc - 6 * c;
-			int ib = (int)((sqrt(8.0 * b + 1.0) - 1.0) * 0.5);
-			while ((ib + 1) * (ib + 2) / 2 <= b) ib++;
-			while (ib * (ib + 1) / 2 > b) ib--;
-			const int jb = b - ib * (ib + 1) / 2;
-			const int row = 6 * ib + rr, col = 6 * jb + c;
-			if (row >= col) __stcg(a.M + (size_t)col * np + row, a.AcP[e]);
+		const long long tot = (long long)tiles(nt) * TT;
+		for (long long e = (long long)cta * blockDim.x + tid; e < tot; e += (long long)G * blockDim.x) {
+			const int t = (int)(e / TT), rc = (int)(e - (long long)t * TT);
+			int I, J;
+			tri_decode(t, I, J);
+			int row = NB * I + (rc >> 5), col = NB * J + (rc & 31);
+			if (row < col) { const int x = row; row = col; col = x; }
+			double v = row == col ? 1.0 : 0.0;
+			if (row < n) {
+				const int ib = row / 6, jb = col / 6;
+				v = a.AcP[((size_t)ib * (ib + 1) / 2 + jb) * 36 + (col - 6 * jb) * 6 + (row - 6 * ib)];
+			}
+			__stcg(a.T + e, v);
 		}
-		for (int i = n + cta * blockDim.x + tid; i < np; i += G * blockDim.x) __stcg(a.M + (size_t)i * np + i, 1.0);
 	}
 	grid_barrier(a.bar, G, gen);
 
-	// ---- phase 1: Cholesky ----
-	for (int k = 0; k < nt; k++) {
+	double* sA = sW + (size_t)wid * 2 * NB * TS;
+	double* sB = sA + NB * TS;
+	const int slot = (wid + WARPS - 1) % WARPS;         // warp 0 factors the pivot: it takes a tile last
+	const int m = nt - 1, ntl = m * (m + 1) / 2;         // trailing tiles per step
+	for (int K = 0; K < nt; K++) {
+		const double* src = a.T + (size_t)(K & 1) * tiles(nt) * TT;
+		double* dst = a.T + (size_t)((K + 1) & 1) * tiles(nt) * TT;
+		const bool last = K == nt - 1;
+		int t = slot * G + cta;
+		int I = 0, J = 0;
+		auto locate = [&](int tt) {
+			int li, lj;
+			tri_decode(tt, li, lj);
+			I = li + (li >= K); J = lj + (lj >= K);
+		};
+		// A_XK of the step: tile (X, K) below the pivot, the transpose of tile (K, X) above it
+		auto issue = [&]() {
+			stage(sA, I > K ? tile(src, I, K) : tile(src, K, I), lane);
+			stage(sB, J > K ? tile(src, J, K) : tile(src, K, J), lane);
+		};
+		if (t < ntl) { locate(t); issue(); }
 		if (wid == 0) {
-			for (int e = lane; e < NB * NB; e += 32) { const int rr = e % NB, cc = e / NB; sD[rr * TS + cc] = rr >= cc ? ldcg(a.M + (size_t)(k * NB + cc) * np + k * NB + rr) : 0.0; }
-			__syncwarp();
-			const bool ok = chol16(sD, sLi, lane);
-			if (!ok && lane == 0) s_fail = 1;
-			if (ok && cta == 0) {
-				for (int e = lane; e < NB * NB; e += 32) {
-					const int rr = e % NB, cc = e / NB;
-					__stcg(a.Lm + (size_t)(k * NB + cc) * np + k * NB + rr, rr >= cc ? sD[rr * TS + cc] : 0.0);
-					__stcg(a.Dinv + (size_t)k * NB * NB + rr * NB + cc, sLi[rr * TS + cc]);
+			// ---- the pivot: every CTA factors A_KK = L L^T in registers (lane i holds row i) and forms L^-1 (lane q: column q) ----
+			double row[NB];
+			const double* g = tile(src, K, K) + lane * NB;
+#pragma unroll
+			for (int i = 0; i < NB; i += 2) { const double2 v = __ldcg(reinterpret_cast<const double2*>(g + i)); row[i] = v.x; row[i + 1] = v.y; }
+			bool ok = true;
+			double rdiag = 0.0;                          // lane i: 1 / L(i, i)
+#pragma unroll
+			for (int k = 0; k < NB; k++) {
+				sRow[lane] = row[k];
+				__syncwarp();
+				const double d = sRow[k];
+				if (!(d > 0)) { ok = false; break; }
+				const double lkk = sqrt(d), rk = 1.0 / lkk;
+				const double lik = lane > k ? row[k] * rk : lane == k ? lkk : 0.0;      // column k of L
+				if (lane == k) rdiag = rk;
+				__syncwarp();
+				sRow[lane] = lik;
+				__syncwarp();
+#pragma unroll
+				for (int j = k + 1; j < NB; j++) row[j] = fma(-lik, sRow[j], row[j]);
+				row[k] = lik;
+				__syncwarp();
+			}
+			if (!ok) { if (lane == 0) s_fail = 1; }
+			else {
+				// row = row `lane` of L (lower); column q of L^-1 by forward substitution, x_i = (delta_iq - sum_{k<i} L_ik x_k) / L_ii
+#pragma unroll
+				for (int i = 0; i < NB; i += 2) *reinterpret_cast<double2*>(sPv + lane * TS + i) = make_double2(row[i], row[i + 1]);
+				sRow[lane] = rdiag;
+				__syncwarp();
+				double x[NB];
+#pragma unroll
+				for (int i = 0; i < NB; i++) {
+					double sum = i == lane ? 1.0 : 0.0;
+#pragma unroll
+					for (int k = 0; k < i; k++) sum = fma(-sPv[i * TS + k], x[k], sum);
+					x[i] = sum * sRow[i];
+				}
+#pragma unroll
+				for (int i = 0; i < NB; i++) sN[i * TS + lane] = x[i];
+				__syncwarp();
+				if (cta == 0) {
+					// the new pivot tile -P = -L^-T L^-1
+					double pp[4][4][2];
+#pragma unroll
+					for (int bi = 0; bi < 4; bi++)
+#pragma unroll
+						for (int bj = 0; bj < 4; bj++) pp[bi][bj][0] = pp[bi][bj][1] = 0.0;
+					mma32(pp, sN, 1, TS, sN, TS, 1, lane);
+					frag_store(sPv, pp, 1.0, lane);
+					__syncwarp();
+					tile_out(sPv, TS, 1, -1.0, true, K, K, tile(dst, K, K), last, a.AcInv, n, lane);
 				}
 			}
 		}
 		__syncthreads();
-		if (s_fail) break;                                 // every CTA sees the same pivots
-		const int m = nt - k - 1;                          // trailing tile rows
-		const int ntile = m * (m + 1) / 2;
-		double* Pi = sP[wid][0];
-		double* Pj = sP[wid][1];
-		for (int t = gw; t < ntile; t += nwarps) {
-			int li = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-			while ((li + 1) * (li + 2) / 2 <= t) li++;
-			while (li * (li + 1) / 2 > t) li--;
-			const int lj = t - li * (li + 1) / 2;
-			const int i = k + 1 + li, j = k + 1 + lj;
-			// P_i = M_ik L_kk^-T : P(r, c) = sum_{m <= c} M_ik(r, m) Linv(c, m); this lane: row r, columns c0..c0+7
+		if (s_fail) { asm volatile("cp.async.wait_group 0;" ::: "memory"); break; }   // every CTA sees the same pivots
+
+		for (bool first = true; t < ntl; t += G * WARPS, first = false) {
+			if (!first) { locate(t); issue(); }
+			const bool trI = I < K, trJ = J < K;
+			// acc = A_IJ (fragment layout), from the copy of this step
+			double acc[4][4][2];
 			{
-				double arow[NB];
+				const double* g = tile(src, I, J) + (lane >> 2) * NB + 2 * (lane & 3);
 #pragma unroll
-				for (int mm = 0; mm < NB; mm++) arow[mm] = ldcg(a.M + (size_t)(k * NB + mm) * np + i * NB + r);
+				for (int bi = 0; bi < 4; bi++)
 #pragma unroll
-				for (int c = 0; c < 8; c++) {
-					const int cc = c0 + c;
-					double s = 0;
-#pragma unroll
-					for (int mm = 0; mm < NB; mm++) if (mm <= cc) s += arow[mm] * sLi[cc * TS + mm];
-					Pi[r * TS + cc] = s;
-				}
-				if (j != i) {
-#pragma unroll
-					for (int mm = 0; mm < NB; mm++) arow[mm] = ldcg(a.M + (size_t)(k * NB + mm) * np + j * NB + r);
-#pragma unroll
-					for (int c = 0; c < 8; c++) {
-						const int cc = c0 + c;
-						double s = 0;
-#pragma unroll
-						for (int mm = 0; mm < NB; mm++) if (mm <= cc) s += arow[mm] * sLi[cc * TS + mm];
-						Pj[r * TS + cc] = s;
+					for (int bj = 0; bj < 4; bj++) {
+						const double2 v = __ldcg(reinterpret_cast<const double2*>(g + 8 * bi * NB + 8 * bj));
+						acc[bi][bj][0] = v.x; acc[bi][bj][1] = v.y;
 					}
-				}
+			}
+			asm volatile("cp.async.wait_group 0;" ::: "memory");
+			__syncwarp();
+			// Q_I = A_IK L^-T into sA over A_IK; -Q_J = -A_JK L^-T into sB over A_JK (tile (I, I): -Q_I)
+			double q[4][4][2];
+#pragma unroll
+			for (int bi = 0; bi < 4; bi++)
+#pragma unroll
+				for (int bj = 0; bj < 4; bj++) q[bi][bj][0] = q[bi][bj][1] = 0.0;
+			mma32(q, sA, trI ? 1 : TS, trI ? TS : 1, sN, 1, TS, lane);
+			__syncwarp();
+			frag_store(sA, q, 1.0, lane);
+			if (I == J) frag_store(sB, q, -1.0, lane);
+			else {
+#pragma unroll
+				for (int bi = 0; bi < 4; bi++)
+#pragma unroll
+					for (int bj = 0; bj < 4; bj++) q[bi][bj][0] = q[bi][bj][1] = 0.0;
+				mma32(q, sB, trJ ? 1 : TS, trJ ? TS : 1, sN, 1, TS, lane);
+				__syncwarp();
+				frag_store(sB, q, -1.0, lane);
 			}
 			__syncwarp();
-			const double* Q = j != i ? Pj : Pi;
-			// M_ij -= P_i P_j^T ; the diagonal tile's warp also publishes L_ik = P_i
+			// A_IJ - A_IK P A_KJ = A_IJ - Q_I Q_J^T
+			mma32(acc, sA, TS, 1, sB, 1, TS, lane);
+			if (I == J) {
+				// the warp of tile (I, I) also forms the new panel tile A_IK P = Q_I L^-1
 #pragma unroll
-			for (int c = 0; c < 8; c++) {
-				const int cc = c0 + c;
-				double s = 0;
+				for (int bi = 0; bi < 4; bi++)
 #pragma unroll
-				for (int mm = 0; mm < NB; mm++) s += Pi[r * TS + mm] * Q[cc * TS + mm];
-				double* dst = a.M + (size_t)(j * NB + cc) * np + i * NB + r;
-				__stcg(dst, ldcg(dst) - s);
-				if (j == i) __stcg(a.Lm + (size_t)(k * NB + cc) * np + i * NB + r, Pi[r * TS + cc]);
+					for (int bj = 0; bj < 4; bj++) q[bi][bj][0] = q[bi][bj][1] = 0.0;
+				mma32(q, sA, TS, 1, sN, TS, 1, lane);
 			}
 			__syncwarp();
+			frag_store(sB, acc, 1.0, lane);
+			__syncwarp();
+			tile_out(sB, TS, 1, 1.0, I == J, I, J, tile(dst, I, J), last, a.AcInv, n, lane);
+			__syncwarp();
+			if (I == J) {
+				// tile (I, K) below the pivot, or its transpose, tile (K, I), above it
+				frag_store(sB, q, 1.0, lane);
+				__syncwarp();
+				if (I > K) tile_out(sB, TS, 1, 1.0, false, I, K, tile(dst, I, K), last, a.AcInv, n, lane);
+				else tile_out(sB, 1, TS, 1.0, false, K, I, tile(dst, K, I), last, a.AcInv, n, lane);
+				__syncwarp();
+			}
 		}
-		grid_barrier(a.bar, G, gen);
+		if (!last) grid_barrier(a.bar, G, gen);
 	}
 	if (s_fail) {
 		for (long long e = (long long)cta * blockDim.x + tid; e < (long long)n * n; e += (long long)G * blockDim.x) a.AcInv[e] = 0.f;
 		if (cta == 0 && tid == 0) *a.info = 1;
 		return;
-	}
-
-	// ---- phase 2: W = L^-1, tile column jt per CTA: W(jt,jt) = Linv_jj, W(i,jt) = -Linv_ii sum_{k=jt}^{i-1} L(i,k) W(k,jt) ----
-	for (int jt = cta; jt < nt; jt += G) {
-		for (int e = tid; e < NB * NB; e += blockDim.x) { const int rr = e / NB, cc = e % NB; __stcg(a.W + (size_t)(jt * NB + cc) * np + jt * NB + rr, ldcg(a.Dinv + (size_t)jt * NB * NB + e)); }
-		__syncthreads();
-		for (int i = jt + 1; i < nt; i++) {
-			// partial sums of this warp over its k's; this lane: row r, columns c0..c0+7
-			double acc[8];
-#pragma unroll
-			for (int c = 0; c < 8; c++) acc[c] = 0.0;
-			for (int k = jt + wid; k < i; k += WARPS) {
-				double lrow[NB];
-#pragma unroll
-				for (int mm = 0; mm < NB; mm++) lrow[mm] = ldcg(a.Lm + (size_t)(k * NB + mm) * np + i * NB + r);     // L(i,k)(r, mm)
-#pragma unroll
-				for (int c = 0; c < 8; c++) {
-					const double* wc = a.W + (size_t)(jt * NB + c0 + c) * np + k * NB;                           // W(k,jt)(:, c)
-					double s = 0;
-#pragma unroll
-					for (int mm = 0; mm < NB; mm++) s += lrow[mm] * ldcg(wc + mm);
-					acc[c] += s;
-				}
-			}
-#pragma unroll
-			for (int c = 0; c < 8; c++) sP[wid][1][r * NB + c0 + c] = acc[c];
-			__syncthreads();
-			if (wid == 0) {
-				// S = sum of the partials (warp order), W(i,jt) = -Linv_ii S
-				double* S = sP[0][0];
-#pragma unroll
-				for (int c = 0; c < 8; c++) {
-					double s = 0;
-#pragma unroll
-					for (int w = 0; w < WARPS; w++) s += sP[w][1][r * NB + c0 + c];
-					S[r * TS + c0 + c] = s;
-				}
-				__syncwarp();
-				double lrow[NB];
-#pragma unroll
-				for (int mm = 0; mm < NB; mm++) lrow[mm] = ldcg(a.Dinv + (size_t)i * NB * NB + r * NB + mm);            // Linv_ii(r, mm), mm <= r
-#pragma unroll
-				for (int c = 0; c < 8; c++) {
-					double s = 0;
-#pragma unroll
-					for (int mm = 0; mm < NB; mm++) if (mm <= r) s += lrow[mm] * S[mm * TS + c0 + c];
-					__stcg(a.W + (size_t)(jt * NB + c0 + c) * np + i * NB + r, -s);
-				}
-			}
-			__syncthreads();
-		}
-	}
-	grid_barrier(a.bar, G, gen);
-
-	// ---- phase 3: Ac^-1 = W^T W: tile (i >= j) = sum_{k >= i} W(k,i)^T W(k,j); one warp per tile ----
-	{
-		const int ntile = nt * (nt + 1) / 2;
-		double* Wi = sP[wid][0];
-		double* Wj = sP[wid][1];
-		for (int t = gw; t < ntile; t += nwarps) {
-			int i = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-			while ((i + 1) * (i + 2) / 2 <= t) i++;
-			while (i * (i + 1) / 2 > t) i--;
-			const int j = t - i * (i + 1) / 2;
-			double acc[8];
-#pragma unroll
-			for (int c = 0; c < 8; c++) acc[c] = 0.0;
-			for (int k = i; k < nt; k++) {
-				// stage W(k,i) and W(k,j) (row-major in shared memory); lane loads row r, columns c0..c0+7 of each
-#pragma unroll
-				for (int c = 0; c < 8; c++) {
-					Wi[r * TS + c0 + c] = ldcg(a.W + (size_t)(i * NB + c0 + c) * np + k * NB + r);
-					Wj[r * TS + c0 + c] = ldcg(a.W + (size_t)(j * NB + c0 + c) * np + k * NB + r);
-				}
-				__syncwarp();
-				// out(r, cc) += sum_m W(k,i)(m, r) W(k,j)(m, cc)
-#pragma unroll
-				for (int c = 0; c < 8; c++) {
-					double s = 0;
-#pragma unroll
-					for (int mm = 0; mm < NB; mm++) s += Wi[mm * TS + r] * Wj[mm * TS + c0 + c];
-					acc[c] += s;
-				}
-				__syncwarp();
-			}
-#pragma unroll
-			for (int c = 0; c < 8; c++) {
-				const int row = i * NB + r, col = j * NB + c0 + c;
-				if (row < n && col < n) {
-					const float v = (float)acc[c];
-					a.AcInv[(size_t)row * n + col] = v;
-					a.AcInv[(size_t)col * n + row] = v;
-				}
-			}
-		}
 	}
 	if (cta == 0 && tid == 0) *a.info = 0;
 }

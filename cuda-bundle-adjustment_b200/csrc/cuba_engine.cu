@@ -197,6 +197,7 @@ struct EngineBase {
 	virtual int dbg_pcg_timing(long long* out, int maxCtas) = 0;
 	virtual int dbg_pcg_info(int32_t* info, double* coarseLambda) = 0;
 	virtual int dbg_coarse(int32_t* rowAgg, double* AcP, float* AcInv) = 0;
+	virtual int dbg_coarse_inverse(const double* AcP, int A, float* AcInv, int* info) = 0;
 };
 
 template <typename T>
@@ -1455,7 +1456,7 @@ struct Engine : EngineBase {
 	DBuf<T> p5Linv, p5R0, p5Zhat, p5RcRow, p5Rc0;
 	DBuf<float> p5AcInv;
 	DBuf<double> p5AcP, p5Lp, p5Wp, p5Ld;
-	DBuf<double> cdM, cdL, cdW, cdDinv;            // dense work matrices of k_coarse_dense
+	DBuf<double> cdT;                              // k_coarse_dense: two copies of the lower 32 x 32 tiles of Ac
 	bool p5Dense = false;
 	DBuf<unsigned long long> p5Boards;
 	void* p5PeerBase[PCG5_MAXWORLD] = { nullptr };   // cudaIpc mappings of the peers' boards (own entry: the local allocation)
@@ -1697,8 +1698,7 @@ struct Engine : EngineBase {
 		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull));
 		CUDA_TRY(p5AcP.alloc(nblkPz * 36)); CUDA_TRY(p5AcInv.alloc((size_t)nc * nc)); CUDA_TRY(p5Lp.alloc(nblkPz * 36)); CUDA_TRY(p5Wp.alloc(nblkPz * 36)); CUDA_TRY(p5Ld.alloc((size_t)A * 36));
 		if (p5Dense) {
-			const size_t ntd = ((size_t)nc + cdense::NB - 1) / cdense::NB, npd = ntd * cdense::NB;
-			CUDA_TRY(cdM.alloc(npd * npd)); CUDA_TRY(cdL.alloc(npd * npd)); CUDA_TRY(cdW.alloc(npd * npd)); CUDA_TRY(cdDinv.alloc(ntd * cdense::NB * cdense::NB));
+			CUDA_TRY(cdT.alloc(2 * cdense::tiles((nc + cdense::NB - 1) / cdense::NB) * cdense::TT));
 			CUDA_TRY(gridBar.alloc(1));
 		}
 		// boards (16-byte words): [2 solve halves][2 pass parities] of w, of the per-CTA partials and of the rank summaries, then the control block
@@ -1727,6 +1727,19 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// blocked symmetric sweep on the whole chip (cuba_coarse_dense.cuh): one persistent cooperative kernel; tiles holds
+	// 2 cdense::tiles(ceil(6A / 32)) tiles, bar a zeroed or reused GridBar
+	int launch_coarse_dense(const double* AcP, int A, double* tiles, float* AcInv, int* info, GridBar* bar)
+	{
+		CUDA_TRY(cudaFuncSetAttribute(cdense::k_coarse_dense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cdense::SMEM));
+		cdense::Args da;
+		da.AcP = AcP; da.A = A; da.T = tiles; da.AcInv = AcInv; da.info = info; da.bar = bar;
+		void* dargs[] = { (void*)&da };
+		CUDA_TRY(cudaLaunchCooperativeKernel((void*)cdense::k_coarse_dense, dim3(numSMs), dim3(cdense::WARPS * 32), dargs, cdense::SMEM, stream));
+		launches++;
+		return CUBA_OK;
+	}
+
 	// coarse matrix Ac = Z^T S Z of the current system and its inverse (fp32), for the aggregates behind (cbPtr, cbList)
 	int launch_coarse_setup(int A, int cluster, size_t invSmem, const int* cbPtr, const int* cbList, double* AcP, float* AcInv, double* Lp, double* Ld, double* Wp, bool dense = false)
 	{
@@ -1734,16 +1747,7 @@ struct Engine : EngineBase {
 		int* infoP = p5InfoSlot();
 		KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, cRowOf.p, fColInd.p, S.nfull, cZx.p, cU.p);
 		KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, cbPtr, cbList, cU.p, nblkP, AcP);
-		if (dense) {
-			// dense tile Cholesky + inverse on the whole chip (cuba_coarse_dense.cuh): one persistent cooperative kernel
-			CUDA_TRY(cudaMemsetAsync(cdM.p, 0, sizeof(double) * cdM.n, stream));
-			cdense::Args da;
-			da.AcP = AcP; da.A = A; da.M = cdM; da.Lm = cdL; da.Dinv = cdDinv; da.W = cdW; da.AcInv = AcInv; da.info = infoP; da.bar = gridBar;
-			void* dargs[] = { (void*)&da };
-			CUDA_TRY(cudaLaunchCooperativeKernel((void*)cdense::k_coarse_dense, dim3(numSMs), dim3(cdense::WARPS * 32), dargs, 0, stream));
-			launches++;
-			return CUBA_OK;
-		}
+		if (dense) return launch_coarse_dense(AcP, A, cdT, AcInv, infoP, gridBar);
 		if (cluster) {
 			// Cholesky in the shared memory of an 8- or 16-CTA cluster, then the triangular inverse (one CTA per block column) and W^T W on the whole chip
 			cudaLaunchConfig_t lc = {};
@@ -2246,6 +2250,26 @@ struct Engine : EngineBase {
 		if (oAcInv) CUDA_TRY(cudaMemcpy(oAcInv, p5AcInv.p, sizeof(float) * (size_t)nc * nc, cudaMemcpyDeviceToHost));
 		return CUBA_OK;
 	}
+	// include/cuba_b200.h: cuba_debug_coarse_inverse -- k_coarse_dense on a caller's packed matrix, in buffers of its own
+	int dbg_coarse_inverse(const double* hAcP, int A, float* hAcInv, int* hInfo) override
+	{
+		if (A < 1 || !hAcP || !hAcInv || !hInfo) return fail(CUBA_ERR_INVALID, "debug_coarse_inverse: A < 1 or a NULL pointer");
+		const size_t nc = 6 * (size_t)A, nblkP = (size_t)A * (A + 1) / 2;
+		DBuf<double> dAcP, dT;
+		DBuf<float> dInv;
+		DBuf<int> dInfo;
+		DBuf<GridBar> dBar;
+		CUDA_TRY(dAcP.alloc(36 * nblkP)); CUDA_TRY(dInv.alloc(nc * nc)); CUDA_TRY(dInfo.alloc(1)); CUDA_TRY(dBar.alloc(1));
+		CUDA_TRY(dT.alloc(2 * cdense::tiles((int)((nc + cdense::NB - 1) / cdense::NB)) * cdense::TT));
+		CUDA_TRY(cudaMemcpyAsync(dAcP.p, hAcP, sizeof(double) * 36 * nblkP, cudaMemcpyHostToDevice, stream));
+		CUDA_TRY(cudaMemsetAsync(dBar.p, 0, sizeof(GridBar), stream));
+		CUDA_TRY(cudaMemsetAsync(dInfo.p, 0xff, sizeof(int), stream));          // -1 unless the kernel reports
+		int rc = launch_coarse_dense(dAcP, A, dT, dInv, dInfo, dBar); if (rc) return rc;
+		CUDA_TRY(cudaMemcpyAsync(hAcInv, dInv.p, sizeof(float) * nc * nc, cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaMemcpyAsync(hInfo, dInfo.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		return CUBA_OK;
+	}
 
 	// ---- micro-benchmarks --------------------------------------------------------------------------------
 	int bench_stage(int stage, int reps, int flush, double lambda, double* ms) override
@@ -2420,6 +2444,7 @@ int cuba_debug_get_schur(cuba_engine* e, double* Hsc, double* bsc, double* invHl
 int cuba_debug_get_delta(cuba_engine* e, double* xp, double* xl) { ENGINE_OR_FAIL(e); return e->impl->dbg_delta(xp, xl); }
 int cuba_debug_get_pcg_info(cuba_engine* e, int32_t* info, double* coarse_lambda) { ENGINE_OR_FAIL(e); return e->impl->dbg_pcg_info(info, coarse_lambda); }
 int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* AcInv) { ENGINE_OR_FAIL(e); return e->impl->dbg_coarse(aggRow, AcP, AcInv); }
+int cuba_debug_coarse_inverse(cuba_engine* e, const double* AcP, int A, float* AcInv, int* info) { ENGINE_OR_FAIL(e); return e->impl->dbg_coarse_inverse(AcP, A, AcInv, info); }
 int cuba_debug_build_structure_host(const cuba_problem* p, int rank, int world, cuba_sizes* sizes,
 	int32_t* hplColPtr, int32_t* hplRowInd, int32_t* edge2Hpl, int32_t* hscRowPtr, int32_t* hscColInd,
 	int32_t* fullRowPtr, int32_t* fullColInd, int32_t* shard)

@@ -238,4 +238,11 @@ CUBA_HD void se3_update(const T upd[6], T q[4], T t[3])
 	for (int i = 0; i < 4; i++) q[i] = invn * r[i];
 }
 
+// D = A B + D on the fp64 tensor pipe, one 8x8x4 product per warp: lane l holds A(l/4, l%4), B(l%4, l/4) and
+// D(l/4, 2 (l%4)) / D(l/4, 2 (l%4) + 1)
+__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
+{
+	asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+}
+
 }  // namespace cuba_b200

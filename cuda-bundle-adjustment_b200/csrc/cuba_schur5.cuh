@@ -33,11 +33,6 @@ struct Smem {
 	int lm[TL];                    // local landmark of each block
 };
 
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
-{
-	asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-
 // lower Cholesky factor of a symmetric positive definite 3x3 given as 00,01,02,11,12,22 -> 00,10,20,11,21,22
 __device__ __forceinline__ void chol3(const double B[6], double L[6])
 {

@@ -240,6 +240,10 @@ int cuba_debug_get_pcg_info(cuba_engine* e, int32_t* info, double* coarse_lambda
  * lower block triangle of Ac = Z^T S Z (block (ib >= jb) at (ib (ib+1)/2 + jb) * 36, column-major 6x6; 36 A (A+1)/2 doubles) and
  * AcInv its fp32 inverse [6A][6A].  Fails when no coarse level has been built.  Any pointer may be NULL. */
 int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* AcInv);
+/* Runs the dense coarse inverse k_coarse_dense, as a two-level solve launches it, on the caller's packed lower block triangle
+ * AcP (layout of cuba_debug_get_coarse, A >= 1 aggregates) in buffers of its own: AcInv [6A][6A] fp32 and info 0 (inverted) or 1
+ * (not positive definite: AcInv all zeros).  Needs a GPU, not a problem; no engine state changes. */
+int cuba_debug_coarse_inverse(cuba_engine* e, const double* AcP, int A, float* AcInv, int* info);
 
 /* Host-only (no CUDA call): builds the index structures from the (iP,iL) lists exactly as
  * cuba_engine_set_problem does and copies them out -- the not-gpu tests check them against the oracle.
