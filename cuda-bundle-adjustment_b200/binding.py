@@ -56,10 +56,10 @@ _lib = None
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
     "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_flush_l2",
-    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_get_profile",
+    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
-    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_bench_stage",
+    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
 ]
 
 
@@ -95,6 +95,9 @@ def load_library():
         "cuba_engine_optimize": [vp, i, vp, C.POINTER(i)],
         "cuba_engine_get_state": [vp, vp, vp, vp],
         "cuba_engine_get_chi2": [vp, vp],
+        "cuba_engine_set_edge_levels": [vp, vp],
+        "cuba_engine_get_edge_levels": [vp, vp],
+        "cuba_engine_classify_edges": [vp, d, d, i, vp],
         "cuba_engine_get_profile": [vp, vp],
         "cuba_engine_get_launch_count": [vp, C.POINTER(C.c_longlong)],
         "cuba_get_transfer_bytes": [C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)],
@@ -117,6 +120,7 @@ def load_library():
         "cuba_debug_pcg5_plan": [C.POINTER(_Problem), i, i, i, vp],
         "cuba_debug_pcg5_plan_apc": [C.POINTER(_Problem), i, i, i, i, vp, C.POINTER(C.c_uint64)],
         "cuba_debug_dropin_problem": [vp, C.POINTER(_Problem)],
+        "cuba_debug_dropin_levels": [vp, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_int32)],
         "cuba_bench_stage": [vp, i, i, i, d, C.POINTER(d)],
     }
     for name, args in sig.items():
@@ -310,6 +314,28 @@ class Engine:
         out = np.zeros(self.sizes["E2"] + self.sizes["E3"])
         _check(self.L.cuba_engine_get_chi2(self.h, _p(out)))
         return out
+
+    # --- edge levels (g2o Edge::setLevel + initializeOptimization(0)) ------------------------------------
+    def set_edge_levels(self, levels):
+        """levels[E2+E3] in edge-id order, 0 = optimised, non-zero = left out of the objective and the normal equations; None = all 0"""
+        if levels is None:
+            _check(self.L.cuba_engine_set_edge_levels(self.h, None))
+            return
+        lv = np.ascontiguousarray(np.asarray(levels) != 0, dtype=np.uint8)
+        assert lv.shape == (self.sizes["E2"] + self.sizes["E3"],), lv.shape
+        _check(self.L.cuba_engine_set_edge_levels(self.h, _p(lv)))
+
+    def edge_levels(self):
+        out = np.zeros(self.sizes["E2"] + self.sizes["E3"], np.uint8)
+        _check(self.L.cuba_engine_get_edge_levels(self.h, _p(out)))
+        return out
+
+    def classify_edges(self, chi2_mono, chi2_stereo, depth=True, reinclude=False):
+        """ORB-SLAM2's outlier test on the device at the current estimate (include/cuba_b200.h: cuba_engine_classify_edges)"""
+        counts = np.zeros(4, np.int32)
+        flags = (1 if depth else 0) | (2 if reinclude else 0)
+        _check(self.L.cuba_engine_classify_edges(self.h, float(chi2_mono), float(chi2_stereo), flags, _p(counts)))
+        return dict(zip(("included_mono", "included_stereo", "excluded", "reincluded"), (int(v) for v in counts)))
 
     def launch_count(self):
         n = C.c_longlong(0)

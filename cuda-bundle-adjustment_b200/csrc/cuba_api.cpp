@@ -14,6 +14,9 @@
 //     the flat arrays live in page-locked memory (the engine's H2D copies are plain DMA) and the edge pass is split over a few
 //     host threads; the pointer -> chi2 map the reference rebuilds in every optimize() (cpp:541-542) is built on the first
 //     chiSquared() call instead.
+// Edge levels (include/cuba_b200_levels.h, which the reference does not have): one byte per list slot beside mono_ / stereo_, so that
+// compaction, the dropping of both-fixed edges and the value-only initialize() carry them; a flat copy in the order of the flat
+// arrays goes to the engine after set_problem only when some level is set; classifyEdges() decisions are fetched lazily.
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
@@ -31,6 +34,7 @@
 
 #include "../../include/cuba_b200.h"
 #include "../../include/cuda_bundle_adjustment.h"
+#include "../../include/cuba_b200_levels.h"
 
 namespace cuba
 {
@@ -113,14 +117,16 @@ public:
 	{
 		if (!member_.insert(e).second) return;
 		edgeVersion_++;
-		mono_.push_back(e);
+		mono_.push_back(e); levMono_.push_back(0);
+		slotValid_ = false;
 		e->vertexP->edges.insert(e); e->vertexL->edges.insert(e);
 	}
 	void addStereoEdge(StereoEdge* e) override
 	{
 		if (!member_.insert(e).second) return;
 		edgeVersion_++;
-		stereo_.push_back(e);
+		stereo_.push_back(e); levStereo_.push_back(0);
+		slotValid_ = false;
 		e->vertexP->edges.insert(e); e->vertexL->edges.insert(e);
 	}
 
@@ -168,6 +174,7 @@ public:
 	void initialize() override
 	{
 		const auto t0 = std::chrono::steady_clock::now();
+		levelsFromDevice();      // classifyEdges() decisions into the lists while their slots still match the uploaded problem
 		compactEdges();
 		if (orderDirty_) {
 			orderP_.clear(); orderL_.clear();
@@ -244,6 +251,8 @@ public:
 		idx2_.resize(2 * mono_.size()); meas2_.resize(2 * mono_.size()); om2_.resize(mono_.size());
 		idx3_.resize(2 * stereo_.size()); meas3_.resize(3 * stereo_.size()); om3_.resize(stereo_.size());
 		const size_t n2 = mono_.size(), n3 = stereo_.size(), total = n2 + n3;
+		lev_.resize(total);
+		levFlatStale_ = false;
 		const unsigned nthreads = host_threads(total, 65536);
 		if (flatValid_ && sameNumbering_ && flatVersion_ == edgeVersion_ && om2_.size() == n2 && om3_.size() == n3) {
 			// same edges in the same order between the same indices, none dropped: the index pairs and the position -> edge lists of
@@ -255,11 +264,13 @@ public:
 						const MonoEdge* ed = mono_[k];
 						meas2_[2 * k] = ed->measurement.data()[0]; meas2_[2 * k + 1] = ed->measurement.data()[1];
 						om2_[k] = ed->information;
+						lev_[k] = levMono_[k];
 					} else {
 						const size_t j = k - n2;
 						const StereoEdge* ed = stereo_[j];
 						for (int c = 0; c < 3; c++) meas3_[3 * j + c] = ed->measurement.data()[c];
 						om3_[j] = ed->information;
+						lev_[k] = levStereo_[j];
 					}
 				}
 			});
@@ -287,6 +298,7 @@ public:
 					idx2_[2 * k] = vp->iP; idx2_[2 * k + 1] = vl->iL;
 					meas2_[2 * k] = ed->measurement.data()[0]; meas2_[2 * k + 1] = ed->measurement.data()[1];
 					om2_[k] = ed->information;
+					lev_[k] = levMono_[k];
 				} else {
 					const size_t j = k - n2;
 					const StereoEdge* ed = stereo_[j];
@@ -296,30 +308,37 @@ public:
 					idx3_[2 * j] = vp->iP; idx3_[2 * j + 1] = vl->iL;
 					for (int c = 0; c < 3; c++) meas3_[3 * j + c] = ed->measurement.data()[c];
 					om3_[j] = ed->information;
+					lev_[k] = levStereo_[j];
 				}
 			}
 			dropped[tix] = drop;
 		});
 		size_t ndrop = 0;
 		for (size_t d : dropped) ndrop += d;
+		flatMono_.clear(); flatStereo_.clear();
 		if (ndrop) {
+			// (the levels close up in place: the stereo levels start behind the kept monocular ones)
 			size_t w = 0;
 			for (size_t k = 0; k < n2; k++) {
 				const MonoEdge* ed = mono_[k];
 				if (ed->vertexP->fixed && ed->vertexL->fixed) continue;
 				(*am)[w] = ed; idx2_[2 * w] = idx2_[2 * k]; idx2_[2 * w + 1] = idx2_[2 * k + 1];
-				meas2_[2 * w] = meas2_[2 * k]; meas2_[2 * w + 1] = meas2_[2 * k + 1]; om2_[w] = om2_[k]; w++;
+				meas2_[2 * w] = meas2_[2 * k]; meas2_[2 * w + 1] = meas2_[2 * k + 1]; om2_[w] = om2_[k]; lev_[w] = lev_[k];
+				flatMono_.push_back(k); w++;
 			}
 			am->resize(w); idx2_.resize(2 * w); meas2_.resize(2 * w); om2_.resize(w);
+			const size_t w2 = w;
 			w = 0;
 			for (size_t j = 0; j < n3; j++) {
 				const StereoEdge* ed = stereo_[j];
 				if (ed->vertexP->fixed && ed->vertexL->fixed) continue;
 				(*as)[w] = ed; idx3_[2 * w] = idx3_[2 * j]; idx3_[2 * w + 1] = idx3_[2 * j + 1];
 				for (int c = 0; c < 3; c++) meas3_[3 * w + c] = meas3_[3 * j + c];
-				om3_[w] = om3_[j]; w++;
+				om3_[w] = om3_[j]; lev_[w2 + w] = lev_[n2 + j];
+				flatStereo_.push_back(j); w++;
 			}
 			as->resize(w); idx3_.resize(2 * w); meas3_.resize(3 * w); om3_.resize(w);
+			lev_.resize(w2 + w);
 		}
 		activeMono_ = am; activeStereo_ = as;
 		flatValid_ = ndrop == 0; flatVersion_ = edgeVersion_;
@@ -341,7 +360,12 @@ public:
 			flatProblem(p);
 			check(cuba_engine_set_problem(engine_, &p));
 			uploaded_ = true;
+			levDevNewer_ = false;
+			// set_problem left every level at 0: lev_ must first take the levels set since initialize() before it is compared with that
+			if (levFlatStale_) rebuildFlatLevels();
+			levUploaded_ = std::none_of(lev_.data(), lev_.data() + lev_.size(), [](unsigned char l) { return l != 0; });
 		}
+		pushLevels();
 		std::vector<cuba_iter_stat> st(niterations > 0 ? niterations : 1);
 		int n = 0;
 		if (niterations > 0) check(cuba_engine_optimize(engine_, niterations, st.data(), &n));
@@ -382,8 +406,45 @@ public:
 		return true;
 	}
 
+	// ---- edge levels (include/cuba_b200_levels.h) ----
+	void setEdgeLevel(BaseEdge* e, int level)
+	{
+		unsigned char& l = levelOf(e);
+		const unsigned char v = level != 0;
+		if (l == v) return;
+		l = v;
+		levFlatStale_ = true; levUploaded_ = false;
+	}
+	int edgeLevel(const BaseEdge* e) { return levelOf(e); }
+	OutlierCounts classifyEdges(const OutlierTest& test)
+	{
+		if (!engine_ || !uploaded_) throw std::logic_error("cuba::classifyEdges: no optimize() since the last initialize()");
+		pushLevels();
+		int32_t c[4] = { 0, 0, 0, 0 };
+		const int flags = (test.requirePositiveDepth ? CUBA_CLASSIFY_DEPTH : 0) | (test.reinclude ? CUBA_CLASSIFY_REINCLUDE : 0);
+		check(cuba_engine_classify_edges(engine_, test.chi2Mono, test.chi2Stereo, flags, c));
+		if (c[2] + c[3] > 0) levDevNewer_ = true;
+		OutlierCounts out;
+		out.includedMono = static_cast<size_t>(c[0]); out.includedStereo = static_cast<size_t>(c[1]);
+		out.excluded = static_cast<size_t>(c[2]); out.reincluded = static_cast<size_t>(c[3]);
+		return out;
+	}
+	// the flat levels with every level set so far applied (also behind cuba_debug_dropin_levels)
+	bool flatLevels(const uint8_t** p, int32_t* n)
+	{
+		if (!initialized_) return false;
+		levelsFromDevice();
+		if (levFlatStale_) rebuildFlatLevels();
+		if (p) *p = lev_.data();
+		if (n) *n = static_cast<int32_t>(lev_.size());
+		return true;
+	}
+
 	void clear() override
 	{
+		levMono_.clear(); levStereo_.clear(); slot_.clear(); slotValid_ = false;
+		flatMono_.clear(); flatStereo_.clear(); lev_.resize(0);
+		levFlatStale_ = false; levUploaded_ = true; levDevNewer_ = false;
 		poses_.clear(); landmarks_.clear(); mono_.clear(); stereo_.clear(); member_.clear(); tombstones_.clear();
 		deadMono_ = deadStereo_ = 0; orderDirty_ = true;
 		edgeVersion_++; flatValid_ = false;
@@ -413,18 +474,64 @@ private:
 	void compactEdges()
 	{
 		if (tombstones_.empty()) return;
-		auto sweep = [this](auto& vec) {
+		auto sweep = [this](auto& vec, std::vector<unsigned char>& lev) {
 			size_t w = 0;
 			for (size_t k = 0; k < vec.size(); k++) {
 				auto it = tombstones_.find(vec[k]);
 				if (it != tombstones_.end()) { if (--it->second == 0) tombstones_.erase(it); continue; }
+				lev[w] = lev[k];
 				vec[w++] = vec[k];
 			}
-			vec.resize(w);
+			vec.resize(w); lev.resize(w);
 		};
-		sweep(mono_); sweep(stereo_);
+		sweep(mono_, levMono_); sweep(stereo_, levStereo_);
 		tombstones_.clear();
 		deadMono_ = deadStereo_ = 0;
+		slotValid_ = false;
+	}
+
+	// the level of the list slot that holds e now (the last one: an edge removed and added again has a new slot)
+	unsigned char& levelOf(const BaseEdge* e)
+	{
+		if (!member_.count(e)) throw std::out_of_range("cuba: the optimizer does not hold this edge");
+		levelsFromDevice();
+		if (!slotValid_) {
+			slot_.clear();
+			slot_.reserve(mono_.size() + stereo_.size());
+			for (size_t k = 0; k < mono_.size(); k++) slot_[mono_[k]] = k;
+			for (size_t k = 0; k < stereo_.size(); k++) slot_[stereo_[k]] = k;
+			slotValid_ = true;
+		}
+		const size_t k = slot_.at(e);
+		return e->dim() == 2 ? levMono_[k] : levStereo_[k];
+	}
+	// list slot of the w-th flat edge of the last initialize() (the identity unless it dropped edges with both ends fixed)
+	size_t monoSlot(size_t w) const { return flatMono_.empty() ? w : flatMono_[w]; }
+	size_t stereoSlot(size_t w) const { return flatStereo_.empty() ? w : flatStereo_[w]; }
+	void rebuildFlatLevels()
+	{
+		const size_t n2 = om2_.size(), n3 = om3_.size();
+		for (size_t w = 0; w < n2; w++) lev_[w] = levMono_[monoSlot(w)];
+		for (size_t w = 0; w < n3; w++) lev_[n2 + w] = levStereo_[stereoSlot(w)];
+		levFlatStale_ = false;
+	}
+	// classifyEdges() changed levels on the device: fetch them into the flat array and the lists (slots are stable until compaction)
+	void levelsFromDevice()
+	{
+		if (!levDevNewer_) return;
+		check(cuba_engine_get_edge_levels(engine_, lev_.data()));
+		const size_t n2 = om2_.size(), n3 = om3_.size();
+		for (size_t w = 0; w < n2; w++) levMono_[monoSlot(w)] = lev_[w];
+		for (size_t w = 0; w < n3; w++) levStereo_[stereoSlot(w)] = lev_[n2 + w];
+		levDevNewer_ = false;
+	}
+	// the levels set since the last upload to the engine (nothing when none changed)
+	void pushLevels()
+	{
+		if (levFlatStale_) rebuildFlatLevels();
+		if (levUploaded_) return;
+		check(cuba_engine_set_edge_levels(engine_, lev_.data()));
+		levUploaded_ = true;
 	}
 
 	// a position -> edge list for chiSquared(): the previous optimize()'s lists stay alive in chiMono_/chiStereo_, so the
@@ -460,6 +567,14 @@ private:
 	bool orderDirty_ = true;
 	std::vector<MonoEdge*> mono_;              // insertion order, may hold tombstoned slots until the next initialize()
 	std::vector<StereoEdge*> stereo_;
+	// edge levels: one byte per list slot (compaction, dropped both-fixed edges and the value-only initialize() carry them)
+	std::vector<unsigned char> levMono_, levStereo_;
+	std::unordered_map<const BaseEdge*, size_t> slot_;   // edge -> its live slot, rebuilt after an add or a compaction
+	bool slotValid_ = false;
+	std::vector<size_t> flatMono_, flatStereo_;          // list slot of every flat edge when the last initialize() dropped edges
+	bool levFlatStale_ = false;   // a level changed since lev_ was built
+	bool levUploaded_ = true;     // the engine holds lev_ (a graph that never uses levels never uploads any)
+	bool levDevNewer_ = false;    // classifyEdges() changed levels on the engine that lev_ and the lists do not have yet
 	std::unordered_set<const BaseEdge*> member_;
 	std::unordered_map<const BaseEdge*, int> tombstones_;
 	size_t deadMono_ = 0, deadStereo_ = 0;
@@ -475,6 +590,7 @@ private:
 	int numP_ = 0, numL_ = 0;
 	HostBuf<double> q_, t_, cam_, Xw_, meas2_, om2_, meas3_, om3_, chi_;
 	HostBuf<int32_t> idx2_, idx3_;
+	HostBuf<unsigned char> lev_;                 // flat levels, order of the flat edge arrays
 	bool initialized_ = false, uploaded_ = false;
 	double initSeconds_ = 0;
 
@@ -497,9 +613,35 @@ static bool dropin_problem(CudaBundleAdjustment* obj, cuba_problem* out)
 }
 CudaBundleAdjustment::~CudaBundleAdjustment() {}
 
+// include/cuba_b200_levels.h: free functions, so that the class keeps the reference's vtable
+static Impl& impl_of(const CudaBundleAdjustment& ba)
+{
+	const Impl* impl = dynamic_cast<const Impl*>(&ba);
+	if (!impl) throw std::invalid_argument("cuba: edge levels need an optimizer made by cuba::CudaBundleAdjustment::create()");
+	return const_cast<Impl&>(*impl);      // reading a level may first fetch the device's decisions into the host lists
+}
+void setEdgeLevel(CudaBundleAdjustment& ba, BaseEdge* e, int level) { impl_of(ba).setEdgeLevel(e, level); }
+int edgeLevel(const CudaBundleAdjustment& ba, const BaseEdge* e) { return impl_of(ba).edgeLevel(e); }
+OutlierCounts classifyEdges(CudaBundleAdjustment& ba, const OutlierTest& test) { return impl_of(ba).classifyEdges(test); }
+
+static bool dropin_levels(CudaBundleAdjustment* obj, const uint8_t** levels, int32_t* n)
+{
+	Impl* impl = dynamic_cast<Impl*>(obj);
+	return impl && impl->flatLevels(levels, n);
+}
+
 } // namespace cuba
 
 extern "C" int cuba_debug_dropin_problem(void* dropin, cuba_problem* out)
 {
 	return cuba::dropin_problem(static_cast<cuba::CudaBundleAdjustment*>(dropin), out) ? CUBA_OK : CUBA_ERR_STATE;
+}
+
+extern "C" int cuba_debug_dropin_levels(void* dropin, const uint8_t** levels, int32_t* n)
+{
+	try {
+		return cuba::dropin_levels(static_cast<cuba::CudaBundleAdjustment*>(dropin), levels, n) ? CUBA_OK : CUBA_ERR_STATE;
+	} catch (const std::exception&) {
+		return CUBA_ERR_CUDA;      // fetching classifyEdges() decisions failed (cuba_last_error has the message)
+	}
 }

@@ -25,6 +25,7 @@
 #include "cuba_peer_reduce.cuh"
 #include "cuba_schur2.cuh"
 #include "cuba_jh4.cuh"
+#include "cuba_levels.cuh"
 #include "cuba_schur3.cuh"
 #include "cuba_schur5.cuh"
 #include "cuba_structure.h"
@@ -198,6 +199,9 @@ struct EngineBase {
 	virtual int dbg_pcg_info(int32_t* info, double* coarseLambda) = 0;
 	virtual int dbg_coarse(int32_t* rowAgg, double* AcP, float* AcInv) = 0;
 	virtual int dbg_coarse_inverse(const double* AcP, int A, float* AcInv, int* info) = 0;
+	virtual int set_edge_levels(const uint8_t* levels) = 0;
+	virtual int get_edge_levels(uint8_t* levels) = 0;
+	virtual int classify_edges(double chi2Mono, double chi2Stereo, int flags, int32_t* counts) = 0;
 };
 
 template <typename T>
@@ -280,6 +284,13 @@ struct Engine : EngineBase {
 	size_t pcg2Smem = 0;
 	// reductions
 	DBuf<double> chiPartial, scalePartialL, scalePartialP, chiSq;
+	// edge levels (cuba_levels.cuh); allocated by the first level call, so that a run without levels keeps its footprint
+	bool lvOn = false;             // levels used since the last set_problem: e_om0 holds the caller's omega, lvLevel the levels
+	long long lvIncluded = 0;      // edges at level 0: all ranks' (under CUBA_DRY_SHARD this rank's own: its optimize() sees no other)
+	DBuf<T> e_om0;                 // landmark-major omega as set_problem scattered it, before the mask
+	DBuf<unsigned char> lvLevel;   // [E] in edge-id order; a rank reads and writes its own edges only
+	DBuf<int> lvPartial;
+	DBuf<double> lvCount;
 	DBuf<Scalars> dScal;
 	Scalars* hScal = nullptr;   // pinned
 	DBuf<double> flushBuf;
@@ -400,6 +411,7 @@ struct Engine : EngineBase {
 			return fail(CUBA_ERR_INVALID, "set_problem: null array with a non-zero count");
 		const auto t0 = std::chrono::steady_clock::now();
 		lastPcgKernel = CUBA_PCG_KERNEL_NONE; p5Rebuilds = 0; bjRetries = 0;
+		lvOn = false;      // every level back to 0: both paths below scatter the caller's omega unmasked
 		// Same topology as the problem this engine already holds (sizes, fixed/free split and every (iP, iL) pair identical): only the
 		// numbers changed -- the estimate after a previous optimize(), new measurements -- so every index structure, tile list,
 		// product list and PCG partition on the device stays valid.  Upload the values and re-run the three kernels that scatter them.
@@ -1986,6 +1998,7 @@ struct Engine : EngineBase {
 	int optimize(int niter, cuba_iter_stat* stats, int* nstats) override
 	{
 		if (!haveProblem) return fail(CUBA_ERR_STATE, "optimize before set_problem");
+		if (lvOn && lvIncluded == 0) { if (nstats) *nstats = 0; return CUBA_OK; }   // every edge at level 1: nothing to optimise
 		const int maxq = 10;
 		const double tau = 1e-5;
 		double nu = 2, lambda = 0, F = 0;
@@ -2107,7 +2120,9 @@ struct Engine : EngineBase {
 		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_chi2 before set_problem");
 		CUDA_TRY(cudaMemsetAsync(chiSq.p, 0, sizeof(double) * (size_t)std::max(S.E, 1), stream));
 		if (S.eLocal > 0) {
-			k_chi_sqs<T><<<(S.eLocal + 255) / 256, 256, 0, stream>>>(chiArgs(cur), e_user, chiSq);
+			ChiArgs<T> a = chiArgs(cur);
+			if (lvOn) a.om = e_om0;      // edges at level 1 report omega |r|^2 with the caller's omega
+			k_chi_sqs<T><<<(S.eLocal + 255) / 256, 256, 0, stream>>>(a, e_user, chiSq);
 			launches++;
 			CUDA_TRY(cudaGetLastError());
 		}
@@ -2115,6 +2130,127 @@ struct Engine : EngineBase {
 		g_d2hBytes += (long long)(sizeof(double) * (size_t)S.E);
 		CUDA_TRY(cudaMemcpyAsync(out, chiSq.p, sizeof(double) * (size_t)S.E, cudaMemcpyDeviceToHost, stream));
 		CUDA_TRY(cudaStreamSynchronize(stream));
+		return CUBA_OK;
+	}
+
+	// ---- edge levels (cuba_levels.cuh) ----------------------------------------------------------------
+	// first level call after a set_problem: keep the unmasked omega, every level 0
+	int levels_init()
+	{
+		if (lvOn) return CUBA_OK;
+		const int eL = S.eLocal;
+		CUDA_TRY(e_om0.alloc(eL));
+		if (eL > 0) CUDA_TRY(cudaMemcpyAsync(e_om0.p, e_om.p, sizeof(T) * (size_t)eL, cudaMemcpyDeviceToDevice, stream));
+		CUDA_TRY(lvLevel.alloc((size_t)std::max(S.E, 1)));
+		CUDA_TRY(cudaMemsetAsync(lvLevel.p, 0, (size_t)std::max(S.E, 1), stream));
+		// the pose-major source list: the device builder keeps it, the host builder has it in S only
+		if (cfg.reserved[1] == 1) CUDA_TRY(g_psrc.upload(S.p_src, stream));
+		lvOn = true;
+		lvIncluded = S.E;
+		return CUBA_OK;
+	}
+	// the mask into the three omega streams; the same streams as a set_problem whose omega is 0 on the edges at level 1
+	int levels_scatter()
+	{
+		const int eL = S.eLocal;
+		KLAUNCH(lv::k_mask_omega<T>, eL, e_om0.p, e_user.p, lvLevel.p, eL, e_om.p);
+		KLAUNCH(lv::k_pose_omega<T>, eL, g_psrc.p, posePtr.p, S.numP, eL, e_om.p, p_om.p);
+		if constexpr (sizeof(T) == 8) {
+			if (jhV4 && ntW > 0) {
+				const int lb = S.lmBeg, N = S.lmEnd - S.lmBeg;
+				KLAUNCH(jh4::k_emit, (long long)N * 32, w_start.p, w_pieces.p, w_base.p, N, lmPtr.p, lb, w_levels.p,
+					e_mx.p, e_my.p, e_mz.p, e_om.p, e_ip.p, e_il.p, e_hpl.p, w_tile.p, w_rec.p, w_tilePose.p, w_tilePieces.p);
+			}
+		}
+		// the system changed: nothing an earlier solve left behind may be reused (as after refresh_values; the estimate stays)
+		trialValid = false;
+		tlActive = false; coarseValid = false; coarseAge = 0; p5CoarseValid = false; p5CoarseAge = 0;
+		return CUBA_OK;
+	}
+	int set_edge_levels(const uint8_t* levels) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "set_edge_levels before set_problem");
+		int rc = levels_init(); if (rc) return rc;
+		const size_t E = (size_t)S.E;
+		long long included = (long long)E;
+		if (levels && E > 0) {
+			std::vector<unsigned char> h(E);
+			for (size_t i = 0; i < E; i++) { h[i] = levels[i] != 0; included -= h[i]; }
+			CUDA_TRY(cudaMemcpyAsync(lvLevel.p, h.data(), E, cudaMemcpyHostToDevice, stream));
+			g_h2dBytes += (long long)E;
+			rc = levels_scatter(); if (rc) return rc;
+			if (world > 1 && !comm) included = own_included(h.data());
+			CUDA_TRY(cudaStreamSynchronize(stream));      // h dies here
+		} else {
+			CUDA_TRY(cudaMemsetAsync(lvLevel.p, 0, std::max<size_t>(E, 1), stream));
+			rc = levels_scatter(); if (rc) return rc;
+			CUDA_TRY(cudaStreamSynchronize(stream));
+			if (world > 1 && !comm) included = S.eLocal;
+		}
+		if (included < 0) return fail(CUBA_ERR_CUDA, "set_edge_levels: reading the shard's edge list failed");
+		lvIncluded = included;
+		return CUBA_OK;
+	}
+	// CUBA_DRY_SHARD (no communicator): optimize() and classify_edges see this rank's edges only, so "no edge included" is judged on
+	// them alone, on every path.  One read-back of the shard's edge ids, on this diagnostic path only; -1 when it fails.
+	long long own_included(const unsigned char* h)
+	{
+		std::vector<int> u((size_t)S.eLocal);
+		if (!u.empty() && cudaMemcpyAsync(u.data(), e_user.p, sizeof(int) * u.size(), cudaMemcpyDeviceToHost, stream) != cudaSuccess) return -1;
+		if (cudaStreamSynchronize(stream) != cudaSuccess) return -1;
+		long long n = 0;
+		for (int v : u) n += h[v] == 0;
+		return n;
+	}
+	int get_edge_levels(uint8_t* out) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_edge_levels before set_problem");
+		const size_t E = (size_t)S.E;
+		if (!lvOn || E == 0) { if (E) memset(out, 0, E); return CUBA_OK; }
+		if (world <= 1) {
+			CUDA_TRY(cudaMemcpyAsync(out, lvLevel.p, E, cudaMemcpyDeviceToHost, stream));
+			CUDA_TRY(cudaStreamSynchronize(stream));
+			g_d2hBytes += (long long)E;
+			return CUBA_OK;
+		}
+		// landmark-sharded: every rank holds its own edges' levels; the per-edge chi2 path collects them
+		CUDA_TRY(cudaMemsetAsync(chiSq.p, 0, sizeof(double) * E, stream));
+		KLAUNCH(lv::k_levels_out, S.eLocal, e_user.p, lvLevel.p, S.eLocal, chiSq.p);
+		int rc = allreduce(chiSq.p, E, false); if (rc) return rc;
+		std::vector<double> h(E);
+		g_d2hBytes += (long long)(sizeof(double) * E);
+		CUDA_TRY(cudaMemcpyAsync(h.data(), chiSq.p, sizeof(double) * E, cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		for (size_t i = 0; i < E; i++) out[i] = h[i] != 0.0;
+		return CUBA_OK;
+	}
+	int classify_edges(double chi2Mono, double chi2Stereo, int flags, int32_t* counts) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "classify_edges before set_problem");
+		int rc = levels_init(); if (rc) return rc;
+		const int eL = S.eLocal, nb = (eL + RED_BLOCK - 1) / RED_BLOCK;
+		CUDA_TRY(lvPartial.alloc(4 * (size_t)std::max(nb, 1))); CUDA_TRY(lvCount.alloc(4));
+		if (eL > 0) {
+			ChiArgs<T> a = chiArgs(cur);
+			a.om = e_om0;
+			lv::k_classify_edges<T><<<nb, RED_BLOCK, 0, stream>>>(a, e_user.p, lvLevel.p, chi2Mono, chi2Stereo, flags, lvPartial.p);
+			launches++;
+			CUDA_TRY(cudaGetLastError());
+		}
+		lv::k_sum_counts<<<1, RED_BLOCK, 0, stream>>>(lvPartial.p, eL > 0 ? nb : 0, lvCount.p);
+		launches++;
+		CUDA_TRY(cudaGetLastError());
+		rc = allreduce(lvCount.p, 4, false); if (rc) return rc;
+		double c[4];
+		g_d2hBytes += (long long)sizeof(c);
+		CUDA_TRY(cudaMemcpyAsync(c, lvCount.p, sizeof(c), cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		// some level changed (on some rank): scatter the mask.  A rank whose own edges kept their levels scatters the same values again.
+		if (c[2] + c[3] > 0) {
+			rc = levels_scatter(); if (rc) return rc;
+		}
+		lvIncluded = (long long)(c[0] + c[1]);      // all ranks; under CUBA_DRY_SHARD this rank's own edges, as in set_edge_levels
+		if (counts) for (int k = 0; k < 4; k++) counts[k] = (int32_t)c[k];
 		return CUBA_OK;
 	}
 
@@ -2411,6 +2547,19 @@ int cuba_engine_get_sizes(const cuba_engine* e, cuba_sizes* out) { ENGINE_OR_FAI
 int cuba_engine_optimize(cuba_engine* e, int niter, cuba_iter_stat* stats, int* nstats) { ENGINE_OR_FAIL(e); return e->impl->optimize(niter, stats, nstats); }
 int cuba_engine_get_state(cuba_engine* e, double* q, double* t, double* Xw) { ENGINE_OR_FAIL(e); return e->impl->get_state(q, t, Xw); }
 int cuba_engine_get_chi2(cuba_engine* e, double* per_edge) { ENGINE_OR_FAIL(e); if (!per_edge) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_chi2(per_edge); }
+int cuba_engine_set_edge_levels(cuba_engine* e, const uint8_t* levels) { ENGINE_OR_FAIL(e); return e->impl->set_edge_levels(levels); }
+int cuba_engine_get_edge_levels(cuba_engine* e, uint8_t* levels)
+{
+	ENGINE_OR_FAIL(e);
+	if (!levels) return fail(CUBA_ERR_INVALID, "null out");
+	return e->impl->get_edge_levels(levels);
+}
+int cuba_engine_classify_edges(cuba_engine* e, double chi2_mono, double chi2_stereo, int flags, int32_t* counts)
+{
+	ENGINE_OR_FAIL(e);
+	if (flags & ~(CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE)) return fail(CUBA_ERR_INVALID, "classify_edges: unknown flag");
+	return e->impl->classify_edges(chi2_mono, chi2_stereo, flags, counts);
+}
 int cuba_engine_get_profile(cuba_engine* e, double* sec) { ENGINE_OR_FAIL(e); if (!sec) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_profile(sec); }
 // debug: per-CTA phase timings of the last k_pcg3 launch (library built with -DCUBA_PCG_TIMING); returns the CTA count
 int cuba_debug_get_pcg_timing(cuba_engine* e, long long* out, int maxCtas)

@@ -178,6 +178,25 @@ int cuba_engine_optimize(cuba_engine* e, int niterations, cuba_iter_stat* stats,
 int cuba_engine_get_state(cuba_engine* e, double* q, double* t, double* Xw);
 /* getChiSqs(): non-robust omega*|r|^2 per edge, edge-id order, [E2+E3] */
 int cuba_engine_get_chi2(cuba_engine* e, double* per_edge);
+/* Edge levels (g2o Edge::setLevel + initializeOptimization(0)).  levels[E2+E3] in edge-id order; 0 = optimised, anything else =
+ * kept in the problem but left out of the objective and the normal equations (and out of the chi2 of cuba_iter_stat).  NULL = all 0.
+ * set_problem resets every level to 0; set_state, reset_state and optimize keep them.  Changing a level keeps the estimate and
+ * drops what earlier solves left behind (the two-level PCG's coarse matrix).  The result is bit for bit that of a set_problem
+ * whose omega is 0 on the edges at level 1.  get_chi2 still reports omega*|r|^2 with the caller's omega for every edge.  With no
+ * edge at level 0, optimize() writes no iteration (*nstats = 0) and leaves the estimate alone.  Landmark-sharded runs: every rank
+ * gets the same full array and applies its own edges. */
+int cuba_engine_set_edge_levels(cuba_engine* e, const uint8_t* levels);
+int cuba_engine_get_edge_levels(cuba_engine* e, uint8_t* levels);          /* 0 or 1 per edge */
+
+/* The outlier test of ORB-SLAM2's local BA / pose optimisation, on the device, against the current estimate: an edge fails when its
+ * non-robust omega*|r|^2 (the value get_chi2 returns) exceeds chi2_mono / chi2_stereo, or, with CUBA_CLASSIFY_DEPTH, when Xc.z <= 0.
+ * Failing edges go to level 1.  Without CUBA_CLASSIFY_REINCLUDE, levels only go 0 -> 1 (local BA).  With it, an edge that passes goes
+ * back to 0 (pose optimisation).  counts[4] (may be NULL): included mono, included stereo, newly excluded, re-included (summed over
+ * the ranks).  One 32-byte read-back is the only host synchronisation. */
+#define CUBA_CLASSIFY_DEPTH 1
+#define CUBA_CLASSIFY_REINCLUDE 2
+int cuba_engine_classify_edges(cuba_engine* e, double chi2_mono, double chi2_stereo, int flags, int32_t* counts);
+
 /* seconds per profile bucket accumulated since set_problem, [CUBA_PROF_NUM] */
 int cuba_engine_get_profile(cuba_engine* e, double* seconds);
 /* number of kernels this library launched since create (for bench.py's gpu_launches) */
@@ -270,6 +289,10 @@ int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int m
  * hands to cuba_engine_set_problem.  `dropin` is the object's address; the pointers stay valid until the next initialize().
  * Needs no GPU (tests of the graph container: tombstones, re-added edges, fixed vertices, vertices without edges). */
 int cuba_debug_dropin_problem(void* dropin, cuba_problem* out);
+/* The flat edge levels of the drop-in class (include/cuba_b200_levels.h), one byte per edge in the order of
+ * cuba_debug_dropin_problem, with the levels set since the last initialize() applied.  The pointer stays valid until the next call
+ * on the object.  Needs no GPU unless classifyEdges() ran since. */
+int cuba_debug_dropin_levels(void* dropin, const uint8_t** levels, int32_t* n);
 
 /* ---- micro-benchmark hooks for bench.py / profiles (device-resident data, CUDA-event timed) ---- */
 /* Runs the named stage `reps` times back to back and returns the average device milliseconds per
