@@ -2,6 +2,7 @@
 for the hot path: initialize()/optimize(n)/batchStatistics()/timeProfile()/chiSquared()
 (reference include/cuda_bundle_adjustment.h:34-125) on a flat problem."""
 import ctypes as C
+import dataclasses
 import os
 
 import numpy as np
@@ -51,12 +52,47 @@ class _Sizes(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("Pall", "numP", "Lall", "numL", "E2", "E3", "nhpl", "nblk", "nmul", "nblk_full")]
 
 
+class _PoseBatch(C.Structure):
+    _fields_ = [("B", C.c_int32), ("E2", C.c_int32), ("E3", C.c_int32), ("q", C.c_void_p), ("t", C.c_void_p), ("cam", C.c_void_p),
+                ("ptr2", C.c_void_p), ("X2", C.c_void_p), ("meas2", C.c_void_p), ("omega2", C.c_void_p),
+                ("ptr3", C.c_void_p), ("X3", C.c_void_p), ("meas3", C.c_void_p), ("omega3", C.c_void_p)]
+
+
+class _PoseRound(C.Structure):
+    _fields_ = [("iterations", C.c_int32), ("kernel_type", C.c_int32 * 2), ("delta", C.c_double * 2), ("restart", C.c_int32),
+                ("chi2_mono", C.c_double), ("chi2_stereo", C.c_double), ("flags", C.c_int32)]
+
+
+POSE_MAX_ROUNDS = 8      # CUBA_POSE_MAX_ROUNDS
+
+
+@dataclasses.dataclass
+class PoseRound:
+    """One round of Engine.optimize_poses (include/cuba_b200.h: cuba_pose_round): optimize(iterations) under kernel / delta
+    (mono, stereo), from the frame's input pose when restart is set, then the outlier test of classify_edges on the result."""
+    iterations: int = 10
+    kernel: tuple = (ROBUST_NONE, ROBUST_NONE)
+    delta: tuple = (0.0, 0.0)
+    restart: bool = True
+    chi2_mono: float = 5.991
+    chi2_stereo: float = 7.815
+    depth: bool = False
+    reinclude: bool = True
+
+
+def orbslam2_pose_schedule():
+    """ORB-SLAM2's Optimizer::PoseOptimization: four rounds of optimize(10) from the frame's pose, Huber in the first two, the chi2
+    test with re-inclusion after each"""
+    huber = dict(kernel=(ROBUST_HUBER, ROBUST_HUBER), delta=(5.991 ** 0.5, 7.815 ** 0.5))
+    return [PoseRound(**(huber if r < 2 else {})) for r in range(4)]
+
+
 _lib = None
 
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
     "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_flush_l2",
-    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_get_profile",
+    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
     "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
@@ -98,6 +134,7 @@ def load_library():
         "cuba_engine_set_edge_levels": [vp, vp],
         "cuba_engine_get_edge_levels": [vp, vp],
         "cuba_engine_classify_edges": [vp, d, d, i, vp],
+        "cuba_engine_optimize_poses": [vp, C.POINTER(_PoseBatch), i, vp, vp, vp, vp, vp, vp, vp],
         "cuba_engine_get_profile": [vp, vp],
         "cuba_engine_get_launch_count": [vp, C.POINTER(C.c_longlong)],
         "cuba_get_transfer_bytes": [C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)],
@@ -336,6 +373,64 @@ class Engine:
         flags = (1 if depth else 0) | (2 if reinclude else 0)
         _check(self.L.cuba_engine_classify_edges(self.h, float(chi2_mono), float(chi2_stereo), flags, _p(counts)))
         return dict(zip(("included_mono", "included_stereo", "excluded", "reincluded"), (int(v) for v in counts)))
+
+    # --- batched pose optimisation (ORB-SLAM2's PoseOptimization over many frames in one launch) ------------------------------------
+    @staticmethod
+    def _rounds_struct(rounds):
+        rs = (_PoseRound * max(len(rounds), 1))()
+        for k, r in enumerate(rounds):
+            rs[k].iterations = int(r.iterations)
+            rs[k].kernel_type[0], rs[k].kernel_type[1] = int(r.kernel[0]), int(r.kernel[1])
+            rs[k].delta[0], rs[k].delta[1] = float(r.delta[0]), float(r.delta[1])
+            rs[k].restart = int(bool(r.restart))
+            rs[k].chi2_mono, rs[k].chi2_stereo = float(r.chi2_mono), float(r.chi2_stereo)
+            rs[k].flags = (1 if r.depth else 0) | (2 if r.reinclude else 0)
+        return rs
+
+    def optimize_poses_flat(self, q, t, cam, ptr2, X2, meas2, omega2, ptr3, X3, meas3, omega3, rounds, B=None, E2=None, E3=None):
+        """cuba_engine_optimize_poses on flat arrays (include/cuba_b200.h); B / E2 / E3 default to the array sizes.  Returns a dict of
+        q [B,4], t [B,3], levels [E2+E3] (mono then stereo), counts [B,R,4], stats [B,sum of iterations] (structured) and nstats [B,R]."""
+        f64 = lambda a, w: np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1, w) if w > 1 else np.asarray(a, dtype=np.float64).reshape(-1))
+        q, t, cam = f64(q, 4), f64(t, 3), f64(cam, 5)
+        X2, meas2, omega2, X3, meas3, omega3 = f64(X2, 3), f64(meas2, 2), f64(omega2, 1), f64(X3, 3), f64(meas3, 3), f64(omega3, 1)
+        ptr2 = np.ascontiguousarray(ptr2, dtype=np.int32); ptr3 = np.ascontiguousarray(ptr3, dtype=np.int32)
+        B = len(q) if B is None else int(B)
+        E2 = len(omega2) if E2 is None else int(E2)
+        E3 = len(omega3) if E3 is None else int(E3)
+        nb, R = max(B, 0), len(rounds)
+        S = sum(max(int(r.iterations), 0) for r in rounds)
+        out = dict(q=np.zeros((nb, 4)), t=np.zeros((nb, 3)), levels=np.zeros(max(E2, 0) + max(E3, 0), np.uint8),
+                   counts=np.zeros((nb, R, 4), np.int32), stats=(_IterStat * max(nb * S, 1))(), nstats=np.zeros((nb, R), np.int32))
+        batch = _PoseBatch(B, E2, E3, _p(q), _p(t), _p(cam), _p(ptr2), _p(X2), _p(meas2), _p(omega2), _p(ptr3), _p(X3), _p(meas3), _p(omega3))
+        _check(self.L.cuba_engine_optimize_poses(self.h, C.byref(batch), R, self._rounds_struct(rounds), _p(out["q"]), _p(out["t"]),
+                                                 _p(out["levels"]), _p(out["counts"]), out["stats"], _p(out["nstats"])))
+        st = np.frombuffer(out["stats"], dtype=np.dtype([("iteration", "<i4"), ("trials", "<i4"), ("chi2", "<f8"), ("lambda_", "<f8"),
+                                                          ("pcg_iters", "<i4"), ("pcg_failed", "<i4")]))
+        out["stats"] = st[:nb * S].reshape(nb, S).copy()
+        return out
+
+    def optimize_poses(self, frames, rounds):
+        """Refines every frame's pose against its fixed points under the round schedule (list of PoseRound) in one launch.  frames:
+        graphio.PoseFrame objects.  Returns, per frame, a dict of q [4], t [3], levels (the frame's mono edges then its stereo edges),
+        counts [R,4] (included mono, included stereo, newly excluded, re-included after each round) and stats (per round, the
+        iteration statistics as optimize() returns them)."""
+        n2 = np.array([len(f.omega2) for f in frames], np.int64); n3 = np.array([len(f.omega3) for f in frames], np.int64)
+        ptr2 = np.concatenate([[0], np.cumsum(n2)]); ptr3 = np.concatenate([[0], np.cumsum(n3)])
+        cat = lambda name, w: np.concatenate([np.asarray(getattr(f, name), np.float64).reshape(-1, w) for f in frames]) if frames else np.zeros((0, w))
+        r = self.optimize_poses_flat(cat("q", 4), cat("t", 3), cat("cam", 5), ptr2, cat("X2", 3), cat("meas2", 2), cat("omega2", 1).ravel(),
+                                     ptr3, cat("X3", 3), cat("meas3", 3), cat("omega3", 1).ravel(), rounds)
+        off = np.concatenate([[0], np.cumsum([int(x.iterations) for x in rounds])])
+        E2 = int(ptr2[-1])
+        res = []
+        for b in range(len(frames)):
+            stats = []
+            for k in range(len(rounds)):
+                rows = r["stats"][b, off[k]:off[k] + r["nstats"][b, k]]
+                stats.append([dict(iteration=int(s["iteration"]), trials=int(s["trials"]), chi2=float(s["chi2"]), lambda_=float(s["lambda_"]),
+                                   pcg_iters=int(s["pcg_iters"]), pcg_failed=int(s["pcg_failed"])) for s in rows])
+            res.append(dict(q=r["q"][b], t=r["t"][b], counts=r["counts"][b], stats=stats,
+                            levels=np.concatenate([r["levels"][ptr2[b]:ptr2[b + 1]], r["levels"][E2 + ptr3[b]:E2 + ptr3[b + 1]]])))
+        return res
 
     def launch_count(self):
         n = C.c_longlong(0)

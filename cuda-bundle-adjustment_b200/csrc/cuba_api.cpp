@@ -19,6 +19,8 @@
 // arrays goes to the engine after set_problem only when some level is set; classifyEdges() decisions are fetched lazily.
 #include <algorithm>
 #include <chrono>
+#include <cmath>
+#include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -35,6 +37,7 @@
 #include "../../include/cuba_b200.h"
 #include "../../include/cuda_bundle_adjustment.h"
 #include "../../include/cuba_b200_levels.h"
+#include "../../include/cuba_b200_pose.h"
 
 namespace cuba
 {
@@ -429,6 +432,12 @@ public:
 		out.excluded = static_cast<size_t>(c[2]); out.reincluded = static_cast<size_t>(c[3]);
 		return out;
 	}
+	// the engine optimizePoses() runs on (include/cuba_b200_pose.h): this object's, created on demand
+	cuba_engine* poseEngine()
+	{
+		ensureEngine();
+		return engine_;
+	}
 	// the flat levels with every level set so far applied (also behind cuba_debug_dropin_levels)
 	bool flatLevels(const uint8_t** p, int32_t* n)
 	{
@@ -623,6 +632,110 @@ static Impl& impl_of(const CudaBundleAdjustment& ba)
 void setEdgeLevel(CudaBundleAdjustment& ba, BaseEdge* e, int level) { impl_of(ba).setEdgeLevel(e, level); }
 int edgeLevel(const CudaBundleAdjustment& ba, const BaseEdge* e) { return impl_of(ba).edgeLevel(e); }
 OutlierCounts classifyEdges(CudaBundleAdjustment& ba, const OutlierTest& test) { return impl_of(ba).classifyEdges(test); }
+
+// include/cuba_b200_pose.h
+std::vector<PoseRound> orbSlam2PoseSchedule()
+{
+	std::vector<PoseRound> s(4);
+	for (size_t r = 0; r < s.size(); r++) {
+		if (r < 2) {
+			s[r].kernelMono = s[r].kernelStereo = RobustKernelType::HUBER;
+			s[r].deltaMono = std::sqrt(5.991); s[r].deltaStereo = std::sqrt(7.815);
+		}
+		s[r].test.chi2Mono = 5.991; s[r].test.chi2Stereo = 7.815;
+		s[r].test.requirePositiveDepth = false; s[r].test.reinclude = true;
+	}
+	return s;
+}
+
+std::vector<PoseResult> optimizePoses(CudaBundleAdjustment& ba, const std::vector<PoseFrame>& frames, const std::vector<PoseRound>& schedule)
+{
+	Impl& impl = impl_of(ba);
+	if (frames.size() > static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizePoses: too many frames");
+	const size_t B = frames.size();
+	std::vector<double> q(4 * B), t(3 * B), cam(5 * B), X2, m2, om2, X3, m3, om3;
+	std::vector<int32_t> ptr2(B + 1, 0), ptr3(B + 1, 0);
+	for (size_t b = 0; b < B; b++) {
+		const PoseFrame& f = frames[b];
+		if (!f.pose) throw std::invalid_argument("cuba::optimizePoses: frame without a pose");
+		for (int k = 0; k < 4; k++) q[4 * b + k] = f.pose->q.coeffs().data()[k];
+		for (int k = 0; k < 3; k++) t[3 * b + k] = f.pose->t.data()[k];
+		const CameraParams& c = f.pose->camera;
+		cam[5 * b] = c.fx; cam[5 * b + 1] = c.fy; cam[5 * b + 2] = c.cx; cam[5 * b + 3] = c.cy; cam[5 * b + 4] = c.bf;
+		for (const BaseEdge* e : f.edges) {
+			if (!e) throw std::invalid_argument("cuba::optimizePoses: null edge");
+			if (e->poseVertex() != f.pose) throw std::invalid_argument("cuba::optimizePoses: an edge's pose vertex is not the frame's pose");
+			const LandmarkVertex* l = e->landmarkVertex();
+			if (!l) throw std::invalid_argument("cuba::optimizePoses: an edge without a landmark");
+			if (e->dim() == 2) {
+				const MonoEdge* me = static_cast<const MonoEdge*>(e);
+				for (int k = 0; k < 3; k++) X2.push_back(l->Xw.data()[k]);
+				m2.push_back(me->measurement.data()[0]); m2.push_back(me->measurement.data()[1]);
+				om2.push_back(me->information);
+			} else if (e->dim() == 3) {
+				const StereoEdge* se = static_cast<const StereoEdge*>(e);
+				for (int k = 0; k < 3; k++) X3.push_back(l->Xw.data()[k]);
+				for (int k = 0; k < 3; k++) m3.push_back(se->measurement.data()[k]);
+				om3.push_back(se->information);
+			} else throw std::invalid_argument("cuba::optimizePoses: an edge that is neither monocular nor stereo");
+		}
+		if (om2.size() + om3.size() > static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizePoses: too many edges");
+		ptr2[b + 1] = static_cast<int32_t>(om2.size()); ptr3[b + 1] = static_cast<int32_t>(om3.size());
+	}
+	std::vector<cuba_pose_round> rounds(schedule.size());
+	size_t perFrame = 0;
+	for (size_t r = 0; r < schedule.size(); r++) {
+		const PoseRound& s = schedule[r];
+		cuba_pose_round& c = rounds[r];
+		c.iterations = s.iterations;
+		c.kernel_type[0] = static_cast<int32_t>(s.kernelMono); c.kernel_type[1] = static_cast<int32_t>(s.kernelStereo);
+		c.delta[0] = s.deltaMono; c.delta[1] = s.deltaStereo;
+		c.restart = s.restart ? 1 : 0;
+		c.chi2_mono = s.test.chi2Mono; c.chi2_stereo = s.test.chi2Stereo;
+		c.flags = (s.test.requirePositiveDepth ? CUBA_CLASSIFY_DEPTH : 0) | (s.test.reinclude ? CUBA_CLASSIFY_REINCLUDE : 0);
+		perFrame += static_cast<size_t>(std::max(s.iterations, 0));
+	}
+	const size_t R = rounds.size();
+	cuba_pose_batch bt;
+	bt.B = static_cast<int32_t>(B); bt.E2 = static_cast<int32_t>(om2.size()); bt.E3 = static_cast<int32_t>(om3.size());
+	bt.q = q.data(); bt.t = t.data(); bt.cam = cam.data();
+	bt.ptr2 = ptr2.data(); bt.X2 = X2.data(); bt.meas2 = m2.data(); bt.omega2 = om2.data();
+	bt.ptr3 = ptr3.data(); bt.X3 = X3.data(); bt.meas3 = m3.data(); bt.omega3 = om3.data();
+	std::vector<double> qo(4 * B), to(3 * B);
+	std::vector<uint8_t> lev(om2.size() + om3.size());
+	std::vector<int32_t> counts(4 * B * std::max<size_t>(R, 1)), nstats(B * std::max<size_t>(R, 1));
+	std::vector<cuba_iter_stat> stats(std::max<size_t>(B * perFrame, 1));
+	// the schedule and the batch are checked by the engine before anything runs: a refusal is the caller's input
+	const int rc = cuba_engine_optimize_poses(impl.poseEngine(), &bt, static_cast<int>(R), rounds.data(), qo.data(), to.data(), lev.data(),
+		counts.data(), stats.data(), nstats.data());
+	if (rc == CUBA_ERR_INVALID) throw std::invalid_argument(std::string("cuba::optimizePoses: ") + cuba_last_error());
+	if (rc != CUBA_OK) throw std::runtime_error(std::string("cuba_b200: ") + cuba_last_error());
+	std::vector<PoseResult> out(B);
+	const size_t E2 = om2.size();
+	for (size_t b = 0; b < B; b++) {
+		PoseVertex* p = frames[b].pose;
+		for (int k = 0; k < 4; k++) p->q.coeffs().data()[k] = qo[4 * b + k];
+		for (int k = 0; k < 3; k++) p->t.data()[k] = to[3 * b + k];
+		PoseResult& res = out[b];
+		size_t i2 = static_cast<size_t>(ptr2[b]), i3 = E2 + static_cast<size_t>(ptr3[b]);
+		for (const BaseEdge* e : frames[b].edges) {
+			const int lv = e->dim() == 2 ? lev[i2++] : lev[i3++];
+			res.levels.push_back(lv);
+			res.inliers += lv == 0;
+		}
+		size_t off = 0;
+		for (size_t r = 0; r < R; r++) {
+			BatchStatistics st;
+			for (int i = 0; i < nstats[b * R + r]; i++) {
+				const cuba_iter_stat& s = stats[b * perFrame + off + i];
+				st.push_back(BatchInfo{ s.iteration, s.chi2 });
+			}
+			res.rounds.push_back(st);
+			off += static_cast<size_t>(rounds[r].iterations);
+		}
+	}
+	return out;
+}
 
 static bool dropin_levels(CudaBundleAdjustment* obj, const uint8_t** levels, int32_t* n)
 {

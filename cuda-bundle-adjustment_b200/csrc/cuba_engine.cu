@@ -26,6 +26,7 @@
 #include "cuba_schur2.cuh"
 #include "cuba_jh4.cuh"
 #include "cuba_levels.cuh"
+#include "cuba_pose_batch.cuh"
 #include "cuba_schur3.cuh"
 #include "cuba_schur5.cuh"
 #include "cuba_structure.h"
@@ -77,6 +78,25 @@ struct PinnedArena {
 		memcpy(p + o, src, bytes);
 		off = o + bytes;
 		return p + o;
+	}
+};
+
+// grow-only page-locked host buffer (the staging area of one packed copy)
+struct PinnedBuf {
+	char* p = nullptr; size_t cap = 0;
+	PinnedBuf() {}
+	PinnedBuf(const PinnedBuf&) = delete;
+	PinnedBuf& operator=(const PinnedBuf&) = delete;
+	~PinnedBuf() { if (p) cudaFreeHost(p); }
+	cudaError_t grow(size_t bytes)
+	{
+		if (p && bytes <= cap) return cudaSuccess;
+		if (p) cudaFreeHost(p);
+		p = nullptr; cap = 0;
+		const cudaError_t e = cudaMallocHost((void**)&p, std::max<size_t>(bytes, 256));
+		if (e == cudaSuccess) cap = std::max<size_t>(bytes, 256);
+		else p = nullptr;
+		return e;
 	}
 };
 
@@ -202,6 +222,8 @@ struct EngineBase {
 	virtual int set_edge_levels(const uint8_t* levels) = 0;
 	virtual int get_edge_levels(uint8_t* levels) = 0;
 	virtual int classify_edges(double chi2Mono, double chi2Stereo, int flags, int32_t* counts) = 0;
+	virtual int optimize_poses(const cuba_pose_batch* bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
+		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) = 0;
 };
 
 template <typename T>
@@ -291,6 +313,9 @@ struct Engine : EngineBase {
 	DBuf<unsigned char> lvLevel;   // [E] in edge-id order; a rank reads and writes its own edges only
 	DBuf<int> lvPartial;
 	DBuf<double> lvCount;
+	// batched pose optimisation (cuba_pose_batch.cuh): the packed batch and the packed results, device and page-locked host copies
+	DBuf<double> pbIn, pbOut;
+	PinnedBuf pbHostIn, pbHostOut;
 	DBuf<Scalars> dScal;
 	Scalars* hScal = nullptr;   // pinned
 	DBuf<double> flushBuf;
@@ -2254,6 +2279,81 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// ---- batched pose optimisation (cuba_pose_batch.cuh): one H2D of the packed batch, one launch, one D2H of the packed results.
+	// Always fp64, on this engine's stream; touches nothing of the engine's problem.  The batch was validated by the caller.
+	int optimize_poses(const cuba_pose_batch* bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
+		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) override
+	{
+		static_assert(sizeof(pb::IterStat) == sizeof(cuba_iter_stat) && sizeof(pb::IterStat) == 32, "cuba_iter_stat layout");
+		const size_t B = (size_t)bt->B, R = (size_t)s.n;
+		if (B == 0) return CUBA_OK;
+		const size_t E2 = (size_t)bt->E2, E3 = (size_t)bt->E3, E = E2 + E3;
+		const size_t nStat = stats ? B * (size_t)s.statOff[s.n] : 0;
+		// input, in doubles: pose [B][8] | cam [B][8] | edges [E][8] | ptr2, ptr3 as int32 [B+1] each
+		const size_t oCam = 8 * B, oEdge = 16 * B, oPtr = oEdge + 8 * E, nIn = oPtr + (B + 1);
+		// results, in doubles: pose [B][8] | stats [nStat] (4 doubles each) | counts [B][R][4], nstats [B][R] as int32 | levels [E] bytes
+		const size_t oStat = 8 * B, oInt = oStat + 4 * nStat, nInt = 5 * B * R, oLev = oInt + (nInt + 1) / 2, nOut = oLev + (E + 7) / 8;
+		CUDA_TRY(pbHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(pbHostOut.grow(sizeof(double) * nOut));
+		CUDA_TRY(pbIn.alloc(nIn)); CUDA_TRY(pbOut.alloc(nOut));
+		double* h = (double*)pbHostIn.p;
+		for (size_t b = 0; b < B; b++) {
+			double* p = h + 8 * b;
+			for (int k = 0; k < 4; k++) p[k] = bt->q[4 * b + k];
+			for (int k = 0; k < 3; k++) p[4 + k] = bt->t[3 * b + k];
+			p[7] = 0;
+			double* c = h + oCam + 8 * b;
+			for (int k = 0; k < 5; k++) c[k] = bt->cam[5 * b + k];
+			c[5] = c[6] = c[7] = 0;
+			// a frame's edges are contiguous, its mono edges first: mono i at ptr3[b] + i, stereo j at ptr2[b+1] + j
+			for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) {
+				double* d = h + oEdge + 8 * ((size_t)bt->ptr3[b] + i);
+				d[0] = bt->X2[3 * i]; d[1] = bt->X2[3 * i + 1]; d[2] = bt->X2[3 * i + 2];
+				d[3] = bt->meas2[2 * i]; d[4] = bt->meas2[2 * i + 1]; d[5] = 0; d[6] = bt->omega2[i]; d[7] = 0;
+			}
+			for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) {
+				double* d = h + oEdge + 8 * ((size_t)bt->ptr2[b + 1] + j);
+				d[0] = bt->X3[3 * j]; d[1] = bt->X3[3 * j + 1]; d[2] = bt->X3[3 * j + 2];
+				d[3] = bt->meas3[3 * j]; d[4] = bt->meas3[3 * j + 1]; d[5] = bt->meas3[3 * j + 2]; d[6] = bt->omega3[j]; d[7] = 0;
+			}
+		}
+		int32_t* hp = (int32_t*)(h + oPtr);
+		memcpy(hp, bt->ptr2, sizeof(int32_t) * (B + 1));
+		memcpy(hp + B + 1, bt->ptr3, sizeof(int32_t) * (B + 1));
+		CUDA_TRY(cudaMemcpyAsync(pbIn.p, h, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
+		g_h2dBytes += (long long)(sizeof(double) * nIn);
+		pb::Args a;
+		a.B = (int)B;
+		a.pose = pbIn.p; a.cam = pbIn.p + oCam; a.edge = pbIn.p + oEdge;
+		a.ptr2 = (const int*)(pbIn.p + oPtr); a.ptr3 = a.ptr2 + B + 1;
+		a.poseOut = pbOut.p;
+		a.stats = stats ? (pb::IterStat*)(pbOut.p + oStat) : nullptr;
+		a.counts = (int*)(pbOut.p + oInt); a.nstats = a.counts + 4 * B * R;
+		a.level = (unsigned char*)(pbOut.p + oLev);
+		pb::k_pose_batch<<<(unsigned)B, pb::BLOCK, 0, stream>>>(a, s);
+		launches++;
+		CUDA_TRY(cudaGetLastError());
+		CUDA_TRY(cudaMemcpyAsync(pbHostOut.p, pbOut.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
+		g_d2hBytes += (long long)(sizeof(double) * nOut);
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		const double* o = (const double*)pbHostOut.p;
+		for (size_t b = 0; b < B; b++) {
+			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
+			for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
+		}
+		if (stats && nStat) memcpy(stats, o + oStat, sizeof(cuba_iter_stat) * nStat);
+		const int32_t* oi = (const int32_t*)(o + oInt);
+		if (counts) memcpy(counts, oi, sizeof(int32_t) * 4 * B * R);
+		if (nstats) memcpy(nstats, oi + 4 * B * R, sizeof(int32_t) * B * R);
+		if (levelsOut) {
+			const unsigned char* lv = (const unsigned char*)(o + oLev);
+			for (size_t b = 0; b < B; b++) {
+				for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) levelsOut[i] = lv[(size_t)bt->ptr3[b] + i];
+				for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) levelsOut[E2 + j] = lv[(size_t)bt->ptr2[b + 1] + j];
+			}
+		}
+		return CUBA_OK;
+	}
+
 	int get_profile(double* sec) override
 	{
 		resolveProfile();
@@ -2560,6 +2660,58 @@ int cuba_engine_classify_edges(cuba_engine* e, double chi2_mono, double chi2_ste
 	if (flags & ~(CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE)) return fail(CUBA_ERR_INVALID, "classify_edges: unknown flag");
 	return e->impl->classify_edges(chi2_mono, chi2_stereo, flags, counts);
 }
+// the batch and the schedule come from outside the program: everything the kernel relies on is checked here, before any work
+static int pose_frames_ok(int B, int E, const int32_t* ptr, const double* X, const double* meas, const double* om, const char* what)
+{
+	if (E < 0) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: negative edge count ") + what);
+	if (!ptr) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: null ptr") + what);
+	if (ptr[0] != 0) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: ptr") + what + "[0] != 0");
+	for (int b = 0; b < B; b++)
+		if (ptr[b + 1] < ptr[b]) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: ptr") + what + " decreases");
+	if (ptr[B] != E) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: ptr") + what + "[B] is not the edge count");
+	if (E > 0 && (!X || !meas || !om)) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: null edge array ") + what);
+	for (int i = 0; i < E; i++)
+		if (!std::isfinite(om[i])) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: non-finite omega") + what);
+	return CUBA_OK;
+}
+
+int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds,
+	double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats)
+{
+	ENGINE_OR_FAIL(e);
+	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_poses: null batch");
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: B < 0");
+	if (nrounds < 1 || nrounds > CUBA_POSE_MAX_ROUNDS || !rounds) return fail(CUBA_ERR_INVALID, "optimize_poses: nrounds outside 1..CUBA_POSE_MAX_ROUNDS");
+	static_assert(CUBA_POSE_MAX_ROUNDS == pb::MAX_ROUNDS, "round limit");
+	pb::Schedule s;
+	memset(&s, 0, sizeof(s));
+	s.n = nrounds;
+	long long off = 0;
+	for (int r = 0; r < nrounds; r++) {
+		const cuba_pose_round& R = rounds[r];
+		if (R.iterations < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: negative iterations");
+		if (R.flags & ~(CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE)) return fail(CUBA_ERR_INVALID, "optimize_poses: unknown flag");
+		for (int k = 0; k < 2; k++) {
+			if (R.kernel_type[k] < CUBA_ROBUST_NONE || R.kernel_type[k] > CUBA_ROBUST_TUKEY) return fail(CUBA_ERR_INVALID, "optimize_poses: unknown kernel type");
+			if (!std::isfinite(R.delta[k])) return fail(CUBA_ERR_INVALID, "optimize_poses: non-finite delta");
+			s.rk[r].type[k] = R.kernel_type[k]; s.rk[r].delta[k] = R.delta[k];
+		}
+		s.r[r].iterations = R.iterations; s.r[r].restart = R.restart != 0; s.r[r].flags = R.flags;
+		s.r[r].chi2[0] = R.chi2_mono; s.r[r].chi2[1] = R.chi2_stereo;
+		s.statOff[r] = (int)off;
+		off += R.iterations;
+		if (off > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many iterations");
+	}
+	s.statOff[nrounds] = (int)off;
+	const int B = bt->B;
+	if (B == 0) return CUBA_OK;
+	if (!bt->q || !bt->t || !bt->cam || !q_out || !t_out) return fail(CUBA_ERR_INVALID, "optimize_poses: null pose array");
+	if ((long long)bt->E2 + bt->E3 > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many edges");
+	int rc = pose_frames_ok(B, bt->E2, bt->ptr2, bt->X2, bt->meas2, bt->omega2, "2"); if (rc) return rc;
+	rc = pose_frames_ok(B, bt->E3, bt->ptr3, bt->X3, bt->meas3, bt->omega3, "3"); if (rc) return rc;
+	return e->impl->optimize_poses(bt, s, q_out, t_out, levels_out, counts, stats, nstats);
+}
+
 int cuba_engine_get_profile(cuba_engine* e, double* sec) { ENGINE_OR_FAIL(e); if (!sec) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_profile(sec); }
 // debug: per-CTA phase timings of the last k_pcg3 launch (library built with -DCUBA_PCG_TIMING); returns the CTA count
 int cuba_debug_get_pcg_timing(cuba_engine* e, long long* out, int maxCtas)

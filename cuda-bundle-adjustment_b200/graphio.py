@@ -143,6 +143,57 @@ def flatten(g) -> FlatProblem:
         pose_rows=prow_order, lm_rows=lrow_order, mono_rows=mrows, stereo_rows=srows)
 
 
+@dataclasses.dataclass
+class PoseFrame:
+    """One frame of Engine.optimize_poses: a free pose and its edges, each carrying its own world point, which is held fixed."""
+    q: np.ndarray       # [4]
+    t: np.ndarray       # [3]
+    cam: np.ndarray     # [5]
+    X2: np.ndarray      # [E2,3]
+    meas2: np.ndarray   # [E2,2]
+    omega2: np.ndarray  # [E2]
+    X3: np.ndarray      # [E3,3]
+    meas3: np.ndarray   # [E3,3]
+    omega3: np.ndarray  # [E3]
+    mono_ids: np.ndarray = None     # edge ids (0..E2-1) of the flat problem the frame was cut from
+    stereo_ids: np.ndarray = None   # ids among the stereo edges (0..E3-1)
+
+    def flat_problem(self, q=None, t=None, keep=None) -> FlatProblem:
+        """The frame as a flat problem (its pose the only vertex, free; one fixed landmark per edge) at pose (q, t) (default: the
+        frame's), with only the edges where keep[mono + stereo] is true (default: all): what the engine optimises for the frame."""
+        E2 = len(self.omega2)
+        keep = np.ones(E2 + len(self.omega3), bool) if keep is None else np.asarray(keep, bool)
+        m, s = keep[:E2], keep[E2:]
+        n2, n3 = int(m.sum()), int(s.sum())
+        q = self.q if q is None else q
+        t = self.t if t is None else t
+        return FlatProblem(
+            Pall=1, numP=1, Lall=n2 + n3, numL=0, q=np.array(q, dtype=np.float64).reshape(1, 4), t=np.array(t, dtype=np.float64).reshape(1, 3),
+            cam=np.array(self.cam, dtype=np.float64).reshape(1, 5), Xw=np.concatenate([self.X2[m], self.X3[s]]).reshape(-1, 3),
+            idx2=np.stack([np.zeros(n2), np.arange(n2)], 1).astype(np.int32), meas2=self.meas2[m].reshape(-1, 2), omega2=self.omega2[m],
+            idx3=np.stack([np.zeros(n3), n2 + np.arange(n3)], 1).astype(np.int32), meas3=self.meas3[s].reshape(-1, 3), omega3=self.omega3[s])
+
+
+def pose_frames(prob: FlatProblem, rows):
+    """The frames of the poses `rows` (indices iP of prob): each pose with all of its edges in edge-id order, the edges' points taken
+    from prob.Xw.  What flatten() gives for the graph of that one pose, free, with its edges and their landmarks, fixed."""
+    def groups(idx):
+        order = np.argsort(idx[:, 0], kind="stable")
+        ptr = np.searchsorted(idx[order, 0], np.arange(prob.Pall + 1))
+        return order, ptr
+    o2, p2 = groups(prob.idx2)
+    o3, p3 = groups(prob.idx3)
+    out = []
+    for p in rows:
+        p = int(p)
+        m = o2[p2[p]:p2[p + 1]]; s = o3[p3[p]:p3[p + 1]]
+        out.append(PoseFrame(q=prob.q[p].copy(), t=prob.t[p].copy(), cam=prob.cam[p].copy(),
+                             X2=prob.Xw[prob.idx2[m, 1]], meas2=prob.meas2[m].copy(), omega2=prob.omega2[m].copy(),
+                             X3=prob.Xw[prob.idx3[s, 1]], meas3=prob.meas3[s].copy(), omega3=prob.omega3[s].copy(),
+                             mono_ids=m, stereo_ids=s))
+    return out
+
+
 def write_back(g, prob: FlatProblem, q, t, Xw):
     """finalize(): reference src/cuda_bundle_adjustment.cpp:512-526 (fixed vertices are written back too)."""
     g["q"][prob.pose_rows] = q

@@ -197,6 +197,52 @@ int cuba_engine_get_edge_levels(cuba_engine* e, uint8_t* levels);          /* 0 
 #define CUBA_CLASSIFY_REINCLUDE 2
 int cuba_engine_classify_edges(cuba_engine* e, double chi2_mono, double chi2_stereo, int flags, int32_t* counts);
 
+/* Pose optimisation of many frames (ORB-SLAM2's Optimizer::PoseOptimization, batched).  A frame is one free SE(3) pose and its
+ * edges, each carrying its own world point, which is held fixed.  Host arrays, fp64; the edges of frame b are [ptr2[b], ptr2[b+1])
+ * and [ptr3[b], ptr3[b+1]), ptr2[0] = ptr3[0] = 0, ptr2[B] = E2, ptr3[B] = E3.  Array pointers of an empty edge type may be NULL. */
+typedef struct cuba_pose_batch {
+	int32_t B, E2, E3;
+	const double* q;       /* [4B] x,y,z,w                                                         */
+	const double* t;       /* [3B]                                                                 */
+	const double* cam;     /* [5B] fx,fy,cx,cy,bf                                                  */
+	const int32_t* ptr2;   /* [B+1]                                                                */
+	const double* X2;      /* [3*E2] world point of each monocular edge                            */
+	const double* meas2;   /* [2*E2]                                                               */
+	const double* omega2;  /* [E2]                                                                 */
+	const int32_t* ptr3;   /* [B+1]                                                                */
+	const double* X3;      /* [3*E3]                                                               */
+	const double* meas3;   /* [3*E3]                                                               */
+	const double* omega3;  /* [E3]                                                                 */
+} cuba_pose_batch;
+
+/* One round of the schedule: optimize(iterations) with the given robust kernels (meaning of cuba_engine_set_robust_kernel, indexed by
+ * CUBA_EDGE_*), from the frame's input pose when restart != 0 (ORB-SLAM2 sets the estimate at the top of every round), else from the
+ * previous round's result; then the outlier test of cuba_engine_classify_edges on the committed pose. */
+#define CUBA_POSE_MAX_ROUNDS 8
+typedef struct cuba_pose_round {
+	int32_t iterations;
+	int32_t kernel_type[2];
+	double delta[2];
+	int32_t restart;
+	double chi2_mono, chi2_stereo;
+	int32_t flags;         /* CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE                         */
+} cuba_pose_round;
+
+/* Runs the schedule on every frame: ONE kernel launch (one CTA per frame), one host->device and one device->host copy.  Every edge
+ * starts at level 0.  Each frame's result is what the engine computes for the frame's sub-problem (set_problem with one free pose
+ * and the edges' points as fixed landmarks; per round set_robust_kernel, set_state on restart, optimize(iterations), classify_edges),
+ * always in fp64; it is bit-reproducible and independent of the other frames of the batch.  A round with no edge at level 0 writes no
+ * iteration and leaves the pose alone.  Runs on the engine's device and stream, ignores set_comm, and neither reads nor changes the
+ * engine's problem, state, levels or solver state.
+ * Outputs: q_out [4B], t_out [3B]; levels_out [E2+E3] (mono then stereo, 0/1 after the last round); counts [B][nrounds][4] (as
+ * classify_edges); stats [B][sum of iterations] (round r of frame b at b * sum + iterations of rounds < r, pcg fields 0); nstats
+ * [B][nrounds] (iterations written per round).  Every output except q_out / t_out may be NULL.  B = 0 does nothing.
+ * CUBA_ERR_INVALID, with nothing run, for a malformed batch or schedule (B < 0, ptr not starting at 0, decreasing or not ending at
+ * the edge count, nrounds outside 1..CUBA_POSE_MAX_ROUNDS, negative iterations, an unknown kernel type or flag, a non-finite omega
+ * or delta). */
+int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* batch, int nrounds, const cuba_pose_round* rounds,
+	double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats);
+
 /* seconds per profile bucket accumulated since set_problem, [CUBA_PROF_NUM] */
 int cuba_engine_get_profile(cuba_engine* e, double* seconds);
 /* number of kernels this library launched since create (for bench.py's gpu_launches) */
