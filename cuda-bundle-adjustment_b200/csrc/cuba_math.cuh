@@ -180,18 +180,38 @@ CUBA_HD bool spd6_inverse(T A[36])
 
 // pose <- Exp([omega;upsilon]) * pose  (cu:551-592): Rodrigues with the theta<1e-5 Taylor branch,
 // R->quaternion by the trace method (cu:492-521), normalisation with w>=0 (cu:531-539).
+// In fp32, a2 = (1 - cos th) / th^2 cancels to nothing between th = 1e-5 and ~3e-4 (V then loses its [w]x upsilon term, an error
+// of th/2 |upsilon|), so the float instantiation uses a2 = 1/2 (sin(th/2) / (th/2))^2 and the series of a3 below th = 0.5.  The
+// double instantiation keeps the reference's formulas (its cancellation costs at most 1.1e-11 |upsilon|).
 template <typename T>
-CUBA_HD void se3_update(const T upd[6], T q[4], T t[3])
+CUBA_HD void se3_coefficients(T theta, T& a1, T& a2, T& a3)
 {
-	const T wx = upd[0], wy = upd[1], wz = upd[2];
-	const T theta = t_sqrt(wx * wx + wy * wy + wz * wz);
-	T a1, a2, a3;
 	if (theta < T(0.00001)) { a1 = T(1); a2 = T(0.5); a3 = T(1) / 6; }
 	else {
 		a1 = t_sin(theta) / theta;
 		a2 = (1 - t_cos(theta)) / (theta * theta);
 		a3 = (theta - t_sin(theta)) / (theta * theta * theta);
 	}
+}
+template <>
+CUBA_HD void se3_coefficients<float>(float theta, float& a1, float& a2, float& a3)
+{
+	if (theta < 0.00001f) { a1 = 1.f; a2 = 0.5f; a3 = 1.f / 6; return; }
+	a1 = sinf(theta) / theta;
+	const float h = 0.5f * theta, s = sinf(h) / h;
+	a2 = 0.5f * s * s;
+	const float t2 = theta * theta;
+	// (th - sin th) / th^3 = 1/6 - th^2/120 + th^4/5040 - th^6/362880 + ..., truncation below 1e-10 at th = 0.5
+	a3 = theta < 0.5f ? (1.f / 6) - t2 * ((1.f / 120) - t2 * ((1.f / 5040) - t2 * (1.f / 362880))) : (theta - sinf(theta)) / (t2 * theta);
+}
+
+template <typename T>
+CUBA_HD void se3_update(const T upd[6], T q[4], T t[3])
+{
+	const T wx = upd[0], wy = upd[1], wz = upd[2];
+	const T theta = t_sqrt(wx * wx + wy * wy + wz * wz);
+	T a1, a2, a3;
+	se3_coefficients(theta, a1, a2, a3);
 	// O1 = [w]x, O2 = [w]x^2 ; M(i,j) row i col j
 	const T O1[3][3] = { { T(0), -wz, wy }, { wz, T(0), -wx }, { -wy, wx, T(0) } };
 	const T xx = wx * wx, yy = wy * wy, zz = wz * wz, xy = wx * wy, yz = wy * wz, zx = wz * wx;
@@ -238,11 +258,13 @@ CUBA_HD void se3_update(const T upd[6], T q[4], T t[3])
 	for (int i = 0; i < 4; i++) q[i] = invn * r[i];
 }
 
+#if defined(__CUDACC__)
 // D = A B + D on the fp64 tensor pipe, one 8x8x4 product per warp: lane l holds A(l/4, l%4), B(l%4, l/4) and
 // D(l/4, 2 (l%4)) / D(l/4, 2 (l%4) + 1)
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
 {
 	asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
+#endif
 
 }  // namespace cuba_b200
