@@ -87,12 +87,35 @@ def orbslam2_pose_schedule():
     return [PoseRound(**(huber if r < 2 else {})) for r in range(4)]
 
 
+class _Sim3Batch(C.Structure):
+    _fields_ = [("B", C.c_int32), ("N", C.c_int32), ("ptr", C.c_void_p), ("q", C.c_void_p), ("t", C.c_void_p), ("s", C.c_void_p),
+                ("cam1", C.c_void_p), ("cam2", C.c_void_p), ("fix_scale", C.c_void_p), ("X1", C.c_void_p), ("X2", C.c_void_p),
+                ("obs1", C.c_void_p), ("obs2", C.c_void_p), ("omega1", C.c_void_p), ("omega2", C.c_void_p)]
+
+
+class _Sim3Params(C.Structure):
+    _fields_ = [("chi2", C.c_double), ("iterations", C.c_int32), ("iterations_bad", C.c_int32), ("iterations_good", C.c_int32),
+                ("min_pairs", C.c_int32)]
+
+
+@dataclasses.dataclass
+class Sim3Params:
+    """OptimizeSim3's schedule (include/cuba_b200.h: cuba_sim3_params), ORB-SLAM2's values by default: optimize(iterations), the pair
+    test at chi2 (also the square of the Huber delta), then, with at least min_pairs pairs left, optimize(iterations_bad) if the test
+    removed a pair, else optimize(iterations_good), and the test again."""
+    chi2: float = 10.0
+    iterations: int = 5
+    iterations_bad: int = 10
+    iterations_good: int = 5
+    min_pairs: int = 10
+
+
 _lib = None
 
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
     "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_flush_l2",
-    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_get_profile",
+    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
     "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
@@ -135,6 +158,7 @@ def load_library():
         "cuba_engine_get_edge_levels": [vp, vp],
         "cuba_engine_classify_edges": [vp, d, d, i, vp],
         "cuba_engine_optimize_poses": [vp, C.POINTER(_PoseBatch), i, vp, vp, vp, vp, vp, vp, vp],
+        "cuba_engine_optimize_sim3": [vp, C.POINTER(_Sim3Batch), C.POINTER(_Sim3Params), vp, vp, vp, vp, vp, vp, vp],
         "cuba_engine_get_profile": [vp, vp],
         "cuba_engine_get_launch_count": [vp, C.POINTER(C.c_longlong)],
         "cuba_get_transfer_bytes": [C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)],
@@ -430,6 +454,57 @@ class Engine:
                                    pcg_iters=int(s["pcg_iters"]), pcg_failed=int(s["pcg_failed"])) for s in rows])
             res.append(dict(q=r["q"][b], t=r["t"][b], counts=r["counts"][b], stats=stats,
                             levels=np.concatenate([r["levels"][ptr2[b]:ptr2[b + 1]], r["levels"][E2 + ptr3[b]:E2 + ptr3[b + 1]]])))
+        return res
+
+    # --- batched Sim(3) alignment (ORB-SLAM2's OptimizeSim3 over many keyframe pairs in one launch) ------------------------------------
+    def optimize_sim3_flat(self, ptr, q, t, s, cam1, cam2, fix_scale, X1, X2, obs1, obs2, omega1, omega2, params=None, B=None, N=None):
+        """cuba_engine_optimize_sim3 on flat arrays (include/cuba_b200.h); fix_scale may be None; B / N default to the array sizes.
+        Returns a dict of q [B,4], t [B,3], s [B], levels [N], ninliers [B], stats [B, iterations + max(bad, good)] (structured) and
+        nstats [B,2]."""
+        params = Sim3Params() if params is None else params
+        f64 = lambda a, w: np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1, w) if w > 1 else np.asarray(a, dtype=np.float64).reshape(-1))
+        q, t, s, cam1, cam2 = f64(q, 4), f64(t, 3), f64(s, 1), f64(cam1, 4), f64(cam2, 4)
+        X1, X2, obs1, obs2, omega1, omega2 = f64(X1, 3), f64(X2, 3), f64(obs1, 2), f64(obs2, 2), f64(omega1, 1), f64(omega2, 1)
+        ptr = np.ascontiguousarray(ptr, dtype=np.int32)
+        fix = None if fix_scale is None else np.ascontiguousarray(fix_scale, dtype=np.int32)
+        B = len(s) if B is None else int(B)
+        N = len(omega1) if N is None else int(N)
+        nb = max(B, 0)
+        S = max(int(params.iterations), 0) + max(int(params.iterations_bad), int(params.iterations_good), 0)
+        out = dict(q=np.zeros((nb, 4)), t=np.zeros((nb, 3)), s=np.zeros(nb), levels=np.zeros(max(N, 0), np.uint8),
+                   ninliers=np.zeros(nb, np.int32), stats=(_IterStat * max(nb * S, 1))(), nstats=np.zeros((nb, 2), np.int32))
+        batch = _Sim3Batch(B, N, _p(ptr), _p(q), _p(t), _p(s), _p(cam1), _p(cam2), _p(fix), _p(X1), _p(X2), _p(obs1), _p(obs2),
+                           _p(omega1), _p(omega2))
+        prm = _Sim3Params(float(params.chi2), int(params.iterations), int(params.iterations_bad), int(params.iterations_good),
+                          int(params.min_pairs))
+        _check(self.L.cuba_engine_optimize_sim3(self.h, C.byref(batch), C.byref(prm), _p(out["q"]), _p(out["t"]), _p(out["s"]),
+                                                _p(out["levels"]), _p(out["ninliers"]), out["stats"], _p(out["nstats"])))
+        st = np.frombuffer(out["stats"], dtype=np.dtype([("iteration", "<i4"), ("trials", "<i4"), ("chi2", "<f8"), ("lambda_", "<f8"),
+                                                          ("pcg_iters", "<i4"), ("pcg_failed", "<i4")]))
+        out["stats"] = st[:nb * S].reshape(nb, S).copy()
+        return out
+
+    def optimize_sim3(self, problems, params=None):
+        """Refines S12 of every problem (graphio.Sim3Problem) under OptimizeSim3's schedule (Sim3Params) in one launch.  Returns, per
+        problem, a dict of q [4], t [3], s, levels (0/1 per pair), ninliers and stats (the iteration statistics of the first and of
+        the second optimize, as optimize() returns them)."""
+        params = Sim3Params() if params is None else params
+        n = np.array([len(p.omega1) for p in problems], np.int64)
+        ptr = np.concatenate([[0], np.cumsum(n)])
+        cat = lambda name, w: np.concatenate([np.asarray(getattr(p, name), np.float64).reshape(-1, w) for p in problems]) if problems else np.zeros((0, w))
+        r = self.optimize_sim3_flat(ptr, cat("q", 4), cat("t", 3), cat("s", 1).ravel(), cat("cam1", 4), cat("cam2", 4),
+                                    np.array([int(bool(p.fix_scale)) for p in problems], np.int32), cat("X1", 3), cat("X2", 3),
+                                    cat("obs1", 2), cat("obs2", 2), cat("omega1", 1).ravel(), cat("omega2", 1).ravel(), params)
+        off = (0, int(params.iterations))
+        res = []
+        for b in range(len(problems)):
+            stats = []
+            for k in range(2):
+                rows = r["stats"][b, off[k]:off[k] + r["nstats"][b, k]]
+                stats.append([dict(iteration=int(x["iteration"]), trials=int(x["trials"]), chi2=float(x["chi2"]), lambda_=float(x["lambda_"]),
+                                   pcg_iters=int(x["pcg_iters"]), pcg_failed=int(x["pcg_failed"])) for x in rows])
+            res.append(dict(q=r["q"][b], t=r["t"][b], s=float(r["s"][b]), levels=r["levels"][ptr[b]:ptr[b + 1]].copy(),
+                            ninliers=int(r["ninliers"][b]), stats=stats))
         return res
 
     def launch_count(self):

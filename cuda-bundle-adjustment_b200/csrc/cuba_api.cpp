@@ -38,6 +38,7 @@
 #include "../../include/cuda_bundle_adjustment.h"
 #include "../../include/cuba_b200_levels.h"
 #include "../../include/cuba_b200_pose.h"
+#include "../../include/cuba_b200_sim3.h"
 
 namespace cuba
 {
@@ -732,6 +733,68 @@ std::vector<PoseResult> optimizePoses(CudaBundleAdjustment& ba, const std::vecto
 			}
 			res.rounds.push_back(st);
 			off += static_cast<size_t>(rounds[r].iterations);
+		}
+	}
+	return out;
+}
+
+// include/cuba_b200_sim3.h
+std::vector<Sim3Result> optimizeSim3(CudaBundleAdjustment& ba, const std::vector<Sim3Problem>& problems, const Sim3Options& options)
+{
+	Impl& impl = impl_of(ba);
+	if (problems.size() > static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizeSim3: too many problems");
+	const size_t B = problems.size();
+	std::vector<double> q(4 * B), t(3 * B), s(B), cam1(4 * B), cam2(4 * B), X1, X2, o1, o2, om1, om2;
+	std::vector<int32_t> ptr(B + 1, 0), fix(B);
+	for (size_t b = 0; b < B; b++) {
+		const Sim3Problem& p = problems[b];
+		for (int k = 0; k < 4; k++) q[4 * b + k] = p.q.coeffs().data()[k];
+		for (int k = 0; k < 3; k++) t[3 * b + k] = p.t.data()[k];
+		s[b] = p.s;
+		const CameraParams* c[2] = { &p.camera1, &p.camera2 };
+		double* cd[2] = { cam1.data() + 4 * b, cam2.data() + 4 * b };
+		for (int k = 0; k < 2; k++) { cd[k][0] = c[k]->fx; cd[k][1] = c[k]->fy; cd[k][2] = c[k]->cx; cd[k][3] = c[k]->cy; }
+		fix[b] = p.fixScale ? 1 : 0;
+		for (const Sim3Match& m : p.matches) {
+			for (int k = 0; k < 3; k++) { X1.push_back(m.X1.data()[k]); X2.push_back(m.X2.data()[k]); }
+			for (int k = 0; k < 2; k++) { o1.push_back(m.obs1.data()[k]); o2.push_back(m.obs2.data()[k]); }
+			om1.push_back(m.information1); om2.push_back(m.information2);
+		}
+		if (om1.size() > static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizeSim3: too many matches");
+		ptr[b + 1] = static_cast<int32_t>(om1.size());
+	}
+	const size_t N = om1.size();
+	cuba_sim3_batch bt;
+	bt.B = static_cast<int32_t>(B); bt.N = static_cast<int32_t>(N); bt.ptr = ptr.data();
+	bt.q = q.data(); bt.t = t.data(); bt.s = s.data(); bt.cam1 = cam1.data(); bt.cam2 = cam2.data(); bt.fix_scale = fix.data();
+	bt.X1 = X1.data(); bt.X2 = X2.data(); bt.obs1 = o1.data(); bt.obs2 = o2.data(); bt.omega1 = om1.data(); bt.omega2 = om2.data();
+	cuba_sim3_params prm;
+	prm.chi2 = options.chi2; prm.iterations = options.iterations; prm.iterations_bad = options.iterationsBad;
+	prm.iterations_good = options.iterationsGood; prm.min_pairs = options.minPairs;
+	const size_t perProblem = static_cast<size_t>(std::max(options.iterations, 0)) +
+		static_cast<size_t>(std::max(std::max(options.iterationsBad, options.iterationsGood), 0));
+	std::vector<double> qo(4 * B), to(3 * B), so(B);
+	std::vector<uint8_t> lev(N);
+	std::vector<int32_t> inl(B), nstats(2 * B);
+	std::vector<cuba_iter_stat> stats(std::max<size_t>(B * perProblem, 1));
+	// the options and the batch are checked by the engine before anything runs: a refusal is the caller's input
+	const int rc = cuba_engine_optimize_sim3(impl.poseEngine(), &bt, &prm, qo.data(), to.data(), so.data(), lev.data(), inl.data(),
+		stats.data(), nstats.data());
+	if (rc == CUBA_ERR_INVALID) throw std::invalid_argument(std::string("cuba::optimizeSim3: ") + cuba_last_error());
+	if (rc != CUBA_OK) throw std::runtime_error(std::string("cuba_b200: ") + cuba_last_error());
+	std::vector<Sim3Result> out(B);
+	for (size_t b = 0; b < B; b++) {
+		Sim3Result& r = out[b];
+		for (int k = 0; k < 4; k++) r.q.coeffs().data()[k] = qo[4 * b + k];
+		for (int k = 0; k < 3; k++) r.t.data()[k] = to[3 * b + k];
+		r.s = so[b];
+		r.inliers = static_cast<size_t>(inl[b]);
+		for (size_t i = static_cast<size_t>(ptr[b]); i < static_cast<size_t>(ptr[b + 1]); i++) r.levels.push_back(lev[i]);
+		for (int k = 0; k < 2; k++) {
+			BatchStatistics st;
+			const size_t off = b * perProblem + (k ? static_cast<size_t>(options.iterations) : 0);
+			for (int i = 0; i < nstats[2 * b + k]; i++) st.push_back(BatchInfo{ stats[off + i].iteration, stats[off + i].chi2 });
+			r.rounds.push_back(st);
 		}
 	}
 	return out;

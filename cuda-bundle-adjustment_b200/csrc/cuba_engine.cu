@@ -27,6 +27,7 @@
 #include "cuba_jh4.cuh"
 #include "cuba_levels.cuh"
 #include "cuba_pose_batch.cuh"
+#include "cuba_sim3_batch.cuh"
 #include "cuba_schur3.cuh"
 #include "cuba_schur5.cuh"
 #include "cuba_structure.h"
@@ -224,6 +225,8 @@ struct EngineBase {
 	virtual int classify_edges(double chi2Mono, double chi2Stereo, int flags, int32_t* counts) = 0;
 	virtual int optimize_poses(const cuba_pose_batch* bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
 		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) = 0;
+	virtual int optimize_sim3(const cuba_sim3_batch* bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
+		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats) = 0;
 };
 
 template <typename T>
@@ -316,6 +319,9 @@ struct Engine : EngineBase {
 	// batched pose optimisation (cuba_pose_batch.cuh): the packed batch and the packed results, device and page-locked host copies
 	DBuf<double> pbIn, pbOut;
 	PinnedBuf pbHostIn, pbHostOut;
+	// batched Sim(3) alignment (cuba_sim3_batch.cuh): the same, for its own packed batch
+	DBuf<double> s3In, s3Out;
+	PinnedBuf s3HostIn, s3HostOut;
 	DBuf<Scalars> dScal;
 	Scalars* hScal = nullptr;   // pinned
 	DBuf<double> flushBuf;
@@ -2354,6 +2360,67 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// ---- batched Sim(3) alignment (cuba_sim3_batch.cuh): one H2D of the packed batch, one launch, one D2H of the packed results.
+	// Always fp64, on this engine's stream; touches nothing of the engine's problem.  The batch was validated by the caller.
+	int optimize_sim3(const cuba_sim3_batch* bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
+		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats) override
+	{
+		static_assert(sizeof(pb::IterStat) == sizeof(cuba_iter_stat) && sizeof(pb::IterStat) == 32, "cuba_iter_stat layout");
+		const size_t B = (size_t)bt->B, N = (size_t)bt->N;
+		if (B == 0) return CUBA_OK;
+		const size_t nStat = stats ? B * (size_t)p.statPer : 0;
+		// input, in doubles: problems [B][PROB] | pairs [N][PAIR] | ptr as int32 [B+1]
+		const size_t oPair = s3::PROB * B, oPtr = oPair + s3::PAIR * N, nIn = oPtr + (B + 2) / 2;
+		// results, in doubles: S [B][8] | stats [nStat] (4 doubles each) | ninliers [B], nstats [B][2] as int32 | levels [N] bytes
+		const size_t oStat = 8 * B, oInt = oStat + 4 * nStat, oLev = oInt + (3 * B + 1) / 2, nOut = oLev + (N + 7) / 8;
+		CUDA_TRY(s3HostIn.grow(sizeof(double) * nIn)); CUDA_TRY(s3HostOut.grow(sizeof(double) * nOut));
+		CUDA_TRY(s3In.alloc(nIn)); CUDA_TRY(s3Out.alloc(nOut));
+		double* h = (double*)s3HostIn.p;
+		for (size_t b = 0; b < B; b++) {
+			double* d = h + s3::PROB * b;
+			for (int k = 0; k < 4; k++) d[k] = bt->q[4 * b + k];
+			for (int k = 0; k < 3; k++) d[4 + k] = bt->t[3 * b + k];
+			d[7] = bt->s[b];
+			for (int k = 0; k < 4; k++) { d[8 + k] = bt->cam1[4 * b + k]; d[12 + k] = bt->cam2[4 * b + k]; }
+			d[16] = bt->fix_scale && bt->fix_scale[b] ? 1.0 : 0.0;
+			d[17] = d[18] = d[19] = 0;
+		}
+		for (size_t i = 0; i < N; i++) {
+			double* d = h + oPair + s3::PAIR * i;
+			for (int k = 0; k < 3; k++) { d[k] = bt->X1[3 * i + k]; d[3 + k] = bt->X2[3 * i + k]; }
+			d[6] = bt->obs1[2 * i]; d[7] = bt->obs1[2 * i + 1]; d[8] = bt->obs2[2 * i]; d[9] = bt->obs2[2 * i + 1];
+			d[10] = bt->omega1[i]; d[11] = bt->omega2[i];
+		}
+		memcpy(h + oPtr, bt->ptr, sizeof(int32_t) * (B + 1));
+		CUDA_TRY(cudaMemcpyAsync(s3In.p, h, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
+		g_h2dBytes += (long long)(sizeof(double) * nIn);
+		s3::Args a;
+		a.B = (int)B;
+		a.prob = s3In.p; a.pair = s3In.p + oPair; a.ptr = (const int*)(s3In.p + oPtr);
+		a.Sout = s3Out.p;
+		a.stats = stats ? (pb::IterStat*)(s3Out.p + oStat) : nullptr;
+		a.ninliers = (int*)(s3Out.p + oInt); a.nstats = a.ninliers + B;
+		a.level = (unsigned char*)(s3Out.p + oLev);
+		s3::k_sim3_batch<<<(unsigned)B, s3::BLOCK, 0, stream>>>(a, p);
+		launches++;
+		CUDA_TRY(cudaGetLastError());
+		CUDA_TRY(cudaMemcpyAsync(s3HostOut.p, s3Out.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
+		g_d2hBytes += (long long)(sizeof(double) * nOut);
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		const double* o = (const double*)s3HostOut.p;
+		for (size_t b = 0; b < B; b++) {
+			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
+			for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
+			sOut[b] = o[8 * b + 7];
+		}
+		if (stats && nStat) memcpy(stats, o + oStat, sizeof(cuba_iter_stat) * nStat);
+		const int32_t* oi = (const int32_t*)(o + oInt);
+		if (ninliers) memcpy(ninliers, oi, sizeof(int32_t) * B);
+		if (nstats) memcpy(nstats, oi + B, sizeof(int32_t) * 2 * B);
+		if (levelsOut && N) memcpy(levelsOut, (const unsigned char*)(o + oLev), N);
+		return CUBA_OK;
+	}
+
 	int get_profile(double* sec) override
 	{
 		resolveProfile();
@@ -2710,6 +2777,53 @@ int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nr
 	int rc = pose_frames_ok(B, bt->E2, bt->ptr2, bt->X2, bt->meas2, bt->omega2, "2"); if (rc) return rc;
 	rc = pose_frames_ok(B, bt->E3, bt->ptr3, bt->X3, bt->meas3, bt->omega3, "3"); if (rc) return rc;
 	return e->impl->optimize_poses(bt, s, q_out, t_out, levels_out, counts, stats, nstats);
+}
+
+static bool all_finite(const double* p, size_t n)
+{
+	for (size_t i = 0; i < n; i++)
+		if (!std::isfinite(p[i])) return false;
+	return true;
+}
+
+int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const cuba_sim3_params* params, double* q_out, double* t_out,
+	double* s_out, uint8_t* levels_out, int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats)
+{
+	ENGINE_OR_FAIL(e);
+	if (!bt || !params) return fail(CUBA_ERR_INVALID, "optimize_sim3: null batch or params");
+	const cuba_sim3_params& P = *params;
+	if (!std::isfinite(P.chi2) || !(P.chi2 > 0)) return fail(CUBA_ERR_INVALID, "optimize_sim3: chi2 not finite and positive");
+	if (P.iterations < 0 || P.iterations_bad < 0 || P.iterations_good < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: negative iterations");
+	if (P.min_pairs < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: negative min_pairs");
+	if ((long long)P.iterations + std::max(P.iterations_bad, P.iterations_good) > INT32_MAX)
+		return fail(CUBA_ERR_INVALID, "optimize_sim3: too many iterations");
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: B < 0");
+	if (bt->N < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: N < 0");
+	const int B = bt->B;
+	if (B == 0) return CUBA_OK;
+	const size_t nb = (size_t)B, N = (size_t)bt->N;
+	if (!bt->ptr) return fail(CUBA_ERR_INVALID, "optimize_sim3: null ptr");
+	if (bt->ptr[0] != 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: ptr[0] != 0");
+	for (int b = 0; b < B; b++)
+		if (bt->ptr[b + 1] < bt->ptr[b]) return fail(CUBA_ERR_INVALID, "optimize_sim3: ptr decreases");
+	if (bt->ptr[B] != bt->N) return fail(CUBA_ERR_INVALID, "optimize_sim3: ptr[B] is not the pair count");
+	if (!bt->q || !bt->t || !bt->s || !bt->cam1 || !bt->cam2 || !q_out || !t_out || !s_out)
+		return fail(CUBA_ERR_INVALID, "optimize_sim3: null problem array");
+	if (N > 0 && (!bt->X1 || !bt->X2 || !bt->obs1 || !bt->obs2 || !bt->omega1 || !bt->omega2))
+		return fail(CUBA_ERR_INVALID, "optimize_sim3: null pair array");
+	if (!all_finite(bt->q, 4 * nb) || !all_finite(bt->t, 3 * nb) || !all_finite(bt->s, nb) || !all_finite(bt->cam1, 4 * nb) ||
+		!all_finite(bt->cam2, 4 * nb))
+		return fail(CUBA_ERR_INVALID, "optimize_sim3: non-finite S12 or intrinsics");
+	for (size_t b = 0; b < nb; b++)
+		if (!(bt->s[b] > 0)) return fail(CUBA_ERR_INVALID, "optimize_sim3: s <= 0");
+	if (!all_finite(bt->X1, 3 * N) || !all_finite(bt->X2, 3 * N) || !all_finite(bt->obs1, 2 * N) || !all_finite(bt->obs2, 2 * N) ||
+		!all_finite(bt->omega1, N) || !all_finite(bt->omega2, N))
+		return fail(CUBA_ERR_INVALID, "optimize_sim3: non-finite pair");
+	s3::Params p;
+	p.chi2 = P.chi2; p.delta = std::sqrt(P.chi2);
+	p.iterations = P.iterations; p.iterationsBad = P.iterations_bad; p.iterationsGood = P.iterations_good; p.minPairs = P.min_pairs;
+	p.statPer = P.iterations + std::max(P.iterations_bad, P.iterations_good);
+	return e->impl->optimize_sim3(bt, p, q_out, t_out, s_out, levels_out, ninliers, stats, nstats);
 }
 
 int cuba_engine_get_profile(cuba_engine* e, double* sec) { ENGINE_OR_FAIL(e); if (!sec) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_profile(sec); }

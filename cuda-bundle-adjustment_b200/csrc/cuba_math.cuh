@@ -135,48 +135,50 @@ CUBA_HD void sym3_inverse(T A00, T A01, T A02, T A11, T A12, T A22, T B[6] /* 00
 	B[5] = id * (A00 * A11 - A01 * A01);
 }
 
-// In-place inverse of a symmetric positive definite 6x6 (column-major) via Cholesky; returns false when
-// a pivot is not positive (block-Jacobi preconditioner of the PCG).
-template <typename T>
-CUBA_HD bool spd6_inverse(T A[36])
+// In-place inverse of a symmetric positive definite NxN (column-major) via Cholesky; returns false when
+// a pivot is not positive.  N = 6: the block-Jacobi preconditioner of the PCG and the pose solves; N = 7: the Sim(3) solve.
+template <int N, typename T>
+CUBA_HD bool spd_inverse(T A[N * N])
 {
-	T L[36];
+	T L[N * N];
 #pragma unroll
-	for (int i = 0; i < 36; i++) L[i] = T(0);
-	for (int j = 0; j < 6; j++) {
-		T d = A[j * 6 + j];
-		for (int k = 0; k < j; k++) d -= L[k * 6 + j] * L[k * 6 + j];
+	for (int i = 0; i < N * N; i++) L[i] = T(0);
+	for (int j = 0; j < N; j++) {
+		T d = A[j * N + j];
+		for (int k = 0; k < j; k++) d -= L[k * N + j] * L[k * N + j];
 		if (!(d > T(0))) return false;
 		d = t_sqrt(d);
-		L[j * 6 + j] = d;
+		L[j * N + j] = d;
 		const T id = 1 / d;
-		for (int i = j + 1; i < 6; i++) {
-			T s = A[j * 6 + i];
-			for (int k = 0; k < j; k++) s -= L[k * 6 + i] * L[k * 6 + j];
-			L[j * 6 + i] = s * id;
+		for (int i = j + 1; i < N; i++) {
+			T s = A[j * N + i];
+			for (int k = 0; k < j; k++) s -= L[k * N + i] * L[k * N + j];
+			L[j * N + i] = s * id;
 		}
 	}
 	// invert L (lower) into Li
-	T Li[36];
+	T Li[N * N];
 #pragma unroll
-	for (int i = 0; i < 36; i++) Li[i] = T(0);
-	for (int j = 0; j < 6; j++) {
-		Li[j * 6 + j] = 1 / L[j * 6 + j];
-		for (int i = j + 1; i < 6; i++) {
+	for (int i = 0; i < N * N; i++) Li[i] = T(0);
+	for (int j = 0; j < N; j++) {
+		Li[j * N + j] = 1 / L[j * N + j];
+		for (int i = j + 1; i < N; i++) {
 			T s = T(0);
-			for (int k = j; k < i; k++) s -= L[k * 6 + i] * Li[j * 6 + k];
-			Li[j * 6 + i] = s / L[i * 6 + i];
+			for (int k = j; k < i; k++) s -= L[k * N + i] * Li[j * N + k];
+			Li[j * N + i] = s / L[i * N + i];
 		}
 	}
 	// A^-1 = Li^T Li
-	for (int j = 0; j < 6; j++)
+	for (int j = 0; j < N; j++)
 		for (int i = 0; i <= j; i++) {
 			T s = T(0);
-			for (int k = j; k < 6; k++) s += Li[i * 6 + k] * Li[j * 6 + k];
-			A[j * 6 + i] = s; A[i * 6 + j] = s;
+			for (int k = j; k < N; k++) s += Li[i * N + k] * Li[j * N + k];
+			A[j * N + i] = s; A[i * N + j] = s;
 		}
 	return true;
 }
+template <typename T>
+CUBA_HD bool spd6_inverse(T A[36]) { return spd_inverse<6, T>(A); }
 
 // pose <- Exp([omega;upsilon]) * pose  (cu:551-592): Rodrigues with the theta<1e-5 Taylor branch,
 // R->quaternion by the trace method (cu:492-521), normalisation with w>=0 (cu:531-539).
@@ -256,6 +258,135 @@ CUBA_HD void se3_update(const T upd[6], T q[4], T t[3])
 	if (r[3] < T(0)) invn = -invn;
 #pragma unroll
 	for (int i = 0; i < 4; i++) q[i] = invn * r[i];
+}
+
+// ---- Sim(3): S = (R(q), t, s), S X = s R X + t (cuba_sim3_batch.cuh); double precision only ----
+
+// W = int_0^1 e^(sigma u) exp(u [w]x) du = A I + B [w]x + C [w]x^2, theta = |w|.  The closed forms (A = expm1(sigma) / sigma and
+// B, C below) cancel as theta and / or sigma go to 0, so inside |(sigma, theta)| <= 1 W is summed as its series: W = sum_n
+// Omega^n / (n+1)!, Omega = sigma I + [w]x, with Omega^n = p I + q [w]x + r [w]x^2 by [w]x^3 = -theta^2 [w]x.  Twenty terms leave a
+// truncation below 1/21! there.  Outside, with es = e^sigma, s1 = sin(theta) / theta and h2 = (1 - cos theta) / theta^2 =
+// (sin(theta/2) / (theta/2))^2 / 2 (neither cancels):
+//   B = (sigma es s1 - expm1(sigma) + es theta^2 h2) / (sigma^2 + theta^2)
+//   C = (A - ((es cos(theta) - 1) sigma + es sin(theta) theta) / (sigma^2 + theta^2)) / theta^2    theta >= 1/2
+//   C = (es sigma^2 h2 + expm1(sigma) - sigma es s1) / (sigma (sigma^2 + theta^2))                  theta < 1/2 (so |sigma| > 0.86)
+CUBA_HD void sim3_coefficients(double sigma, double theta, double& A, double& B, double& C)
+{
+	const double th2 = theta * theta, c = sigma * sigma + th2;
+	if (c <= 1) {
+		double p = 1, q = 0, r = 0, f = 1;
+		A = 1; B = 0; C = 0;
+		for (int n = 1; n <= 20; n++) {
+			const double pn = sigma * p, qn = sigma * q + p - th2 * r, rn = sigma * r + q;
+			p = pn; q = qn; r = rn;
+			f /= (n + 1);
+			A += f * p; B += f * q; C += f * r;
+		}
+		return;
+	}
+	const double es = exp(sigma), em1 = expm1(sigma);
+	const double h = 0.5 * theta, sh = theta > 0 ? sin(h) / h : 1.0;
+	const double s1 = theta > 0 ? sin(theta) / theta : 1.0, h2 = 0.5 * sh * sh;
+	A = sigma != 0 ? em1 / sigma : 1.0;
+	B = (sigma * es * s1 - em1 + es * th2 * h2) / c;
+	if (theta >= 0.5) C = (A - ((em1 - es * th2 * h2) * sigma + es * s1 * th2) / c) / th2;
+	else C = (es * sigma * sigma * h2 + em1 - sigma * es * s1) / (sigma * c);
+}
+
+// S <- Exp(xi) S, xi = (omega, upsilon, sigma) (g2o's VertexSim3Expmap::oplusImpl): R <- Rodrigues(omega) R, t <- e^sigma
+// Rodrigues(omega) t + W upsilon, s <- e^sigma s.  The rotation and its quaternion are se3_update's (with upsilon = 0), so with
+// sigma = 0 this is se3_update up to the rounding of W = V.  sigma = 0 leaves s bit for bit.
+CUBA_HD void sim3_update(const double upd[7], double q[4], double t[3], double& s)
+{
+	const double w[3] = { upd[0], upd[1], upd[2] }, v[3] = { upd[3], upd[4], upd[5] }, sigma = upd[6];
+	double A, B, C;
+	sim3_coefficients(sigma, sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]), A, B, C);
+	const double wv[3] = { w[1] * v[2] - w[2] * v[1], w[2] * v[0] - w[0] * v[2], w[0] * v[1] - w[1] * v[0] };
+	const double wwv[3] = { w[1] * wv[2] - w[2] * wv[1], w[2] * wv[0] - w[0] * wv[2], w[0] * wv[1] - w[1] * wv[0] };
+	const double es = exp(sigma);
+	for (int i = 0; i < 3; i++) t[i] *= es;
+	const double rot[6] = { w[0], w[1], w[2], 0.0, 0.0, 0.0 };
+	se3_update(rot, q, t);
+	for (int i = 0; i < 3; i++) t[i] += A * v[i] + B * wv[i] + C * wwv[i];
+	s *= es;
+}
+
+// Y = S X = s R(q) X + t
+CUBA_HD void sim3_map(const double q[4], const double t[3], double s, const double X[3], double Y[3])
+{
+	rotate(q, X, Y);
+	for (int i = 0; i < 3; i++) Y[i] = s * Y[i] + t[i];
+}
+
+// Z = S^-1 X = R(q)^T (X - t) / s
+CUBA_HD void sim3_inverse_map(const double q[4], const double t[3], double s, const double X[3], double Z[3])
+{
+	const double qc[4] = { -q[0], -q[1], -q[2], q[3] }, d[3] = { X[0] - t[0], X[1] - t[1], X[2] - t[2] };
+	rotate(qc, d, Z);
+	for (int i = 0; i < 3; i++) Z[i] /= s;
+}
+
+// r = pi(P) - obs, pi(P) = (fx P.x / P.z + cx, fy P.y / P.z + cy), cam = fx, fy, cx, cy (the projection of edge_residual)
+CUBA_HD void sim3_project(const double cam[4], const double P[3], const double obs[2], double r[2])
+{
+	const double invZ = 1 / P[2];
+	r[0] = cam[0] * invZ * P[0] + cam[2] - obs[0];
+	r[1] = cam[1] * invZ * P[1] + cam[3] - obs[1];
+}
+
+// d pi / dP (2x3)
+CUBA_HD void sim3_project_jacobian(const double cam[4], const double P[3], double Jp[2][3])
+{
+	const double invZ = 1 / P[2];
+	Jp[0][0] = cam[0] * invZ; Jp[0][1] = 0;               Jp[0][2] = -cam[0] * P[0] * invZ * invZ;
+	Jp[1][0] = 0;             Jp[1][1] = cam[1] * invZ; Jp[1][2] = -cam[1] * P[1] * invZ * invZ;
+}
+
+// e12 of a matched pair: r = pi1(S X2) - obs1; Y = S X2 is returned for the Jacobian
+CUBA_HD void sim3_residual12(const double q[4], const double t[3], double s, const double cam1[4], const double X2[3], const double obs1[2],
+	double Y[3], double r[2])
+{
+	sim3_map(q, t, s, X2, Y);
+	sim3_project(cam1, Y, obs1, r);
+}
+
+// e21 of a matched pair: r = pi2(S^-1 X1) - obs2; Z = S^-1 X1 is returned for the Jacobian
+CUBA_HD void sim3_residual21(const double q[4], const double t[3], double s, const double cam2[4], const double X1[3], const double obs2[2],
+	double Z[3], double r[2])
+{
+	sim3_inverse_map(q, t, s, X1, Z);
+	sim3_project(cam2, Z, obs2, r);
+}
+
+// dr/dxi of e12 for the update Exp(xi) S (2x7, columns omega, upsilon, sigma): d pi1 / dY [-[Y]x, I, Y]
+CUBA_HD void sim3_jacobian12(const double cam1[4], const double Y[3], double J[2][7])
+{
+	double Jp[2][3];
+	sim3_project_jacobian(cam1, Y, Jp);
+	for (int m = 0; m < 2; m++) {
+		const double* a = Jp[m];
+		// row m of -Jp [Y]x is Y x a
+		J[m][0] = Y[1] * a[2] - Y[2] * a[1]; J[m][1] = Y[2] * a[0] - Y[0] * a[2]; J[m][2] = Y[0] * a[1] - Y[1] * a[0];
+		J[m][3] = a[0]; J[m][4] = a[1]; J[m][5] = a[2];
+		J[m][6] = a[0] * Y[0] + a[1] * Y[1] + a[2] * Y[2];
+	}
+}
+
+// dr/dxi of e21 (2x7): d pi2 / dZ (1/s) R^T [[X1]x, -I, -X1]
+CUBA_HD void sim3_jacobian21(const double q[4], double s, const double cam2[4], const double X1[3], const double Z[3], double J[2][7])
+{
+	double Jp[2][3];
+	sim3_project_jacobian(cam2, Z, Jp);
+	for (int m = 0; m < 2; m++) {
+		// row m of M = Jp R^T / s is (R Jp[m]) / s
+		double a[3];
+		rotate(q, Jp[m], a);
+		for (int i = 0; i < 3; i++) a[i] /= s;
+		// row m of M [X1]x is a x X1
+		J[m][0] = a[1] * X1[2] - a[2] * X1[1]; J[m][1] = a[2] * X1[0] - a[0] * X1[2]; J[m][2] = a[0] * X1[1] - a[1] * X1[0];
+		J[m][3] = -a[0]; J[m][4] = -a[1]; J[m][5] = -a[2];
+		J[m][6] = -(a[0] * X1[0] + a[1] * X1[1] + a[2] * X1[2]);
+	}
 }
 
 #if defined(__CUDACC__)

@@ -194,6 +194,75 @@ def pose_frames(prob: FlatProblem, rows):
     return out
 
 
+@dataclasses.dataclass
+class Sim3Problem:
+    """One problem of Engine.optimize_sim3 (ORB-SLAM2's OptimizeSim3): S12 = (q, t, s), S12 X = s R(q) X + t, from camera 2 into
+    camera 1, and N matched pairs: X1 / X2 the point in camera-1 / camera-2 coordinates, obs1 / obs2 its keypoints, omega1 / omega2
+    their scalar informations."""
+    q: np.ndarray       # [4] x,y,z,w
+    t: np.ndarray       # [3]
+    s: float
+    cam1: np.ndarray    # [4] fx,fy,cx,cy
+    cam2: np.ndarray    # [4]
+    X1: np.ndarray      # [N,3]
+    X2: np.ndarray      # [N,3]
+    obs1: np.ndarray    # [N,2]
+    obs2: np.ndarray    # [N,2]
+    omega1: np.ndarray  # [N]
+    omega2: np.ndarray  # [N]
+    fix_scale: bool = False
+    landmarks: np.ndarray = None   # [N] landmark ids (iL) of the flat problem the pairs were cut from
+
+
+def _rotation(q):
+    x, y, z, w = (float(v) for v in q)
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
+def _quaternion(R):
+    """the unit quaternion (x, y, z, w), w >= 0, of a rotation matrix"""
+    K = np.array([[R[0, 0] - R[1, 1] - R[2, 2], R[1, 0] + R[0, 1], R[2, 0] + R[0, 2], R[2, 1] - R[1, 2]],
+                  [R[1, 0] + R[0, 1], R[1, 1] - R[0, 0] - R[2, 2], R[2, 1] + R[1, 2], R[0, 2] - R[2, 0]],
+                  [R[2, 0] + R[0, 2], R[2, 1] + R[1, 2], R[2, 2] - R[0, 0] - R[1, 1], R[1, 0] - R[0, 1]],
+                  [R[2, 1] - R[1, 2], R[0, 2] - R[2, 0], R[1, 0] - R[0, 1], R[0, 0] + R[1, 1] + R[2, 2]]]) / 3
+    w, v = np.linalg.eigh(K)
+    q = v[:, np.argmax(w)]
+    return q if q[3] >= 0 else -q
+
+
+def sim3_problems(prob: FlatProblem, pairs, scale=1.0, fix_scale=False):
+    """The Sim3 problems of the pose pairs (i, j) (indices iP of prob): one matched pair per landmark both poses observe, in landmark
+    order; obs = (u, v) of the pose's edge to the landmark, (u_left, v) for a stereo edge (the first edge in edge-id order where a
+    pose has several); X1 / X2 = the landmark's point in camera i / camera j, X2 divided by the pair's scale drift s0 (`scale`: one
+    value, or one per pair).  S12 is set to the planted value (R_i R_j^T, t_i - R_i R_j^T t_j, s0), which maps X2 onto X1 exactly."""
+    P = np.concatenate([prob.idx2[:, 0], prob.idx3[:, 0]]).astype(np.int64)
+    L = np.concatenate([prob.idx2[:, 1], prob.idx3[:, 1]]).astype(np.int64)
+    uv = np.concatenate([np.asarray(prob.meas2).reshape(-1, 2), np.asarray(prob.meas3).reshape(-1, 3)[:, :2]])
+    om = np.concatenate([prob.omega2, prob.omega3])
+    order = np.lexsort((np.arange(len(P)), L, P))
+    P, L, uv, om = P[order], L[order], uv[order], om[order]
+    first = np.ones(len(P), bool)
+    first[1:] = (P[1:] != P[:-1]) | (L[1:] != L[:-1])
+    P, L, uv, om = P[first], L[first], uv[first], om[first]
+    ptr = np.searchsorted(P, np.arange(prob.Pall + 1))
+    pairs = [(int(i), int(j)) for i, j in pairs]
+    s0 = np.broadcast_to(np.asarray(scale, dtype=np.float64), (len(pairs),))
+    out = []
+    for k, (i, j) in enumerate(pairs):
+        common, a, b = np.intersect1d(L[ptr[i]:ptr[i + 1]], L[ptr[j]:ptr[j + 1]], assume_unique=True, return_indices=True)
+        a, b = a + ptr[i], b + ptr[j]
+        Ri, Rj = _rotation(prob.q[i]), _rotation(prob.q[j])
+        X = np.asarray(prob.Xw)[common].reshape(-1, 3)
+        R12 = Ri @ Rj.T
+        out.append(Sim3Problem(
+            q=_quaternion(R12), t=prob.t[i] - R12 @ prob.t[j], s=float(s0[k]), cam1=np.array(prob.cam[i][:4], dtype=np.float64),
+            cam2=np.array(prob.cam[j][:4], dtype=np.float64), X1=X @ Ri.T + prob.t[i], X2=(X @ Rj.T + prob.t[j]) / s0[k],
+            obs1=uv[a].copy(), obs2=uv[b].copy(), omega1=om[a].copy(), omega2=om[b].copy(), fix_scale=bool(fix_scale), landmarks=common))
+    return out
+
+
 def write_back(g, prob: FlatProblem, q, t, Xw):
     """finalize(): reference src/cuda_bundle_adjustment.cpp:512-526 (fixed vertices are written back too)."""
     g["q"][prob.pose_rows] = q

@@ -243,6 +243,56 @@ typedef struct cuba_pose_round {
 int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* batch, int nrounds, const cuba_pose_round* rounds,
 	double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats);
 
+/* Sim(3) alignment of many keyframe pairs (ORB-SLAM2's Optimizer::OptimizeSim3, batched).  Problem b is keyframes 1 and 2 and the
+ * matched pairs [ptr[b], ptr[b+1]); ptr[0] = 0, ptr[B] = N.  Pair i: X1 (point of keyframe 1 in camera-1 coordinates), X2 (its match
+ * in camera-2 coordinates), obs1 / obs2 (the keypoints in keyframes 1 / 2), omega1 / omega2 (scalar informations).  The unknown is
+ * S12 = (R(q), t, s), S12 X = s R X + t.  Each pair gives two monocular edges, r12 = pi1(S12 X2) - obs1 and r21 = pi2(S12^-1 X1) -
+ * obs2, pi(Y) = (fx Y.x / Y.z + cx, fy Y.y / Y.z + cy), each under a Huber kernel with delta = sqrt(chi2).  With fix_scale[b] != 0
+ * the scale is held (s_out is s bit for bit).  Host arrays, fp64; pair arrays may be NULL when N = 0. */
+typedef struct cuba_sim3_batch {
+	int32_t B, N;
+	const int32_t* ptr;        /* [B+1]                                                                */
+	const double* q;           /* [4B] x,y,z,w                                                         */
+	const double* t;           /* [3B]                                                                 */
+	const double* s;           /* [B]  > 0                                                             */
+	const double* cam1;        /* [4B] fx,fy,cx,cy of keyframe 1                                       */
+	const double* cam2;        /* [4B] fx,fy,cx,cy of keyframe 2                                       */
+	const int32_t* fix_scale;  /* [B], or NULL: scale free everywhere                                  */
+	const double* X1;          /* [3N]                                                                 */
+	const double* X2;          /* [3N]                                                                 */
+	const double* obs1;        /* [2N]                                                                 */
+	const double* obs2;        /* [2N]                                                                 */
+	const double* omega1;      /* [N]                                                                  */
+	const double* omega2;      /* [N]                                                                  */
+} cuba_sim3_batch;
+
+/* OptimizeSim3(pKF1, pKF2, matches, S12, th2, bFixScale): optimize(iterations); the pair test (a pair fails when either edge's
+ * non-robust omega |r|^2 exceeds chi2; failed pairs go to level 1); with fewer than min_pairs pairs left, 0 inliers and S out = S in;
+ * else optimize(iterations_bad if the test removed a pair, else iterations_good) over the pairs left and the test again.  The defaults
+ * are ORB-SLAM2's: CUBA_SIM3_DEFAULT_*. */
+#define CUBA_SIM3_DEFAULT_CHI2 10.0
+#define CUBA_SIM3_DEFAULT_ITERATIONS 5
+#define CUBA_SIM3_DEFAULT_ITERATIONS_BAD 10
+#define CUBA_SIM3_DEFAULT_ITERATIONS_GOOD 5
+#define CUBA_SIM3_DEFAULT_MIN_PAIRS 10
+typedef struct cuba_sim3_params {
+	double chi2;
+	int32_t iterations, iterations_bad, iterations_good, min_pairs;
+} cuba_sim3_params;
+
+/* Runs the schedule on every problem: ONE kernel launch (one CTA per problem), one host->device and one device->host copy.  The LM
+ * rules are those of cuba_engine_optimize (lambda from the largest of the 7 diagonal entries); the update is S <- Exp(xi) S, xi =
+ * (omega, upsilon, sigma), with analytic Jacobians.  Always fp64; each problem's result is bit-reproducible and independent of the
+ * other problems of the batch.  Runs on the engine's device and stream, ignores set_comm, and neither reads nor changes the engine's
+ * problem, state, levels or solver state.
+ * Outputs: q_out [4B], t_out [3B], s_out [B]; levels_out [N] (0/1 after the last test); ninliers [B]; stats [B][iterations +
+ * max(iterations_bad, iterations_good)] (the second optimize of problem b from b * that + iterations, pcg fields 0); nstats [B][2]
+ * (iterations written by each optimize).  Every output except q_out / t_out / s_out may be NULL.  B = 0 does nothing.
+ * CUBA_ERR_INVALID, with nothing run, for B < 0, a malformed ptr, a non-finite input, s <= 0, negative iterations or min_pairs, or a
+ * chi2 that is not finite and positive. */
+int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* batch, const cuba_sim3_params* params, double* q_out, double* t_out,
+	double* s_out, uint8_t* levels_out, int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats);
+
 /* seconds per profile bucket accumulated since set_problem, [CUBA_PROF_NUM] */
 int cuba_engine_get_profile(cuba_engine* e, double* seconds);
 /* number of kernels this library launched since create (for bench.py's gpu_launches) */
