@@ -19,7 +19,7 @@ PROFILE_ITEMS = ("0: Initialize Optimizer", "1: Build Structure", "2: Compute Er
 PCG_INFO_LEN = 16
 PCG_INFO_FIELDS = ("kernel", "two_level", "aggs_per_cta", "G", "gs", "A", "maxRows", "capBlocks", "zhInSmem", "coarse_kernel",
                    "cinfo", "status", "iters", "coarse_rebuilds", "bj_retries", "bad_rebuilds")
-PCG_KERNELS = ("none", "k_pcg", "k_pcg2", "k_pcg3", "k_pcg4", "k_pcg5", "k_pcg5_big", "k_pcg5t")
+PCG_KERNELS = ("none", "k_pcg", "k_pcg2", "k_pcg3", "k_pcg4", "k_pcg5", "k_pcg5_big", "k_pcg5t")   # "k_pcg" (retired) is never reported
 COARSE_KERNELS = ("none", "k_coarse_invert", "cluster2<8>", "cluster2<16>", "k_coarse_dense", "k_coarse_chol_cluster")
 
 
@@ -270,7 +270,16 @@ def pcg5_plan_apc_host(prob, aggs_per_cta, world=1, num_sms=132, max_aggregates=
 
 
 class Engine:
-    """One optimizer instance on one GPU (reference: one CudaBundleAdjustment per thread/device)."""
+    """One optimizer instance on one GPU (reference: one CudaBundleAdjustment per thread/device).
+
+    The kernel-selecting options take only the values that name a kernel (cuba_config.reserved[] in include/cuba_b200.h);
+    any other makes the constructor raise CubaError before a device is touched:
+      pcg_variant    0 automatic (default), 7 / 8 automatic with the rows never / always distributed over the ranks,
+                     2 k_pcg2, 3 k_pcg4, 4 k_pcg3, 5 two-level k_pcg5, 6 block-Jacobi k_pcg5
+      jh_variant     0 k_linearize_landmark4 (default), 7 / 8 / 9 its three-stage / 5 / 6 CTAs-per-SM shapes,
+                     1..4 the first-generation kernel's tile shapes
+      schur_variant  0 / 3 k_schur3 (default), 5 landmark tiles on the fp64 tensor pipe (k_schur3 where that cannot run)
+    """
 
     def __init__(self, device=-1, use_fp32=False, pcg_max_iters=0, pcg_tol=0.0, pcg_variant=0, structure_on_host=False, jh_variant=0, schur_variant=0,
                  coarse_refresh=0, two_level_switch=0, max_aggregates=0):

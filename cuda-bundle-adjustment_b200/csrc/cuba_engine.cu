@@ -23,7 +23,6 @@
 #include "cuba_pcg5t.cuh"
 #include "cuba_coarse_dense.cuh"
 #include "cuba_peer_reduce.cuh"
-#include "cuba_schur2.cuh"
 #include "cuba_jh4.cuh"
 #include "cuba_levels.cuh"
 #include "cuba_pose_batch.cuh"
@@ -237,9 +236,7 @@ struct Engine : EngineBase {
 	int ntiles = 0, nPoseBlocks = 0, nChiBlocks = 0;
 	int tileSize = TILE;    // 256 or 128, from cfg.reserved[2]
 	int jhMinBlocks = 2;
-	bool jhV2 = true;       // k_linearize_landmark2 (pose window in smem + TMA bulk store of Hpl)
-	bool jhV3 = true;       // k_linearize_landmark3 (v2 + persistent CTAs with a cp.async double-buffered input stage)
-	int jh3Grid = 0, nChiLin = 0;
+	int nChiLin = 0;
 	// warp-tile J+H landmark pass (cuba_jh4.cuh)
 	bool jhV4 = true;
 	int ntW = 0, jh4Grid = 0, jh4HasBig = 0, jh4MinB = 4, jh4Nst = 2;
@@ -250,21 +247,17 @@ struct Engine : EngineBase {
 	DBuf<jh4::WTile> w_tile;
 	DBuf<jh4::Rec> w_rec;
 	DBuf<double> w_bigPartial;
-	DBuf<TileInfo> tileInfo;
-	// tile-local Schur (cuba_schur2.cuh)
-	bool useSchur2 = true;
-	bool useSchur5 = false;  // landmark tiles + DMMA (cuba_schur5.cuh), fp64 only
+	// landmark-tile Schur complement on the tensor pipe (cuba_schur5.cuh), fp64 only; k_schur3 (cuba_schur3.cuh) otherwise
+	bool useSchur5 = false;
 	int s5Ntiles = 0;
 	DBuf<int> s5TileLm;
 	DBuf<TileInfo> s5TileInfo;
 	DBuf<int4> s5SegRec;
 	DBuf<unsigned int> s5Off;
-	int s2Nseg = 0, s2Nvalid = 0;
-	DBuf<unsigned long long> s2_key, s2_keyS, s2_key3, s2_key3S;
-	DBuf<int> s2_val, s2_valS, s2_head, s2_segId, s2_segStart, s2_segTile, s2_segDest, s2_val3, s2_val3S, s2_segRank, s2_rankDest, s2_tileSegPtr, s2_destSegPtr, s2_p2i, s2_p2j;
-	DBuf<schur2::Counts> s2_counts;
-	DBuf<T> s2_partial;
-	DBuf<int> tilePose0, tilePoseN;
+	DBuf<unsigned long long> s5_key, s5_keyS, s5_key3, s5_key3S;
+	DBuf<int> s5_val, s5_valS, s5_head, s5_segId, s5_segStart, s5_segTile, s5_segDest, s5_val3, s5_val3S, s5_segRank, s5_rankDest, s5_tileSegPtr, s5_destSegPtr, s5_p2i, s5_p2j;
+	DBuf<schur5::Counts> s5_counts;
+	DBuf<T> s5_partial;
 	int cur = 0;            // current state buffer
 	bool trialValid = false;
 	// state
@@ -280,11 +273,6 @@ struct Engine : EngineBase {
 	bool mixed = false;
 	bool upperReduce = false;   // k_schur3 writes the upper blocks into uVal; one all-reduce of uVal | bsc, then k_expand_upper
 	DBuf<int> prodPtr, prodI, prodJ, prodL, blkRow, blkCol, u2f, u2fT, fRowPtr, fColInd;
-	bool useSchur3 = true;
-	// pcg
-	DBuf<T> pr, pz, pq, pp0, pp1, Minv;
-	DBuf<double> pcgPartial;
-	int pcgGrid = 0;
 	// pcg v2 (cuba_pcg2.cuh)
 	DBuf<T> fHat, Linv, vR0, vR1, vS0, vS1, vW0, vW1, vP, vY;
 	DBuf<int> fLocal, ctaRow, needPtr, needCol;
@@ -456,21 +444,19 @@ struct Engine : EngineBase {
 		reusable = false;
 		hostStructureValid = false;
 		shardBoundValid = false;
-		// landmark-tile variant: 0/1 = 256 edges, 2 CTAs/SM; 2 = 256, 3 CTAs/SM; 3 = 128, 4 CTAs/SM; 4 = 128, 6 CTAs/SM
+		// landmark-tile shape of the first-generation kernel: 1 = 256 edges, 2 CTAs/SM; 2 = 256, 3 CTAs/SM; 3 = 128, 4 CTAs/SM;
+		// 4 = 128, 6 CTAs/SM; otherwise LM_TILE edges, 4 CTAs/SM
 		switch (cfg.reserved[2]) {
 		case 2: tileSize = 256; jhMinBlocks = 3; break;
 		case 3: tileSize = 128; jhMinBlocks = 4; break;
 		case 4: tileSize = 128; jhMinBlocks = 6; break;
 		case 1: tileSize = 256; jhMinBlocks = 2; break;
-		default: tileSize = JH2_TL; jhMinBlocks = 4; break;
+		default: tileSize = LM_TILE; jhMinBlocks = 4; break;
 		}
 		// k_linearize_landmark4: 0 = two-stage pipeline, 4 CTAs of 4 warps per SM (default); 8/9 = 5/6 CTAs per SM; 7 = three stages
 		jhV4 = (cfg.reserved[2] == 0 || (cfg.reserved[2] >= 7 && cfg.reserved[2] <= 9)) && sizeof(T) == 8;
 		jh4Nst = cfg.reserved[2] == 7 ? 3 : 2;
 		jh4MinB = cfg.reserved[2] == 8 ? 5 : (cfg.reserved[2] == 9 ? 6 : 4);
-		jhV3 = cfg.reserved[2] == 6 && sizeof(T) == 8;
-		jhV2 = cfg.reserved[2] == 5 && sizeof(T) == 8;
-		if (cfg.reserved[2] == 5) { tileSize = JH2_TL; jhMinBlocks = 4; }
 		// (the bulk copy needs 16-byte multiples: 144-byte fp64 blocks qualify, 72-byte fp32 blocks do not)
 		if (cfg.reserved[2] == 0 && sizeof(T) != 8) { tileSize = 128; jhMinBlocks = 6; }
 		int rc = (cfg.reserved[1] == 1) ? build_on_host(p) : build_on_gpu(p);
@@ -671,7 +657,7 @@ struct Engine : EngineBase {
 		KLAUNCH(k_tile_ptr, numL + 2, lmPtr.p, numL, eL, tilePtr.p);
 		const int tb = std::min(S.lmBeg, numL), te = std::min(S.lmEnd, numL) + (S.lmEnd > numL ? 1 : 0);
 		// windows a little shorter than the CTA so that the tail of a tile's last landmark usually still fits one chunk
-		const int window = tileSize == 128 ? JH3_WINDOW : tileSize - 16;
+		const int window = tileSize - 16;
 		const int nt = (eL + window - 1) / window;
 		CUDA_TRY(tileLm.alloc((size_t)nt + 1));
 		KLAUNCH(k_tiles, nt + 1, tilePtr.p, tb, te, window, nt, tileLm.p);
@@ -787,7 +773,14 @@ struct Engine : EngineBase {
 		else CUDA_TRY(Hpl.alloc(18 * (size_t)S.nhplLocal));
 		CUDA_TRY(invHll.alloc(9 * nL));
 		CUDA_TRY(fVal.alloc(36 * (size_t)S.nfull + 6 * nP)); bsc.alias(fVal.p + 36 * (size_t)S.nfull, 6 * nP);
-		upperReduce = world > 1 && (cfg.reserved[3] == 0 || cfg.reserved[3] == 3 || cfg.use_fp32 == 2) && S.numP > 0 && S.numL > 0;
+		// Schur kernel: 0 / 3 = k_schur3 (destination-sorted products, six lanes per product; default), 5 = landmark tiles on the fp64
+		// tensor pipe (k_schur_tiles_mma + k_schur_reduce, cuba_schur5.cuh: 12 % faster on the banded 5 M-edge graph, on par on
+		// kitti00_shaped, 2x slower on the real ba_kitti_00 whose loop closures leave 4.4 products per (tile, destination) segment ->
+		// opt-in).  A request for 5 that schur5 cannot serve (host-built structure, fp32 or mixed precision, no products on this rank)
+		// runs k_schur3.  upperReduce depends on the request only, so that every rank of a sharded run joins the same collective.
+		const bool schur5Asked = cfg.reserved[3] == 5 && cfg.reserved[1] != 1 && cfg.use_fp32 != 2 && sizeof(T) == 8;
+		useSchur5 = schur5Asked && S.numP > 0 && S.numL > 0 && ntiles > 0 && S.eLocal > 0 && S.nmulLocal > 0;
+		upperReduce = world > 1 && !schur5Asked && S.numP > 0 && S.numL > 0;
 		if (upperReduce) {
 			uCount = 36 * (size_t)S.nblk + 6 * nP;
 			const size_t need = ((uCount + 1) & ~(size_t)1) + 64;          // + the signal block of the peer all-reduce
@@ -812,8 +805,6 @@ struct Engine : EngineBase {
 			}
 		}
 		CUDA_TRY(xp.alloc(6 * nP)); CUDA_TRY(xl.alloc(3 * nL));
-		CUDA_TRY(pr.alloc(6 * nP)); CUDA_TRY(pz.alloc(6 * nP)); CUDA_TRY(pq.alloc(6 * nP)); CUDA_TRY(pp0.alloc(6 * nP)); CUDA_TRY(pp1.alloc(6 * nP));
-		CUDA_TRY(Minv.alloc(36 * nP));
 		// landmarks outside this rank's shard keep zero Hll/bl/xl (they are never touched locally)
 		if (nL) CUDA_TRY(cudaMemsetAsync(Hll.p, 0, sizeof(T) * 9 * nL, stream));
 		if (nL) CUDA_TRY(cudaMemsetAsync(bl.p, 0, sizeof(T) * 3 * nL, stream));
@@ -821,52 +812,12 @@ struct Engine : EngineBase {
 		if (nP) CUDA_TRY(cudaMemsetAsync(xp.p, 0, sizeof(T) * 6 * nP, stream));
 		if (nP) CUDA_TRY(cudaMemsetAsync(Hpp.p, 0, sizeof(T) * 36 * nP, stream));
 		if (nP) CUDA_TRY(cudaMemsetAsync(bp.p, 0, sizeof(T) * 6 * nP, stream));
-		CUDA_TRY(tilePose0.alloc((size_t)std::max(ntiles, 1))); CUDA_TRY(tilePoseN.alloc((size_t)std::max(ntiles, 1)));
-		if (ntiles > 0) {
-			k_tile_info<<<ntiles, 128, 0, stream>>>(tilePtr.p, tileLm.p, e_ip.p, ntiles, tilePose0.p, tilePoseN.p);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
-			CUDA_TRY(tileInfo.alloc((size_t)ntiles));
-			k_tile_info3<<<ntiles, 128, 0, stream>>>(tilePtr.p, tileLm.p, e_ip.p, e_hpl.p, S.eLocal, S.nhplLocal, ntiles, tileInfo.p);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
-		}
-		CUDA_TRY(cudaFuncSetAttribute(k_linearize_landmark3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Jh3Smem)));
-		jh3Grid = std::max(1, std::min(ntiles, numSMs * 4));
-		// the tile-local Schur pair is correct but was measured slower than k_schur on kitti00_shaped -> opt-in
-		useSchur2 = cfg.reserved[3] == 2 && S.numP > 0 && S.numL > 0 && ntiles > 0;
-		// 0 / 3 = k_schur3 (destination-sorted products, six lanes per product; default), 5 = landmark tiles on the fp64 tensor pipe
-		// (k_schur_tiles_mma + k_schur_reduce, cuba_schur5.cuh: 12 % faster on the banded 5 M-edge graph, on par on kitti00_shaped,
-		// 2x slower on the real ba_kitti_00 whose loop closures leave 4.4 products per (tile, destination) segment -> opt-in),
-		// 4 = k_schur4 (k_schur3 + cooperative cp.async block loads: slower, kept for the record), 1 = k_schur (lane per product),
-		// 2 = tile-local pair without tensor cores
-		useSchur5 = cfg.reserved[3] == 5 && cfg.reserved[1] != 1 && sizeof(T) == 8 && S.numP > 0 && S.numL > 0 && ntiles > 0 && S.eLocal > 0;
-		useSchur3 = cfg.reserved[3] == 0 || cfg.reserved[3] == 3 || cfg.reserved[3] == 4 || cfg.use_fp32 == 2;
-		if (cfg.use_fp32 == 2) { useSchur2 = false; useSchur5 = false; }
-		if (useSchur3 && S.nmulLocal > 0) {
+		if (!useSchur5 && S.nmulLocal > 0) {
 			CUDA_TRY(prodL.alloc((size_t)S.nmulLocal));
 			KLAUNCH(schur3::k_prod_landmark, S.nmulLocal, prodI.p, hplLm.p, (int)S.nmulLocal, prodL.p);
 		}
-		if (useSchur5) {
-			// the Schur stage cuts its own, larger landmark tiles (windows of 448 edges)
-			const int tb5 = std::min(S.lmBeg, S.numL), te5 = std::min(S.lmEnd, S.numL) + (S.lmEnd > S.numL ? 1 : 0);
-			s5Ntiles = (S.eLocal + schur5::WINDOW - 1) / schur5::WINDOW;
-			CUDA_TRY(s5TileLm.alloc((size_t)s5Ntiles + 1)); CUDA_TRY(s5TileInfo.alloc((size_t)s5Ntiles));
-			KLAUNCH(sgpu::k_tiles, s5Ntiles + 1, tilePtr.p, tb5, te5, schur5::WINDOW, s5Ntiles, s5TileLm.p);
-			k_tile_info3<<<s5Ntiles, 128, 0, stream>>>(tilePtr.p, s5TileLm.p, e_ip.p, e_hpl.p, S.eLocal, S.nhplLocal, s5Ntiles, s5TileInfo.p);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
-			int rc = setup_schur2(s5TileInfo.p, s5Ntiles); if (rc) return rc;
-			if (useSchur5) {
-				CUDA_TRY(s5SegRec.alloc((size_t)std::max(s2Nseg, 1)));
-				KLAUNCH(schur5::k_seg_records, s2Nseg, s2_segStart.p, s2_segDest.p, s2_segRank.p, s2_segTile.p, blkRow.p, blkCol.p, s5TileInfo.p, s2_p2i.p, s2_p2j.p, s2Nseg, s5SegRec.p);
-				CUDA_TRY(s5Off.alloc((size_t)std::max(s2Nvalid, 1)));
-				KLAUNCH(schur5::k_prod_offsets, s2Nvalid, s2_segStart.p, s2_segTile.p, s5TileInfo.p, s2_p2i.p, s2_p2j.p, s2Nseg, s2Nvalid, s5Off.p);
-				CUDA_TRY(cudaFuncSetAttribute(schur5::k_schur_tiles_mma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(schur5::Smem)));
-			}
-		}
-		else if (useSchur2) { int rc = setup_schur2(tileInfo.p, ntiles); if (rc) return rc; }
-		tmark("alloc + tile info queued");
+		if (useSchur5) { int rc = setup_schur5(); if (rc) return rc; }
+		tmark("alloc + Schur setup queued");
 		if (jhV4) { int rc = setup_jh4(); if (rc) return rc; }
 		tmark("jh4 queued");
 		if (S.numP > 0) { int rc = setup_pcg2(); if (rc) return rc; }        // host-heavy: overlaps the warp-tile kernels queued above
@@ -874,23 +825,13 @@ struct Engine : EngineBase {
 		tmark("pcg partition (host)");
 		if (jhV4) { int rc = setup_jh4_finish(); if (rc) return rc; }
 		tmark("jh4 finish");
-		nChiLin = jhV4 ? jh4Grid : (jhV3 ? jh3Grid : ntiles);
+		nChiLin = jhV4 ? jh4Grid : ntiles;
 		nPoseBlocks = (S.numP + RED_BLOCK - 1) / RED_BLOCK;
 		nChiBlocks = std::max(1, std::min((eL + RED_BLOCK - 1) / RED_BLOCK, numSMs * 8));
 		CUDA_TRY(chiPartial.alloc((size_t)std::max(std::max(ntiles, nChiBlocks), jh4Grid) + 1));
 		CUDA_TRY(scalePartialL.alloc((size_t)std::max(ntiles, (S.numL + RED_BLOCK - 1) / RED_BLOCK) + 1));
 		CUDA_TRY(scalePartialP.alloc((size_t)nPoseBlocks + 1));
 		CUDA_TRY(chiSq.alloc((size_t)S.E));
-		// cooperative grid of the first-generation PCG kernel
-		{
-			int perSM = 0;
-			CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_pcg<T>, PCG_BLOCK, 0));
-			if (perSM < 1) return fail(CUBA_ERR_CUDA, "k_pcg cannot be resident");
-			const int wantWarps = std::max(1, S.numP);
-			const int wantBlocks = (wantWarps + PCG_BLOCK / 32 - 1) / (PCG_BLOCK / 32);
-			pcgGrid = std::max(1, std::min(wantBlocks, numSMs * std::min(perSM, 2)));
-			CUDA_TRY(pcgPartial.alloc(2 * (size_t)pcgGrid));
-		}
 		return CUBA_OK;
 	}
 
@@ -1001,18 +942,6 @@ struct Engine : EngineBase {
 #endif
 			}
 		}
-		else if (jhV3) {
-			if constexpr (sizeof(T) == 8) {
-				LinLm3Args b;
-				b.base = a; b.info = tileInfo; b.ntiles = ntiles;
-				k_linearize_landmark3<<<jh3Grid, JH3_TL, sizeof(Jh3Smem), stream>>>(b);
-			}
-		}
-		else if (jhV2) {
-			LinLm2Args<T> b;
-			b.base = a; b.tilePose0 = tilePose0; b.tilePoseN = tilePoseN; b.eLocal = S.eLocal; b.nhplLocal = S.nhplLocal;
-			k_linearize_landmark2<T><<<ntiles, JH2_TL, 0, stream>>>(b);
-		}
 		else if (tileSize == 128 && jhMinBlocks >= 6) k_linearize_landmark<T, 128, 6><<<ntiles, 128, 0, stream>>>(a);
 		else if (tileSize == 128) k_linearize_landmark<T, 128, 4><<<ntiles, 128, 0, stream>>>(a);
 		else if (jhMinBlocks >= 3) k_linearize_landmark<T, 256, 3><<<ntiles, 256, 0, stream>>>(a);
@@ -1122,31 +1051,24 @@ struct Engine : EngineBase {
 	int launch_schur(T lambda)
 	{
 		ProfScope ps(this, CUBA_PROF_SCHUR_COMPLEMENT);
-		if (useSchur2 || useSchur5) {
-			schur2::TileArgs<T> ta;
-			ta.Hpl = Hpl; ta.Hll = Hll; ta.bl = bl; ta.info = tileInfo; ta.hplLm = hplLm;
-			ta.tileSegPtr = s2_tileSegPtr; ta.segStart = s2_segStart; ta.segDest = s2_segDest; ta.segRank = s2_segRank; ta.p2i = s2_p2i; ta.p2j = s2_p2j;
-			ta.blkRow = blkRow; ta.blkCol = blkCol; ta.numL = S.numL; ta.lambda = lambda; ta.invHll = invHll; ta.partial = s2_partial;
-			if (useSchur5) {
-				if constexpr (sizeof(T) == 8) {
-					schur5::Args sa;
-					sa.Hpl = Hpl; sa.Hll = Hll; sa.bl = bl; sa.info = s5TileInfo; sa.hplLm = hplLm; sa.tileSegPtr = s2_tileSegPtr; sa.segRec = s5SegRec; sa.off = s5Off;
-					sa.p2i = s2_p2i; sa.p2j = s2_p2j; sa.numL = S.numL; sa.lambda = lambda; sa.invHll = invHll; sa.partial = s2_partial;
-					schur5::k_schur_tiles_mma<<<s5Ntiles, schur5::WARPS * 32, sizeof(schur5::Smem), stream>>>(sa);
+		if (useSchur5) {
+			if constexpr (sizeof(T) == 8) {
+				schur5::Args sa;
+				sa.Hpl = Hpl; sa.Hll = Hll; sa.bl = bl; sa.info = s5TileInfo; sa.hplLm = hplLm; sa.tileSegPtr = s5_tileSegPtr; sa.segRec = s5SegRec; sa.off = s5Off;
+				sa.p2i = s5_p2i; sa.p2j = s5_p2j; sa.numL = S.numL; sa.lambda = lambda; sa.invHll = invHll; sa.partial = s5_partial;
+				schur5::k_schur_tiles_mma<<<s5Ntiles, schur5::WARPS * 32, sizeof(schur5::Smem), stream>>>(sa);
+				launches++;
+				CUDA_TRY(cudaGetLastError());
+				schur5::ReduceArgs<T> ra;
+				ra.partial = s5_partial; ra.destSegPtr = s5_destSegPtr; ra.Hpp = Hpp; ra.bp = bp;
+				ra.blkRow = blkRow; ra.blkCol = blkCol; ra.u2f = u2f; ra.u2fT = u2fT; ra.nblk = S.nblk; ra.lambda = lambda;
+				ra.addDiag = rank == 0 ? 1 : 0; ra.fVal = fVal; ra.bsc = bsc;
+				schur5::k_schur_reduce<T><<<(S.nblk + 3) / 4, 128, 0, stream>>>(ra);
+				launches++;
+				CUDA_TRY(cudaGetLastError());
+				if (world > 1) {
+					int rc = allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true); if (rc) return rc;   // Hsc | bsc: one buffer
 				}
-			}
-			else schur2::k_schur_tiles<T><<<ntiles, schur2::TL, 0, stream>>>(ta);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
-			schur2::ReduceArgs<T> ra;
-			ra.partial = s2_partial; ra.destSegPtr = s2_destSegPtr; ra.Hpp = Hpp; ra.bp = bp;
-			ra.blkRow = blkRow; ra.blkCol = blkCol; ra.u2f = u2f; ra.u2fT = u2fT; ra.nblk = S.nblk; ra.lambda = lambda;
-			ra.addDiag = rank == 0 ? 1 : 0; ra.fVal = fVal; ra.bsc = bsc;
-			schur2::k_schur_reduce<T><<<(S.nblk + 3) / 4, 128, 0, stream>>>(ra);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
-			if (world > 1) {
-				int rc = allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true); if (rc) return rc;   // Hsc | bsc: one buffer
 			}
 			return CUBA_OK;
 		}
@@ -1159,7 +1081,7 @@ struct Engine : EngineBase {
 				CUDA_TRY(cudaGetLastError());
 			}
 		}
-		if (useSchur3 && S.numP > 0 && S.numL > 0) {
+		if (S.numP > 0 && S.numL > 0) {
 			schur3::Args<T> a;
 			a.Hpl = Hpl; a.invHll = invHll; a.bl = bl; a.Hpp = Hpp; a.bp = bp;
 			a.prodPtr = prodPtr; a.prodI = prodI; a.prodJ = prodJ; a.prodL = prodL;
@@ -1173,8 +1095,7 @@ struct Engine : EngineBase {
 					schur3::k_schur3<double, float><<<(S.nblk + schur3::WARPS - 1) / schur3::WARPS, schur3::WARPS * 32, 0, stream>>>(m);
 				}
 			}
-			else if (cfg.reserved[3] != 4) schur3::k_schur3<T><<<(S.nblk + schur3::WARPS - 1) / schur3::WARPS, schur3::WARPS * 32, 0, stream>>>(a);
-			else schur3::k_schur4<T><<<(S.nblk + schur3::WARPS - 1) / schur3::WARPS, schur3::WARPS * 32, 0, stream>>>(a);
+			else schur3::k_schur3<T><<<(S.nblk + schur3::WARPS - 1) / schur3::WARPS, schur3::WARPS * 32, 0, stream>>>(a);
 			launches++;
 			CUDA_TRY(cudaGetLastError());
 			if (upperReduce) {
@@ -1194,20 +1115,6 @@ struct Engine : EngineBase {
 				}
 			}
 			else if (world > 1) {
-				int rc = allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true); if (rc) return rc;   // Hsc | bsc: one buffer
-			}
-		}
-		else if (S.numP > 0 && S.numL > 0) {
-			SchurArgs<T> a;
-			a.Hpl = Hpl; a.invHll = invHll; a.bl = bl; a.Hpp = Hpp; a.bp = bp;
-			a.prodPtr = prodPtr; a.prodI = prodI; a.prodJ = prodJ; a.hplLm = hplLm;
-			a.blkRow = blkRow; a.blkCol = blkCol; a.u2f = u2f; a.u2fT = u2fT; a.nblk = S.nblk;
-			a.lambda = lambda; a.addDiag = rank == 0 ? 1 : 0; a.fVal = fVal; a.bsc = bsc;
-			const int wpb = SCHUR_BLOCK / 32;
-			k_schur<T><<<(S.nblk + wpb - 1) / wpb, SCHUR_BLOCK, 0, stream>>>(a);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
-			if (world > 1) {
 				int rc = allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true); if (rc) return rc;   // Hsc | bsc: one buffer
 			}
 		}
@@ -1262,37 +1169,48 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// (tile, destination) segments of the block products for the tile-local Schur kernels
-	int setup_schur2(const TileInfo* tinfo, int nt)
+	// landmark tiles of the Schur stage (its own, larger ones: windows of schur5::WINDOW edges), (tile, destination) segments of
+	// the block products, segment records and operand offsets of k_schur_tiles_mma
+	int setup_schur5()
 	{
-		using namespace schur2;
+		using namespace schur5;
 		const int N = (int)S.nmulLocal, nblk = S.nblk;
-		if (N <= 0) { useSchur2 = false; useSchur5 = false; return CUBA_OK; }
-		CUDA_TRY(s2_key.alloc(N)); CUDA_TRY(s2_keyS.alloc(N)); CUDA_TRY(s2_val.alloc(N)); CUDA_TRY(s2_valS.alloc(N));
-		CUDA_TRY(s2_head.alloc(N)); CUDA_TRY(s2_segId.alloc(N)); CUDA_TRY(s2_counts.alloc(1));
-		KLAUNCH(schur2::k_keys, N, prodPtr.p, nblk, prodI.p, N, tinfo, nt, s2_key.p, s2_val.p);
-		int rc = sortPairs(s2_key.p, s2_keyS.p, s2_val.p, s2_valS.p, N, 64); if (rc) return rc;
-		KLAUNCH(schur2::k_heads, N, s2_keyS.p, N, s2_head.p);
-		rc = exclusiveSum(s2_head.p, s2_segId.p, N); if (rc) return rc;
-		schur2::k_counts<<<1, 32, 0, stream>>>(s2_keyS.p, s2_head.p, s2_segId.p, N, s2_counts.p);
+		const int tb5 = std::min(S.lmBeg, S.numL), te5 = std::min(S.lmEnd, S.numL) + (S.lmEnd > S.numL ? 1 : 0);
+		const int nt = s5Ntiles = (S.eLocal + WINDOW - 1) / WINDOW;
+		CUDA_TRY(s5TileLm.alloc((size_t)nt + 1)); CUDA_TRY(s5TileInfo.alloc((size_t)nt));
+		KLAUNCH(sgpu::k_tiles, nt + 1, tilePtr.p, tb5, te5, WINDOW, nt, s5TileLm.p);
+		k_tile_info3<<<nt, 128, 0, stream>>>(tilePtr.p, s5TileLm.p, e_ip.p, e_hpl.p, S.eLocal, S.nhplLocal, nt, s5TileInfo.p);
 		launches++;
-		schur2::Counts hc;
-		CUDA_TRY(cudaMemcpyAsync(&hc, s2_counts.p, sizeof(hc), cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaGetLastError());
+		CUDA_TRY(s5_key.alloc(N)); CUDA_TRY(s5_keyS.alloc(N)); CUDA_TRY(s5_val.alloc(N)); CUDA_TRY(s5_valS.alloc(N));
+		CUDA_TRY(s5_head.alloc(N)); CUDA_TRY(s5_segId.alloc(N)); CUDA_TRY(s5_counts.alloc(1));
+		KLAUNCH(k_keys, N, prodPtr.p, nblk, prodI.p, N, s5TileInfo.p, nt, s5_key.p, s5_val.p);
+		int rc = sortPairs(s5_key.p, s5_keyS.p, s5_val.p, s5_valS.p, N, 64); if (rc) return rc;
+		KLAUNCH(k_heads, N, s5_keyS.p, N, s5_head.p);
+		rc = exclusiveSum(s5_head.p, s5_segId.p, N); if (rc) return rc;
+		k_counts<<<1, 32, 0, stream>>>(s5_keyS.p, s5_head.p, s5_segId.p, N, s5_counts.p);
+		launches++;
+		Counts hc;
+		CUDA_TRY(cudaMemcpyAsync(&hc, s5_counts.p, sizeof(hc), cudaMemcpyDeviceToHost, stream));
 		CUDA_TRY(cudaStreamSynchronize(stream));
-		const int nseg = hc.nseg;
-		s2Nseg = nseg; s2Nvalid = hc.nvalid;
-		CUDA_TRY(s2_segStart.alloc((size_t)nseg + 1)); CUDA_TRY(s2_segTile.alloc(nseg)); CUDA_TRY(s2_segDest.alloc(nseg));
-		CUDA_TRY(s2_key3.alloc(nseg)); CUDA_TRY(s2_key3S.alloc(nseg)); CUDA_TRY(s2_val3.alloc(nseg)); CUDA_TRY(s2_val3S.alloc(nseg));
-		CUDA_TRY(s2_segRank.alloc(nseg)); CUDA_TRY(s2_rankDest.alloc(nseg));
-		CUDA_TRY(s2_tileSegPtr.alloc((size_t)nt + 1)); CUDA_TRY(s2_destSegPtr.alloc((size_t)nblk + 1));
-		CUDA_TRY(s2_p2i.alloc(N)); CUDA_TRY(s2_p2j.alloc(N));
-		KLAUNCH(schur2::k_segments, N + 1, s2_keyS.p, s2_valS.p, s2_head.p, s2_segId.p, prodI.p, prodJ.p, N, nseg, hc.nvalid,
-			s2_segStart.p, s2_segTile.p, s2_segDest.p, s2_p2i.p, s2_p2j.p, s2_key3.p, s2_val3.p);
-		KLAUNCH(schur2::k_ptr_from_field, nt + 1, s2_segTile.p, nseg, nt, s2_tileSegPtr.p);
-		rc = sortPairs(s2_key3.p, s2_key3S.p, s2_val3.p, s2_val3S.p, nseg, 32 + sgpu::bits_for((unsigned long long)std::max(nblk, 1))); if (rc) return rc;
-		KLAUNCH(schur2::k_rank, nseg, s2_key3S.p, s2_val3S.p, nseg, s2_segRank.p, s2_rankDest.p);
-		KLAUNCH(schur2::k_ptr_from_field, nblk + 1, s2_rankDest.p, nseg, nblk, s2_destSegPtr.p);
-		CUDA_TRY(s2_partial.alloc((size_t)schur2::PW * std::max(nseg, 1)));
+		const int nseg = hc.nseg, nvalid = hc.nvalid;
+		CUDA_TRY(s5_segStart.alloc((size_t)nseg + 1)); CUDA_TRY(s5_segTile.alloc(nseg)); CUDA_TRY(s5_segDest.alloc(nseg));
+		CUDA_TRY(s5_key3.alloc(nseg)); CUDA_TRY(s5_key3S.alloc(nseg)); CUDA_TRY(s5_val3.alloc(nseg)); CUDA_TRY(s5_val3S.alloc(nseg));
+		CUDA_TRY(s5_segRank.alloc(nseg)); CUDA_TRY(s5_rankDest.alloc(nseg));
+		CUDA_TRY(s5_tileSegPtr.alloc((size_t)nt + 1)); CUDA_TRY(s5_destSegPtr.alloc((size_t)nblk + 1));
+		CUDA_TRY(s5_p2i.alloc(N)); CUDA_TRY(s5_p2j.alloc(N));
+		KLAUNCH(k_segments, N + 1, s5_keyS.p, s5_valS.p, s5_head.p, s5_segId.p, prodI.p, prodJ.p, N, nseg, nvalid,
+			s5_segStart.p, s5_segTile.p, s5_segDest.p, s5_p2i.p, s5_p2j.p, s5_key3.p, s5_val3.p);
+		KLAUNCH(k_ptr_from_field, nt + 1, s5_segTile.p, nseg, nt, s5_tileSegPtr.p);
+		rc = sortPairs(s5_key3.p, s5_key3S.p, s5_val3.p, s5_val3S.p, nseg, 32 + sgpu::bits_for((unsigned long long)std::max(nblk, 1))); if (rc) return rc;
+		KLAUNCH(k_rank, nseg, s5_key3S.p, s5_val3S.p, nseg, s5_segRank.p, s5_rankDest.p);
+		KLAUNCH(k_ptr_from_field, nblk + 1, s5_rankDest.p, nseg, nblk, s5_destSegPtr.p);
+		CUDA_TRY(s5_partial.alloc((size_t)PW * std::max(nseg, 1)));
+		CUDA_TRY(s5SegRec.alloc((size_t)std::max(nseg, 1)));
+		KLAUNCH(k_seg_records, nseg, s5_segStart.p, s5_segDest.p, s5_segRank.p, s5_segTile.p, blkRow.p, blkCol.p, s5TileInfo.p, s5_p2i.p, s5_p2j.p, nseg, s5SegRec.p);
+		CUDA_TRY(s5Off.alloc((size_t)std::max(nvalid, 1)));
+		KLAUNCH(k_prod_offsets, nvalid, s5_segStart.p, s5_segTile.p, s5TileInfo.p, s5_p2i.p, s5_p2j.p, nseg, nvalid, s5Off.p);
+		CUDA_TRY(cudaFuncSetAttribute(k_schur_tiles_mma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)));
 		return CUBA_OK;
 	}
 
@@ -1612,7 +1530,7 @@ struct Engine : EngineBase {
 		const int numP = S.numP;
 		if (numP < 1) return CUBA_OK;
 		const int mode = cfg.reserved[0];
-		if (mode == 1 || mode == 2 || mode == 3 || mode == 4) return CUBA_OK;          // an older kernel was asked for explicitly
+		if (mode == 2 || mode == 3 || mode == 4) return CUBA_OK;          // an older kernel was asked for explicitly
 		const bool wantDist = world > 1 && comm && mode != 7 && (mode == 8 || numP >= 2048);
 		const int W = wantDist ? world : 1;
 		int smemMax = 0;
@@ -1904,31 +1822,17 @@ struct Engine : EngineBase {
 		lastPcgTwoLevel = false;
 		// 0 (also 7, 8): automatic = block-Jacobi while a solve converges quickly, two-level afterwards -- k_pcg5 for the two-level solves
 		// (and, when the rows are distributed over the ranks, for every solve), k_pcg3 for the quick block-Jacobi ones on one GPU;
-		// 5: always two-level k_pcg5; 6: always block-Jacobi k_pcg5; 3: always k_pcg4; 4: always k_pcg3; 2: k_pcg2; 1: k_pcg
-		{
-			const int m = cfg.reserved[0];
-			const bool two = tlActive && !forceBlockJacobi;
-			if (p5Ok && (m == 5 || m == 6)) return launch_pcg5(m == 5 && !forceBlockJacobi);
-			if (p5Ok && (m == 0 || m == 7 || m == 8) && (p5Dist || two)) return launch_pcg5(two);
-			if ((m == 0 || m == 7 || m == 8) && !(pcg4Ok && two)) return launch_pcg2(pcg3Ok);
-			if ((m == 0 || m == 7 || m == 8) && pcg4Ok && two) return launch_pcg4();
-		}
-		if (pcg4Ok && cfg.reserved[0] == 3 && !forceBlockJacobi) return launch_pcg4();
-		if (cfg.reserved[0] == 0 || cfg.reserved[0] == 3 || cfg.reserved[0] == 4) return launch_pcg2(pcg3Ok);  // k_pcg3: flag-synchronised exchange (k_pcg2 beyond ~85 rows per CTA)
-		if (cfg.reserved[0] == 2) return launch_pcg2(false);   // k_pcg2: one grid barrier per iteration
-		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
-		PcgArgs<T> a;
-		a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fVal = fVal; a.b = bsc; a.numP = S.numP;
-		a.x = xp; a.r = pr; a.z = pz; a.q = pq; a.p0 = pp0; a.p1 = pp1; a.Minv = Minv; a.partial = pcgPartial;
-		a.maxIters = cfg.pcg_max_iters > 0 ? cfg.pcg_max_iters : std::max(200, 40 * S.numP);
-		const double tol = cfg.pcg_tol > 0 ? cfg.pcg_tol : (sizeof(T) == 8 ? 1e-11 : 1e-6);
-		a.tol2 = tol * tol;
-		a.status = &dScal.p->pcg;
-		void* args[] = { (void*)&a };
-		CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg<T>, dim3(pcgGrid), dim3(PCG_BLOCK), args, 0, stream));
-		launches++;
-		lastPcgKernel = CUBA_PCG_KERNEL_PCG;
-		return CUBA_OK;
+		// 5: always two-level k_pcg5; 6: always block-Jacobi k_pcg5; 3: always k_pcg4; 4: always k_pcg3; 2: k_pcg2.
+		// Whatever was asked for, a solve the chosen kernel cannot take (no k_pcg5 plan, no k_pcg4 partition) is block-Jacobi
+		// k_pcg3 -- k_pcg2 beyond k_pcg3's rows per CTA.
+		const int m = cfg.reserved[0];
+		const bool automatic = m == 0 || m == 7 || m == 8;
+		const bool two = tlActive && !forceBlockJacobi;
+		if (p5Ok && (m == 5 || m == 6)) return launch_pcg5(m == 5 && !forceBlockJacobi);
+		if (p5Ok && automatic && (p5Dist || two)) return launch_pcg5(two);
+		if (pcg4Ok && ((automatic && two) || (m == 3 && !forceBlockJacobi))) return launch_pcg4();
+		if (m == 2) return launch_pcg2(false);   // k_pcg2: one grid barrier per iteration
+		return launch_pcg2(pcg3Ok);              // k_pcg3: flag-synchronised exchange
 	}
 
 	int launch_backsub(T lambda)
@@ -2647,6 +2551,14 @@ int cuba_engine_create(const cuba_config* cfg, cuba_engine** out)
 	memset(&c, 0, sizeof(c));
 	c.device = -1; c.deterministic = 1;
 	if (cfg) c = *cfg;
+	// kernel-selecting slots: a value that names no kernel is an error, not a silent default
+	const int r0 = c.reserved[0], r2 = c.reserved[2], r3 = c.reserved[3];
+	if (r0 != 0 && (r0 < 2 || r0 > 8))
+		return fail(CUBA_ERR_INVALID, "create: reserved[0] = " + std::to_string(r0) + " names no PCG kernel (0, 2..8)");
+	if (r2 < 0 || r2 == 5 || r2 == 6 || r2 > 9)
+		return fail(CUBA_ERR_INVALID, "create: reserved[2] = " + std::to_string(r2) + " names no J+H kernel (0..4, 7..9)");
+	if (r3 != 0 && r3 != 3 && r3 != 5)
+		return fail(CUBA_ERR_INVALID, "create: reserved[3] = " + std::to_string(r3) + " names no Schur kernel (0, 3, 5)");
 	std::unique_ptr<EngineBase> impl;
 	int rc;
 	if (c.use_fp32 == 1) { auto* e = new Engine<float>(); e->cfg = c; impl.reset(e); rc = e->init(); }

@@ -1,9 +1,9 @@
 // cuba_jh4.cuh -- fourth generation of the Jacobian+Hessian landmark pass: WARP tiles.
 //
 // Replaces computeActiveErrorsKernel + constructQuadraticFormKernel (reference src/cuda_block_solver.cu:732-839)
-// for the landmark-side outputs (Hpl, Hll, bl, chi2), like k_linearize_landmark{,2,3} in cuba_kernels.cuh.
+// for the landmark-side outputs (Hpl, Hll, bl, chi2), like k_linearize_landmark in cuba_kernels.cuh.
 //
-// Where the ncu source view of k_linearize_landmark3 put the samples: mostly in the per-landmark reduction loop through
+// Where the ncu source view of the third generation (CTA tiles with a cp.async input stage, since retired) put the samples: mostly in the per-landmark reduction loop through
 // shared memory (branchy, a third of all instructions), then in the cp.async issue code and at CTA barriers.  This kernel
 // removes all three:
 //   * the unit of work is a WARP tile: whole landmarks packed greedily into <= 32 edge slots (a landmark with

@@ -1,10 +1,9 @@
 // cuba_pcg2.cuh -- persistent, shared-memory-resident block-Jacobi PCG (second generation).
 //
-// Same mathematics as k_pcg (block-Jacobi preconditioned CG on the reduced pose system) but organised
-// for latency instead of generality:
+// Block-Jacobi preconditioned CG on the reduced pose system, organised for latency:
 //   * split preconditioning: with M_i = L_i L_i^T (Cholesky of the 6x6 diagonal blocks) the kernel forms
 //     A^ = L^-1 S L^-T once per solve (diagonal blocks become I) and runs plain CG on A^ y = L^-1 b,
-//     x = L^-T y.  r^.r^ = r' M^-1 r, so the stopping rule is the same as k_pcg's.
+//     x = L^-T y.  r^.r^ = r' M^-1 r, so the stopping rule sqrt(r'z / r0'z0) <= tol is that of plain PCG.
 //   * one CTA per SM, each owning a contiguous range of block rows whose A^ blocks live in shared memory
 //     for the whole solve (227 KB/CTA, 33 MB across the chip -- ba_kitti_00's Schur matrix is 23 MB);
 //     rows that do not fit are streamed from the global copy.

@@ -10,20 +10,121 @@
 // segment's products  C += V_i V_j^T  with one `mma.sync.m8n8k4.f64` each: A fragment = V_i (6x3 padded to 8x4), B fragment
 // = V_j^T (3x6 padded to 4x8; column 6 carries u = L^T bl of the landmark on diagonal destinations, so the bsc contribution
 // Hpl_i inv bl = V_i u rides in the same instruction), both read from shared memory with ONE 8-byte load per lane.
-// The 6x6 (+6) partial of the segment goes to a buffer; schur2::k_schur_reduce adds the partials of every destination in a
+// The 6x6 (+6) partial of the segment goes to a buffer; k_schur_reduce adds the partials of every destination in a
 // fixed order (tiles ascending) and applies the Hpp / lambda / sign epilogue.  No atomics, bit-reproducible.
 // Replaces computeBschureKernel / initializeHschurKernel / computeHschureKernel (reference src/cuda_block_solver.cu:933-977).
 #pragma once
 
-#include "cuba_schur2.cuh"
+#include "cuba_kernels.cuh"
 
 namespace cuba_b200 {
+
+// landmark tiles of the Schur stage: landmarks [l0, l1), edges [e0, e1), poses [pose0, pose0 + poseN), Hpl blocks [h0, h1)
+struct TileInfo { int l0, l1, e0, e1, pose0, poseN, h0, h1; };   // h0/h1: Hpl block index at e0 / e1
+
+__global__ void k_tile_info3(const int* __restrict__ tilePtr, const int* __restrict__ tileLm, const int* __restrict__ ip,
+	const int* __restrict__ hpl, int eLocal, int nhplLocal, int ntiles, TileInfo* info)
+{
+	__shared__ int s_min, s_max;
+	if (threadIdx.x == 0) { s_min = 0x7fffffff; s_max = -1; }
+	__syncthreads();
+	const int l0 = tileLm[blockIdx.x], l1 = tileLm[blockIdx.x + 1];
+	const int e0 = tilePtr[l0], e1 = tilePtr[l1];
+	int mn = 0x7fffffff, mx = -1;
+	for (int e = e0 + threadIdx.x; e < e1; e += blockDim.x) { const int p = ip[e] & 0x7fffffff; mn = p < mn ? p : mn; mx = p > mx ? p : mx; }
+	atomicMin(&s_min, mn); atomicMax(&s_max, mx);
+	__syncthreads();
+	if (threadIdx.x == 0) {
+		auto rankAt = [&](int e) { if (e >= eLocal) return nhplLocal; const int x = hpl[e]; return x >= 0 ? x : -1 - x; };
+		TileInfo ti;
+		ti.l0 = l0; ti.l1 = l1; ti.e0 = e0; ti.e1 = e1;
+		ti.pose0 = s_max >= 0 ? s_min : 0; ti.poseN = s_max >= 0 ? s_max - s_min + 1 : 0;
+		ti.h0 = rankAt(e0); ti.h1 = rankAt(e1);
+		info[blockIdx.x] = ti;
+	}
+}
+
 namespace schur5 {
 
 constexpr int TL = 512;            // Hpl blocks staged per tile
 constexpr int BS = 21;             // doubles per staged block: V (6x3, column-major) followed by u (3)
 constexpr int WINDOW = 448;        // edges per tile window of the structure builder: leaves 64 slots for the last landmark's tail
 constexpr int WARPS = 8;
+constexpr int PW = 42;             // doubles per partial: 36 (block) + 6 (bsc part, zero off the diagonal)
+
+// ---- (tile, destination) segments of the block products, built once per structure (Engine::setup_schur5) ----
+
+// key = (tile << 32) | destination block, for every real product of the destination-sorted list
+__global__ void k_keys(const int* __restrict__ prodPtr, int nblk, const int* __restrict__ prodI, int N, const TileInfo* __restrict__ info, int ntiles,
+	unsigned long long* key, int* val)
+{
+	const int n = blockIdx.x * blockDim.x + threadIdx.x;
+	if (n >= N) return;
+	val[n] = n;
+	const int i = prodI[n];
+	if (i < 0) { key[n] = ~0ull; return; }
+	int lo = 0, hi = ntiles - 1;                 // first tile with h1 > i
+	while (lo < hi) { const int mid = (lo + hi) >> 1; if (info[mid].h1 > i) hi = mid; else lo = mid + 1; }
+	const int tile = lo;
+	lo = 0; hi = nblk - 1;                       // destination k: last k with prodPtr[k] <= n
+	while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (prodPtr[mid] <= n) lo = mid; else hi = mid - 1; }
+	key[n] = ((unsigned long long)(unsigned)tile << 32) | (unsigned)lo;
+}
+
+__global__ void k_heads(const unsigned long long* __restrict__ key, int N, int* head)
+{
+	const int n = blockIdx.x * blockDim.x + threadIdx.x;
+	if (n >= N) return;
+	head[n] = (key[n] != ~0ull && (n == 0 || key[n] != key[n - 1])) ? 1 : 0;
+}
+
+struct Counts { int nseg; int nvalid; };
+
+__global__ void k_counts(const unsigned long long* __restrict__ key, const int* __restrict__ head, const int* __restrict__ segId, int N, Counts* out)
+{
+	if (blockIdx.x != 0 || threadIdx.x != 0) return;
+	out->nseg = N > 0 ? segId[N - 1] + head[N - 1] : 0;
+	int lo = 0, hi = N;                          // first sentinel
+	while (lo < hi) { const int mid = (lo + hi) >> 1; if (key[mid] == ~0ull) hi = mid; else lo = mid + 1; }
+	out->nvalid = lo;
+}
+
+__global__ void k_segments(const unsigned long long* __restrict__ key, const int* __restrict__ valSorted, const int* __restrict__ head,
+	const int* __restrict__ segId, const int* __restrict__ prodI, const int* __restrict__ prodJ, int N, int nseg, int nvalid,
+	int* segStart, int* segTile, int* segDest, int* p2i, int* p2j, unsigned long long* key3, int* val3)
+{
+	const int n = blockIdx.x * blockDim.x + threadIdx.x;
+	if (n > N) return;
+	if (n == N) { segStart[nseg] = nvalid; return; }
+	if (key[n] == ~0ull) return;
+	if (head[n]) {
+		const int s = segId[n];
+		const int tile = (int)(key[n] >> 32), dest = (int)(key[n] & 0xffffffffu);
+		segStart[s] = n; segTile[s] = tile; segDest[s] = dest;
+		key3[s] = ((unsigned long long)(unsigned)dest << 32) | (unsigned)tile;
+		val3[s] = s;
+	}
+	const int src = valSorted[n];
+	p2i[n] = prodI[src]; p2j[n] = prodJ[src];
+}
+
+// ptr[i] = first segment (sorted by the given 32-bit field, ascending) with field >= i
+__global__ void k_ptr_from_field(const int* __restrict__ field, int n, int m, int* ptr)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i > m) return;
+	int lo = 0, hi = n;
+	while (lo < hi) { const int mid = (lo + hi) >> 1; if (field[mid] < i) lo = mid + 1; else hi = mid; }
+	ptr[i] = lo;
+}
+
+__global__ void k_rank(const unsigned long long* __restrict__ key3Sorted, const int* __restrict__ val3Sorted, int nseg, int* segRank, int* rankDest)
+{
+	const int r = blockIdx.x * blockDim.x + threadIdx.x;
+	if (r >= nseg) return;
+	segRank[val3Sorted[r]] = r;
+	rankDest[r] = (int)(key3Sorted[r] >> 32);
+}
 
 struct Smem {
 	double V[TL * BS];             // per block: V = Hpl chol(inv(Hll + lambda I)) and u = L^T bl of its landmark:
@@ -211,12 +312,47 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_schur_tiles_mma(const Args a)
 			}
 		}
 		// C[g][2q], C[g][2q+1]: the 6x6 block (column-major) and, in column 6, the bsc part
-		double* out = a.partial + (size_t)schur2::PW * rec.z;
+		double* out = a.partial + (size_t)PW * rec.z;
 		if (g < 6) {
 			if (q < 3) { out[(2 * q) * 6 + g] = c0; out[(2 * q + 1) * 6 + g] = c1; }
 			else out[36 + g] = c0;
 		}
 		rec = recN; recN = recNN; cur = nxt;
+	}
+}
+
+template <typename T>
+struct ReduceArgs {
+	const T* partial; const int* destSegPtr;
+	const T* Hpp; const T* bp;
+	const int* blkRow; const int* blkCol; const int* u2f; const int* u2fT;
+	int nblk; T lambda; int addDiag;
+	T* fVal; T* bsc;
+};
+
+// one warp per destination block: fixed-order sum of its partials (tiles ascending), then the Hpp / lambda / sign epilogue
+template <typename T>
+__global__ void __launch_bounds__(128) k_schur_reduce(const ReduceArgs<T> a)
+{
+	const int lane = threadIdx.x & 31;
+	const int k = blockIdx.x * 4 + (threadIdx.x >> 5);
+	if (k >= a.nblk) return;
+	const int ra = a.blkRow[k], cb = a.blkCol[k];
+	const bool diag = ra == cb;
+	const int r0 = a.destSegPtr[k], r1 = a.destSegPtr[k + 1];
+	for (int e = lane; e < PW; e += 32) {
+		T s = T(0);
+		for (int r = r0; r < r1; r++) s += a.partial[(size_t)PW * r + e];
+		if (e < 36) {
+			const int c = e / 6, rr = e - 6 * c;
+			T val = -s;
+			if (diag && a.addDiag) val += a.Hpp[36 * (size_t)ra + e] + (rr == c ? a.lambda : T(0));
+			a.fVal[36 * (size_t)a.u2f[k] + e] = val;
+			if (!diag) a.fVal[36 * (size_t)a.u2fT[k] + rr * 6 + c] = val;
+		} else if (diag) {
+			const int rr = e - 36;
+			a.bsc[6 * (size_t)ra + rr] = (a.addDiag ? a.bp[6 * (size_t)ra + rr] : T(0)) - s;
+		}
 	}
 }
 

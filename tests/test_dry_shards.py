@@ -205,12 +205,11 @@ def _world1_schur(pkg, prob, rk, **engine_kw):
     return out
 
 
-PATHS = {"default": {}, "schur1": dict(schur_variant=1), "schur2": dict(schur_variant=2), "schur4": dict(schur_variant=4),
-         "schur5": dict(schur_variant=5), "jh1": dict(jh_variant=1), "jh2": dict(jh_variant=2), "jh3": dict(jh_variant=3),
-         "jh4": dict(jh_variant=4), "jh5": dict(jh_variant=5), "jh6": dict(jh_variant=6), "jh7": dict(jh_variant=7),
-         "jh8": dict(jh_variant=8), "jh9": dict(jh_variant=9), "mixed": dict(use_fp32="mixed")}
-SMALL_PATHS = ("default", "schur1", "schur2", "schur4", "schur5", "jh6", "jh5", "jh4", "mixed")
-SHARD_EDGE_PATHS = ("default", "jh7", "jh8", "jh9", "jh6", "jh5", "jh4")
+PATHS = {"default": {}, "schur5": dict(schur_variant=5), "jh1": dict(jh_variant=1), "jh2": dict(jh_variant=2), "jh3": dict(jh_variant=3),
+         "jh4": dict(jh_variant=4), "jh7": dict(jh_variant=7), "jh8": dict(jh_variant=8), "jh9": dict(jh_variant=9),
+         "mixed": dict(use_fp32="mixed")}
+SMALL_PATHS = ("default", "schur5", "jh4", "mixed")
+SHARD_EDGE_PATHS = ("default", "jh7", "jh8", "jh9", "jh4")
 CASES = ([(n, w, "default", "huber") for n in ("tiny", "tiny-mixed", "tiny-pose_only", "tiny-landmark_only") for w in (2, 3, 8)]
          + [("small", w, p, "huber") for w in (2, 3) for p in SMALL_PATHS] + [("small", 2, "default", "none"), ("small", 3, "default", "tukey")]
          + [("kitti07_shaped", w, p, "huber") for w in (2, 8) for p in ("default", "schur5", "mixed")]

@@ -234,9 +234,9 @@ def _check_equivalent(a, b):
 
 
 EQUIV = [(n, k, "default") for n in ("tiny", "small", "kitti07_shaped", "kitti00_shaped", "shard_edges") for k in ("none", "huber", "tukey")] + \
-        [("small", "huber", v) for v in ("jh6", "jh5", "jh1", "host", "fp32", "mixed", "pcg5", "pcg6", "clean")] + \
+        [("small", "huber", v) for v in ("jh1", "host", "fp32", "mixed", "pcg5", "pcg6", "clean")] + \
         [("kitti00_shaped", "huber", "pcg5")]
-VARIANT = {"default": {}, "jh6": dict(jh_variant=6), "jh5": dict(jh_variant=5), "jh1": dict(jh_variant=1), "host": {},
+VARIANT = {"default": {}, "jh1": dict(jh_variant=1), "host": {},
            "fp32": dict(use_fp32=True), "mixed": dict(use_fp32="mixed"), "pcg5": dict(pcg_variant=5), "pcg6": dict(pcg_variant=6),
            "clean": {}}
 

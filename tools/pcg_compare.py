@@ -1,4 +1,4 @@
-"""PCG kernel comparison: iterations and device time of k_pcg2 vs k_pcg on one linearised system."""
+"""PCG kernel comparison: iterations and device time of k_pcg5 (default and 74-aggregate bound) vs k_pcg3 on one linearised system."""
 import os
 import sys
 

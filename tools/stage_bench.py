@@ -1,5 +1,5 @@
 """Per-stage device times (L2 flushed) for one or more workloads and Schur variants.
-usage: python tools/stage_bench.py [--schur 0,1] <workload | ba_kitti_00> ..."""
+usage: python tools/stage_bench.py [--schur 0,5] <workload | ba_kitti_00> ..."""
 import os
 import sys
 
