@@ -23,6 +23,10 @@ PCG_KERNELS = ("none", "k_pcg", "k_pcg2", "k_pcg3", "k_pcg4", "k_pcg5", "k_pcg5_
 COARSE_KERNELS = ("none", "k_coarse_invert", "cluster2<8>", "cluster2<16>", "k_coarse_dense", "k_coarse_chol_cluster")
 
 
+# cuba_debug_pcg5_plan: info[] fields; w_cols_tuned / w_cols_legacy are the columns of w each launch shape's staging holds
+PCG5_PLAN_FIELDS = ("ok", "G", "gs", "A", "needMax", "maxRows", "maxNeedAgg", "halo_rows", "blkMax", "w_cols_tuned", "w_cols_legacy")
+
+
 class CubaError(RuntimeError):
     pass
 
@@ -241,9 +245,9 @@ def pcg_partition_host(prob, n_ctas=148, max_aggregates=74):
     lists of the two-level PCG); the library verifies their invariants and raises CubaError if one fails."""
     L = load_library()
     P, keep = _problem_struct(prob)
-    info = np.zeros(8, np.int32)
+    info = np.zeros(9, np.int32)
     _check(L.cuba_debug_pcg_partition(C.byref(P), int(n_ctas), int(max_aggregates), _p(info)))
-    return dict(zip(("G", "gs", "A", "needMax", "maxRows", "blkMax", "maxNeedAgg", "coarse_list_size"), (int(v) for v in info)))
+    return dict(zip(("G", "gs", "A", "needMax", "maxRows", "blkMax", "maxNeedAgg", "coarse_list_size", "pcg3_fixed_bytes"), (int(v) for v in info)))
 
 
 def pcg5_plan_host(prob, world=1, num_sms=148, max_aggregates=74):
@@ -251,9 +255,9 @@ def pcg5_plan_host(prob, world=1, num_sms=148, max_aggregates=74):
     the library verifies its invariants and raises CubaError if one fails."""
     L = load_library()
     P, keep = _problem_struct(prob)
-    info = np.zeros(8, np.int32)
+    info = np.zeros(len(PCG5_PLAN_FIELDS), np.int32)
     _check(L.cuba_debug_pcg5_plan(C.byref(P), int(world), int(num_sms), int(max_aggregates), _p(info)))
-    return dict(zip(("ok", "G", "gs", "A", "needMax", "maxRows", "maxNeedAgg", "halo_rows"), (int(v) for v in info)))
+    return dict(zip(PCG5_PLAN_FIELDS, (int(v) for v in info)))
 
 
 def pcg5_plan_apc_host(prob, aggs_per_cta, world=1, num_sms=132, max_aggregates=148):
@@ -261,10 +265,10 @@ def pcg5_plan_apc_host(prob, aggs_per_cta, world=1, num_sms=132, max_aggregates=
     FNV-1a hash over every array of the plan"""
     L = load_library()
     P, keep = _problem_struct(prob)
-    info = np.zeros(8, np.int32)
+    info = np.zeros(len(PCG5_PLAN_FIELDS), np.int32)
     h = C.c_uint64(0)
     _check(L.cuba_debug_pcg5_plan_apc(C.byref(P), int(world), int(num_sms), int(max_aggregates), int(aggs_per_cta), _p(info), C.byref(h)))
-    out = dict(zip(("ok", "G", "gs", "A", "needMax", "maxRows", "maxNeedAgg", "halo_rows"), (int(v) for v in info)))
+    out = dict(zip(PCG5_PLAN_FIELDS, (int(v) for v in info)))
     out["hash"] = int(h.value)
     return out
 

@@ -37,6 +37,16 @@ namespace cuba_b200 {
 static thread_local std::string g_err;
 static int fail(int code, const std::string& msg) { g_err = msg; return code; }
 
+// fixed shared-memory footprint of k_pcg3 (a superset of k_pcg2's): r,s per needed column, p,y per own row, index lists
+static size_t pcg3_fixed_bytes(int needMax, int maxRows, size_t scalar)
+{
+	return (size_t)needMax * (12 * scalar + 8) + (size_t)maxRows * (12 * scalar + 4) + ((size_t)maxRows + 1) * 4 + (size_t)PCG3_CHUNK * 6 * scalar;
+}
+
+// columns of w a k_pcg5 / k_pcg5t layout's staging region `cc` holds between passes (it ends where the next region, rc, begins)
+template <typename L>
+static int32_t w_staging_columns(const L& lay) { return (int32_t)((lay.rc - lay.cc) / (6 * sizeof(double))); }
+
 #define CUDA_TRY(expr)                                                                                      \
 	do {                                                                                                    \
 		cudaError_t _e = (expr);                                                                            \
@@ -1229,10 +1239,16 @@ struct Engine : EngineBase {
 		build_pcg_partition(numP, S.nfull, S.fRowPtr, S.fColInd, G, PP);
 		const std::vector<int>& rows = PP.rows; const std::vector<int>& nptr = PP.nptr; const std::vector<int>& ncol = PP.ncol; const std::vector<int>& local = PP.local;
 		const int needMax = PP.needMax, blkMax = PP.blkMax, maxRows = PP.maxRows;
-		// fixed shared-memory footprint of k_pcg3 (a superset of k_pcg2's): r,s per needed column, p,y per own row, index lists
-		const size_t needBytes = (size_t)needMax * (12 * sizeof(T) + 8) + (size_t)maxRows * (12 * sizeof(T) + 4) + ((size_t)maxRows + 1) * 4
-			+ (size_t)PCG3_CHUNK * 6 * sizeof(T);
-		pcg3Ok = maxRows * 6 <= PCG3_BLOCK && 2 * G <= 2 * PCG3_BLOCK;   // k_pcg3: one (row,component) pair per thread, two partial words per thread
+		const size_t needBytes = pcg3_fixed_bytes(needMax, maxRows, sizeof(T));
+		// k_pcg3 / k_pcg2 keep every needed column in shared memory and are the solver of last resort: without them no solve can run
+		if (needBytes > budget) {
+			const size_t perNeed = 12 * sizeof(T) + 8, rest = needBytes - (size_t)needMax * perNeed;
+			const size_t fit = budget > rest ? (budget - rest) / perNeed : 0;
+			return fail(CUBA_ERR_INVALID, "set_problem: a CTA of the block-Jacobi PCG needs " + std::to_string(needMax) + " columns of the reduced camera system ("
+				+ std::to_string(needBytes) + " bytes of shared memory, " + std::to_string(budget) + " available: at most " + std::to_string(fit)
+				+ " columns with " + std::to_string(maxRows) + " rows per CTA); the poses are too densely covisible for this engine");
+		}
+		pcg3Ok =maxRows * 6 <= PCG3_BLOCK && 2 * G <= 2 * PCG3_BLOCK;   // k_pcg3: one (row,component) pair per thread, two partial words per thread
 		size_t cap = budget > needBytes ? (budget - needBytes) / (36 * sizeof(T) + 4) : 0;
 		cap = std::min<size_t>(cap, (size_t)blkMax);
 		pcg2Grid = G; pcg2Cap = (int)cap; pcg2NeedMax = needMax; pcg2MaxRows = maxRows;
@@ -1567,7 +1583,7 @@ struct Engine : EngineBase {
 			p5t::Pcg5Dims t{};
 			t.needMax = PP.needMax; t.maxRows = PP.maxRows; t.nc = nc; t.maxNeedAgg = CP.maxNeedAgg;
 			t.npv = d.npv; t.nls = NR; t.sliceRows = d.sliceRows;
-			t.ccCap = PP.blkMax >= TS::CHUNK ? TS::CHUNK : std::max((std::max(PP.blkMax, PP.needMax) + 31) / 32 * 32, 32);
+			t.ccCap = p5t::pcg5t_cc_cap(PP.blkMax, PP.needMax);
 			t.sqWords = p5t::pcg5t_np(apc) * (TS::BLOCK / 32);
 			t.capBlocks = 0; t.zhInSmem = 0;
 			const size_t base = p5t::Pcg5Layout<T>(t).total + 64;
@@ -2822,7 +2838,10 @@ int cuba_debug_pcg_partition(const cuba_problem* p, int nCtas, int maxAgg, int32
 	build_coarse_lists(S.numP, S.nfull, S.fRowPtr, S.fColInd, C);
 	const char* bad = check_pcg_partition(S.numP, S.nfull, S.fRowPtr, S.fColInd, P, C);
 	if (bad) return fail(CUBA_ERR_INVALID, std::string("pcg_partition self-check: ") + bad);
-	if (info) { info[0] = P.G; info[1] = C.gs; info[2] = C.A; info[3] = P.needMax; info[4] = P.maxRows; info[5] = P.blkMax; info[6] = C.maxNeedAgg; info[7] = (int32_t)C.cbList.size(); }
+	if (info) {
+		info[0] = P.G; info[1] = C.gs; info[2] = C.A; info[3] = P.needMax; info[4] = P.maxRows; info[5] = P.blkMax; info[6] = C.maxNeedAgg; info[7] = (int32_t)C.cbList.size();
+		info[8] = (int32_t)pcg3_fixed_bytes(P.needMax, P.maxRows, sizeof(double));
+	}
 	return CUBA_OK;
 }
 
@@ -2841,7 +2860,7 @@ int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int m
 	if (!build_structure(p->Pall, p->numP, p->Lall, p->numL, p->E2, p->idx2, p->E3, p->idx3, 0, 1, TILE, S, &err)) return fail(CUBA_ERR_INVALID, err);
 	Pcg5Plan plan;
 	build_pcg5_plan(S.numP, S.nfull, S.fRowPtr, S.fColInd, world, numSMs, maxAgg, 2 * PCG5_BLOCK / 6, plan, nullptr, aggsPerCta);
-	if (info) for (int i = 0; i < 8; i++) info[i] = 0;
+	if (info) for (int i = 0; i < 11; i++) info[i] = 0;
 	if (hash) *hash = 0;
 	if (!plan.ok) return CUBA_OK;
 	const char* bad = check_pcg5_plan(S.numP, S.nfull, S.fRowPtr, S.fColInd, plan);
@@ -2850,6 +2869,14 @@ int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int m
 		int halo = 0;
 		for (unsigned char m : plan.rowPeers) if (m) halo++;
 		info[0] = 1; info[1] = plan.G; info[2] = plan.gs; info[3] = plan.A; info[4] = plan.P.needMax; info[5] = plan.P.maxRows; info[6] = plan.C.maxNeedAgg; info[7] = halo;
+		info[8] = plan.P.blkMax;
+		// the two launch shapes' layouts as setup_pcg5 sizes them (the staging does not depend on the cached-block count)
+		p5t::Pcg5Dims t{};
+		t.needMax = plan.P.needMax; t.maxRows = plan.P.maxRows; t.ccCap = p5t::pcg5t_cc_cap(plan.P.blkMax, plan.P.needMax);
+		Pcg5Dims d{};
+		d.needMax = plan.P.needMax; d.maxRows = plan.P.maxRows;
+		info[9] = w_staging_columns(p5t::Pcg5Layout<double>(t));
+		info[10] = w_staging_columns(Pcg5Layout<double>(d));
 	}
 	if (hash) {
 		uint64_t h = 1469598103934665603ull;

@@ -65,7 +65,9 @@ struct Pcg5Layout {
 		u = take((size_t)d.needMax * 6 * sizeof(T), 8);
 		p = take((size_t)d.maxRows * 6 * sizeof(T), 8);
 		y = take((size_t)d.maxRows * 6 * sizeof(T), 8);
-		cc = take((size_t)PCG5_CHUNK * 6 * sizeof(double), 8);      // block-product staging; polled w entries (double) between passes
+		// block-product staging ([6][PCG5_CHUNK] T); between passes the polled w entries of the needed columns ([needMax][6] double),
+		// so a dense row block (needMax > PCG5_CHUNK) widens it
+		cc = take((size_t)(d.needMax > PCG5_CHUNK ? d.needMax : PCG5_CHUNK) * 6 * sizeof(double), 8);
 		rc = take((size_t)d.nc * sizeof(T), 8);
 		sc = take((size_t)d.nc * sizeof(T), 8);
 		c = take((size_t)d.maxNeedAgg * 6 * sizeof(T), 8);

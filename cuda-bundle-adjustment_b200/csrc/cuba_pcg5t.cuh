@@ -43,6 +43,14 @@ struct Pcg5Dims {
 	int sqWords;  // doubles of the partial-product staging: 9 * maxRows * 6
 };
 
+// Pcg5Dims::ccCap of a plan: the shape's CHUNK, or less when a CTA never owns that many blocks; never less than needMax, because the
+// same storage holds the polled w entries of the needed columns
+inline int pcg5t_cc_cap(int blkMax, int needMax)
+{
+	const int c = blkMax >= Pcg5Shape::CHUNK ? Pcg5Shape::CHUNK : std::max((std::max(blkMax, needMax) + 31) / 32 * 32, 32);
+	return std::max(c, needMax);
+}
+
 // shared-memory carve-up, one definition for the host (size) and the device (pointers)
 template <typename T>
 struct Pcg5Layout {

@@ -373,12 +373,14 @@ int cuba_debug_build_structure_host(const cuba_problem* p, int rank, int world, 
 
 /* CPU-only check of the host side of the PCG setup (row partition over nCtas persistent CTAs, need lists, pose aggregates and
  * coarse lists of the two-level PCG, csrc/cuba_structure.cpp): builds them for the problem and verifies their invariants.
- * info[8] = G, gs, A, needMax, maxRows, blkMax, maxNeedAgg, size of the coarse lists.  No device needed. */
+ * info[9] = G, gs, A, needMax, maxRows, blkMax, maxNeedAgg, size of the coarse lists, bytes of k_pcg3's fp64 shared memory that do
+ * not hold cached blocks (set_problem fails with CUBA_ERR_INVALID when they exceed the device's budget).  No device needed. */
 int cuba_debug_pcg_partition(const cuba_problem* p, int nCtas, int maxAgg, int32_t* info);
 
 /* CPU-only check of the plan of the row-distributed two-level PCG (k_pcg5; csrc/cuba_structure.cpp): rows over world x G virtual
- * CTAs, aggregates aligned with the ranks, halo masks.  info[8] = ok (0: system too small for this kernel), G, gs, A, needMax,
- * maxRows, maxNeedAgg, number of halo rows.  No device needed. */
+ * CTAs, aggregates aligned with the ranks, halo masks.  info[11] = ok (0: system too small for this kernel; then all zero), G, gs,
+ * A, needMax, maxRows, maxNeedAgg, number of halo rows, blkMax, and the columns of w the polled-w staging of the fp64 shared-memory
+ * layout holds in the tuned (k_pcg5t) and the legacy (k_pcg5) launch shape; a CTA polls needMax of them.  No device needed. */
 int cuba_debug_pcg5_plan(const cuba_problem* p, int world, int numSMs, int maxAgg, int32_t* info);
 /* The same with aggsPerCta aggregates per CTA (the one-GPU tuned kernel; 1: the plan of cuba_debug_pcg5_plan).  hash (may be null):
  * FNV-1a over every array of the plan, to compare plans across builds. */
