@@ -122,7 +122,7 @@ _SYMBOLS = [
     "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
-    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
+    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
 ]
 
 
@@ -184,6 +184,7 @@ def load_library():
         "cuba_debug_pcg_partition": [C.POINTER(_Problem), i, i, vp],
         "cuba_debug_pcg5_plan": [C.POINTER(_Problem), i, i, i, vp],
         "cuba_debug_pcg5_plan_apc": [C.POINTER(_Problem), i, i, i, i, vp, C.POINTER(C.c_uint64)],
+        "cuba_debug_pcg5t_layout": [C.POINTER(_Problem), i, i, i, C.c_int64, vp],
         "cuba_debug_dropin_problem": [vp, C.POINTER(_Problem)],
         "cuba_debug_dropin_levels": [vp, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_int32)],
         "cuba_bench_stage": [vp, i, i, i, d, C.POINTER(d)],
@@ -271,6 +272,21 @@ def pcg5_plan_apc_host(prob, aggs_per_cta, world=1, num_sms=132, max_aggregates=
     out = dict(zip(PCG5_PLAN_FIELDS, (int(v) for v in info)))
     out["hash"] = int(h.value)
     return out
+
+
+PCG5T_LAYOUT_FIELDS = ("ok", "aggs_per_cta", "capBlocks", "streamed_blocks", "zhInSmem", "total_bytes", "blk_bytes", "rsu_bytes",
+                       "staging_bytes", "rc_bytes", "zh_bytes", "slice_bytes")
+H100_SMEM_BUDGET = 227 * 1024 - 2048     # what set_problem leaves to k_pcg5t's dynamic shared memory on an H100
+
+
+def pcg5t_layout_host(prob, aggs_per_cta_top=2, num_sms=132, scalar_bytes=8, smem_budget=H100_SMEM_BUDGET):
+    """Shared-memory layout of the one-GPU tuned PCG kernel as set_problem would pick it (the largest number of aggregates per CTA
+    <= aggs_per_cta_top whose plan fits smem_budget bytes), on the CPU"""
+    L = load_library()
+    P, keep = _problem_struct(prob)
+    info = np.zeros(len(PCG5T_LAYOUT_FIELDS), np.int32)
+    _check(L.cuba_debug_pcg5t_layout(C.byref(P), int(num_sms), int(aggs_per_cta_top), int(scalar_bytes), int(smem_budget), _p(info)))
+    return dict(zip(PCG5T_LAYOUT_FIELDS, (int(v) for v in info)))
 
 
 class Engine:

@@ -47,6 +47,19 @@ static size_t pcg3_fixed_bytes(int needMax, int maxRows, size_t scalar)
 template <typename L>
 static int32_t w_staging_columns(const L& lay) { return (int32_t)((lay.rc - lay.cc) / (6 * sizeof(double))); }
 
+// Pcg5Dims of the tuned one-GPU shape (cuba_pcg5t.cuh) for a plan on one GPU; p5t::pcg5t_fit sizes the caches
+static p5t::Pcg5Dims pcg5t_plan_dims(const Pcg5Plan& plan)
+{
+	p5t::Pcg5Dims t{};
+	const int G = plan.G, nc = 6 * plan.A, NR = 3 + 6 * (G / plan.gs), np = p5t::pcg5t_np(plan.apc);
+	t.needMax = plan.P.needMax; t.maxRows = plan.P.maxRows; t.nc = nc; t.maxNeedAgg = plan.C.maxNeedAgg;
+	t.npv = std::max(std::max(G * np, NR), 6 * plan.C.maxNeedAgg); t.nls = NR;
+	t.sliceRows = (nc + G - 1) / G;
+	t.ccCap = p5t::pcg5t_cc_cap(plan.P.blkMax);
+	t.sqWords = np * (p5t::Pcg5Shape::BLOCK / 32);
+	return t;
+}
+
 #define CUDA_TRY(expr)                                                                                      \
 	do {                                                                                                    \
 		cudaError_t _e = (expr);                                                                            \
@@ -1580,20 +1593,8 @@ struct Engine : EngineBase {
 			wantCache = PP.blkMax > PCG5_REGBLK ? (size_t)(PP.blkMax - PCG5_REGBLK) : 0;
 			if (!tryTuned) break;
 			using TS = p5t::Pcg5Shape;
-			p5t::Pcg5Dims t{};
-			t.needMax = PP.needMax; t.maxRows = PP.maxRows; t.nc = nc; t.maxNeedAgg = CP.maxNeedAgg;
-			t.npv = d.npv; t.nls = NR; t.sliceRows = d.sliceRows;
-			t.ccCap = p5t::pcg5t_cc_cap(PP.blkMax, PP.needMax);
-			t.sqWords = p5t::pcg5t_np(apc) * (TS::BLOCK / 32);
-			t.capBlocks = 0; t.zhInSmem = 0;
-			const size_t base = p5t::Pcg5Layout<T>(t).total + 64;
-			const size_t zhBytes = (size_t)t.needMax * 36 * sizeof(T);
-			size_t used = base + wantCache * per, cap = wantCache;
-			if (used + zhBytes <= budget) { t.zhInSmem = 1; used += zhBytes; }
-			// apc > 1: the larger slice of Ac^-1 may take the place of cached blocks (the rest is read from the global copy)
-			if (apc > 1 && used > budget && base <= budget) { cap = std::min(wantCache, (budget - base) / per); used = base + cap * per; }
-			if (PP.maxRows * 6 <= TS::BLOCK && used <= budget) {
-				t.capBlocks = (int)cap;
+			p5t::Pcg5Dims t = pcg5t_plan_dims(plan);
+			if (PP.maxRows * 6 <= TS::BLOCK && p5t::pcg5t_fit<T>(t, PP.blkMax, apc, budget)) {
 				p5tDims = t;
 				p5tDimsBJ = t; p5tDimsBJ.nc = 0; p5tDimsBJ.maxNeedAgg = 0; p5tDimsBJ.zhInSmem = 0; p5tDimsBJ.sliceRows = 0; p5tDimsBJ.nls = 3; p5tDimsBJ.npv = std::max(G * 3, W * 3);
 				const size_t smemT = std::max(p5t::Pcg5Layout<T>(p5tDims).total, p5t::Pcg5Layout<T>(p5tDimsBJ).total);
@@ -1759,7 +1760,7 @@ struct Engine : EngineBase {
 		}
 		if (twoLevel) KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, cZx.p);
 		Pcg5PrepArgs<T> pa;
-		pa.fRowPtr = fRowPtr; pa.fColInd = fColInd; pa.fVal = fVal; pa.b = bsc; pa.Zx = cZx; pa.numP = numP; pa.A = A; pa.aggRow = p5AggRow;
+		pa.fRowPtr = fRowPtr; pa.fColInd = fColInd; pa.fVal = fVal; pa.b = bsc; pa.Zx = cZx; pa.numP = numP; pa.A = A; pa.aggRow = p5AggRow; pa.zhatFp32 = p5Tuned ? 1 : 0;
 		pa.Linv = p5Linv; pa.R0 = p5R0; pa.Zhat = p5Zhat; pa.rcRow = p5RcRow; pa.rc0 = p5Rc0; pa.ctl = p5Ctl(p5Boards.p);
 		k_pcg5_prep_rows<T><<<(numP + 127) / 128, 128, 0, stream>>>(pa);
 		launches++;
@@ -2872,7 +2873,7 @@ int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int m
 		info[8] = plan.P.blkMax;
 		// the two launch shapes' layouts as setup_pcg5 sizes them (the staging does not depend on the cached-block count)
 		p5t::Pcg5Dims t{};
-		t.needMax = plan.P.needMax; t.maxRows = plan.P.maxRows; t.ccCap = p5t::pcg5t_cc_cap(plan.P.blkMax, plan.P.needMax);
+		t.needMax = plan.P.needMax; t.maxRows = plan.P.maxRows; t.ccCap = p5t::pcg5t_cc_cap(plan.P.blkMax);
 		Pcg5Dims d{};
 		d.needMax = plan.P.needMax; d.maxRows = plan.P.maxRows;
 		info[9] = w_staging_columns(p5t::Pcg5Layout<double>(t));
@@ -2891,6 +2892,32 @@ int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int m
 			&plan.C.naList, &plan.C.needAgg, &plan.C.rowOf, &plan.C.cbPtr, &plan.C.cbList }) vec(*v);
 		mix(plan.rowPeers.data(), plan.rowPeers.size());
 		*hash = h;
+	}
+	return CUBA_OK;
+}
+
+int cuba_debug_pcg5t_layout(const cuba_problem* p, int numSMs, int aggsPerCtaTop, int scalarBytes, int64_t smemBudget, int32_t* info)
+{
+	if (!p || numSMs < 1 || aggsPerCtaTop < 1 || aggsPerCtaTop > 3 || (scalarBytes != 4 && scalarBytes != 8) || smemBudget < 0 || !info)
+		return fail(CUBA_ERR_INVALID, "pcg5t_layout: bad arguments");
+	Structure S;
+	const char* err = "";
+	if (!build_structure(p->Pall, p->numP, p->Lall, p->numL, p->E2, p->idx2, p->E3, p->idx3, 0, 1, TILE, S, &err)) return fail(CUBA_ERR_INVALID, err);
+	for (int i = 0; i < 12; i++) info[i] = 0;
+	for (int apc = aggsPerCtaTop; apc >= 1; apc--) {
+		Pcg5Plan plan;
+		build_pcg5_plan(S.numP, S.nfull, S.fRowPtr, S.fColInd, 1, numSMs, PCG5_MAXAGG, 2 * PCG5_BLOCK / 6, plan, nullptr, apc);
+		if (!plan.ok || plan.P.maxRows * 6 > p5t::Pcg5Shape::BLOCK) continue;
+		p5t::Pcg5Dims t = pcg5t_plan_dims(plan);
+		auto report = [&](auto lay) {
+			const int cached = std::max(plan.P.blkMax - p5t::Pcg5Shape::REGBLK, 0);
+			const size_t vals[12] = { 1, (size_t)apc, (size_t)t.capBlocks, (size_t)(cached - t.capBlocks), (size_t)t.zhInSmem, lay.total,
+				lay.r - lay.blk, lay.p - lay.r, lay.rc - lay.cc, lay.c - lay.rc, lay.ls - lay.zh, lay.loc - lay.ai };
+			for (int i = 0; i < 12; i++) info[i] = (int32_t)vals[i];
+		};
+		if (scalarBytes == 8) { if (!p5t::pcg5t_fit<double>(t, plan.P.blkMax, apc, (size_t)smemBudget)) continue; report(p5t::Pcg5Layout<double>(t)); }
+		else { if (!p5t::pcg5t_fit<float>(t, plan.P.blkMax, apc, (size_t)smemBudget)) continue; report(p5t::Pcg5Layout<float>(t)); }
+		break;
 	}
 	return CUBA_OK;
 }

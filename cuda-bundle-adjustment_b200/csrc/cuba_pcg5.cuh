@@ -166,6 +166,7 @@ template <typename T>
 struct Pcg5PrepArgs {
 	const int* fRowPtr; const int* fColInd; const T* fVal; const T* b; const T* Zx;
 	int numP, A; const int* aggRow;
+	int zhatFp32;   // 1: Z^ is rounded to fp32 before it is stored and used for rc0 (k_pcg5t keeps it in fp32 in shared memory)
 	T* Linv; T* R0; T* Zhat; T* rcRow; T* rc0; Pcg5Ctl* ctl;
 };
 
@@ -217,6 +218,7 @@ __global__ void k_pcg5_prep_rows(const Pcg5PrepArgs<T> a)
 				T s = T(0);
 #pragma unroll
 				for (int k = 0; k < 6; k++) if (k >= r) s += L[r * 6 + k] * zq[k];       // Z^(r,q) = sum_{k>=r} L(k,r) Z(k,q)
+				if (a.zhatFp32) s = (T)(float)s;
 				a.Zhat[36 * (size_t)i + q * 6 + r] = s;
 				rcq += s * bh[r];
 			}

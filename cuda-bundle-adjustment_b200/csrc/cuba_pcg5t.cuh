@@ -7,7 +7,12 @@
 //   * the three scalars are summed by three warps (one each) instead of by all sixteen; the 3 + 6K partial products of the
 //     (row, component) threads are added by warp butterflies instead of through a shared-memory staging array;
 //   * K = 1, 2 or 3 aggregates per CTA on the coarse level (k_pcg5: one per group of gs CTAs);
-//   * up to two blocks per thread in one product round (register block, then one cached block), the staging sized by what a CTA owns.
+//   * one block per thread and product round (the register blocks, then the cached ones), the row sums accumulating over the
+//     rounds: 512 staging slots instead of 1 024;
+//   * Z^ of the needed columns in shared memory in fp32, the polled partial words behind the polled w inside the product staging,
+//     and the needed column (not its six board offsets) per w entry: what makes room for the K = 2 slice of Ac^-1.  The rounded
+//     Z^ is the prolongator in both places of the iteration and in rc0 (k_pcg5_prep_rows rounds the global copy), so
+//     M^-1 = I + Z^ Ac^-1 Z^^T stays symmetric positive definite and rc stays Z^^T r;
 // cuba_pcg5.cuh keeps the multi-GPU and large-graph shape: the same source restructured to serve both shapes ran slower on the
 // streamed (BIG) path, so the shapes live in two files.
 // The engine picks this kernel for world == 1 solves whose blocks fit on chip (CUBA_PCG5_LEGACY=1 forces the other one).
@@ -23,15 +28,16 @@ struct Pcg5Shape {
 	static constexpr int BLOCK = 512;
 	static constexpr int BPT = 1;                      // register-resident A^ blocks per thread
 	static constexpr int REGBLK = BLOCK * BPT;         // 512, as in cuba_pcg5.cuh (PCG5_REGBLK)
-	static constexpr int CPT = 2;                      // blocks per thread and product round: the register block, then one cached block
+	static constexpr int CPT = 1;                      // blocks per thread and product round
 	static constexpr int CHUNK = BLOCK * CPT;
 	static constexpr int PCH = 3;                      // polled words in flight per thread
 };
 
 // aggregates per CTA the engine tries first (then fewer, until the plan exists and the shared memory fits).  1: on ba_kitti_00
-// (one H100 80GB HBM3, 700 W) K = 2 cut the iterations per LM step from 1561 to 1250 but cost 18.1 instead of 11.2 us per
-// iteration (71 fewer cached blocks and Z^ from L2 to make room for the 76 KB slice of Ac^-1) and 4.2 instead of 1.5 ms per
-// coarse rebuild: 29.0 instead of 24.0 ms per step.  K = 3 does not fit in shared memory.
+// (one H100 80GB HBM3, 700 W limit) K = 2 fits with every Z^ and all but 22 of the 182 cached blocks of the fullest CTA on chip and
+// cuts the iterations per LM step from 1560 to 1251, but an iteration takes 14.5 instead of 9.8 us (every phase grows: 15
+// instead of 9 partial words, 12 instead of 6 rows of Ac^-1 over 1584 instead of 792 columns; DESIGN.md section 7) and a coarse
+// rebuild 1.6 instead of 0.5 ms: 24.4 instead of 21.6 ms per step.  K = 2 pays below about 11.4 us per iteration.
 constexpr int DEFAULT_APC = 1;
 
 struct Pcg5Dims {
@@ -43,18 +49,17 @@ struct Pcg5Dims {
 	int sqWords;  // doubles of the partial-product staging: 9 * maxRows * 6
 };
 
-// Pcg5Dims::ccCap of a plan: the shape's CHUNK, or less when a CTA never owns that many blocks; never less than needMax, because the
-// same storage holds the polled w entries of the needed columns
-inline int pcg5t_cc_cap(int blkMax, int needMax)
+// Pcg5Dims::ccCap of a plan: the shape's CHUNK, or less when a CTA never owns that many blocks (Pcg5Layout sizes the storage for
+// the polled words it also holds)
+inline int pcg5t_cc_cap(int blkMax)
 {
-	const int c = blkMax >= Pcg5Shape::CHUNK ? Pcg5Shape::CHUNK : std::max((std::max(blkMax, needMax) + 31) / 32 * 32, 32);
-	return std::max(c, needMax);
+	return blkMax >= Pcg5Shape::CHUNK ? Pcg5Shape::CHUNK : std::max((blkMax + 31) / 32 * 32, 32);
 }
 
 // shared-memory carve-up, one definition for the host (size) and the device (pointers)
 template <typename T>
 struct Pcg5Layout {
-	size_t blk, r, s, u, p, y, cc, rc, sc, c, zh, pv, ls, sq, ai, loc, rowPtr, woff, own, nagg, alist, diag, total;
+	size_t blk, r, s, u, p, y, cc, rc, c, zh, pv, ls, sq, ai, loc, rowPtr, col, own, nagg, alist, diag, total;
 	__host__ __device__ explicit Pcg5Layout(const Pcg5Dims& d)
 	{
 		size_t o = 0;
@@ -65,18 +70,20 @@ struct Pcg5Layout {
 		u = take((size_t)d.needMax * 6 * sizeof(T), 8);
 		p = take((size_t)d.maxRows * 6 * sizeof(T), 8);
 		y = take((size_t)d.maxRows * 6 * sizeof(T), 8);
-		cc = take((size_t)d.ccCap * 6 * sizeof(double), 8);      // block-product staging; polled w entries (double) between passes
+		// block-product staging; between the passes the polled w entries of the needed columns and, behind them, the polled
+		// partial words (both double): they are consumed before the next products are staged
+		const size_t polled = (size_t)d.needMax * 6 + (size_t)d.npv, staged = (size_t)d.ccCap * 6;
+		cc = take((polled > staged ? polled : staged) * sizeof(double), 8);
+		pv = cc + (size_t)d.needMax * 6 * sizeof(double);
 		rc = take((size_t)d.nc * sizeof(T), 8);
-		sc = take((size_t)d.nc * sizeof(T), 8);
 		c = take((size_t)d.maxNeedAgg * 6 * sizeof(T), 8);
-		zh = take(d.zhInSmem ? (size_t)d.needMax * 36 * sizeof(T) : 0, 8);
-		pv = take((size_t)d.npv * sizeof(double), 8);
+		zh = take(d.zhInSmem ? (size_t)d.needMax * 36 * sizeof(float) : 0, 8);
 		ls = take((size_t)d.nls * sizeof(double), 8);
 		sq = take((size_t)d.sqWords * sizeof(double), 8);           // nine products of every (row, component) thread
 		ai = take((size_t)d.sliceRows * d.nc * sizeof(float), 16);
 		loc = take((size_t)d.capBlocks * sizeof(int), 4);
 		rowPtr = take(((size_t)d.maxRows + 1) * sizeof(int), 4);
-		woff = take((size_t)d.needMax * 6 * sizeof(int), 4);
+		col = take((size_t)d.needMax * sizeof(int), 4);
 		own = take((size_t)d.needMax * sizeof(int), 4);
 		nagg = take((size_t)d.needMax * sizeof(int), 4);
 		alist = take((size_t)d.maxNeedAgg * sizeof(int), 4);
@@ -84,6 +91,39 @@ struct Pcg5Layout {
 		total = (o + 15) / 16 * 16;
 	}
 };
+
+// entries of the coarse search direction sc = wc + beta sc a thread keeps in registers (entry tid + i BLOCK in slot i; only the thread
+// that advances rc(q) ever reads sc(q)): a plan needs nc <= BLOCK * pcg5t_nsc(K)
+__host__ __device__ constexpr int pcg5t_nsc(int K) { return 2 * K; }
+
+// blocks of a CTA that a plan with K > 1 aggregates per CTA may leave to the global copy (read from L2 in every pass) to make room
+// for the K-fold slice of Ac^-1: one warp's share of a product round
+constexpr int MAX_STREAMED_BLOCKS = 32;
+
+// Sizes the caches of a plan (every other field of `t` set) for `budget` bytes of shared memory: capBlocks and zhInSmem.
+// One aggregate per CTA: every block past the registers is cached (a solve that streams blocks is cuba_pcg5.cuh's BIG shape), Z^
+// if it still fits.  Several: Z^ is cached and at most MAX_STREAMED_BLOCKS blocks are not.  False: the plan does not fit.
+template <typename T>
+inline bool pcg5t_fit(Pcg5Dims& t, int blkMax, int aggsPerCta, size_t budget)
+{
+	const size_t per = 36 * sizeof(T) + sizeof(int);              // s_blk + s_loc
+	const size_t want = blkMax > Pcg5Shape::REGBLK ? (size_t)(blkMax - Pcg5Shape::REGBLK) : 0;
+	t.capBlocks = 0; t.zhInSmem = 0;
+	if (t.nc > Pcg5Shape::BLOCK * pcg5t_nsc(aggsPerCta)) return false;
+	const size_t base = Pcg5Layout<T>(t).total + 64;              // + what the alignment of the regions behind s_blk can add
+	const size_t zh = (size_t)t.needMax * 36 * sizeof(float);
+	if (aggsPerCta > 1) {
+		if (base + zh > budget) return false;
+		const size_t cap = std::min(want, (budget - base - zh) / per);
+		if (want - cap > (size_t)MAX_STREAMED_BLOCKS) return false;
+		t.capBlocks = (int)cap; t.zhInSmem = 1;
+		return true;
+	}
+	if (base + want * per > budget) return false;
+	t.capBlocks = (int)want;
+	t.zhInSmem = base + want * per + zh <= budget ? 1 : 0;
+	return true;
+}
 
 template <typename T>
 struct Pcg5Args {
@@ -166,6 +206,7 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 	// the names of cuba_pcg5.cuh's constants, bound to this shape
 	constexpr int PCG5_BLOCK = Shape::BLOCK, PCG5_BPT = Shape::BPT, PCG5_CPT = Shape::CPT, PCG5_CHUNK = Shape::CHUNK, PCG5_PCH = Shape::PCH;
 	constexpr int NPK = pcg5t_np(K);
+	constexpr int NSC = pcg5t_nsc(K);
 	constexpr int PPCH = K == 1 ? PCG5_PCH : 2 * K;        // polled partial words in flight per thread: G (3 + 6K) in one round on 132 CTAs
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const Pcg5Layout<T> lay(a.dims);
@@ -179,15 +220,14 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 	T* s_cc = reinterpret_cast<T*>(smem_raw + lay.cc);              // [6][ccCap] block products, component-major
 	double* s_w = reinterpret_cast<double*>(smem_raw + lay.cc);     // polled w entries of the needed columns (same storage, other phase)
 	T* s_rc = reinterpret_cast<T*>(smem_raw + lay.rc);              // [nc] coarse residual Z^^T r
-	T* s_sc = reinterpret_cast<T*>(smem_raw + lay.sc);              // [nc]
 	T* s_c = reinterpret_cast<T*>(smem_raw + lay.c);                // [maxNeedAgg][6]
-	T* s_zh = reinterpret_cast<T*>(smem_raw + lay.zh);              // [needMax][36]
-	double* s_pv = reinterpret_cast<double*>(smem_raw + lay.pv);    // polled partials, later polled rank summaries
+	float* s_zh = reinterpret_cast<float*>(smem_raw + lay.zh);      // [needMax][36] Z^ of the needed columns
+	double* s_pv = reinterpret_cast<double*>(smem_raw + lay.pv);    // polled partials, later polled rank summaries (behind s_w)
 	double* s_ls = reinterpret_cast<double*>(smem_raw + lay.ls);    // [NR] this rank's summary
 	float* s_ai = reinterpret_cast<float*>(smem_raw + lay.ai);      // [nagg*6][nc] slices of AcInv
 	int* s_loc = reinterpret_cast<int*>(smem_raw + lay.loc);
 	int* s_rowPtr = reinterpret_cast<int*>(smem_raw + lay.rowPtr);
-	int* s_woff = reinterpret_cast<int*>(smem_raw + lay.woff);      // [needMax*6] board offset of every needed w entry
+	int* s_col = reinterpret_cast<int*>(smem_raw + lay.col);        // [needMax] the needed columns: w entry (c, comp) is word 6 s_col[c] + comp of a board
 	int* s_own = reinterpret_cast<int*>(smem_raw + lay.own);
 	int* s_nagg = reinterpret_cast<int*>(smem_raw + lay.nagg);
 	int* s_alist = reinterpret_cast<int*>(smem_raw + lay.alist);
@@ -225,22 +265,22 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 	for (int i = tid; i <= nrows; i += PCG5_BLOCK) s_rowPtr[i] = a.fRowPtr[row0 + i] - blk0;
 	for (int i = tid; i < nneed; i += PCG5_BLOCK) {
 		const int j = a.needCol[need0 + i];
+		s_col[i] = j;
 		s_own[i] = (j >= row0 && j < row1) ? j - row0 : -1;
 		if (coarse) s_nagg[i] = a.needAgg[need0 + i];
 	}
-	for (int i = tid; i < nneed * 6; i += PCG5_BLOCK) s_woff[i] = 6 * a.needCol[need0 + i / 6] + (i % 6);
 	if (coarse) {
 		const int na0 = a.naPtr[cta];
 		nagg = a.naPtr[cta + 1] - na0;
 		for (int i = tid; i < nagg; i += PCG5_BLOCK) s_alist[i] = a.naList[na0 + i];
-		for (int i = tid; i < nc; i += PCG5_BLOCK) { s_rc[i] = a.rc0[i]; s_sc[i] = T(0); }
+		for (int i = tid; i < nc; i += PCG5_BLOCK) s_rc[i] = a.rc0[i];
 	}
 	for (int i = tid; i < nrows * 6; i += PCG5_BLOCK) { s_p[i] = T(0); s_y[i] = T(0); }
 	__syncthreads();
 	for (int i = tid; i < nneed; i += PCG5_BLOCK) if (s_own[i] >= 0) s_diag[s_own[i]] = i;
 	if (coarse) {
 		if (a.dims.zhInSmem)
-			for (int wi = tid; wi < nneed * 36; wi += PCG5_BLOCK) s_zh[wi] = __ldcg(a.Zhat + 36 * (size_t)a.needCol[need0 + wi / 36] + (wi % 36));
+			for (int wi = tid; wi < nneed * 36; wi += PCG5_BLOCK) s_zh[wi] = (float)__ldcg(a.Zhat + 36 * (size_t)a.needCol[need0 + wi / 36] + (wi % 36));
 		for (int wi = tid; wi < (srow1 - srow0) * nc; wi += PCG5_BLOCK) s_ai[wi] = __ldg(a.AcInv + (size_t)srow0 * nc + wi);
 	}
 
@@ -303,12 +343,15 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 		}
 	}
 	for (int wi = tid; wi < nneed * 6; wi += PCG5_BLOCK) {
-		s_r[wi] = a.R0[s_woff[wi]];
+		s_r[wi] = a.R0[6 * (size_t)s_col[wi / 6] + (wi % 6)];
 		s_s[wi] = T(0);
 		s_u[wi] = T(0);
 	}
 	__syncthreads();
 
+	T scReg[NSC];
+#pragma unroll
+	for (int i = 0; i < NSC; i++) scReg[i] = T(0);
 	int status = 1, it = 0, kExit = 0;
 	double gamma = 0, rho0 = 0, rho = 0, alpha = 0, beta = 0;
 #ifdef CUBA_PCG_TIMING
@@ -349,7 +392,7 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 					const unsigned long long* pB = a.pBoard + 2 * (pHalf + (size_t)par * pStride + (size_t)rep * nPl);
 					// two lists, one after the other (one mixed list, the loads of both boards in flight together, was slower on
 					// ba_kitti_00 with 256 and with 512 threads)
-					bool ok = ll_poll_many<PCG5_BLOCK, PCG5_PCH>(nW, [&](int i) { return wB + 2 * (size_t)s_woff[i]; }, s_w, tag, a.ctl);
+					bool ok = ll_poll_many<PCG5_BLOCK, PCG5_PCH>(nW, [&](int i) { return wB + 2 * (size_t)(6 * s_col[i / 6] + (i % 6)); }, s_w, tag, a.ctl);
 					ok = ok && ll_poll_many<PCG5_BLOCK, PPCH>(nPl, [&](int i) { return pB + 2 * (size_t)i; }, s_pv, tag, a.ctl);
 					if (!ok) s_abort = 1;
 				}
@@ -426,7 +469,10 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 				//      cross the L2 while this CTA still has work to do ----
 				if (!coarse) advance_vectors();
 				if (coarse)
-					for (int q = tid; q < nc; q += PCG5_BLOCK) {
+#pragma unroll
+					for (int i = 0; i < NSC; i++) {
+						const int q = tid + i * PCG5_BLOCK;
+						if (q >= nc) break;
 						// global aggregate q/6 = rank r, local aggregate al
 						double wcv;
 						if (world > 1) wcv = s_pv[(q / (6 * Aloc)) * NR + 3 + (q % (6 * Aloc))];
@@ -436,8 +482,8 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 							wcv = 0;
 							for (int c = c0; c < c0 + a.gs; c++) wcv += s_pv[c * NP + 3 + 6 * j + comp];
 						}
-						const T sc = (T)wcv + (T)beta * s_sc[q];
-						s_sc[q] = sc;
+						const T sc = (T)wcv + (T)beta * scReg[i];
+						scReg[i] = sc;
 						s_rc[q] -= (T)alpha * sc;
 					}
 				__syncthreads();
@@ -477,11 +523,11 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 					const T* cc = s_c + 6 * (size_t)s_nagg[c];
 					T u = s_r[wi];
 					if (a.dims.zhInSmem) {
-						const T* Zh = s_zh + 36 * (size_t)c + comp;
+						const float* Zh = s_zh + 36 * (size_t)c + comp;
 #pragma unroll
-						for (int q = 0; q < 6; q++) u += Zh[6 * q] * cc[q];
+						for (int q = 0; q < 6; q++) u += (T)Zh[6 * q] * cc[q];
 					} else {
-						const T* Zh = a.Zhat + 36 * (size_t)(s_woff[wi] / 6) + comp;
+						const T* Zh = a.Zhat + 36 * (size_t)s_col[c] + comp;
 #pragma unroll
 						for (int q = 0; q < 6; q++) u += __ldcg(Zh + 6 * q) * cc[q];
 					}
@@ -533,12 +579,14 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 									for (int r = 0; r < 6; r++) y[r] += B[(c * 6 + r) * st] * rc;
 								}
 							} else {
+								// the few blocks a K > 1 plan leaves to the global copy: written by this CTA before the first pass and never
+								// again, so they may stay in the L1 (plain loads)
 								const T* B = a.fHat + overBase + (m - ncached);
 #pragma unroll 1
 								for (int c = 0; c < 6; c++) {
 									const T rc = rj[c];
 #pragma unroll
-									for (int r = 0; r < 6; r++) { y[r] += __ldcg(B) * rc; B += nover; }
+									for (int r = 0; r < 6; r++) { y[r] += *B * rc; B += nover; }
 								}
 							}
 						}
@@ -601,13 +649,14 @@ __global__ void __launch_bounds__(Pcg5Shape::BLOCK, 1) k_pcg5t(const Pcg5Args<T>
 				q9[1] += (double)wv1 * (double)ui;
 				q9[2] += (double)ri * (double)ri;
 				if (coarse) {
-					const T* Zh = a.dims.zhInSmem ? s_zh + 36 * (size_t)dl + comp : a.Zhat + 36 * (size_t)(row0 + li) + comp;
+					const float* ZhS = s_zh + 36 * (size_t)dl + comp;
+					const T* ZhG = a.Zhat + 36 * (size_t)(row0 + li) + comp;
 					int ja = 0;                                                    // the row's aggregate within this CTA
 #pragma unroll
 					for (int j = 0; j + 1 < K; j++) ja += li >= aggCut[j] ? 1 : 0;
 #pragma unroll
 					for (int q = 0; q < 6; q++) {
-						const double z = (double)(Zh[6 * q] * wv1);                  // (Z^^T w)(q) = sum_comp Z^(comp,q) w(comp)
+						const double z = (double)((a.dims.zhInSmem ? (T)ZhS[6 * q] : ZhG[6 * q]) * wv1);   // (Z^^T w)(q) = sum_comp Z^(comp,q) w(comp)
 #pragma unroll
 						for (int j = 0; j < K; j++) if (ja == j) q9[3 + 6 * j + q] += z;
 					}

@@ -385,6 +385,13 @@ int cuba_debug_pcg5_plan(const cuba_problem* p, int world, int numSMs, int maxAg
 /* The same with aggsPerCta aggregates per CTA (the one-GPU tuned kernel; 1: the plan of cuba_debug_pcg5_plan).  hash (may be null):
  * FNV-1a over every array of the plan, to compare plans across builds. */
 int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int maxAgg, int aggsPerCta, int32_t* info, uint64_t* hash);
+/* CPU-only: the shared-memory layout the one-GPU tuned kernel (k_pcg5t, csrc/cuba_pcg5t.cuh) gets on a device with numSMs SMs and
+ * smemBudget bytes of shared memory per CTA, as set_problem picks it: the largest number of aggregates per CTA <= aggsPerCtaTop whose
+ * plan exists and fits.  scalarBytes: 8 (fp64 engine) or 4.  info[12] = ok (0: no such plan; then all zero), aggregates per CTA,
+ * blocks cached in shared memory per CTA, blocks of the fullest CTA left to the global copy, Z^ in shared memory, total bytes, and
+ * the bytes of the cached blocks, of r / s / u, of the product staging (with the polled words), of rc, of Z^ and of the slice
+ * of Ac^-1.  No device needed. */
+int cuba_debug_pcg5t_layout(const cuba_problem* p, int numSMs, int aggsPerCtaTop, int scalarBytes, int64_t smemBudget, int32_t* info);
 /* The flat arrays the drop-in class (cuba::CudaBundleAdjustment, csrc/cuba_api.cpp) built in its last initialize(): what optimize()
  * hands to cuba_engine_set_problem.  `dropin` is the object's address; the pointers stay valid until the next initialize().
  * Needs no GPU (tests of the graph container: tombstones, re-added edges, fixed vertices, vertices without edges). */
