@@ -20,7 +20,7 @@ PCG_INFO_LEN = 16
 PCG_INFO_FIELDS = ("kernel", "two_level", "aggs_per_cta", "G", "gs", "A", "maxRows", "capBlocks", "zhInSmem", "coarse_kernel",
                    "cinfo", "status", "iters", "coarse_rebuilds", "bj_retries", "bad_rebuilds")
 PCG_KERNELS = ("none", "k_pcg", "k_pcg2", "k_pcg3", "k_pcg4", "k_pcg5", "k_pcg5_big", "k_pcg5t")   # "k_pcg" (retired) is never reported
-COARSE_KERNELS = ("none", "k_coarse_invert", "cluster2<8>", "cluster2<16>", "k_coarse_dense", "k_coarse_chol_cluster")
+COARSE_KERNELS = ("none", "k_coarse_invert", "cluster2<8>", "cluster2<16>", "k_coarse_dense", "k_coarse_chol_cluster")   # the cluster kernels (retired) are never reported
 
 
 # cuba_debug_pcg5_plan: info[] fields; w_cols_tuned / w_cols_legacy are the columns of w each launch shape's staging holds

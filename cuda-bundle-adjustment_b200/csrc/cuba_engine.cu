@@ -21,7 +21,7 @@
 #include "cuba_pcg4.cuh"
 #include "cuba_pcg5.cuh"
 #include "cuba_pcg5t.cuh"
-#include "cuba_coarse_dense.cuh"
+#include "cuba_coarse.cuh"
 #include "cuba_peer_reduce.cuh"
 #include "cuba_jh4.cuh"
 #include "cuba_levels.cuh"
@@ -304,14 +304,16 @@ struct Engine : EngineBase {
 	DBuf<long long> pcgTiming;
 	DBuf<unsigned long long> llFlags;   // k_pcg3: [wFlag 2*6numP*2 | pFlag 2*2G*2 | abort word]
 	int pcg2Grid = 0, pcg2Cap = 0, pcg2NeedMax = 0, pcg2MaxRows = 0;
-	// two-level PCG (cuba_pcg4.cuh)
+	// two-level PCG (cuba_pcg4.cuh; its coarse level: cuba_coarse.cuh)
 	DBuf<T> cZx, cZhat;
 	DBuf<float> cAcInv;
-	DBuf<double> cAcP, cPart, cU, cLp, cLd, cWp;
+	DBuf<double> cAcP, cPart, cU;
+	DBuf<double> cdT;               // k_coarse_dense: two copies of the lower 32 x 32 tiles of Ac, sized by setup_pcg2 and setup_pcg5 for
+	                                // the larger of their coarse matrices (DBuf only grows)
 	DBuf<int> cAggRow, cNaPtr, cNaList, cNeedAgg, cInfo, cRowOf, cCbPtr, cCbList;
 	int pcg4A = 0, pcg4Gs = 1, pcg4MaxNeedAgg = 0, pcg4Cap = 0, pcg4SliceInSmem = 0, pcg4ZhInSmem = 0;
-	size_t pcg4Smem = 0, pcg4InvSmem = 0;
-	bool pcg4Ok = false, tlActive = false, pcg4Cluster = false;
+	size_t pcg4Smem = 0;
+	bool pcg4Ok = false, tlActive = false;
 	PinnedArena arena;
 	bool coarseValid = false;       // cAcInv holds the inverse coarse matrix of an earlier solve of this problem
 	int coarseAge = 0;              // two-level solves since the coarse matrix was last rebuilt
@@ -369,6 +371,8 @@ struct Engine : EngineBase {
 		memset(hScal, 0, sizeof(Scalars));
 		CUDA_TRY(dScal.alloc(1));
 		CUDA_TRY(cudaMemsetAsync(dScal.p, 0, sizeof(Scalars), stream));
+		// for every coarse matrix k_coarse_invert takes (launch_coarse_setup), whichever solver it belongs to
+		CUDA_TRY(cudaFuncSetAttribute(k_coarse_invert<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coarse_invert_smem(PCG4_MAXAGG1)));
 		return CUBA_OK;
 	}
 
@@ -1288,12 +1292,11 @@ struct Engine : EngineBase {
 		//      beyond k_pcg5's 85 rows per CTA; otherwise its host lists and uploads are skipped (k_pcg5 has its own plan) ----
 		pcg4Ok = false;
 		if (cfg.reserved[0] == 3 || sizeof(T) != 8 || numP > 80 * numSMs * (world > 1 && numP >= 2048 ? world : 1)) {
-			// up to 74 aggregates (coarse inverse in the shared memory of an 8-CTA cluster), 37 with cfg.reserved[6] == 37 (one CTA)
+			// up to 74 aggregates, fewer with cfg.reserved[6] (37 or fewer: the coarse inverse of one CTA, k_coarse_invert)
 			const int maxAgg = (cfg.reserved[6] > 0 && cfg.reserved[6] < PCG4_MAXAGG) ? cfg.reserved[6] : PCG4_MAXAGG;
 			CoarsePartition CP;
 			build_coarse_partition(numP, PP, maxAgg, CP);
 			const int gs = CP.gs, A = CP.A, nc = 6 * A;
-			pcg4Cluster = A > PCG4_MAXAGG1;
 			pcg4A = A; pcg4Gs = gs; pcg4MaxNeedAgg = CP.maxNeedAgg;
 			size_t fixed4 = (size_t)needMax * (12 * sizeof(T) + 8) + (size_t)maxRows * (6 * sizeof(T) + 8) + 8 + 2 * (size_t)nc * sizeof(T)
 				+ (size_t)pcg4MaxNeedAgg * (6 * sizeof(T) + 4) + 64;
@@ -1311,14 +1314,9 @@ struct Engine : EngineBase {
 			pcg4Smem = (size_t)cap4 * (36 * sizeof(T) + 4) + fixed4;
 			if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg4: G %d A %d gs %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceInSmem %d cap %d smem %zu\n",
 				G, A, gs, needMax, maxRows, blkMax, pcg4MaxNeedAgg, pcg4ZhInSmem, pcg4SliceInSmem, pcg4Cap, pcg4Smem);
-			const size_t nblkPz = (size_t)A * (A + 1) / 2;
-			pcg4InvSmem = pcg4Cluster ? (((nblkPz + PCG4_CL - 1) / PCG4_CL + 2 * (size_t)A) * 36 * sizeof(double) + 2 * nblkPz + 16)
-			                          : ((nblkPz + 2 * (size_t)A) * 36 * sizeof(double));
-			pcg4Ok = budget > fixed4 && nc + 64 <= PCG4_BLOCK && pcg4InvSmem + 1024 <= (size_t)smemMax && numP >= 2 * A;
+			pcg4Ok = budget > fixed4 && nc + 64 <= PCG4_BLOCK && numP >= 2 * A;
 			if (pcg4Ok) {
 				CUDA_TRY(cudaFuncSetAttribute(k_pcg4<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcg4Smem));
-				if (pcg4Cluster) CUDA_TRY(cudaFuncSetAttribute(k_coarse_chol_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcg4InvSmem));
-				else CUDA_TRY(cudaFuncSetAttribute(k_coarse_invert<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcg4InvSmem));
 				int perSM4 = 0;
 				CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM4, k_pcg4<T>, PCG4_BLOCK, pcg4Smem));
 				if (perSM4 < 1) pcg4Ok = false;
@@ -1331,7 +1329,7 @@ struct Engine : EngineBase {
 				CUDA_TRY(cRowOf.upload(CP.rowOf, stream, arena)); CUDA_TRY(cCbPtr.upload(CP.cbPtr, stream, arena)); CUDA_TRY(cCbList.upload(CP.cbList, stream, arena));
 				CUDA_TRY(cZx.alloc(36 * (size_t)numP)); CUDA_TRY(cZhat.alloc(36 * (size_t)numP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull));
 				CUDA_TRY(cAcP.alloc((size_t)A * (A + 1) / 2 * 36)); CUDA_TRY(cAcInv.alloc((size_t)nc * nc));
-				CUDA_TRY(cLp.alloc((size_t)A * (A + 1) / 2 * 36)); CUDA_TRY(cWp.alloc((size_t)A * (A + 1) / 2 * 36)); CUDA_TRY(cLd.alloc((size_t)A * 36));
+				if (A > PCG4_MAXAGG1) CUDA_TRY(cdT.alloc(cdense::scratch_doubles(A)));
 				CUDA_TRY(cPart.alloc(2 * (size_t)G * PCG4_PSTRIDE)); CUDA_TRY(cInfo.alloc(1));
 				CUDA_TRY(cudaMemsetAsync(cPart.p, 0, sizeof(double) * cPart.n, stream));
 				// (no synchronisation: the uploads above read the pinned arena, or were staged by the driver before returning)
@@ -1345,29 +1343,10 @@ struct Engine : EngineBase {
 	int launch_pcg4()
 	{
 		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
-		const int numP = S.numP, A = pcg4A, nblkP = A * (A + 1) / 2;
+		const int numP = S.numP, A = pcg4A;
 		KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, cZx.p);
-		// The coarse matrix Ac = Z^T S Z and its inverse are rebuilt only now and then: ANY symmetric positive definite
-		// stand-in for Ac^-1 keeps M^-1 = D^-1 + Z B Z^T a valid preconditioner, and the coarse operator of an earlier
-		// damping / linearisation preconditions as well as the current one (CPU prototype: 26..201 iterations over ten LM
-		// iterations with a fresh inverse, 26..193 with one that is refreshed every fifth iteration).
-		// Measured limits of that freedom: a coarse inverse from an 81x larger damping costs nothing, one from a 1e5x larger damping
-		// costs 8x the iterations (1 276 vs 149 on kitti00_shaped) -> it is also rebuilt when the damping moved by more than 300x.
-		const int refreshEvery = cfg.reserved[4] > 0 ? cfg.reserved[4] : 8;
-		const double lamRatio = (coarseValid && coarseLambda > 0 && curLambda > 0) ? std::max(curLambda / coarseLambda, coarseLambda / curLambda) : 1.0;
-		if (!coarseValid || coarseAge >= refreshEvery || lamRatio > 300.0) {
-			KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, cRowOf.p, fColInd.p, S.nfull, cZx.p, cU.p);
-			KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, cCbPtr.p, cCbList.p, cU.p, nblkP, cAcP.p);
-			if (pcg4Cluster) {
-				// Cholesky in the shared memory of an 8-CTA cluster, then the triangular inverse (one CTA per block column) and W^T W on the whole chip
-				k_coarse_chol_cluster<<<PCG4_CL, 1024, pcg4InvSmem, stream>>>(cAcP.p, A, cLp.p, cLd.p, cAcInv.p, cInfo.p);
-				k_coarse_trinv<<<A, 256, (size_t)A * 36 * sizeof(double), stream>>>(cLp.p, cLd.p, A, cWp.p, cInfo.p);
-				k_coarse_wtw<<<(nblkP * 36 + 255) / 256, 256, 0, stream>>>(cWp.p, A, cAcInv.p, cInfo.p);
-				launches += 2;
-			}
-			else k_coarse_invert<T><<<1, 1024, pcg4InvSmem, stream>>>(cAcP.p, A, cAcInv.p, cInfo.p);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
+		if (coarse_due(coarseValid, coarseAge, coarseLambda)) {
+			int rc = launch_coarse_setup(A, cCbPtr, cCbList, cAcP, cAcInv, cInfo.p); if (rc) return rc;     // slot 0 of cInfo
 			coarseValid = true; coarseAge = 0; coarseLambda = curLambda;
 		}
 		coarseAge++;
@@ -1445,9 +1424,7 @@ struct Engine : EngineBase {
 	DBuf<unsigned char> p5RowPeers;
 	DBuf<T> p5Linv, p5R0, p5Zhat, p5RcRow, p5Rc0;
 	DBuf<float> p5AcInv;
-	DBuf<double> p5AcP, p5Lp, p5Wp, p5Ld;
-	DBuf<double> cdT;                              // k_coarse_dense: two copies of the lower 32 x 32 tiles of Ac
-	bool p5Dense = false;
+	DBuf<double> p5AcP;
 	DBuf<unsigned long long> p5Boards;
 	void* p5PeerBase[PCG5_MAXWORLD] = { nullptr };   // cudaIpc mappings of the peers' boards (own entry: the local allocation)
 	void* p5MappedFor = nullptr;                   // local allocation the mappings were exchanged for
@@ -1460,9 +1437,7 @@ struct Engine : EngineBase {
 	p5t::Pcg5Dims p5tDims{}, p5tDimsBJ{};            // the tuned one-GPU shape (cuba_pcg5t.cuh), when p5Tuned
 	const void* p5Fn = nullptr;
 	int p5Block = PCG5_BLOCK;
-	int p5Cluster = 0;                             // CTAs of the cluster that factors the coarse matrix (0: one CTA)
 	bool p5CoarseValid = false; int p5CoarseAge = 0; double p5CoarseLambda = 0;
-	size_t p5InvSmem = 0;
 	int p5Apc = 1;                                 // aggregates per CTA of the plan (k_pcg5t)
 	// read by cuba_debug_get_pcg_info only: the kernel of the last solve (CUBA_PCG_KERNEL_*), counters since set_problem, and a
 	// log of the cInfo flag of every k_pcg5 coarse rebuild -- rebuild n writes slot 1 + n % P5_INFO_LOG of cInfo (k_pcg4 keeps
@@ -1647,23 +1622,7 @@ struct Engine : EngineBase {
 		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: world %d G %d gs %d A %d aggsPerCta %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceRows %d cap %d smem %zu\n",
 			W, G, gs, A, plan.apc, d.needMax, d.maxRows, PP.blkMax, d.maxNeedAgg, d.zhInSmem, d.sliceRows, d.capBlocks, p5Smem);
 		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: shape %s, %d threads\n", p5Big ? "big" : p5Tuned ? "tuned" : "legacy", p5Block);
-		// coarse inverse: k_coarse_dense on the whole chip (A > 37; the only one past A = 148), or the packed block triangle in the
-		// shared memory of one CTA (A <= 37), of an 8-CTA cluster (A <= 74) or of a 16-CTA cluster (A <= 148; non-portable cluster size)
-		p5Dense = A > PCG4_MAXAGG1 && (A > PCG5_MAXAGG || !getenv("CUBA_COARSE_CLUSTER"));
-		p5Cluster = A > PCG5_MAXAGG ? 0 : A > PCG4_MAXAGG1 ? (A > PCG4_MAXAGG ? 16 : 8) : 0;
 		const size_t nblkPz = (size_t)A * (A + 1) / 2;
-		if (A > PCG5_MAXAGG) p5InvSmem = 0;
-		else if (p5Cluster) {
-			const size_t nloc = (nblkPz + p5Cluster - 1) / p5Cluster;
-			p5InvSmem = nloc * 36 * sizeof(double) + 2 * nloc + 16;
-		} else p5InvSmem = (nblkPz + 2 * (size_t)A) * 36 * sizeof(double);
-		if (p5InvSmem + 1024 > (size_t)smemMax) return CUBA_OK;
-		if (p5Cluster == 16) {
-			CUDA_TRY(cudaFuncSetAttribute(k_coarse_chol_cluster2<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p5InvSmem));
-			CUDA_TRY(cudaFuncSetAttribute(k_coarse_chol_cluster2<16>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-		} else if (p5Cluster == 8) CUDA_TRY(cudaFuncSetAttribute(k_coarse_chol_cluster2<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p5InvSmem));
-		else if (!p5Dense) CUDA_TRY(cudaFuncSetAttribute(k_coarse_invert<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(p5InvSmem, (!pcg4Cluster && pcg4Ok) ? pcg4InvSmem : 0)));
-		if (p5Cluster && (size_t)A * 36 * sizeof(double) > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(k_coarse_trinv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)A * 36 * sizeof(double))));
 		CUDA_TRY(p5CtaRow.upload(PP.rows, stream, arena)); CUDA_TRY(p5NeedPtr.upload(PP.nptr, stream, arena)); CUDA_TRY(p5NeedCol.upload(PP.ncol, stream, arena));
 		CUDA_TRY(p5Local.upload(PP.local, stream, arena)); CUDA_TRY(p5RowPeers.upload(peers, stream, arena));
 		CUDA_TRY(p5AggRow.upload(CP.aggRow, stream, arena)); CUDA_TRY(p5NaPtr.upload(CP.naPtr, stream, arena)); CUDA_TRY(p5NaList.upload(CP.naList, stream, arena));
@@ -1674,9 +1633,9 @@ struct Engine : EngineBase {
 		CUDA_TRY(cZx.alloc(36 * nP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(cInfo.alloc(1 + P5_INFO_LOG));
 		CUDA_TRY(cudaMemsetAsync(cInfo.p, 0, sizeof(int) * cInfo.n, stream));
 		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull));
-		CUDA_TRY(p5AcP.alloc(nblkPz * 36)); CUDA_TRY(p5AcInv.alloc((size_t)nc * nc)); CUDA_TRY(p5Lp.alloc(nblkPz * 36)); CUDA_TRY(p5Wp.alloc(nblkPz * 36)); CUDA_TRY(p5Ld.alloc((size_t)A * 36));
-		if (p5Dense) {
-			CUDA_TRY(cdT.alloc(2 * cdense::tiles((nc + cdense::NB - 1) / cdense::NB) * cdense::TT));
+		CUDA_TRY(p5AcP.alloc(nblkPz * 36)); CUDA_TRY(p5AcInv.alloc((size_t)nc * nc));
+		if (A > PCG4_MAXAGG1) {
+			CUDA_TRY(cdT.alloc(cdense::scratch_doubles(A)));
 			CUDA_TRY(gridBar.alloc(1));
 		}
 		// boards (16-byte words): [2 solve halves][2 pass parities] of w, of the per-CTA partials and of the rank summaries, then the control block
@@ -1705,8 +1664,8 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// blocked symmetric sweep on the whole chip (cuba_coarse_dense.cuh): one persistent cooperative kernel; tiles holds
-	// 2 cdense::tiles(ceil(6A / 32)) tiles, bar a zeroed or reused GridBar
+	// blocked symmetric sweep on the whole chip (cuba_coarse.cuh): one persistent cooperative kernel; tiles holds
+	// cdense::scratch_doubles(A) doubles, bar a zeroed or reused GridBar
 	int launch_coarse_dense(const double* AcP, int A, double* tiles, float* AcInv, int* info, GridBar* bar)
 	{
 		CUDA_TRY(cudaFuncSetAttribute(cdense::k_coarse_dense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cdense::SMEM));
@@ -1718,31 +1677,33 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// coarse matrix Ac = Z^T S Z of the current system and its inverse (fp32), for the aggregates behind (cbPtr, cbList)
-	int launch_coarse_setup(int A, int cluster, size_t invSmem, const int* cbPtr, const int* cbList, double* AcP, float* AcInv, double* Lp, double* Ld, double* Wp, bool dense = false)
+	// coarse matrix Ac = Z^T S Z of the current system (basis cZx) and its inverse (fp32), for the aggregates behind (cbPtr, cbList);
+	// info: 0 inverted, 1 not positive definite (AcInv zeroed).  The inverse: one CTA while the packed triangle fits its shared
+	// memory (A <= PCG4_MAXAGG1), the blocked sweep on the whole chip above.
+	int launch_coarse_setup(int A, const int* cbPtr, const int* cbList, double* AcP, float* AcInv, int* info)
 	{
 		const int nblkP = A * (A + 1) / 2;
-		int* infoP = p5InfoSlot();
 		KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, cRowOf.p, fColInd.p, S.nfull, cZx.p, cU.p);
 		KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, cbPtr, cbList, cU.p, nblkP, AcP);
-		if (dense) return launch_coarse_dense(AcP, A, cdT, AcInv, infoP, gridBar);
-		if (cluster) {
-			// Cholesky in the shared memory of an 8- or 16-CTA cluster, then the triangular inverse (one CTA per block column) and W^T W on the whole chip
-			cudaLaunchConfig_t lc = {};
-			lc.gridDim = dim3(cluster); lc.blockDim = dim3(1024); lc.dynamicSmemBytes = invSmem; lc.stream = stream;
-			cudaLaunchAttribute at[1];
-			at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-			lc.attrs = at; lc.numAttrs = 1;
-			if (cluster == 16) CUDA_TRY(cudaLaunchKernelEx(&lc, k_coarse_chol_cluster2<16>, (const double*)AcP, A, Lp, Ld, AcInv, infoP));
-			else CUDA_TRY(cudaLaunchKernelEx(&lc, k_coarse_chol_cluster2<8>, (const double*)AcP, A, Lp, Ld, AcInv, infoP));
-			k_coarse_trinv<<<A, 256, (size_t)A * 36 * sizeof(double), stream>>>(Lp, Ld, A, Wp, infoP);
-			k_coarse_wtw<<<(nblkP * 36 + 255) / 256, 256, 0, stream>>>(Wp, A, AcInv, infoP);
-			launches += 2;
-		}
-		else k_coarse_invert<T><<<1, 1024, invSmem, stream>>>(AcP, A, AcInv, infoP);
+		if (A > PCG4_MAXAGG1) return launch_coarse_dense(AcP, A, cdT, AcInv, info, gridBar);
+		k_coarse_invert<T><<<1, 1024, coarse_invert_smem(A), stream>>>(AcP, A, AcInv, info);
 		launches++;
 		CUDA_TRY(cudaGetLastError());
 		return CUBA_OK;
+	}
+
+	// The coarse matrix Ac = Z^T S Z and its inverse are rebuilt only now and then: ANY symmetric positive definite stand-in for
+	// Ac^-1 keeps M^-1 = D^-1 + Z B Z^T a valid preconditioner, and the coarse operator of an earlier damping / linearisation
+	// preconditions as well as the current one (CPU prototype: 26..201 iterations over ten LM iterations with a fresh inverse,
+	// 26..193 with one that is refreshed every fifth iteration).
+	// Measured limits of that freedom: a coarse inverse from an 81x larger damping costs nothing, one from a 1e5x larger damping
+	// costs 8x the iterations (1 276 vs 149 on kitti00_shaped) -> it is also rebuilt when the damping moved by more than 300x.
+	// valid / age / lambda: whether the solver holds an inverse, its two-level solves since the rebuild, the damping of the rebuild.
+	bool coarse_due(bool valid, int age, double lambda) const
+	{
+		const int refreshEvery = cfg.reserved[4] > 0 ? cfg.reserved[4] : 8;
+		const double lamRatio = (valid && lambda > 0 && curLambda > 0) ? std::max(curLambda / lambda, lambda / curLambda) : 1.0;
+		return !valid || age >= refreshEvery || lamRatio > 300.0;
 	}
 
 	int launch_pcg5(bool twoLevel)
@@ -1767,11 +1728,8 @@ struct Engine : EngineBase {
 		if (twoLevel) {
 			k_pcg5_prep_rc<T><<<(6 * A + 127) / 128, 128, 0, stream>>>(pa);
 			launches++;
-			// The coarse inverse is rebuilt only now and then (see launch_pcg4: any SPD stand-in keeps M^-1 a valid preconditioner).
-			const int refreshEvery = cfg.reserved[4] > 0 ? cfg.reserved[4] : 8;
-			const double lamRatio = (p5CoarseValid && p5CoarseLambda > 0 && curLambda > 0) ? std::max(curLambda / p5CoarseLambda, p5CoarseLambda / curLambda) : 1.0;
-			if (!p5CoarseValid || p5CoarseAge >= refreshEvery || lamRatio > 300.0) {
-				int rc = launch_coarse_setup(A, p5Cluster, p5InvSmem, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5Lp, p5Ld, p5Wp, p5Dense); if (rc) return rc;
+			if (coarse_due(p5CoarseValid, p5CoarseAge, p5CoarseLambda)) {
+				int rc = launch_coarse_setup(A, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5InfoSlot()); if (rc) return rc;
 				p5CoarseValid = true; p5CoarseAge = 0; p5CoarseLambda = curLambda; p5Rebuilds++;
 			}
 			p5CoarseAge++;
@@ -2443,10 +2401,10 @@ struct Engine : EngineBase {
 			for (int v : log) if (v != 0) bad++;
 			last = log[(int)((p5Rebuilds - 1) % P5_INFO_LOG)];
 		}
+		auto coarseOf = [](int A) { return A > PCG4_MAXAGG1 ? CUBA_COARSE_KERNEL_DENSE : CUBA_COARSE_KERNEL_INVERT; };   // launch_coarse_setup's rule
 		int coarseKernel = CUBA_COARSE_KERNEL_NONE;
-		if (lastPcgTwoLevel && lastPcgKernel == CUBA_PCG_KERNEL_PCG4) coarseKernel = pcg4Cluster ? CUBA_COARSE_KERNEL_PCG4_CLUSTER : CUBA_COARSE_KERNEL_INVERT;
-		else if (lastPcgTwoLevel && p5Ok)
-			coarseKernel = p5Dense ? CUBA_COARSE_KERNEL_DENSE : p5Cluster == 16 ? CUBA_COARSE_KERNEL_CLUSTER16 : p5Cluster == 8 ? CUBA_COARSE_KERNEL_CLUSTER8 : CUBA_COARSE_KERNEL_INVERT;
+		if (lastPcgTwoLevel && lastPcgKernel == CUBA_PCG_KERNEL_PCG4) coarseKernel = coarseOf(pcg4A);
+		else if (lastPcgTwoLevel && p5Ok) coarseKernel = coarseOf(p5A);
 		const bool tuned = p5Ok && p5Tuned;
 		const int32_t v[CUBA_PCG_INFO_LEN] = {
 			lastPcgKernel, lastPcgKernel != CUBA_PCG_KERNEL_NONE && lastPcgTwoLevel ? 1 : 0,
@@ -2484,7 +2442,7 @@ struct Engine : EngineBase {
 		DBuf<int> dInfo;
 		DBuf<GridBar> dBar;
 		CUDA_TRY(dAcP.alloc(36 * nblkP)); CUDA_TRY(dInv.alloc(nc * nc)); CUDA_TRY(dInfo.alloc(1)); CUDA_TRY(dBar.alloc(1));
-		CUDA_TRY(dT.alloc(2 * cdense::tiles((int)((nc + cdense::NB - 1) / cdense::NB)) * cdense::TT));
+		CUDA_TRY(dT.alloc(cdense::scratch_doubles(A)));
 		CUDA_TRY(cudaMemcpyAsync(dAcP.p, hAcP, sizeof(double) * 36 * nblkP, cudaMemcpyHostToDevice, stream));
 		CUDA_TRY(cudaMemsetAsync(dBar.p, 0, sizeof(GridBar), stream));
 		CUDA_TRY(cudaMemsetAsync(dInfo.p, 0xff, sizeof(int), stream));          // -1 unless the kernel reports
@@ -2520,7 +2478,7 @@ struct Engine : EngineBase {
 			case 6: rc = launch_chi2(cur, 0); break;
 			case 7:   // one rebuild of the coarse inverse of k_pcg5 / k_pcg5t (projection, assembly, inverse) from the current system
 				if (!p5Ok || p5A < 1) rc = fail(CUBA_ERR_STATE, "bench_stage: no two-level k_pcg5 plan");
-				else rc = launch_coarse_setup(p5A, p5Cluster, p5InvSmem, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5Lp, p5Ld, p5Wp, p5Dense);
+				else rc = launch_coarse_setup(p5A, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5InfoSlot());
 				break;
 			default: rc = fail(CUBA_ERR_INVALID, "bench_stage: unknown stage");
 			}

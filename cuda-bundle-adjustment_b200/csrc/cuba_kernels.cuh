@@ -9,7 +9,6 @@
 //   Hsc: symmetric-full BSR (fRowPtr,fColInd,fVal[nfull][36]) for the PCG; upper view for parity.
 #pragma once
 
-#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 

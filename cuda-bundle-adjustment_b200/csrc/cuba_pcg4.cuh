@@ -18,7 +18,7 @@
 //     partials, the six numbers Z^_own^T w -- so every CTA can advance the coarse residual rc = Z^^T r by the same
 //     recurrences as r itself (sc = wc + beta sc, rc -= alpha sc);
 //   * c = Ac^-1 rc is needed only for the aggregates of a CTA's own and neighbouring rows: a few 6-row slices of the
-//     explicit inverse (computed per solve by k_coarse_invert) times rc;
+//     explicit inverse (rebuilt now and then by the coarse level of cuba_coarse.cuh, as for k_pcg5) times rc;
 //   * u_j = r_j + Z^_j c_a(j) for every needed column j, then w = A^ u from shared memory as before.
 // All sums are in fixed order: bit-reproducible.
 // Replaces convertBSRToCSR + cuSOLVER csrchol (reference cuda_linear_solver.cpp:301-335) like the other PCG kernels.
@@ -30,9 +30,7 @@ namespace cuba_b200 {
 
 constexpr int PCG4_BLOCK = 512;
 constexpr int PCG4_PSTRIDE = 12;    // doubles per CTA on the partial board: gamma, delta, rho, -, wc[6], -, -
-constexpr int PCG4_MAXAGG = 74;     // k_coarse_invert_cluster: the packed block triangle lives in the shared memory of an 8-CTA cluster
-constexpr int PCG4_MAXAGG1 = 37;    // k_coarse_invert: ... of one CTA
-constexpr int PCG4_CL = 8;          // CTAs per cluster of k_coarse_invert_cluster
+constexpr int PCG4_MAXAGG = 74;     // aggregates: threads 64 .. 64 + nc advance the coarse residual, so nc + 64 <= PCG4_BLOCK
 constexpr int PCG4_TPR = 16;        // threads per row of the coarse slice product
 
 template <typename T>
@@ -443,527 +441,6 @@ __global__ void __launch_bounds__(PCG4_BLOCK, 1) k_pcg4(const Pcg4Args<T> aa)
 	if (tid == 0 && aa.timing) { for (int i = 0; i < 7; i++) aa.timing[(size_t)cta * 8 + i] = tacc[i]; aa.timing[(size_t)cta * 8 + 7] = it; }
 #endif
 	if (cta == 0 && tid == 0) { a.status->iters = it; a.status->status = status; a.status->rz0 = rho0; a.status->rz = rho; }
-}
-
-// ---- coarse-level setup ------------------------------------------------------------------------------------------
-
-// Z_i = Ad(T_i) for every free pose: delta = [omega; upsilon], Ad = [[R, 0], [[t]x R, R]] (column-major 6x6)
-template <typename T>
-__global__ void k_coarse_basis(const T* __restrict__ pose, int numP, T* Zx)
-{
-	const int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= numP) return;
-	const T* p = pose + 8 * (size_t)i;
-	const T x = p[0], y = p[1], z = p[2], w = p[3], tx = p[4], ty = p[5], tz = p[6];
-	T R[3][3];
-	R[0][0] = 1 - 2 * (y * y + z * z); R[0][1] = 2 * (x * y - z * w); R[0][2] = 2 * (x * z + y * w);
-	R[1][0] = 2 * (x * y + z * w); R[1][1] = 1 - 2 * (x * x + z * z); R[1][2] = 2 * (y * z - x * w);
-	R[2][0] = 2 * (x * z - y * w); R[2][1] = 2 * (y * z + x * w); R[2][2] = 1 - 2 * (x * x + y * y);
-	const T K[3][3] = { { T(0), -tz, ty }, { tz, T(0), -tx }, { -ty, tx, T(0) } };
-	T* Z = Zx + 36 * (size_t)i;
-	for (int c = 0; c < 3; c++)
-		for (int r = 0; r < 3; r++) {
-			Z[c * 6 + r] = R[r][c];                              // top-left R
-			Z[(c + 3) * 6 + r] = T(0);                           // top-right 0
-			Z[(c + 3) * 6 + r + 3] = R[r][c];                    // bottom-right R
-			Z[c * 6 + r + 3] = K[r][0] * R[0][c] + K[r][1] * R[1][c] + K[r][2] * R[2][c];   // bottom-left [t]x R
-		}
-}
-
-// U_n = Z_i^T S_n Z_j for every block n = (i,j) of the symmetric-full BSR: one thread per (block, entry)
-template <typename T>
-__global__ void k_coarse_project(const T* __restrict__ fVal, const int* __restrict__ fRowOf, const int* __restrict__ fColInd, int nfull,
-	const T* __restrict__ Zx, double* U)
-{
-	const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-	if (e >= 36LL * nfull) return;
-	const int n = (int)(e / 36), rc = (int)(e - 36LL * n), c = rc / 6, r = rc - 6 * c;
-	const T* Sb = fVal + 36 * (size_t)n;
-	const T* Zi = Zx + 36 * (size_t)fRowOf[n] + r * 6;        // column r of Z_i
-	const T* Zj = Zx + 36 * (size_t)fColInd[n] + c * 6;       // column c of Z_j
-	double zj[6];
-#pragma unroll
-	for (int m = 0; m < 6; m++) zj[m] = (double)Zj[m];
-	double s = 0;
-#pragma unroll
-	for (int k = 0; k < 6; k++) {
-		double t = 0;
-#pragma unroll
-		for (int m = 0; m < 6; m++) t += (double)Sb[m * 6 + k] * zj[m];      // (S Z_j)(k,c)
-		s += (double)Zi[k] * t;
-	}
-	U[e] = s;
-}
-
-// Ac = Z^T S Z, lower block triangle, packed: block (ib >= jb) at (ib (ib+1)/2 + jb) * 36, column-major 6x6.
-// cbPtr/cbList: the fine blocks of every coarse block in ascending order (built on the host) -> fixed-order sums.
-__global__ void k_coarse_assemble(const int* __restrict__ cbPtr, const int* __restrict__ cbList, const double* __restrict__ U, int nblkP, double* AcP)
-{
-	const int e = blockIdx.x * blockDim.x + threadIdx.x;
-	if (e >= nblkP * 36) return;
-	const int bp = e / 36, rc = e - 36 * bp;
-	double s0 = 0, s1 = 0;
-	int k = cbPtr[bp];
-	const int k1 = cbPtr[bp + 1];
-	for (; k + 1 < k1; k += 2) { s0 += U[36 * (size_t)cbList[k] + rc]; s1 += U[36 * (size_t)cbList[k + 1] + rc]; }
-	if (k < k1) s0 += U[36 * (size_t)cbList[k] + rc];
-	AcP[e] = s0 + s1;
-}
-
-// AcInv = Ac^-1 by block Cholesky (6x6 blocks) of the packed lower triangle in shared memory: ONE CTA.
-// On a non-positive pivot the inverse is zeroed (the preconditioner degrades to block-Jacobi, still valid).
-template <typename T>
-__global__ void __launch_bounds__(1024, 1) k_coarse_invert(const double* __restrict__ AcP, int A, float* AcInv, int* info)
-{
-	extern __shared__ __align__(16) unsigned char smem_raw[];
-	double* B = reinterpret_cast<double*>(smem_raw);             // [nblkP][36] packed blocks
-	const int nblkP = A * (A + 1) / 2, nc = 6 * A;
-	double* sLi = B + (size_t)nblkP * 36;                        // [A][36] inverses of the diagonal factors
-	double* sRow = sLi + (size_t)A * 36;                         // [A][36] scratch row
-	__shared__ int s_fail;
-	__shared__ unsigned char s_ib[PCG4_MAXAGG1 * (PCG4_MAXAGG1 + 1) / 2], s_jb[PCG4_MAXAGG1 * (PCG4_MAXAGG1 + 1) / 2];   // packed index -> (ib, jb)
-	__shared__ double s_L[36], s_id[6];
-	const int tid = threadIdx.x, NT = blockDim.x;
-	auto idx = [](int ib, int jb) { return (size_t)(ib * (ib + 1) / 2 + jb) * 36; };
-	for (int e = tid; e < nblkP * 36; e += NT) B[e] = AcP[e];
-	for (int ib = tid; ib < A; ib += NT) for (int jb = 0; jb <= ib; jb++) { s_ib[ib * (ib + 1) / 2 + jb] = (unsigned char)ib; s_jb[ib * (ib + 1) / 2 + jb] = (unsigned char)jb; }
-	if (tid == 0) s_fail = 0;
-	__syncthreads();
-	// ---- phase 1: block Cholesky, L overwrites the triangle ----
-	for (int kb = 0; kb < A; kb++) {
-		if (tid < 32) {
-			// 6x6 Cholesky of the diagonal block in place (lane r owns row r), then L^-1 column by column (lane q owns column q)
-			double* D = B + idx(kb, kb);
-			const int r = tid;
-			for (int j = 0; j < 6; j++) {
-				const double d = D[j * 6 + j];
-				if (!(d > 0)) { if (r == 0) s_fail = 1; break; }
-				const double sq = sqrt(d);
-				__syncwarp();
-				if (r == j) D[j * 6 + j] = sq;
-				else if (r > j && r < 6) D[j * 6 + r] = D[j * 6 + r] / sq;
-				__syncwarp();
-				if (r > j && r < 6)
-					for (int c = j + 1; c <= r; c++) D[c * 6 + r] -= D[j * 6 + r] * D[j * 6 + c];
-				__syncwarp();
-			}
-			__syncwarp();
-			if (r < 6) {
-				for (int c = r + 1; c < 6; c++) D[c * 6 + r] = 0.0;       // the strict upper part is not part of L
-				s_id[r] = 1.0 / D[r * 6 + r];
-			}
-			__syncwarp();
-			if (r < 6) {
-				const int q = r;                                           // column q of Li = L^-1
-				double col[6];
-				for (int i = 0; i < 6; i++) col[i] = 0.0;
-				col[q] = s_id[q];
-				for (int i = q + 1; i < 6; i++) {
-					double sum = 0;
-					for (int k = q; k < i; k++) sum += D[k * 6 + i] * col[k];
-					col[i] = -sum * s_id[i];
-				}
-				for (int i = 0; i < 6; i++) sLi[(size_t)kb * 36 + q * 6 + i] = col[i];
-			}
-		}
-		__syncthreads();
-		if (s_fail) break;
-		// panel: B(ib,kb) <- B(ib,kb) L_kk^-T, one thread per (block, row)
-		const double* Li = sLi + (size_t)kb * 36;
-		for (int w = tid; w < (A - kb - 1) * 6; w += NT) {
-			const int ib = kb + 1 + w / 6, r = w % 6;
-			double* X = B + idx(ib, kb);
-			double x[6], y[6];
-			for (int k = 0; k < 6; k++) x[k] = X[k * 6 + r];
-			for (int c = 0; c < 6; c++) { double s = 0; for (int k = 0; k <= c; k++) s += x[k] * Li[k * 6 + c]; y[c] = s; }   // (X Li^T)(r,c) = sum_k X(r,k) Li(c,k)
-			for (int c = 0; c < 6; c++) X[c * 6 + r] = y[c];
-		}
-		__syncthreads();
-		// trailing update: B(ib,jb) -= B(ib,kb) B(jb,kb)^T for kb < jb <= ib
-		const int m = A - kb - 1;
-		const int nent = m * (m + 1) / 2 * 36;
-		for (int w = tid; w < nent; w += NT) {
-			const int bq = w / 36, rc = w - 36 * bq, c = rc / 6, r = rc - 6 * c;
-			const int ib = kb + 1 + s_ib[bq], jb = kb + 1 + s_jb[bq];
-			const double* P = B + idx(ib, kb);
-			const double* Q = B + idx(jb, kb);
-			double s = 0;
-			for (int k = 0; k < 6; k++) s += P[k * 6 + r] * Q[k * 6 + c];
-			B[idx(ib, jb) + c * 6 + r] -= s;
-		}
-		__syncthreads();
-	}
-	if (s_fail) {
-		for (int e = tid; e < nc * nc; e += NT) AcInv[e] = 0.f;
-		if (tid == 0 && info) *info = 1;
-		return;
-	}
-	// ---- phase 2: W = L^-1 (block lower triangular), row by row: W(ib,jb) = -L_ii^-1 sum_{k=jb}^{ib-1} L(ib,k) W(k,jb) ----
-	for (int ib = 0; ib < A; ib++) {
-		for (int w = tid; w < ib * 36; w += NT) {
-			const int jb = w / 36, rc = w - 36 * jb, c = rc / 6, r = rc - 6 * c;
-			double s = 0;
-			for (int k = jb; k < ib; k++) {
-				const double* Lb = B + idx(ib, k);
-				const double* Wb = B + idx(k, jb);               // rows < ib already hold W (diagonal blocks: W(k,k) = L_kk^-1)
-				for (int mm = 0; mm < 6; mm++) s += Lb[mm * 6 + r] * Wb[c * 6 + mm];
-			}
-			sRow[(size_t)jb * 36 + c * 6 + r] = s;
-		}
-		__syncthreads();
-		const double* Li = sLi + (size_t)ib * 36;
-		for (int w = tid; w < (ib + 1) * 36; w += NT) {
-			const int jb = w / 36, rc = w - 36 * jb, c = rc / 6, r = rc - 6 * c;
-			double v;
-			if (jb == ib) v = Li[c * 6 + r];
-			else {
-				double s = 0;
-				for (int k = 0; k <= r; k++) s += Li[k * 6 + r] * sRow[(size_t)jb * 36 + c * 6 + k];   // Li lower: Li(r,k), k <= r
-				v = -s;
-			}
-			B[idx(ib, jb) + c * 6 + r] = v;
-		}
-		__syncthreads();
-	}
-	// ---- phase 3: Ac^-1 = W^T W; block (ib,jb), ib >= jb: sum_{k >= ib} W(k,ib)^T W(k,jb) ----
-	for (int w = tid; w < nblkP * 36; w += NT) {
-		const int bq = w / 36, rc = w - 36 * bq, c = rc / 6, r = rc - 6 * c;
-		const int ib = s_ib[bq], jb = s_jb[bq];
-		double s = 0;
-		for (int k = ib; k < A; k++) {
-			const double* Wa = B + idx(k, ib);
-			const double* Wb = B + idx(k, jb);
-			for (int mm = 0; mm < 6; mm++) s += Wa[r * 6 + mm] * Wb[c * 6 + mm];
-		}
-		AcInv[(size_t)(ib * 6 + r) * nc + jb * 6 + c] = (float)s;
-		AcInv[(size_t)(jb * 6 + c) * nc + ib * 6 + r] = (float)s;
-	}
-	if (tid == 0 && info) *info = 0;
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// The same inversion for up to PCG4_MAXAGG aggregates: the packed triangle (74 aggregates: 2 775 blocks, 800 KB) is
-// spread over the shared memory of an 8-CTA thread-block cluster, block b in CTA b % 8 (distributed shared memory);
-// every CTA updates the blocks it owns and reads the others' through cluster.map_shared_rank.  cluster.sync() between
-// phases.  Same arithmetic and summation order as k_coarse_invert.
-// ------------------------------------------------------------------------------------------------------------------
-__global__ void __cluster_dims__(PCG4_CL, 1, 1) __launch_bounds__(1024, 1)
-k_coarse_chol_cluster(const double* __restrict__ AcP, int A, double* Lp, double* Ld, float* AcInv, int* info)
-{
-	namespace cgx = cooperative_groups;
-	cgx::cluster_group cluster = cgx::this_cluster();
-	extern __shared__ __align__(16) unsigned char smem_raw[];
-	const int nblkP = A * (A + 1) / 2, nc = 6 * A;
-	const int nloc = (nblkP + PCG4_CL - 1) / PCG4_CL;              // blocks per CTA
-	double* Bl = reinterpret_cast<double*>(smem_raw);              // [nloc][36] own blocks: local slot lb holds block lb * 8 + rank
-	double* sLiL = Bl + (size_t)nloc * 36;                         // [A][36] inverses of the diagonal factors (rank 0's copy is the one in use)
-	double* sScr = sLiL + (size_t)A * 36;                          // [A][36] scratch (phase 2), [36] scratch of the diagonal factorisation
-	unsigned char* s_ib = reinterpret_cast<unsigned char*>(sScr + (size_t)A * 36);   // [nblkP] packed index -> (ib, jb)
-	unsigned char* s_jb = s_ib + nblkP;
-	__shared__ int s_fail;
-	const int rank = (int)cluster.block_rank(), tid = threadIdx.x, NT = blockDim.x;
-	double* base[PCG4_CL];
-#pragma unroll
-	for (int r = 0; r < PCG4_CL; r++) base[r] = cluster.map_shared_rank(Bl, r);
-	double* sLi0 = cluster.map_shared_rank(sLiL, 0);
-	int* fail0 = cluster.map_shared_rank(&s_fail, 0);
-	auto blk = [&](int ib, int jb) -> double* { const int b = ib * (ib + 1) / 2 + jb; return base[b & (PCG4_CL - 1)] + (size_t)(b / PCG4_CL) * 36; };
-	for (int e = tid; e < nloc * 36; e += NT) {
-		const int b = (e / 36) * PCG4_CL + rank;
-		Bl[e] = b < nblkP ? AcP[(size_t)b * 36 + (e % 36)] : 0.0;
-	}
-	for (int ib = tid; ib < A; ib += NT) for (int jb = 0; jb <= ib; jb++) { s_ib[ib * (ib + 1) / 2 + jb] = (unsigned char)ib; s_jb[ib * (ib + 1) / 2 + jb] = (unsigned char)jb; }
-	if (tid == 0) s_fail = 0;
-	cluster.sync();
-	// ---- phase 1: block Cholesky.  Every CTA factors the (already final) diagonal block itself -- two cluster barriers per
-	//      block column instead of three, and the panel reads its own copy of L_kk^-1 ----
-	for (int kb = 0; kb < A; kb++) {
-		if (tid < 32) {
-			double* D = sScr;
-			const double* Dg = blk(kb, kb);                     // raw diagonal block: nobody writes it any more
-			for (int e = tid; e < 36; e += 32) D[e] = Dg[e];
-			__syncwarp();
-			const int r = tid;
-			for (int j = 0; j < 6; j++) {
-				const double d = D[j * 6 + j];
-				if (!(d > 0)) { if (r == 0) s_fail = 1; break; }
-				const double sq = sqrt(d);
-				__syncwarp();
-				if (r == j) D[j * 6 + j] = sq;
-				else if (r > j && r < 6) D[j * 6 + r] = D[j * 6 + r] / sq;
-				__syncwarp();
-				if (r > j && r < 6)
-					for (int c = j + 1; c <= r; c++) D[c * 6 + r] -= D[j * 6 + r] * D[j * 6 + c];
-				__syncwarp();
-			}
-			__syncwarp();
-			__shared__ double s_id[6];
-			if (r < 6) {
-				for (int c = r + 1; c < 6; c++) D[c * 6 + r] = 0.0;
-				s_id[r] = 1.0 / D[r * 6 + r];
-			}
-			__syncwarp();
-			if (r < 6) {
-				const int q = r;
-				double col[6];
-				for (int i = 0; i < 6; i++) col[i] = 0.0;
-				col[q] = s_id[q];
-				for (int i = q + 1; i < 6; i++) {
-					double sum = 0;
-					for (int k = q; k < i; k++) sum += D[k * 6 + i] * col[k];
-					col[i] = -sum * s_id[i];
-				}
-				for (int i = 0; i < 6; i++) sLiL[(size_t)kb * 36 + q * 6 + i] = col[i];
-			}
-			__syncwarp();
-			// the factor of the diagonal block goes straight to the output (its shared-memory copy stays raw)
-			if (rank == (((kb * (kb + 1)) / 2 + kb) & (PCG4_CL - 1))) for (int e = tid; e < 36; e += 32) Lp[((size_t)kb * (kb + 1) / 2 + kb) * 36 + e] = D[e];
-		}
-		__syncthreads();
-		if (s_fail) { *fail0 = 1; }                                // every CTA computes the same verdict; rank 0's flag is the shared one
-		// panel of the blocks this CTA owns
-		const double* Li = sLiL + (size_t)kb * 36;
-		if (!s_fail)
-		for (int w = tid; w < nloc * 6; w += NT) {            // panel: one thread per (own block, row)
-			const int lb = w / 6, r = w - 6 * lb, b = lb * PCG4_CL + rank;
-			if (b >= nblkP) continue;
-			const int ib = s_ib[b], jb = s_jb[b];
-			if (jb != kb || ib <= kb) continue;
-			double* X = Bl + (size_t)lb * 36;
-			double x[6], y[6];
-			for (int k = 0; k < 6; k++) x[k] = X[k * 6 + r];
-			for (int c = 0; c < 6; c++) { double sm = 0; for (int k = 0; k <= c; k++) sm += x[k] * Li[k * 6 + c]; y[c] = sm; }
-			for (int c = 0; c < 6; c++) X[c * 6 + r] = y[c];
-		}
-		cluster.sync();
-		if (*fail0) break;
-		for (int w = tid; w < nloc * 36; w += NT) {           // trailing: one thread per (own block, entry)
-			const int lb = w / 36, rc = w - 36 * lb, c = rc / 6, r = rc - 6 * c, b = lb * PCG4_CL + rank;
-			if (b >= nblkP) continue;
-			const int ib = s_ib[b], jb = s_jb[b];
-			if (jb <= kb) continue;                            // ib >= jb > kb
-			const double* P = blk(ib, kb);
-			const double* Q = blk(jb, kb);
-			double sm = 0;
-			for (int k = 0; k < 6; k++) sm += P[k * 6 + r] * Q[k * 6 + c];
-			Bl[(size_t)lb * 36 + rc] -= sm;
-		}
-		cluster.sync();
-	}
-	if (*fail0) {
-		for (int e = rank * NT + tid; e < nc * nc; e += PCG4_CL * NT) AcInv[e] = 0.f;
-		if (rank == 0 && tid == 0 && info) *info = 1;
-		cluster.sync();
-		return;
-	}
-	// ---- the factor L (packed, block b at Lp + 36 b) and the inverses of its diagonal blocks leave for k_coarse_trinv ----
-	for (int e = tid; e < nloc * 36; e += NT) {
-		const int b = (e / 36) * PCG4_CL + rank;
-		if (b < nblkP && s_ib[b] != s_jb[b]) Lp[(size_t)b * 36 + (e % 36)] = Bl[e];     // diagonal factors were written in phase 1
-	}
-	if (rank == 0) for (int e = tid; e < A * 36; e += NT) Ld[e] = sLiL[e];
-	if (rank == 0 && tid == 0 && info) *info = 0;
-	cluster.sync();                                            // nobody leaves while its shared memory may still be read
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// Second generation of the cluster Cholesky, for up to 148 aggregates (k_pcg5: one aggregate per CTA, ~9 poses): the packed
-// triangle (148 aggregates: 11 026 blocks, 3.2 MB) needs the shared memory of a 16-CTA cluster (non-portable size, allowed on
-// sm_90 with cudaFuncAttributeNonPortableClusterSizeAllowed), so everything but the blocks themselves had to leave shared memory: the inverses of the diagonal factors go straight
-// to global memory, the packed-index -> (ib, jb) map is kept only for the CTA's own blocks (2 bytes each).  Same arithmetic
-// and summation order as k_coarse_chol_cluster; CL = 8 or 16 CTAs per cluster, launched with cudaLaunchKernelEx.
-// ------------------------------------------------------------------------------------------------------------------
-constexpr int PCG5_MAXAGG = 148;
-
-template <int CL>
-__global__ void __launch_bounds__(1024, 1) k_coarse_chol_cluster2(const double* __restrict__ AcP, int A, double* Lp, double* Ld, float* AcInv, int* info)
-{
-	namespace cgx = cooperative_groups;
-	cgx::cluster_group cluster = cgx::this_cluster();
-	extern __shared__ __align__(16) unsigned char smem_raw[];
-	const int nblkP = A * (A + 1) / 2, nc = 6 * A;
-	const int nloc = (nblkP + CL - 1) / CL;                        // blocks per CTA
-	double* Bl = reinterpret_cast<double*>(smem_raw);              // [nloc][36] own blocks: local slot lb holds block lb * CL + rank
-	unsigned char* s_ib = reinterpret_cast<unsigned char*>(Bl + (size_t)nloc * 36);   // [nloc] (ib, jb) of the own blocks
-	unsigned char* s_jb = s_ib + nloc;
-	__shared__ int s_fail;
-	__shared__ double s_D[36], s_Li[36], s_id[6];
-	const int rank = (int)cluster.block_rank(), tid = threadIdx.x, NT = blockDim.x;
-	double* base[CL];
-#pragma unroll
-	for (int r = 0; r < CL; r++) base[r] = cluster.map_shared_rank(Bl, r);
-	int* fail0 = cluster.map_shared_rank(&s_fail, 0);
-	auto blk = [&](int ib, int jb) -> double* { const int b = ib * (ib + 1) / 2 + jb; return base[b % CL] + (size_t)(b / CL) * 36; };
-	for (int e = tid; e < nloc * 36; e += NT) {
-		const int b = (e / 36) * CL + rank;
-		Bl[e] = b < nblkP ? AcP[(size_t)b * 36 + (e % 36)] : 0.0;
-	}
-	for (int lb = tid; lb < nloc; lb += NT) {
-		const int b = lb * CL + rank;
-		int ib = (int)((sqrt(8.0 * b + 1.0) - 1.0) * 0.5);
-		while ((ib + 1) * (ib + 2) / 2 <= b) ib++;
-		while (ib * (ib + 1) / 2 > b) ib--;
-		s_ib[lb] = (unsigned char)(b < nblkP ? ib : 255); s_jb[lb] = (unsigned char)(b < nblkP ? b - ib * (ib + 1) / 2 : 255);
-	}
-	if (tid == 0) s_fail = 0;
-	cluster.sync();
-	for (int kb = 0; kb < A; kb++) {
-		if (tid < 32) {
-			// every CTA factors the (already final) diagonal block itself: 6x6 Cholesky (lane r owns row r), then L^-1 column by column
-			double* D = s_D;
-			const double* Dg = blk(kb, kb);
-			for (int e = tid; e < 36; e += 32) D[e] = Dg[e];
-			__syncwarp();
-			const int r = tid;
-			for (int j = 0; j < 6; j++) {
-				const double d = D[j * 6 + j];
-				if (!(d > 0)) { if (r == 0) s_fail = 1; break; }
-				const double sq = sqrt(d);
-				__syncwarp();
-				if (r == j) D[j * 6 + j] = sq;
-				else if (r > j && r < 6) D[j * 6 + r] = D[j * 6 + r] / sq;
-				__syncwarp();
-				if (r > j && r < 6)
-					for (int c = j + 1; c <= r; c++) D[c * 6 + r] -= D[j * 6 + r] * D[j * 6 + c];
-				__syncwarp();
-			}
-			__syncwarp();
-			if (r < 6) {
-				for (int c = r + 1; c < 6; c++) D[c * 6 + r] = 0.0;
-				s_id[r] = 1.0 / D[r * 6 + r];
-			}
-			__syncwarp();
-			if (r < 6) {
-				const int q = r;
-				double col[6];
-				for (int i = 0; i < 6; i++) col[i] = 0.0;
-				col[q] = s_id[q];
-				for (int i = q + 1; i < 6; i++) {
-					double sum = 0;
-					for (int k = q; k < i; k++) sum += D[k * 6 + i] * col[k];
-					col[i] = -sum * s_id[i];
-				}
-				for (int i = 0; i < 6; i++) s_Li[q * 6 + i] = col[i];
-			}
-			__syncwarp();
-			// the factor of the diagonal block and its inverse go straight to the outputs (the shared-memory copy stays raw)
-			if (rank == (((kb * (kb + 1)) / 2 + kb) % CL)) for (int e = tid; e < 36; e += 32) { Lp[((size_t)kb * (kb + 1) / 2 + kb) * 36 + e] = D[e]; Ld[(size_t)kb * 36 + e] = s_Li[e]; }
-		}
-		__syncthreads();
-		if (s_fail) { *fail0 = 1; }                                // every CTA computes the same verdict; rank 0's flag is the shared one
-		if (!s_fail)
-		for (int w = tid; w < nloc * 6; w += NT) {                 // panel: one thread per (own block, row)
-			const int lb = w / 6, r = w - 6 * lb;
-			const int ib = s_ib[lb], jb = s_jb[lb];
-			if (jb != kb || ib <= kb || ib == 255) continue;
-			double* X = Bl + (size_t)lb * 36;
-			double x[6], y[6];
-			for (int k = 0; k < 6; k++) x[k] = X[k * 6 + r];
-			for (int c = 0; c < 6; c++) { double sm = 0; for (int k = 0; k <= c; k++) sm += x[k] * s_Li[k * 6 + c]; y[c] = sm; }
-			for (int c = 0; c < 6; c++) X[c * 6 + r] = y[c];
-		}
-		cluster.sync();
-		if (*fail0) break;
-		for (int w = tid; w < nloc * 36; w += NT) {               // trailing: one thread per (own block, entry)
-			const int lb = w / 36, rc = w - 36 * lb, c = rc / 6, r = rc - 6 * c;
-			const int ib = s_ib[lb], jb = s_jb[lb];
-			if (jb <= kb || ib == 255) continue;                   // ib >= jb > kb
-			const double* P = blk(ib, kb);
-			const double* Q = blk(jb, kb);
-			double sm = 0;
-			for (int k = 0; k < 6; k++) sm += P[k * 6 + r] * Q[k * 6 + c];
-			Bl[(size_t)lb * 36 + rc] -= sm;
-		}
-		cluster.sync();
-	}
-	if (*fail0) {
-		for (int e = rank * NT + tid; e < nc * nc; e += CL * NT) AcInv[e] = 0.f;
-		if (rank == 0 && tid == 0 && info) *info = 1;
-		cluster.sync();
-		return;
-	}
-	// the off-diagonal blocks of the factor L (packed, block b at Lp + 36 b) leave for k_coarse_trinv
-	for (int e = tid; e < nloc * 36; e += NT) {
-		const int lb = e / 36, b = lb * CL + rank;
-		if (b < nblkP && s_ib[lb] != s_jb[lb]) Lp[(size_t)b * 36 + (e % 36)] = Bl[e];
-	}
-	if (rank == 0 && tid == 0 && info) *info = 0;
-	cluster.sync();                                            // nobody leaves while its shared memory may still be read
-}
-
-// W = L^-1 (block lower triangular), one CTA per block column jb: W(jb,jb) = L_jj^-1,
-// W(ib,jb) = -L_ii^-1 sum_{k=jb}^{ib-1} L(ib,k) W(k,jb).  The columns are independent; a column is sequential in ib.
-constexpr int PCG4_KS = 7;      // k-slices of the inner sum (36 entries x 7 slices = 252 threads)
-__global__ void __launch_bounds__(256) k_coarse_trinv(const double* __restrict__ Lp, const double* __restrict__ Ld, int A, double* Wp, const int* __restrict__ info)
-{
-	extern __shared__ __align__(16) unsigned char smem_raw[];
-	double* Wcol = reinterpret_cast<double*>(smem_raw);          // [A][36] this column of W (rows < jb unused)
-	__shared__ double s_part[PCG4_KS][36], s_S[36];
-	if (*info != 0) return;
-	const int jb = blockIdx.x, tid = threadIdx.x;
-	const int e = tid % 36, sl = tid / 36, c = e / 6, r = e - 6 * c;
-	auto pidx = [](int ib, int kb) { return (size_t)(ib * (ib + 1) / 2 + kb) * 36; };
-	if (tid < 36) { const double v = Ld[(size_t)jb * 36 + tid]; Wcol[(size_t)jb * 36 + tid] = v; Wp[pidx(jb, jb) + tid] = v; }
-	__syncthreads();
-	for (int ib = jb + 1; ib < A; ib++) {
-		if (sl < PCG4_KS) {
-			double sm = 0;
-			for (int k = jb + sl; k < ib; k += PCG4_KS) {
-				const double* Lb = Lp + pidx(ib, k);
-				const double* Wb = Wcol + (size_t)k * 36;
-#pragma unroll
-				for (int mm = 0; mm < 6; mm++) sm += Lb[mm * 6 + r] * Wb[c * 6 + mm];
-			}
-			s_part[sl][e] = sm;
-		}
-		__syncthreads();
-		if (tid < 36) {
-			double sm = 0;
-#pragma unroll
-			for (int q = 0; q < PCG4_KS; q++) sm += s_part[q][tid];
-			s_S[tid] = sm;
-		}
-		__syncthreads();
-		if (tid < 36) {
-			const double* Li = Ld + (size_t)ib * 36;
-			double sm = 0;
-			for (int k = 0; k <= r; k++) sm += Li[k * 6 + r] * s_S[c * 6 + k];
-			Wcol[(size_t)ib * 36 + tid] = -sm;
-			Wp[pidx(ib, jb) + tid] = -sm;
-		}
-		__syncthreads();
-	}
-}
-
-// Ac^-1 = W^T W: one thread per entry of the lower block triangle, written to both triangles of the full fp32 matrix
-__global__ void k_coarse_wtw(const double* __restrict__ Wp, int A, float* AcInv, const int* __restrict__ info)
-{
-	const int w = blockIdx.x * blockDim.x + threadIdx.x;
-	const int nblkP = A * (A + 1) / 2, nc = 6 * A;
-	if (w >= nblkP * 36 || *info != 0) return;
-	const int bq = w / 36, rc = w - 36 * bq, c = rc / 6, r = rc - 6 * c;
-	int ib = (int)((sqrt(8.0 * bq + 1.0) - 1.0) * 0.5);
-	while ((ib + 1) * (ib + 2) / 2 <= bq) ib++;
-	while (ib * (ib + 1) / 2 > bq) ib--;
-	const int jb = bq - ib * (ib + 1) / 2;
-	double s0 = 0, s1 = 0;
-	int k = ib;
-	for (; k + 1 < A; k += 2) {
-		const double* Wa = Wp + (size_t)(k * (k + 1) / 2 + ib) * 36, *Wb = Wp + (size_t)(k * (k + 1) / 2 + jb) * 36;
-		const double* Wa1 = Wp + (size_t)((k + 1) * (k + 2) / 2 + ib) * 36, *Wb1 = Wp + (size_t)((k + 1) * (k + 2) / 2 + jb) * 36;
-#pragma unroll
-		for (int mm = 0; mm < 6; mm++) { s0 += Wa[r * 6 + mm] * Wb[c * 6 + mm]; s1 += Wa1[r * 6 + mm] * Wb1[c * 6 + mm]; }
-	}
-	if (k < A) {
-		const double* Wa = Wp + (size_t)(k * (k + 1) / 2 + ib) * 36, *Wb = Wp + (size_t)(k * (k + 1) / 2 + jb) * 36;
-#pragma unroll
-		for (int mm = 0; mm < 6; mm++) s0 += Wa[r * 6 + mm] * Wb[c * 6 + mm];
-	}
-	const float v = (float)(s0 + s1);
-	AcInv[(size_t)(ib * 6 + r) * nc + jb * 6 + c] = v;
-	AcInv[(size_t)(jb * 6 + c) * nc + ib * 6 + r] = v;
 }
 
 }  // namespace cuba_b200

@@ -40,6 +40,7 @@ constexpr int PCG5_REPL = 8;                       // replicas of the partial / 
 constexpr int PCG5_MAXWORLD = 8;
 constexpr int PCG5_PCH = 8;                        // polled words in flight per thread
 constexpr int PCG5_TPR = 16;                       // threads per row of the coarse slice product
+constexpr int PCG5_MAXAGG = 148;                   // aggregates of a k_pcg5 plan (build_pcg5_plan's maxAgg) unless cfg.reserved[6] asks for fewer
 
 // device-resident solve bookkeeping: read by every CTA at its start, changed only BETWEEN solves by k_pcg5_commit
 struct Pcg5Ctl { unsigned int tagBase; unsigned int solve; int abort; int nbad; unsigned int advance; int pad[3]; };

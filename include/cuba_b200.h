@@ -347,11 +347,11 @@ int cuba_debug_get_delta(cuba_engine* e, double* xp /*6*numP*/, double* xl /*3*n
 #define CUBA_PCG_KERNEL_PCG5_BIG 6        /* k_pcg5<T, true> */
 #define CUBA_PCG_KERNEL_PCG5T 7           /* k_pcg5t<T, K>, K = info[2] */
 #define CUBA_COARSE_KERNEL_NONE 0
-#define CUBA_COARSE_KERNEL_INVERT 1       /* k_coarse_invert: one CTA */
-#define CUBA_COARSE_KERNEL_CLUSTER8 2     /* k_coarse_chol_cluster2<8> */
-#define CUBA_COARSE_KERNEL_CLUSTER16 3    /* k_coarse_chol_cluster2<16> */
-#define CUBA_COARSE_KERNEL_DENSE 4        /* cdense::k_coarse_dense: the whole chip */
-#define CUBA_COARSE_KERNEL_PCG4_CLUSTER 5 /* k_coarse_chol_cluster of k_pcg4 */
+#define CUBA_COARSE_KERNEL_INVERT 1       /* k_coarse_invert: one CTA, A <= 37 */
+#define CUBA_COARSE_KERNEL_CLUSTER8 2     /* the retired k_coarse_chol_cluster2<8>: never reported, the number stays taken */
+#define CUBA_COARSE_KERNEL_CLUSTER16 3    /* the retired k_coarse_chol_cluster2<16>: never reported, the number stays taken */
+#define CUBA_COARSE_KERNEL_DENSE 4        /* cdense::k_coarse_dense: the whole chip, A > 37 */
+#define CUBA_COARSE_KERNEL_PCG4_CLUSTER 5 /* the retired k_coarse_chol_cluster of k_pcg4: never reported, the number stays taken */
 int cuba_debug_get_pcg_info(cuba_engine* e, int32_t* info, double* coarse_lambda);
 /* The coarse level of k_pcg5 as the last two-level solve applied it: aggRow[numP] the aggregate of every free pose, AcP the packed
  * lower block triangle of Ac = Z^T S Z (block (ib >= jb) at (ib (ib+1)/2 + jb) * 36, column-major 6x6; 36 A (A+1)/2 doubles) and

@@ -1,4 +1,4 @@
-"""k_coarse_dense (csrc/cuba_coarse_dense.cuh), the dense coarse inverse of the two-level PCG, on matrices of our own through
+"""k_coarse_dense (csrc/cuba_coarse.cuh), the dense coarse inverse of the two-level PCG, on matrices of our own through
 cuba_debug_coarse_inverse: the fp32 inverse against fp64, bit-reproducibility and the not-positive-definite path, which a solve
 never takes (block-Jacobi alone carries on, silently).
 

@@ -558,13 +558,19 @@ def test_jh4_and_first_generation_agree(pkg, oracle, problems, name):
 @pytest.mark.parametrize("name", ["kitti07_shaped", "kitti00_shaped"])
 def test_two_level_pcg_converges_faster_to_the_same_solution(pkg, problems, name, two_level):
     """k_pcg4 (block-Jacobi + rigid-aggregate coarse correction) vs k_pcg3 (block-Jacobi) on the same reduced system at a low
-    damping: same solution to the CG tolerance, several times fewer iterations"""
+    damping: same solution to the CG tolerance, several times fewer iterations.  Both two-level solvers invert the coarse matrix
+    the same way: in one CTA on kitti07_shaped (31 CTAs, so 31 aggregates), on the whole chip on kitti00_shaped (k_pcg4: 66,
+    k_pcg5t: 132 aggregates)."""
     prob = problems(name); rk = KERNELS["huber"]
     a = make_engine(pkg, prob, rk, pcg_variant=two_level); b = make_engine(pkg, prob, rk, pcg_variant=4)
     a.linearize(); b.linearize()
     lam = 1e-8 * a.max_diagonal()
     ia, oka = a.solve(lam); ib, okb = b.solve(lam)
     assert oka and okb
+    info = a.pcg_info()
+    want_coarse = {"kitti07_shaped": "k_coarse_invert", "kitti00_shaped": "k_coarse_dense"}[name]
+    assert info["kernel"] == ("k_pcg4" if two_level == 3 else "k_pcg5t") and info["two_level"], info
+    assert info["coarse_kernel"] == want_coarse, info
     for nme, x, y in zip(("xp", "xl"), a.delta(), b.delta()):
         assert relerr(x, y) < 1e-7, (nme, ia, ib, relerr(x, y))
     assert ia * 1.5 < ib, (ia, ib)

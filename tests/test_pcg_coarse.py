@@ -217,14 +217,13 @@ def _oracle_ladder(oracle, prob, name):
 
 # The plan sizes follow from the 132 SMs of an H100; `plan` holds what that GPU gives.  Each case checks it, so that a case that
 # drifts to another path fails instead of testing something else.  nc = 6A is a multiple of 16 (k_coarse_dense's tile) in
-# k00_two_per_cta (1584) and not in k00_dense / k00_legacy / r11k_* (792, padded) or k07_three_per_cta (558).
+# k00_two_per_cta (1584) and not in k00_gs2 (396), k00_dense / k00_legacy / r11k_* (792, padded) or k07_three_per_cta (558).
 PATH_CASES = {
     # id: (graph, Engine kwargs, environment, kernel, coarse kernel, plan)
     "k07_invert": ("kitti07_shaped", {}, {}, "k_pcg5t", "k_coarse_invert", dict(aggs_per_cta=1, G=31, gs=1, A=31)),
     "k00_span_ctas": ("kitti00_shaped", dict(max_aggregates=37), {}, "k_pcg5t", "k_coarse_invert", dict(aggs_per_cta=1, G=132, gs=4, A=33)),
     "k00_dense": ("kitti00_shaped", {}, {}, "k_pcg5t", "k_coarse_dense", dict(aggs_per_cta=1, G=132, gs=1, A=132)),
-    "k00_cluster8": ("kitti00_shaped", dict(max_aggregates=66), {"CUBA_COARSE_CLUSTER": "1"}, "k_pcg5t", "cluster2<8>", dict(aggs_per_cta=1, G=132, gs=2, A=66)),
-    "k00_cluster16": ("kitti00_shaped", {}, {"CUBA_COARSE_CLUSTER": "1"}, "k_pcg5t", "cluster2<16>", dict(aggs_per_cta=1, G=132, gs=1, A=132)),
+    "k00_gs2": ("kitti00_shaped", dict(max_aggregates=66), {}, "k_pcg5t", "k_coarse_dense", dict(aggs_per_cta=1, G=132, gs=2, A=66)),
     "k00_two_per_cta": ("kitti00_shaped", {}, {"CUBA_PCG5_AGGS_PER_CTA": "2"}, "k_pcg5t", "k_coarse_dense", dict(aggs_per_cta=2, G=132, gs=1, A=264)),
     "k07_three_per_cta": ("kitti07_shaped", {}, {"CUBA_PCG5_AGGS_PER_CTA": "3"}, "k_pcg5t", "k_coarse_dense", dict(aggs_per_cta=3, G=31, gs=1, A=93)),
     "k00_legacy": ("kitti00_shaped", {}, {"CUBA_PCG5_LEGACY": "1"}, "k_pcg5", "k_coarse_dense", dict(G=132, gs=1, A=132)),
@@ -239,16 +238,16 @@ def test_pcg5_coarse_level_on_every_path(pkg, oracle, problems, monkeypatch, cas
     """a. the kernel and the coarse-inverse kernel the case names ran;  b. Ac = Z^T S Z;  c. the fp32 inverse against fp64;
     d. x against the direct solve, no breakdown;  e. the iteration count against restated_pcg5 fed the engine's own inverse.
 
-    Measured on one H100 80GB HBM3 (400 W limit), all ten cases x three dampings:
+    Measured on one H100 80GB HBM3 (700 W limit), all nine cases x three dampings:
       b. Ac against Z^T S Z from the engine's own Schur complement <= 1.4e-14, from the oracle's <= 3.1e-12 (rows_11k, lambda 0.1);
-      c. Ac^-1 against the fp64 inverse <= 5.2e-8 of its largest entry.  |AcInv Ac - I|_max reaches 6.5 on kitti00_shaped and
-         1.1e3 on rows_11k at lambda 0.1: Ac is that ill-conditioned (about 1e11 on kitti00_shaped; the rigid-motion basis
+      c. Ac^-1 against the fp64 inverse <= 5.2e-8 of its largest entry.  |AcInv Ac - I|_max reaches 7.3 on kitti00_shaped and
+         about 1e3 on rows_11k at lambda 0.1: Ac is that ill-conditioned (about 1e11 on kitti00_shaped; the rigid-motion basis
          carries translations of kilometres), and the same residual follows from rounding the fp64 inverse once to fp32.  The
          check is therefore against that floor: measured 0.90 .. 1.00 times it, bound INV_RESIDUAL_FACTOR;
-      d. the solution is as close to the direct solve as the restatement's (within 2 % everywhere);
-      e. the kernel's iteration count equals the restatement's in all 30 solves (18 .. 590 iterations).  count_bound allows
-         max(3, 3 %); the broken coarse levels of test_restatement_sees_a_broken_coarse_level move the count by 9 and 112.
-    The ten cases take about 70 s, most of it the CPU restatement on rows_11k (590 iterations on 10.7 M non-zeros).
+      d. the solution is as close to the direct solve as the restatement's (within a few per cent everywhere);
+      e. the kernel's iteration count is within one of the restatement's in all 27 solves (18 .. 589 iterations).  count_bound
+         allows max(3, 3 %); the broken coarse levels of test_restatement_sees_a_broken_coarse_level move the count by 9 and 112.
+    The nine cases take about 80 s, most of it the CPU restatement on rows_11k (590 iterations on 10.7 M non-zeros).
     """
     name, kw, env, want_kernel, want_coarse, want_plan = PATH_CASES[case]
     for k, v in env.items():
