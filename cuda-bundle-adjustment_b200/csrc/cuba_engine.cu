@@ -700,7 +700,7 @@ struct Engine : EngineBase {
 		// 5. block products keyed by destination block, + one dummy per diagonal
 		CUDA_TRY(g_cnt.alloc((size_t)nhpl + 1)); CUDA_TRY(g_off.alloc((size_t)nhpl + 1));
 		CUDA_TRY(cudaMemsetAsync(g_cnt.p, 0, sizeof(int) * ((size_t)nhpl + 1), stream));
-		KLAUNCH(k_prod_count, nhpl, g_hplLmG.p, g_hplColPtr.p, nhpl, g_cnt.p);
+		KLAUNCH(k_prod_count, nhpl, g_hplLmG.p, g_hplColPtr.p, g_hplRowInd.p, nhpl, g_cnt.p, g_meta.p);
 		rc = exclusiveSum(g_cnt.p, g_off.p, nhpl + 1); if (rc) return rc;
 		long long nmul = 0;
 		{
@@ -730,6 +730,7 @@ struct Engine : EngineBase {
 		tmark("sync 3");
 		const int nblk = hMeta->nblk;
 		S.nblk = nblk;
+		S.repeatedPairs = hMeta->repeats != 0;
 		CUDA_TRY(blkRow.alloc(nblk)); CUDA_TRY(blkCol.alloc(nblk)); CUDA_TRY(prodPtr.alloc((size_t)nblk + 1));
 		CUDA_TRY(prodI.alloc((size_t)N)); CUDA_TRY(prodJ.alloc((size_t)N));
 		KLAUNCH(k_blocks, N + 1, g_pkeyS.p, g_pvalS.p, g_head.p, g_blkId.p, g_pi.p, g_pj.p, (int)N, blkRow.p, blkCol.p, prodPtr.p, prodI.p, prodJ.p);
@@ -803,10 +804,11 @@ struct Engine : EngineBase {
 		// Schur kernel: 0 / 3 = k_schur3 (destination-sorted products, six lanes per product; default), 5 = landmark tiles on the fp64
 		// tensor pipe (k_schur_tiles_mma + k_schur_reduce, cuba_schur5.cuh: 12 % faster on the banded 5 M-edge graph, on par on
 		// kitti00_shaped, 2x slower on the real ba_kitti_00 whose loop closures leave 4.4 products per (tile, destination) segment ->
-		// opt-in).  A request for 5 that schur5 cannot serve (host-built structure, fp32 or mixed precision, no products on this rank)
+		// opt-in).  A request for 5 that schur5 cannot serve (host-built structure, fp32 or mixed precision, no products on this rank,
+		// a repeated (pose, landmark) pair anywhere in the graph: its bsc term rides on every product of a diagonal destination)
 		// runs k_schur3.  upperReduce depends on the request only, so that every rank of a sharded run joins the same collective.
 		const bool schur5Asked = cfg.reserved[3] == 5 && cfg.reserved[1] != 1 && cfg.use_fp32 != 2 && sizeof(T) == 8;
-		useSchur5 = schur5Asked && S.numP > 0 && S.numL > 0 && ntiles > 0 && S.eLocal > 0 && S.nmulLocal > 0;
+		useSchur5 = schur5Asked && S.numP > 0 && S.numL > 0 && ntiles > 0 && S.eLocal > 0 && S.nmulLocal > 0 && !S.repeatedPairs;
 		upperReduce = world > 1 && !schur5Asked && S.numP > 0 && S.numL > 0;
 		if (upperReduce) {
 			uCount = 36 * (size_t)S.nblk + 6 * nP;
@@ -2764,7 +2766,8 @@ int cuba_debug_build_structure_host(const cuba_problem* p, int rank, int world, 
 	cp(hplColPtr, S.hplColPtr); cp(hplRowInd, S.hplRowInd); cp(edge2Hpl, S.edge2Hpl);
 	cp(hscRowPtr, S.hscRowPtr); cp(hscColInd, S.hscColInd); cp(fullRowPtr, S.fRowPtr); cp(fullColInd, S.fColInd);
 	if (shard) { shard[0] = S.lmBeg; shard[1] = S.lmEnd; shard[2] = S.eLocal; shard[3] = (int32_t)S.nmulLocal; }
-	// internal consistency (cheap): tiles cover the shard, products reference blocks of one landmark with row(i)<=row(j)
+	// internal consistency (cheap): tiles cover the shard, products reference blocks of one landmark with row(i)<=row(j), and
+	// with i<=j except between two blocks of one pose
 	if ((int)S.tileLm.size() < 1 || S.tileLm.front() != S.lmBeg || S.tileLm.back() != S.lmEnd) return fail(CUBA_ERR_INVALID, "structure self-check: tiles");
 	for (size_t t = 0; t + 1 < S.tileLm.size(); t++) {
 		const int nl = S.tileLm[t + 1] - S.tileLm[t];
@@ -2774,7 +2777,9 @@ int cuba_debug_build_structure_host(const cuba_problem* p, int rank, int world, 
 	for (int k = 0; k < S.nblk; k++)
 		for (int n = S.prodPtr[k]; n < S.prodPtr[k + 1]; n++) {
 			const int i = S.prodI[n] + S.hplBase, j = S.prodJ[n] + S.hplBase;
-			if (S.hplRowInd[i] != S.blkRow[k] || S.hplRowInd[j] != S.blkCol[k] || S.hplLm[S.prodI[n]] != S.hplLm[S.prodJ[n]] || i > j)
+			// i > j only between two blocks of one pose (a repeated pair), on its diagonal destination
+			if (S.hplRowInd[i] != S.blkRow[k] || S.hplRowInd[j] != S.blkCol[k] || S.hplLm[S.prodI[n]] != S.hplLm[S.prodJ[n]] ||
+				(i > j && S.blkRow[k] != S.blkCol[k]))
 				return fail(CUBA_ERR_INVALID, "structure self-check: product list");
 		}
 	return CUBA_OK;

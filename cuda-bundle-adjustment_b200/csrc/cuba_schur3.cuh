@@ -8,7 +8,8 @@
 // Here lane = (product slot s = lane / 6, row r = lane % 6): a lane owns one row of the 6x6 product (6 + 1
 // accumulators), the landmark of a product comes with the product list (no dependent lookup), the indices of
 // the next step are fetched while the current one is computed, and five products are in flight per warp step.
-//   Hsc(a,b) = [a==b](Hpp_a + lambda I) - sum_products (Hpl_i invHll_l) Hpl_j^T      bsc(a) = bp_a - sum (Hpl_i invHll_l) bl_l
+//   Hsc(a,b) = [a==b](Hpp_a + lambda I) - sum_products (Hpl_i invHll_l) Hpl_j^T      bsc(a) = bp_a - sum_{products i==j} (Hpl_i invHll_l) bl_l
+// (i == j on every product of a diagonal destination unless the pose observes the landmark through more than one edge)
 #pragma once
 
 #include "cuba_kernels.cuh"
@@ -79,7 +80,7 @@ __global__ void __launch_bounds__(WARPS * 32, 3) k_schur3(const Args<T, TH> a)
 			const T w2 = a0 * i2 + a1 * i4 + a2 * i5;
 #pragma unroll
 			for (int c = 0; c < 6; c++) C[c] += w0 * B[c] + w1 * B[6 + c] + w2 * B[12 + c];
-			if (diag) {
+			if (ci == cj) {         // bsc takes Hpl_i invHll bl once per block: not from the (i, j) pairs of a repeated pair
 				const T* b3 = a.bl + 3 * (size_t)cl;
 				vr += w0 * __ldg(b3) + w1 * __ldg(b3 + 1) + w2 * __ldg(b3 + 2);
 			}

@@ -261,7 +261,8 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_schur_tiles_mma(const Args a)
 		unsigned int nxt = 0;
 		if (s + WARPS < s1 && lane < recN.y) nxt = __ldg(a.off + recN.x + lane);
 		const bool diag = (rec.w & 1) != 0;
-		// column 6 of the B fragment carries u on diagonal destinations (there the product pairs a block with itself)
+		// column 6 of the B fragment carries u on diagonal destinations (there the product pairs a block with itself: the engine
+		// runs k_schur3 instead on a graph with a repeated (pose, landmark) pair, whose diagonal destinations also pair two blocks)
 		const bool useU = diag && g == 6 && q < 3;
 		const double* bBase = inAB ? sm.V + fo : (useU ? sm.V + 18 + q : sm.zero);
 		const int bMul = (inAB || useU) ? 1 : 0;

@@ -128,10 +128,19 @@ bool build_structure(int Pall, int numP, int Lall, int numL, int E2, const int32
 		std::vector<int> fill(rowPtrH.begin(), rowPtrH.end() - 1);
 		for (int h = 0; h < S.nhpl; h++) rowList[fill[S.hplRowInd[h]]++] = h;
 	}
+	// Block i of landmark l emits the products (i, j) with j from first(i) to the end of l's column.  first(i) = i unless the pose
+	// observes l through more than one edge (a repeated pair, e.g. a mono and a stereo edge): then the column holds several blocks
+	// of that pose next to each other, and the diagonal destination needs every ordered pair of them -- first(i) is the first.
+	auto first = [&](int i) {
+		int j = i;
+		while (j > S.hplColPtr[hplLmG[i]] && S.hplRowInd[j - 1] == S.hplRowInd[i]) j--;
+		return j;
+	};
 	std::vector<int> mark(numP, 0), cntLoc(numP, 0), touched;
 	std::vector<int> prodCount;
 	S.hscRowPtr.assign(numP + 1, 0);
 	S.nmul = 0; S.nmulLocal = 0;
+	S.repeatedPairs = false;
 	for (int a = 0; a < numP; a++) {
 		touched.clear();
 		touched.push_back(a); mark[a] = 1;     // the diagonal block always exists
@@ -140,12 +149,14 @@ bool build_structure(int Pall, int numP, int Lall, int numL, int E2, const int32
 			const int l = hplLmG[i];
 			const bool local = l >= S.lmBeg && l < S.lmEnd;
 			const int cend = S.hplColPtr[l + 1];
-			for (int j = i; j < cend; j++) {
+			const int j0 = first(i);
+			if (j0 < i) S.repeatedPairs = true;
+			for (int j = j0; j < cend; j++) {
 				const int b = S.hplRowInd[j];
 				if (!mark[b]) { mark[b] = 1; touched.push_back(b); }
 				if (local) cntLoc[b]++;
 			}
-			S.nmul += cend - i;
+			S.nmul += cend - j0;
 		}
 		std::sort(touched.begin(), touched.end());
 		for (int b : touched) {
@@ -171,7 +182,7 @@ bool build_structure(int Pall, int numP, int Lall, int numL, int E2, const int32
 				const int l = hplLmG[i];
 				if (l < S.lmBeg || l >= S.lmEnd) continue;
 				const int cend = S.hplColPtr[l + 1];
-				for (int j = i; j < cend; j++) {
+				for (int j = first(i); j < cend; j++) {
 					const int pos = off[S.hplRowInd[j]]++;
 					S.prodI[pos] = i - S.hplBase;
 					S.prodJ[pos] = j - S.hplBase;

@@ -28,6 +28,7 @@ struct Structure {
 	int hplBase = 0;       // first global Hpl index of the shard
 	int nhplLocal = 0;
 	long long nmulLocal = 0;
+	bool repeatedPairs = false;   // some free pose observes some free landmark through more than one edge
 
 	// global structures (bit-exact contract with the reference)
 	std::vector<int> hplColPtr;   // [numL+1]
@@ -53,7 +54,8 @@ struct Structure {
 	// destination-sorted product list of the shard's landmarks
 	std::vector<int> blkRow, blkCol;   // [nblk]
 	std::vector<int> prodPtr;          // [nblk+1]
-	std::vector<int> prodI, prodJ;     // [nmulLocal] LOCAL Hpl indices, row(prodI) <= row(prodJ)
+	std::vector<int> prodI, prodJ;     // [nmulLocal] LOCAL Hpl indices, row(prodI) <= row(prodJ); on a diagonal destination
+	                                   // every ordered pair of the pose's blocks of one landmark (both (i, j) and (j, i))
 
 	// symmetric-full BSR
 	std::vector<int> fRowPtr;     // [numP+1]

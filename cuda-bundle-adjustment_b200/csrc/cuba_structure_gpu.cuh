@@ -28,6 +28,7 @@ struct Meta {            // small device->host record, one copy per sync point
 	int nblk;
 	int npe;             // pose-major entries
 	int bounds[9];       // first landmark of every rank's shard (world <= 8), bounds[world] = Lall
+	int repeats;         // 1: some free pose observes some free landmark through more than one edge
 };
 
 // (iL, iP) sort keys of the user-order edges; validates the indices.
@@ -197,15 +198,28 @@ __global__ void k_pose_stream(const int* __restrict__ src, const int* __restrict
 	pmx[k] = mx[e]; pmy[k] = my[e]; pmz[k] = mz[e]; pom[k] = om[e];
 }
 
-// number of block products emitted by Hpl block i: its column partners j >= i
-__global__ void k_prod_count(const int* __restrict__ hplLmG, const int* __restrict__ hplColPtr, int nhpl, int* cnt)
+// first column partner of Hpl block i: i itself, or -- when its pose observes the landmark through more than one edge (a
+// repeated pair) -- the first of that pose's blocks in the column, so that the diagonal destination gets every ordered pair
+__device__ __forceinline__ int first_partner(const int* __restrict__ hplRowInd, int colBeg, int i)
+{
+	int j = i;
+	while (j > colBeg && hplRowInd[j - 1] == hplRowInd[i]) j--;
+	return j;
+}
+
+// number of block products emitted by Hpl block i: its column partners j >= first_partner(i)
+__global__ void k_prod_count(const int* __restrict__ hplLmG, const int* __restrict__ hplColPtr, const int* __restrict__ hplRowInd, int nhpl,
+	int* cnt, Meta* meta)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= nhpl) return;
-	cnt[i] = hplColPtr[hplLmG[i] + 1] - i;
+	const int l = hplLmG[i];
+	const int j0 = first_partner(hplRowInd, hplColPtr[l], i);
+	if (j0 < i) meta->repeats = 1;
+	cnt[i] = hplColPtr[l + 1] - j0;
 }
 
-// products (i,j), i<=j in one landmark column, keyed by destination block (row_i,row_j); products of foreign
+// products (i,j), j >= first_partner(i) in one landmark column, keyed by destination block (row_i,row_j); products of foreign
 // landmarks (other ranks) keep their key (global pattern) but are marked pi = -1
 __global__ void k_prod_emit(const int* __restrict__ hplLmG, const int* __restrict__ hplColPtr, const int* __restrict__ hplRowInd,
 	const int* __restrict__ off, int nhpl, int lmBeg, int lmEnd, int hplBase, unsigned long long* pkey, int* pval, int* pi, int* pj)
@@ -217,7 +231,7 @@ __global__ void k_prod_emit(const int* __restrict__ hplLmG, const int* __restric
 	const bool local = l >= lmBeg && l < lmEnd;
 	const unsigned long long hi = (unsigned long long)(unsigned)hplRowInd[i] << 32;
 	int n = off[i];
-	for (int j = i; j < cend; j++, n++) {
+	for (int j = first_partner(hplRowInd, hplColPtr[l], i); j < cend; j++, n++) {
 		pkey[n] = hi | (unsigned)hplRowInd[j];
 		pval[n] = n;
 		pi[n] = local ? i - hplBase : -1;

@@ -89,7 +89,8 @@ typedef struct cuba_config {
 	                          reserved[2]: J+H landmark kernel, 0 = k_linearize_landmark4 (warp tiles, default; 8/9 = 5/6 CTAs per SM,
 	                          7 = three pipeline stages), 1-4 = first generation (tile shapes; the fp32 engine's kernel)
 	                          reserved[3]: Schur kernel, 0 / 3 = k_schur3 (six lanes per product, default), 5 = landmark tiles on the
-	                          fp64 tensor pipe (cuba_schur5.cuh, DMMA m8n8k4; wins only on banded graphs; k_schur3 where it cannot run)
+	                          fp64 tensor pipe (cuba_schur5.cuh, DMMA m8n8k4; wins only on banded graphs; k_schur3 where it cannot run:
+	                          fp32 or mixed precision, host-built structures, and a graph with a repeated (pose, landmark) pair)
 	                          reserved[0], [2] and [3] accept only the values listed: cuba_engine_create returns CUBA_ERR_INVALID
 	                          for any other, before it touches a device
 	                          reserved[4]: two-level PCG: solves between rebuilds of the coarse matrix (<=0: 8)

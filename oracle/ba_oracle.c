@@ -216,6 +216,16 @@ static void build_hpl_structure(bao* h)
 	free(cntP); free(byP); free(fill);
 }
 
+/* First column partner of Hpl block i of landmark l: i, or -- when its pose observes l through more than one edge (a repeated
+ * pair, which g2o sums and so does the engine; the reference pairs only i <= j and leaves Hsc(a,a) without W_j Hpl_i^T) -- the
+ * first of that pose's blocks in the column (the column is sorted by pose). */
+static int first_partner(const bao* h, int l, int i)
+{
+	int j = i;
+	while (j > h->hplColPtr[l] && h->hplRowInd[j - 1] == h->hplRowInd[i]) j--;
+	return j;
+}
+
 /* Upper-triangular BSR pattern of Hsc from landmark co-visibility:
  * sparse_block_matrix.cpp:55-133 (constructFromVertices), columns ascending per row. */
 static void build_hsc_structure(bao* h)
@@ -223,10 +233,8 @@ static void build_hsc_structure(bao* h)
 	const int numP = h->numP, numL = h->numL;
 	/* count products and collect (row,col) pairs */
 	long nmul = 0;
-	for (int l = 0; l < numL; l++) {
-		const long d = h->hplColPtr[l + 1] - h->hplColPtr[l];
-		nmul += d * (d + 1) / 2;
-	}
+	for (int l = 0; l < numL; l++)
+		for (int i = h->hplColPtr[l]; i < h->hplColPtr[l + 1]; i++) nmul += h->hplColPtr[l + 1] - first_partner(h, l, i);
 	h->nmul = (int)nmul;
 	/* + one (p,p) key per free pose: the reference only gets a diagonal block when the pose has a
 	 * free-free edge (and then mis-addresses Hpp otherwise, cu:955-962); we always keep the diagonal. */
@@ -236,7 +244,7 @@ static void build_hsc_structure(bao* h)
 	for (int p = 0; p < numP; p++) keys[m++] = ((int64_t)p << 32) | (uint32_t)p;
 	for (int l = 0; l < numL; l++)
 		for (int i = h->hplColPtr[l]; i < h->hplColPtr[l + 1]; i++)
-			for (int j = i; j < h->hplColPtr[l + 1]; j++)
+			for (int j = first_partner(h, l, i); j < h->hplColPtr[l + 1]; j++)
 				keys[m++] = ((int64_t)h->hplRowInd[i] << 32) | (uint32_t)h->hplRowInd[j];
 	/* radix-free: sort 64-bit keys with two counting passes (col then row) */
 	int64_t* tmp = (int64_t*)malloc(sizeof(int64_t) * (nmul > 0 ? nmul : 1));
@@ -647,9 +655,9 @@ int bao_solve(bao* h, double lambda)
 				const int rowi = h->hplRowInd[i];
 				double* bs = h->bsc + 6 * (size_t)rowi;
 				for (int r = 0; r < 6; r++) { double s = 0; for (int k = 0; k < 3; k++) s += W[k * 6 + r] * bl[k]; bs[r] -= s; }
-				/* cu:964-1000: Hsc(row_i,row_j) -= W_i * Hpl_j^T for i <= j */
+				/* cu:964-1000: Hsc(row_i,row_j) -= W_i * Hpl_j^T for i <= j, and for j < i on the same pose (first_partner) */
 				int k = h->hscRowPtr[rowi];
-				for (int j = i; j < h->hplColPtr[l + 1]; j++) {
+				for (int j = first_partner(h, l, i); j < h->hplColPtr[l + 1]; j++) {
 					const int rowj = h->hplRowInd[j];
 					while (h->hscColInd[k] < rowj) k++;
 					const double* B = h->Hpl + 18 * (size_t)j;

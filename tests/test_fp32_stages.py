@@ -182,6 +182,10 @@ def schur_restated(eng, sysE, invHll, lam):
             pi.append(starts[m] + a); pj.append(starts[m] + b)
     pi = np.concatenate(pi) if pi else np.zeros(0, int); pj = np.concatenate(pj) if pj else np.zeros(0, int)
     ri, rj = rowInd[pi], rowInd[pj]
+    # a pose that observes the landmark more than once: its diagonal block also takes W_j Hpl_i^T of every such pair
+    rep = (ri == rj) & (pi != pj)
+    pi, pj = np.concatenate([pi, pj[rep]]), np.concatenate([pj, pi[rep]])
+    ri, rj = rowInd[pi], rowInd[pj]
     sw = ri > rj
     pi[sw], pj[sw] = pj[sw].copy(), pi[sw].copy()
     ri, rj = rowInd[pi], rowInd[pj]
