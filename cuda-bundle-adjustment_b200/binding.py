@@ -122,7 +122,7 @@ _SYMBOLS = [
     "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
-    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
+    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_peer_allreduce", "cuba_debug_pcg5_ranks", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
 ]
 
 
@@ -180,6 +180,8 @@ def load_library():
         "cuba_debug_get_pcg_info": [vp, vp, C.POINTER(d)],
         "cuba_debug_get_coarse": [vp, vp, vp, vp],
         "cuba_debug_coarse_inverse": [vp, vp, i, vp, vp],
+        "cuba_debug_peer_allreduce": [vp, i, C.c_int64, i, vp, vp],
+        "cuba_debug_pcg5_ranks": [vp, i, i, i, vp, vp, vp, vp, vp],
         "cuba_debug_build_structure_host": [C.POINTER(_Problem), i, i, C.POINTER(_Sizes), vp, vp, vp, vp, vp, vp, vp, vp],
         "cuba_debug_pcg_partition": [C.POINTER(_Problem), i, i, vp],
         "cuba_debug_pcg5_plan": [C.POINTER(_Problem), i, i, i, vp],
@@ -274,6 +276,8 @@ def pcg5_plan_apc_host(prob, aggs_per_cta, world=1, num_sms=132, max_aggregates=
     return out
 
 
+# cuba_debug_pcg5_ranks: plan[] fields
+PCG5_RANKS_PLAN_FIELDS = ("G", "gs", "A", "needMax", "maxRows", "halo", "big", "cinfo")
 PCG5T_LAYOUT_FIELDS = ("ok", "aggs_per_cta", "capBlocks", "streamed_blocks", "zhInSmem", "total_bytes", "blk_bytes", "rsu_bytes",
                        "staging_bytes", "rc_bytes", "zh_bytes", "slice_bytes")
 H100_SMEM_BUDGET = 227 * 1024 - 2048     # what set_problem leaves to k_pcg5t's dynamic shared memory on an H100
@@ -633,6 +637,29 @@ class Engine:
         info = C.c_int(-1)
         _check(self.L.cuba_debug_coarse_inverse(self.h, _p(AcP), A, _p(AcInv), C.byref(info)))
         return AcInv, info.value
+
+    def peer_allreduce(self, parts):
+        """the peer all-reduce of a `world`-rank run emulated on this GPU (include/cuba_b200.h: cuba_debug_peer_allreduce): parts
+        [calls][world][n], each call's parts loaded in the engine's scalar type; returns every rank's buffer after every call, same shape"""
+        parts = np.ascontiguousarray(parts, dtype=np.float64)
+        calls, world, n = parts.shape
+        out = np.zeros_like(parts)
+        _check(self.L.cuba_debug_peer_allreduce(self.h, int(world), int(n), int(calls), _p(parts), _p(out)))
+        return out
+
+    def pcg5_ranks(self, world, two_level, nsolves=3):
+        """the row-distributed k_pcg5 of a `world`-rank run emulated on this GPU, on the current reduced system (include/cuba_b200.h:
+        cuba_debug_pcg5_ranks).  Returns x [nsolves][numP][6], status [nsolves][world] and iters [nsolves][world] of every rank,
+        plan (dict of PCG5_RANKS_PLAN_FIELDS), aggRow [A+1] and the fp32 AcInv [6A][6A] (zeros for block-Jacobi)."""
+        P = self.sizes["numP"]
+        amax = min(P, 148)
+        x = np.zeros((nsolves, P, 6)); st = np.zeros((nsolves, world, 2), np.int32); plan = np.zeros(len(PCG5_RANKS_PLAN_FIELDS), np.int32)
+        agg = np.zeros(amax + 1, np.int32); AcInv = np.zeros(36 * amax * amax, np.float32)
+        _check(self.L.cuba_debug_pcg5_ranks(self.h, int(world), int(bool(two_level)), int(nsolves), _p(x), _p(st), _p(plan), _p(agg), _p(AcInv)))
+        pl = dict(zip(PCG5_RANKS_PLAN_FIELDS, (int(v) for v in plan)))
+        A = pl["A"]
+        return dict(x=x, status=st[:, :, 0].copy(), iters=st[:, :, 1].copy(), plan=pl, aggRow=agg[:A + 1].copy(),
+                    AcInv=AcInv[:36 * A * A].reshape(6 * A, 6 * A).copy())
 
     def bench_stage(self, stage, reps=10, flush_l2=True, lam=1.0):
         ms = C.c_double(0)

@@ -242,6 +242,8 @@ struct EngineBase {
 	virtual int dbg_pcg_info(int32_t* info, double* coarseLambda) = 0;
 	virtual int dbg_coarse(int32_t* rowAgg, double* AcP, float* AcInv) = 0;
 	virtual int dbg_coarse_inverse(const double* AcP, int A, float* AcInv, int* info) = 0;
+	virtual int dbg_peer_allreduce(int world, size_t n, int calls, const double* parts, double* out) = 0;
+	virtual int dbg_pcg5_ranks(int world, int twoLevel, int nsolves, double* x, int32_t* status, int32_t* plan, int32_t* aggRow, float* AcInv) = 0;
 	virtual int set_edge_levels(const uint8_t* levels) = 0;
 	virtual int get_edge_levels(uint8_t* levels) = 0;
 	virtual int classify_edges(double chi2Mono, double chi2Stereo, int flags, int32_t* counts) = 0;
@@ -1529,6 +1531,60 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	int pcg5_max_agg() const { return (cfg.reserved[6] > 0 && cfg.reserved[6] < PCG5_MAXAGG) ? cfg.reserved[6] : PCG5_MAXAGG; }
+
+	// The dimensions of a k_pcg5 plan over W ranks that do not depend on the launch shape (capBlocks and zhInSmem stay 0).
+	static Pcg5Dims pcg5_plan_dims(const Pcg5Plan& plan, int W)
+	{
+		const int G = plan.G, nc = 6 * plan.A, NR = 3 + 6 * (G / plan.gs);
+		Pcg5Dims d{};
+		d.needMax = plan.P.needMax; d.maxRows = plan.P.maxRows; d.nc = nc; d.maxNeedAgg = plan.C.maxNeedAgg;
+		d.npv = std::max(std::max(G * p5t::pcg5t_np(plan.apc), W * NR), 6 * plan.C.maxNeedAgg); d.nls = NR;
+		d.sliceRows = (nc + G - 1) / G;
+		return d;
+	}
+
+	// k_pcg5's legacy (256-thread) shape for a plan: the blocks cached in shared memory, Z^ in shared memory or not, BIG or not, the
+	// block-Jacobi dimensions, the dynamic shared memory and the kernel -- k_pcg5, or with `ranks` k_pcg5_ranks (W ranks emulated in
+	// one launch, cuba_debug_pcg5_ranks), so that the emulation runs the shape a W-GPU run would.  perSM: CTAs per SM, 0 when the
+	// plan does not fit.
+	struct P5Shape { Pcg5Dims dims{}, dimsBJ{}; size_t smem = 0; bool big = false; const void* fn = nullptr; int perSM = 0; };
+	int pcg5_legacy_shape(const Pcg5Plan& plan, Pcg5Dims d, int W, bool ranks, P5Shape& sh)
+	{
+		sh = P5Shape{};
+		int smemMax = 0;
+		CUDA_TRY(cudaDeviceGetAttribute(&smemMax, cudaDevAttrMaxSharedMemoryPerBlockOptin, devOrdinal));
+		const size_t budget = (size_t)smemMax > 4096 ? (size_t)smemMax - 2048 : 0;   // static arrays of k_pcg5: < 1 KB
+		const PcgPartition& PP = plan.P;
+		const size_t per = 36 * sizeof(T) + 4;
+		const size_t wantCache = PP.blkMax > PCG5_REGBLK ? (size_t)(PP.blkMax - PCG5_REGBLK) : 0;
+		bool big = PP.maxRows * 6 > PCG5_BLOCK;
+		{
+			d.capBlocks = 0; d.zhInSmem = 0;
+			const size_t base = Pcg5Layout<T>(d).total + 64;
+			if (base > budget) return CUBA_OK;
+			const size_t zhBytes = (size_t)d.needMax * 36 * sizeof(T);
+			size_t used = base + wantCache * per;
+			if (used + zhBytes <= budget) { d.zhInSmem = 1; used += zhBytes; }
+			const size_t fixed = used - wantCache * per;
+			d.capBlocks = (int)std::min(wantCache, (budget - fixed) / per);
+			// blocks would have to be streamed from the global copy every pass: the variant without register-resident blocks streams
+			// with eighteen 16-byte loads in flight per thread (the register variant can afford six 8-byte loads)
+			if ((size_t)d.capBlocks < wantCache) big = true;
+			if (big) d.capBlocks = (int)std::min((size_t)PP.blkMax, (budget - fixed) / per);
+		}
+		Pcg5Dims dBJ = d; dBJ.nc = 0; dBJ.maxNeedAgg = 0; dBJ.zhInSmem = 0; dBJ.sliceRows = 0; dBJ.nls = 3; dBJ.npv = std::max(plan.G * 3, W * 3);
+		const size_t smem = std::max(Pcg5Layout<T>(d).total, Pcg5Layout<T>(dBJ).total);
+		if (smem > (size_t)smemMax - 1024) return CUBA_OK;
+		const void* fn = ranks ? (big ? (const void*)k_pcg5_ranks<T, true> : (const void*)k_pcg5_ranks<T, false>)
+		                       : (big ? (const void*)k_pcg5<T, true> : (const void*)k_pcg5<T, false>);
+		CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+		int perSM = 0;
+		CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fn, PCG5_BLOCK, smem));
+		sh.dims = d; sh.dimsBJ = dBJ; sh.smem = smem; sh.big = big; sh.fn = fn; sh.perSM = perSM;
+		return CUBA_OK;
+	}
+
 	// Partition of the rows over world x G virtual CTAs, aggregates aligned with the ranks, shared-memory budget, boards.
 	int setup_pcg5()
 	{
@@ -1544,7 +1600,7 @@ struct Engine : EngineBase {
 		const size_t budget = (size_t)smemMax > 4096 ? (size_t)smemMax - 2048 : 0;   // static arrays of k_pcg5: < 1 KB
 		// rows over world x G virtual CTAs (about eight rows each, never more than 42: one thread per (row, component) pair in the
 		// row sums), rank-aligned aggregates, halo masks: cuba_structure.cpp (CPU-tested through cuba_debug_pcg5_plan)
-		const int maxAgg = (cfg.reserved[6] > 0 && cfg.reserved[6] < PCG5_MAXAGG) ? cfg.reserved[6] : PCG5_MAXAGG;
+		const int maxAgg = pcg5_max_agg();
 		// the tuned shape (cuba_pcg5t.cuh): a solve on one GPU whose blocks fit registers + shared memory, with apc aggregates per
 		// CTA -- the largest apc <= p5t::DEFAULT_APC (CUBA_PCG5_AGGS_PER_CTA: another bound, 1 = one aggregate per CTA group as
 		// k_pcg5) whose plan exists and whose shared memory fits; every other shape: one aggregate per group of gs CTAs
@@ -1555,19 +1611,13 @@ struct Engine : EngineBase {
 		Pcg5Plan plan;
 		Pcg5Dims d{};
 		int NR = 0;
-		const size_t per = 36 * sizeof(T) + 4;
-		size_t wantCache = 0;
 		for (int apc = tryTuned ? apcTop : 1; apc >= 1 && !p5Tuned; apc--) {
 			build_pcg5_plan(numP, S.nfull, S.fRowPtr, S.fColInd, W, numSMs, maxAgg, 2 * PCG5_BLOCK / 6, plan, &hostPP, apc);
 			if (!plan.ok) continue;
-			const int G = plan.G, nc = 6 * plan.A;
-			const PcgPartition& PP = plan.P; const CoarsePartition& CP = plan.C;
-			NR = 3 + 6 * (G / plan.gs);
-			d = Pcg5Dims{};
-			d.needMax = PP.needMax; d.maxRows = PP.maxRows; d.nc = nc; d.maxNeedAgg = CP.maxNeedAgg;
-			d.npv = std::max(std::max(G * p5t::pcg5t_np(apc), W * NR), 6 * CP.maxNeedAgg); d.nls = NR;
-			d.sliceRows = (nc + G - 1) / G;
-			wantCache = PP.blkMax > PCG5_REGBLK ? (size_t)(PP.blkMax - PCG5_REGBLK) : 0;
+			const int G = plan.G;
+			const PcgPartition& PP = plan.P;
+			d = pcg5_plan_dims(plan, W);
+			NR = d.nls;
 			if (!tryTuned) break;
 			using TS = p5t::Pcg5Shape;
 			p5t::Pcg5Dims t = pcg5t_plan_dims(plan);
@@ -1593,33 +1643,11 @@ struct Engine : EngineBase {
 		const std::vector<unsigned char>& peers = plan.rowPeers;
 		const int nc = 6 * A;
 		if (!p5Tuned) {
-		bool big = PP.maxRows * 6 > PCG5_BLOCK;
-		{
-			d.capBlocks = 0; d.zhInSmem = 0;
-			const size_t base = Pcg5Layout<T>(d).total + 64;
-			if (base > budget) return CUBA_OK;
-			const size_t zhBytes = (size_t)d.needMax * 36 * sizeof(T);
-			size_t used = base + wantCache * per;
-			if (used + zhBytes <= budget) { d.zhInSmem = 1; used += zhBytes; }
-			const size_t fixed = used - wantCache * per;
-			d.capBlocks = (int)std::min(wantCache, (budget - fixed) / per);
-			// blocks would have to be streamed from the global copy every pass: the variant without register-resident blocks streams
-			// with eighteen 16-byte loads in flight per thread (the register variant can afford six 8-byte loads)
-			if ((size_t)d.capBlocks < wantCache) big = true;
-			if (big) d.capBlocks = (int)std::min((size_t)PP.blkMax, (budget - fixed) / per);
-		}
-		p5Dims = d;
-		p5DimsBJ = d; p5DimsBJ.nc = 0; p5DimsBJ.maxNeedAgg = 0; p5DimsBJ.zhInSmem = 0; p5DimsBJ.sliceRows = 0; p5DimsBJ.nls = 3; p5DimsBJ.npv = std::max(G * 3, W * 3);
-		p5Smem = std::max(Pcg5Layout<T>(p5Dims).total, Pcg5Layout<T>(p5DimsBJ).total);
-		if (p5Smem > (size_t)smemMax - 1024) return CUBA_OK;
-		p5Big = big;
-		p5Fn = p5Big ? (const void*)k_pcg5<T, true> : (const void*)k_pcg5<T, false>;
-		p5Block = PCG5_BLOCK;
-		CUDA_TRY(cudaFuncSetAttribute(p5Fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p5Smem));
-		int perSM = 0;
-		if (p5Big) CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_pcg5<T, true>, PCG5_BLOCK, p5Smem));
-		else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_pcg5<T, false>, PCG5_BLOCK, p5Smem));
-		if (perSM < 1) return CUBA_OK;
+			P5Shape sh;
+			int rc = pcg5_legacy_shape(plan, d, W, false, sh); if (rc) return rc;
+			if (sh.perSM < 1) return CUBA_OK;
+			d = sh.dims; p5Dims = sh.dims; p5DimsBJ = sh.dimsBJ; p5Smem = sh.smem; p5Big = sh.big; p5Fn = sh.fn;
+			p5Block = PCG5_BLOCK;
 		}
 		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: world %d G %d gs %d A %d aggsPerCta %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceRows %d cap %d smem %zu\n",
 			W, G, gs, A, plan.apc, d.needMax, d.maxRows, PP.blkMax, d.maxNeedAgg, d.zhInSmem, d.sliceRows, d.capBlocks, p5Smem);
@@ -1684,10 +1712,16 @@ struct Engine : EngineBase {
 	// memory (A <= PCG4_MAXAGG1), the blocked sweep on the whole chip above.
 	int launch_coarse_setup(int A, const int* cbPtr, const int* cbList, double* AcP, float* AcInv, int* info)
 	{
+		return launch_coarse_setup(A, cbPtr, cbList, cRowOf, cZx, cU, cdT, gridBar, AcP, AcInv, info);
+	}
+	// the same on a plan's own aggregate map rowOf and basis Zx, with scratch U [36 nfull], and tiles and bar for A > PCG4_MAXAGG1
+	int launch_coarse_setup(int A, const int* cbPtr, const int* cbList, const int* rowOf, const T* Zx, double* U, double* tiles, GridBar* bar,
+		double* AcP, float* AcInv, int* info)
+	{
 		const int nblkP = A * (A + 1) / 2;
-		KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, cRowOf.p, fColInd.p, S.nfull, cZx.p, cU.p);
-		KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, cbPtr, cbList, cU.p, nblkP, AcP);
-		if (A > PCG4_MAXAGG1) return launch_coarse_dense(AcP, A, cdT, AcInv, info, gridBar);
+		KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, rowOf, fColInd.p, S.nfull, Zx, U);
+		KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, cbPtr, cbList, U, nblkP, AcP);
+		if (A > PCG4_MAXAGG1) return launch_coarse_dense(AcP, A, tiles, AcInv, info, bar);
 		k_coarse_invert<T><<<1, 1024, coarse_invert_smem(A), stream>>>(AcP, A, AcInv, info);
 		launches++;
 		CUDA_TRY(cudaGetLastError());
@@ -1708,11 +1742,18 @@ struct Engine : EngineBase {
 		return !valid || age >= refreshEvery || lamRatio > 300.0;
 	}
 
+	int pcg5_max_iters() const { return cfg.pcg_max_iters > 0 ? cfg.pcg_max_iters : std::max(200, 40 * S.numP); }
+	double pcg5_tol2() const
+	{
+		const double tol = cfg.pcg_tol > 0 ? cfg.pcg_tol : (sizeof(T) == 8 ? 1e-11 : 1e-6);
+		return tol * tol;
+	}
+
 	int launch_pcg5(bool twoLevel)
 	{
 		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
 		const int numP = S.numP, A = twoLevel ? p5A : 0;
-		const int maxIters = cfg.pcg_max_iters > 0 ? cfg.pcg_max_iters : std::max(200, 40 * numP);
+		const int maxIters = pcg5_max_iters();
 		// tags are 32 bits: long before the device tag base can wrap, every rank (same arithmetic everywhere) clears its boards
 		p5TagBound += (long long)maxIters + 8;
 		if (p5TagBound > (1LL << 31)) {
@@ -1745,8 +1786,7 @@ struct Engine : EngineBase {
 			a.numP = numP; a.G = p5G; a.rank = p5Dist ? rank : 0; a.world = p5W;
 			a.Linv = p5Linv; a.R0 = p5R0; a.Zhat = p5Zhat; a.rc0 = p5Rc0; a.x = xp;
 			a.maxIters = maxIters;
-			const double tol = cfg.pcg_tol > 0 ? cfg.pcg_tol : (sizeof(T) == 8 ? 1e-11 : 1e-6);
-			a.tol2 = tol * tol;
+			a.tol2 = pcg5_tol2();
 			a.status = &dScal.p->pcg;
 			a.AcInv = p5AcInv; a.naPtr = p5NaPtr; a.naList = p5NaList; a.needAgg = p5NeedAgg; a.A = A; a.gs = p5Gs;
 			for (int r = 0; r < PCG5_MAXWORLD; r++) { a.peerW[r] = nullptr; a.peerR[r] = nullptr; a.peerCtl[r] = nullptr; }
@@ -2455,6 +2495,163 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// include/cuba_b200.h: cuba_debug_peer_allreduce -- `world` ranks of k_peer_allreduce emulated on this GPU by one cooperative
+	// launch of k_peer_allreduce_ranks (numSMs / world CTAs per rank), in buffers of its own
+	int dbg_peer_allreduce(int W, size_t n, int calls, const double* parts, double* out) override
+	{
+		if (W < 1 || W > peer::MAXW || n < 1 || calls < 1 || !parts || !out)
+			return fail(CUBA_ERR_INVALID, "debug_peer_allreduce: world outside 1..8, n < 1, calls < 1 or a NULL pointer");
+		unsigned int nctas = numSMs / W;
+		int perSM = 0;
+		CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, peer::k_peer_allreduce_ranks<T>, peer::BLOCK, 0));
+		if ((long long)perSM * numSMs < (long long)W * nctas)
+			return fail(CUBA_ERR_INVALID, "debug_peer_allreduce: " + std::to_string(W * nctas) + " CTAs, but only " + std::to_string(perSM * numSMs) + " can be resident at once");
+		// every rank's buffer as launch_peer_allreduce lays it out (n elements, the signal block at the next even element), 16-byte aligned
+		const size_t sigOff = (n + 1) & ~(size_t)1;
+		const size_t sigElems = (2 * peer::MAXW * sizeof(unsigned int) + sizeof(T) - 1) / sizeof(T);
+		const size_t stride = (sigOff + sigElems + 31) / 32 * 32;
+		DBuf<T> buf; DBuf<GridBar> bars; DBuf<peer::Args<T>> dArgs;
+		CUDA_TRY(buf.alloc(stride * W)); CUDA_TRY(bars.alloc(W));
+		CUDA_TRY(cudaMemsetAsync(buf.p, 0, sizeof(T) * stride * W, stream));
+		CUDA_TRY(cudaMemsetAsync(bars.p, 0, sizeof(GridBar) * W, stream));
+		std::vector<peer::Args<T>> ha(W);
+		for (int r = 0; r < W; r++) {
+			peer::Args<T>& a = ha[r];
+			for (int q = 0; q < peer::MAXW; q++) { a.peers[q] = nullptr; a.sigPeer[q] = nullptr; }
+			for (int q = 0; q < W; q++) { a.peers[q] = buf.p + stride * q; a.sigPeer[q] = (unsigned int*)(buf.p + stride * q + sigOff); }
+			a.local = a.peers[r]; a.sigLocal = a.sigPeer[r]; a.n = n; a.rank = r; a.world = W; a.bar = bars.p + r;
+		}
+		std::vector<T> h((size_t)W * n);
+		for (int c = 0; c < calls; c++) {
+			for (int r = 0; r < W; r++) ha[r].epoch = (unsigned int)c + 1;           // consecutive epochs on the same signal blocks
+			CUDA_TRY(dArgs.upload(ha.data(), W, stream));
+			for (size_t i = 0; i < (size_t)W * n; i++) h[i] = (T)parts[(size_t)c * W * n + i];
+			for (int r = 0; r < W; r++) CUDA_TRY(cudaMemcpyAsync(buf.p + stride * r, h.data() + (size_t)r * n, sizeof(T) * n, cudaMemcpyHostToDevice, stream));
+			const peer::Args<T>* pa = dArgs.p;
+			void* args[] = { (void*)&pa, (void*)&nctas };
+			CUDA_TRY(cudaLaunchCooperativeKernel((void*)peer::k_peer_allreduce_ranks<T>, dim3(W * nctas), dim3(peer::BLOCK), args, 0, stream));
+			launches++;
+			for (int r = 0; r < W; r++) CUDA_TRY(cudaMemcpyAsync(h.data() + (size_t)r * n, buf.p + stride * r, sizeof(T) * n, cudaMemcpyDeviceToHost, stream));
+			CUDA_TRY(cudaStreamSynchronize(stream));
+			for (size_t i = 0; i < (size_t)W * n; i++) out[(size_t)c * W * n + i] = (double)h[i];
+		}
+		return CUBA_OK;
+	}
+
+	// include/cuba_b200.h: cuba_debug_pcg5_ranks -- the row-distributed k_pcg5 of a `world`-rank run on the current reduced system,
+	// every rank's boards in this GPU's memory and all ranks in one cooperative launch of k_pcg5_ranks, in buffers of its own
+	int dbg_pcg5_ranks(int W, int twoLevel, int nsolves, double* xOut, int32_t* statusOut, int32_t* planOut, int32_t* aggRowOut, float* acInvOut) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "no problem");
+		if (W < 1 || W > PCG5_MAXWORLD || nsolves < 1 || !xOut || !statusOut || !planOut)
+			return fail(CUBA_ERR_INVALID, "debug_pcg5_ranks: world outside 1..8, nsolves < 1 or a NULL pointer");
+		const int numP = S.numP;
+		if (numP < 1 || S.numL < 1) return fail(CUBA_ERR_STATE, "debug_pcg5_ranks: no reduced system");
+		Pcg5Plan plan;
+		build_pcg5_plan(numP, S.nfull, S.fRowPtr, S.fColInd, W, numSMs / W, pcg5_max_agg(), 2 * PCG5_BLOCK / 6, plan, nullptr, 1);
+		if (!plan.ok) return fail(CUBA_ERR_INVALID, "debug_pcg5_ranks: no k_pcg5 plan for " + std::to_string(W) + " ranks of " + std::to_string(numSMs / W) + " CTAs");
+		P5Shape sh;
+		int rc = pcg5_legacy_shape(plan, pcg5_plan_dims(plan, W), W, true, sh); if (rc) return rc;
+		const int G = plan.G, A = twoLevel ? plan.A : 0, nc = 6 * plan.A;
+		if ((long long)sh.perSM * numSMs < (long long)W * G)
+			return fail(CUBA_ERR_INVALID, "debug_pcg5_ranks: " + std::to_string(W * G) + " CTAs, but only " + std::to_string(sh.perSM * numSMs) + " can be resident at once");
+		const PcgPartition& PP = plan.P; const CoarsePartition& CP = plan.C;
+		const size_t nP = (size_t)numP;
+		DBuf<int> dCtaRow, dNeedPtr, dNeedCol, dLocal, dAggRow, dNaPtr, dNaList, dNeedAgg, dCbPtr, dCbList, dRowOf, dInfo;
+		DBuf<unsigned char> dRowPeers;
+		DBuf<T> dLinv, dR0, dZhat, dRcRow, dRc0, dZx, dHat, dx;
+		DBuf<double> dU, dAcP, dTiles;
+		DBuf<float> dAcInv;
+		DBuf<GridBar> dBar;
+		DBuf<PcgStatus> dStatus;
+		DBuf<unsigned long long> boards;
+		DBuf<Pcg5Args<T>> dArgs;
+		CUDA_TRY(dCtaRow.upload(PP.rows, stream)); CUDA_TRY(dNeedPtr.upload(PP.nptr, stream)); CUDA_TRY(dNeedCol.upload(PP.ncol, stream));
+		CUDA_TRY(dLocal.upload(PP.local, stream)); CUDA_TRY(dRowPeers.upload(plan.rowPeers, stream));
+		CUDA_TRY(dAggRow.upload(CP.aggRow, stream)); CUDA_TRY(dNaPtr.upload(CP.naPtr, stream)); CUDA_TRY(dNaList.upload(CP.naList, stream));
+		CUDA_TRY(dNeedAgg.upload(CP.needAgg, stream)); CUDA_TRY(dCbPtr.upload(CP.cbPtr, stream)); CUDA_TRY(dCbList.upload(CP.cbList, stream));
+		CUDA_TRY(dRowOf.upload(CP.rowOf, stream));
+		CUDA_TRY(dLinv.alloc(36 * nP)); CUDA_TRY(dR0.alloc(6 * nP)); CUDA_TRY(dZhat.alloc(36 * nP)); CUDA_TRY(dRcRow.alloc(6 * nP)); CUDA_TRY(dRc0.alloc(std::max(nc, 1)));
+		CUDA_TRY(dZx.alloc(36 * nP)); CUDA_TRY(dU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(dHat.alloc(36 * (size_t)S.nfull)); CUDA_TRY(dx.alloc(6 * nP));
+		CUDA_TRY(dAcP.alloc(36 * ((size_t)plan.A * (plan.A + 1) / 2))); CUDA_TRY(dAcInv.alloc((size_t)nc * nc)); CUDA_TRY(dInfo.alloc(1));
+		CUDA_TRY(dBar.alloc(1)); CUDA_TRY(dStatus.alloc(W));
+		CUDA_TRY(cudaMemsetAsync(dAcInv.p, 0, sizeof(float) * (size_t)nc * nc, stream));
+		CUDA_TRY(cudaMemsetAsync(dInfo.p, 0, sizeof(int), stream));
+		CUDA_TRY(cudaMemsetAsync(dBar.p, 0, sizeof(GridBar), stream));
+		// W board sets laid out as setup_pcg5 lays out one GPU's, zeroed: [2 solve halves][2 pass parities] of w, partials, rank
+		// summaries and coarse corrections, then the control block
+		const int NR = 3 + 6 * (G / plan.gs);
+		const size_t wW = 4 * 6 * nP, pW = 4 * (size_t)PCG5_REPL * G * p5t::pcg5t_np(plan.apc), rW = 4 * (size_t)PCG5_REPL * W * NR, cW = 4 * (size_t)PCG5_REPL * nc;
+		const size_t words2 = 2 * (wW + pW + rW + cW) + (sizeof(Pcg5Ctl) + 7) / 8 + 2;
+		CUDA_TRY(boards.alloc(words2 * W));
+		CUDA_TRY(cudaMemsetAsync(boards.p, 0, sizeof(unsigned long long) * words2 * W, stream));
+		auto base = [&](int r) { return boards.p + words2 * r; };
+		auto ctlOf = [&](int r) { return (Pcg5Ctl*)(base(r) + 2 * (wW + pW + rW + cW)); };
+		// the preparation and the coarse level, as launch_pcg5 runs them on every rank (the rows of Linv, R0, Z^ and rc0 are the
+		// same on every rank: computed once; each rank's breakdown counter gets its own count)
+		if (A > 0) KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, dZx.p);
+		Pcg5PrepArgs<T> pa;
+		pa.fRowPtr = fRowPtr; pa.fColInd = fColInd; pa.fVal = fVal; pa.b = bsc; pa.Zx = dZx; pa.numP = numP; pa.A = A; pa.aggRow = dAggRow; pa.zhatFp32 = 0;
+		pa.Linv = dLinv; pa.R0 = dR0; pa.Zhat = dZhat; pa.rcRow = dRcRow; pa.rc0 = dRc0;
+		for (int r = 0; r < W; r++) {
+			pa.ctl = ctlOf(r);
+			k_pcg5_prep_rows<T><<<(numP + 127) / 128, 128, 0, stream>>>(pa);
+			launches++;
+		}
+		if (A > 0) {
+			k_pcg5_prep_rc<T><<<(6 * A + 127) / 128, 128, 0, stream>>>(pa);
+			launches++;
+			if (A > PCG4_MAXAGG1) CUDA_TRY(dTiles.alloc(cdense::scratch_doubles(A)));
+			rc = launch_coarse_setup(A, dCbPtr, dCbList, dRowOf, dZx, dU, dTiles.p, dBar, dAcP, dAcInv, dInfo); if (rc) return rc;
+		}
+		CUDA_TRY(cudaGetLastError());
+		std::vector<Pcg5Args<T>> ha(W);
+		for (int r = 0; r < W; r++) {
+			Pcg5Args<T>& a = ha[r];
+			a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = dLocal; a.fVal = fVal; a.fHat = dHat;
+			a.ctaRow = dCtaRow; a.needPtr = dNeedPtr; a.needCol = dNeedCol;
+			a.numP = numP; a.G = G; a.rank = r; a.world = W;
+			a.Linv = dLinv; a.R0 = dR0; a.Zhat = dZhat; a.rc0 = dRc0; a.x = dx;
+			a.dims = A > 0 ? sh.dims : sh.dimsBJ;
+			a.dims.capBlocks = sh.dims.capBlocks;
+			a.maxIters = pcg5_max_iters(); a.tol2 = pcg5_tol2();
+			a.status = dStatus.p + r;
+			a.AcInv = dAcInv; a.naPtr = dNaPtr; a.naList = dNaList; a.needAgg = dNeedAgg; a.A = A; a.gs = plan.gs;
+			for (int q = 0; q < PCG5_MAXWORLD; q++) { a.peerW[q] = nullptr; a.peerR[q] = nullptr; a.peerCtl[q] = nullptr; }
+			for (int q = 0; q < W; q++) { a.peerW[q] = base(q); a.peerR[q] = base(q) + 2 * (wW + pW); a.peerCtl[q] = ctlOf(q); }
+			a.wBoard = base(r); a.pBoard = base(r) + 2 * wW; a.rBoard = base(r) + 2 * (wW + pW); a.cBoard = base(r) + 2 * (wW + pW + rW);
+			a.rowPeers = dRowPeers; a.ctl = ctlOf(r);
+			a.timing = nullptr;
+		}
+		CUDA_TRY(dArgs.upload(ha.data(), W, stream));
+		std::vector<T> hx(6 * nP);
+		std::vector<PcgStatus> hs(W);
+		for (int k = 0; k < nsolves; k++) {
+			CUDA_TRY(cudaMemsetAsync(dx.p, 0xff, sizeof(T) * 6 * nP, stream));         // NaN: a row no rank writes stays visible
+			const Pcg5Args<T>* pArgs = dArgs.p;
+			int g = G;
+			void* args[] = { (void*)&pArgs, (void*)&g };
+			CUDA_TRY(cudaLaunchCooperativeKernel(sh.fn, dim3(W * G), dim3(PCG5_BLOCK), args, sh.smem, stream));
+			for (int r = 0; r < W; r++) k_pcg5_commit<<<1, 1, 0, stream>>>(ctlOf(r));
+			launches += 1 + W;
+			CUDA_TRY(cudaGetLastError());
+			CUDA_TRY(cudaMemcpyAsync(hx.data(), dx.p, sizeof(T) * 6 * nP, cudaMemcpyDeviceToHost, stream));
+			CUDA_TRY(cudaMemcpyAsync(hs.data(), dStatus.p, sizeof(PcgStatus) * W, cudaMemcpyDeviceToHost, stream));
+			CUDA_TRY(cudaStreamSynchronize(stream));
+			for (size_t i = 0; i < 6 * nP; i++) xOut[(size_t)k * 6 * nP + i] = (double)hx[i];
+			for (int r = 0; r < W; r++) { statusOut[((size_t)k * W + r) * 2] = hs[r].status; statusOut[((size_t)k * W + r) * 2 + 1] = hs[r].iters; }
+		}
+		int cinfo = 0;
+		CUDA_TRY(cudaMemcpy(&cinfo, dInfo.p, sizeof(int), cudaMemcpyDeviceToHost));
+		int halo = 0;
+		for (unsigned char m : plan.rowPeers) if (m) halo++;
+		const int32_t v[8] = { G, plan.gs, plan.A, PP.needMax, PP.maxRows, halo, sh.big ? 1 : 0, cinfo };
+		memcpy(planOut, v, sizeof(v));
+		if (aggRowOut) memcpy(aggRowOut, CP.aggRow.data(), sizeof(int) * (plan.A + 1));
+		if (acInvOut) CUDA_TRY(cudaMemcpy(acInvOut, dAcInv.p, sizeof(float) * (size_t)nc * nc, cudaMemcpyDeviceToHost));
+		return CUBA_OK;
+	}
+
 	// ---- micro-benchmarks --------------------------------------------------------------------------------
 	int bench_stage(int stage, int reps, int flush, double lambda, double* ms) override
 	{
@@ -2749,6 +2946,17 @@ int cuba_debug_get_delta(cuba_engine* e, double* xp, double* xl) { ENGINE_OR_FAI
 int cuba_debug_get_pcg_info(cuba_engine* e, int32_t* info, double* coarse_lambda) { ENGINE_OR_FAIL(e); return e->impl->dbg_pcg_info(info, coarse_lambda); }
 int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* AcInv) { ENGINE_OR_FAIL(e); return e->impl->dbg_coarse(aggRow, AcP, AcInv); }
 int cuba_debug_coarse_inverse(cuba_engine* e, const double* AcP, int A, float* AcInv, int* info) { ENGINE_OR_FAIL(e); return e->impl->dbg_coarse_inverse(AcP, A, AcInv, info); }
+int cuba_debug_peer_allreduce(cuba_engine* e, int world, int64_t n, int calls, const double* parts, double* out)
+{
+	ENGINE_OR_FAIL(e);
+	if (n < 1) return fail(CUBA_ERR_INVALID, "debug_peer_allreduce: n < 1");
+	return e->impl->dbg_peer_allreduce(world, (size_t)n, calls, parts, out);
+}
+int cuba_debug_pcg5_ranks(cuba_engine* e, int world, int two_level, int nsolves, double* x, int32_t* status, int32_t* plan, int32_t* aggRow, float* AcInv)
+{
+	ENGINE_OR_FAIL(e);
+	return e->impl->dbg_pcg5_ranks(world, two_level, nsolves, x, status, plan, aggRow, AcInv);
+}
 int cuba_debug_build_structure_host(const cuba_problem* p, int rank, int world, cuba_sizes* sizes,
 	int32_t* hplColPtr, int32_t* hplRowInd, int32_t* edge2Hpl, int32_t* hscRowPtr, int32_t* hscColInd,
 	int32_t* fullRowPtr, int32_t* fullColInd, int32_t* shard)

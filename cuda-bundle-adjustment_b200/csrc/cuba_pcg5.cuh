@@ -278,9 +278,10 @@ __device__ __forceinline__ bool ll_poll_many(int n, SlotOf slotOf, double* dst, 
 	return true;
 }
 
-// BIG: the CTA may own more than 42 rows (up to 85): every thread then serves two (row, component) pairs in the row sums
-template <typename T, bool BIG = false>
-__global__ void __launch_bounds__(PCG5_BLOCK, 1) k_pcg5(const Pcg5Args<T> a)
+// BIG: the CTA may own more than 42 rows (up to 85): every thread then serves two (row, component) pairs in the row sums.
+// lc: this CTA's index among the G CTAs of its rank (blockIdx.x in k_pcg5); the body reads neither blockIdx nor gridDim.
+template <typename T, bool BIG>
+__device__ __forceinline__ void pcg5_body(const Pcg5Args<T>& a, const int lc)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const Pcg5Layout<T> lay(a.dims);
@@ -310,7 +311,7 @@ __global__ void __launch_bounds__(PCG5_BLOCK, 1) k_pcg5(const Pcg5Args<T> a)
 	__shared__ int s_abort;
 
 	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-	const int G = a.G, lc = blockIdx.x, cta = a.rank * G + lc, world = a.world;
+	const int G = a.G, cta = a.rank * G + lc, world = a.world;
 	const bool coarse = a.A > 0;
 	const int Aloc = coarse ? G / a.gs : 0;             // aggregates hosted by one rank (gs divides G)
 	const int NP = coarse ? 9 : 3, NR = 3 + 6 * Aloc;
@@ -746,6 +747,14 @@ __global__ void __launch_bounds__(PCG5_BLOCK, 1) k_pcg5(const Pcg5Args<T> a)
 		a.ctl->advance = (unsigned int)(kExit + 3);
 	}
 }
+
+template <typename T, bool BIG = false>
+__global__ void __launch_bounds__(PCG5_BLOCK, 1) k_pcg5(const Pcg5Args<T> a) { pcg5_body<T, BIG>(a, blockIdx.x); }
+
+// W ranks emulated on one GPU (cuba_debug_pcg5_ranks): one cooperative launch of W * G CTAs, CTA b acting as CTA b % G of rank
+// b / G with that rank's arguments args[b / G].  The ranks exchange through device memory only, as on W GPUs.
+template <typename T, bool BIG>
+__global__ void __launch_bounds__(PCG5_BLOCK, 1) k_pcg5_ranks(const Pcg5Args<T>* args, int G) { pcg5_body<T, BIG>(args[blockIdx.x / G], blockIdx.x % G); }
 
 // between solves: move the tag base past every tag the finished solve used, flip the solve parity, clear the breakdown counter
 __global__ void k_pcg5_commit(Pcg5Ctl* ctl)

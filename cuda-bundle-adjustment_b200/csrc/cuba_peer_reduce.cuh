@@ -37,29 +37,41 @@ template <typename T> struct Vec2;
 template <> struct Vec2<double> { static __device__ __forceinline__ void ld(const double* p, double& a, double& b) { asm volatile("ld.volatile.global.v2.f64 {%0, %1}, [%2];" : "=d"(a), "=d"(b) : "l"(p) : "memory"); } };
 template <> struct Vec2<float> { static __device__ __forceinline__ void ld(const float* p, float& a, float& b) { asm volatile("ld.volatile.global.v2.f32 {%0, %1}, [%2];" : "=f"(a), "=f"(b) : "l"(p) : "memory"); } };
 
-// every rank signals phase `ph` to all ranks and waits until all ranks have signalled it (CTA 0), then the grid proceeds
-template <typename T>
-__device__ __forceinline__ void rank_barrier(const Args<T>& a, int ph, unsigned int& gen)
+// The CTAs of one rank: this CTA's index lc() among them and their number nctas().  k_peer_allreduce reads blockIdx.x and
+// gridDim.x where it uses them (OneRank), k_peer_allreduce_ranks takes them from its rank's share of the grid (RankShare).
+struct OneRank {
+	__device__ __forceinline__ unsigned int lc() const { return blockIdx.x; }
+	__device__ __forceinline__ unsigned int nctas() const { return gridDim.x; }
+};
+struct RankShare {
+	unsigned int l, n;
+	__device__ __forceinline__ unsigned int lc() const { return l; }
+	__device__ __forceinline__ unsigned int nctas() const { return n; }
+};
+
+// every rank signals phase `ph` to all ranks and waits until all ranks have signalled it (CTA 0), then the rank's CTAs proceed
+template <typename T, typename Ctas>
+__device__ __forceinline__ void rank_barrier(const Args<T>& a, int ph, unsigned int& gen, const Ctas& g)
 {
-	if (blockIdx.x == 0 && threadIdx.x < a.world) {
+	if (g.lc() == 0 && threadIdx.x < a.world) {
 		__threadfence_system();
 		st_sys_u32(a.sigPeer[threadIdx.x] + ph * MAXW + a.rank, a.epoch);
 		while ((int)(ld_sys_u32(a.sigLocal + ph * MAXW + threadIdx.x) - a.epoch) < 0) { }
 		__threadfence_system();
 	}
-	grid_barrier(a.bar, gridDim.x, gen);
+	grid_barrier(a.bar, g.nctas(), gen);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(BLOCK, 1) k_peer_allreduce(const Args<T> a)
+template <typename T, typename Ctas>
+__device__ __forceinline__ void allreduce_body(const Args<T>& a, const Ctas& g)
 {
 	__shared__ unsigned int s_gen;
 	if (threadIdx.x == 0) s_gen = ld_acquire_u32(&a.bar->gen);
 	__syncthreads();
 	unsigned int gen = s_gen;
 	const size_t per = ((a.n + a.world - 1) / a.world + 1) & ~(size_t)1;      // slice length, even (two-element vector loads)
-	const size_t stride = (size_t)gridDim.x * BLOCK * 2, first = ((size_t)blockIdx.x * BLOCK + threadIdx.x) * 2;
-	rank_barrier(a, 0, gen);                                                     // everybody's partial sums are in place
+	const size_t stride = (size_t)g.nctas() * BLOCK * 2, first = ((size_t)g.lc() * BLOCK + threadIdx.x) * 2;
+	rank_barrier(a, 0, gen, g);                                                     // everybody's partial sums are in place
 	{
 		const size_t lo = per * a.rank, hi = lo + per < a.n ? lo + per : a.n;
 		for (size_t i = lo + first; i < hi; i += stride) {
@@ -75,8 +87,8 @@ __global__ void __launch_bounds__(BLOCK, 1) k_peer_allreduce(const Args<T> a)
 			if (two) __stcg(a.local + i + 1, s1);
 		}
 	}
-	grid_barrier(a.bar, gridDim.x, gen);
-	rank_barrier(a, 1, gen);                                                     // every slice is reduced at its owner
+	grid_barrier(a.bar, g.nctas(), gen);
+	rank_barrier(a, 1, gen, g);                                                     // every slice is reduced at its owner
 	for (int q = 0; q < a.world; q++) {
 		if (q == a.rank) continue;
 		const size_t lo = per * q, hi = lo + per < a.n ? lo + per : a.n;
@@ -89,6 +101,17 @@ __global__ void __launch_bounds__(BLOCK, 1) k_peer_allreduce(const Args<T> a)
 			if (two) __stcg(a.local + i + 1, v1);
 		}
 	}
+}
+
+template <typename T>
+__global__ void __launch_bounds__(BLOCK, 1) k_peer_allreduce(const Args<T> a) { allreduce_body(a, OneRank{}); }
+
+// W ranks emulated on one GPU (cuba_debug_peer_allreduce): one cooperative launch of W * nctas CTAs, CTA b acting as CTA
+// b % nctas of rank b / nctas with that rank's arguments (and GridBar) args[b / nctas]
+template <typename T>
+__global__ void __launch_bounds__(BLOCK, 1) k_peer_allreduce_ranks(const Args<T>* args, unsigned int nctas)
+{
+	allreduce_body(args[blockIdx.x / nctas], RankShare{ blockIdx.x % nctas, nctas });
 }
 
 }  // namespace peer

@@ -362,6 +362,26 @@ int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* A
  * AcP (layout of cuba_debug_get_coarse, A >= 1 aggregates) in buffers of its own: AcInv [6A][6A] fp32 and info 0 (inverted) or 1
  * (not positive definite: AcInv all zeros).  Needs a GPU, not a problem; no engine state changes. */
 int cuba_debug_coarse_inverse(cuba_engine* e, const double* AcP, int A, float* AcInv, int* info);
+/* The two kernels of a landmark-sharded run that exchange through peer memory, with `world` ranks (1..8) emulated on this GPU:
+ * the boards of every rank live in this device's memory and ONE cooperative launch runs all ranks, CTA b acting as CTA b % G of
+ * rank b / G.  Both use buffers of their own and change no engine state; both fail with CUBA_ERR_INVALID when the world * G CTAs
+ * cannot all be resident at once.  A rank here has numSMs / world CTAs, where a W-GPU run gives every rank the whole GPU.
+ *
+ * cuba_debug_peer_allreduce: `calls` consecutive all-reduces (k_peer_allreduce, G = numSMs / world, consecutive epochs on the same
+ * buffers and signal blocks).  Before call c every rank's buffer is loaded with parts[c][rank][0..n) in the engine's scalar type;
+ * out[c][rank][0..n) is that rank's buffer after the call. */
+int cuba_debug_peer_allreduce(cuba_engine* e, int world, int64_t n, int calls, const double* parts, double* out);
+/* cuba_debug_pcg5_ranks: the row-distributed k_pcg5 of a `world`-rank run on the engine's current reduced system (Hsc, bsc and the
+ * poses after a Schur stage, e.g. cuba_bench_stage 3 at lambda).  The plan is build_pcg5_plan's for world ranks of numSMs / world
+ * CTAs, in the launch shape setup_pcg5 gives such a plan; the preparation and one coarse setup (two_level != 0) run first, then
+ * `nsolves` solves on the same boards (one launch and every rank's commit each), two-level or block-Jacobi.
+ *   x [nsolves][6 numP]: the solution of each solve (rows no rank wrote are NaN);  status [nsolves][world][2]: each rank's status
+ *   (0 converged, 1 iteration cap, 2 breakdown, 3 exchange abandoned) and iterations;  plan [8]: G, gs, A, needMax, maxRows, rows
+ *   some other rank needs (halo rows), BIG shape (0/1), info of the coarse inverse (0 inverted, 1 not positive definite);
+ *   aggRow [A+1] (may be NULL): first row of every aggregate;  AcInv [6A][6A] (may be NULL): the fp32 coarse inverse the two-level
+ *   solves applied (zeros for block-Jacobi).  A <= min(numP, 148). */
+int cuba_debug_pcg5_ranks(cuba_engine* e, int world, int two_level, int nsolves, double* x, int32_t* status, int32_t* plan, int32_t* aggRow,
+	float* AcInv);
 
 /* Host-only (no CUDA call): builds the index structures from the (iP,iL) lists exactly as
  * cuba_engine_set_problem does and copies them out -- the not-gpu tests check them against the oracle.

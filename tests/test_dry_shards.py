@@ -5,8 +5,8 @@ stage output is rank r's partial result: the Hll / bl / Hpl blocks and edges of 
 Schur complement, and Hpp + lambda I and bp on the diagonal of rank 0 only.  Each rank is checked against the CPU oracle run on the
 sub-problem made of the shard's edges (sharding.sub_problem).  Rank 0's partial reduced system is the Schur complement of that
 sub-problem, so rank 0's solve, update and whole optimize() are the sub-problem's LM run; the other ranks never solve (their
-partial Hsc has no Hpp and is not SPD).  What one GPU cannot show: the peer all-reduce, the row-distributed k_pcg5 and the NCCL
-landmark gather."""
+partial Hsc has no Hpp and is not SPD).  The peer all-reduce and the row-distributed k_pcg5 run with the ranks emulated on one GPU
+in test_emulated_ranks.py; what one GPU cannot show is the NCCL landmark gather."""
 import numpy as np
 import pytest
 
