@@ -12,6 +12,7 @@
 #include <cstring>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/cuba_b200.h"
@@ -47,18 +48,40 @@ static size_t pcg3_fixed_bytes(int needMax, int maxRows, size_t scalar)
 template <typename L>
 static int32_t w_staging_columns(const L& lay) { return (int32_t)((lay.rc - lay.cc) / (6 * sizeof(double))); }
 
+// The dimensions of a k_pcg5 plan over W ranks that do not depend on the launch shape (capBlocks and zhInSmem stay 0).
+static Pcg5Dims pcg5_plan_dims(const Pcg5Plan& plan, int W)
+{
+	const int G = plan.G, nc = 6 * plan.A, NR = 3 + 6 * (G / plan.gs);
+	Pcg5Dims d{};
+	d.needMax = plan.P.needMax; d.maxRows = plan.P.maxRows; d.nc = nc; d.maxNeedAgg = plan.C.maxNeedAgg;
+	d.npv = std::max(std::max(G * p5t::pcg5t_np(plan.apc), W * NR), 6 * plan.C.maxNeedAgg); d.nls = NR;
+	d.sliceRows = (nc + G - 1) / G;
+	return d;
+}
+
 // Pcg5Dims of the tuned one-GPU shape (cuba_pcg5t.cuh) for a plan on one GPU; p5t::pcg5t_fit sizes the caches
 static p5t::Pcg5Dims pcg5t_plan_dims(const Pcg5Plan& plan)
 {
+	const Pcg5Dims d = pcg5_plan_dims(plan, 1);
 	p5t::Pcg5Dims t{};
-	const int G = plan.G, nc = 6 * plan.A, NR = 3 + 6 * (G / plan.gs), np = p5t::pcg5t_np(plan.apc);
-	t.needMax = plan.P.needMax; t.maxRows = plan.P.maxRows; t.nc = nc; t.maxNeedAgg = plan.C.maxNeedAgg;
-	t.npv = std::max(std::max(G * np, NR), 6 * plan.C.maxNeedAgg); t.nls = NR;
-	t.sliceRows = (nc + G - 1) / G;
+	t.needMax = d.needMax; t.maxRows = d.maxRows; t.nc = d.nc; t.maxNeedAgg = d.maxNeedAgg;
+	t.npv = d.npv; t.nls = d.nls; t.sliceRows = d.sliceRows;
 	t.ccCap = p5t::pcg5t_cc_cap(plan.P.blkMax);
-	t.sqWords = np * (p5t::Pcg5Shape::BLOCK / 32);
+	t.sqWords = p5t::pcg5t_np(plan.apc) * (p5t::Pcg5Shape::BLOCK / 32);
 	return t;
 }
+
+// the block-Jacobi dimensions of a k_pcg5 / k_pcg5t shape from its two-level ones: no coarse level, three words per rank summary
+template <typename D>
+static D block_jacobi_dims(D d, int G, int W)
+{
+	d.nc = 0; d.maxNeedAgg = 0; d.zhInSmem = 0; d.sliceRows = 0; d.nls = 3; d.npv = std::max(G * 3, W * 3);
+	return d;
+}
+
+// the kernel that inverts a coarse matrix of A aggregates: one CTA while the packed triangle fits its shared memory, the blocked
+// sweep on the whole chip above
+static int coarse_kernel(int A) { return A > PCG4_MAXAGG1 ? CUBA_COARSE_KERNEL_DENSE : CUBA_COARSE_KERNEL_INVERT; }
 
 #define CUDA_TRY(expr)                                                                                      \
 	do {                                                                                                    \
@@ -149,12 +172,49 @@ struct DBuf {
 		return cudaMemcpyAsync(p, h, sizeof(U) * count, cudaMemcpyHostToDevice, s);
 	}
 	cudaError_t upload(const std::vector<U>& h, cudaStream_t s) { return upload(h.data(), h.size(), s); }
-	cudaError_t upload(const std::vector<U>& h, cudaStream_t s, PinnedArena& arena)
+	// through the pinned arena when one is given
+	cudaError_t upload(const std::vector<U>& h, cudaStream_t s, PinnedArena* arena)
 	{
-		const void* src = h.empty() ? nullptr : arena.put(h.data(), sizeof(U) * h.size());
+		const void* src = h.empty() || !arena ? nullptr : arena->put(h.data(), sizeof(U) * h.size());
 		return upload(src ? (const U*)src : h.data(), h.size(), s);
 	}
 	operator U*() const { return p; }
+};
+
+// One coarse level of a two-level PCG (cuba_coarse.cuh): the device lists of a CoarsePartition, the packed coarse matrix Ac
+// (fp64) and its inverse (fp32), and when that inverse was built.  k_pcg4 and k_pcg5 each own one.
+struct CoarseLevel {
+	int A = 0;
+	DBuf<int> aggRow, naPtr, naList, needAgg, rowOf, cbPtr, cbList;
+	DBuf<double> AcP;
+	DBuf<float> AcInv;
+	bool valid = false;   // AcInv holds the inverse coarse matrix of an earlier solve of this problem
+	int age = 0;          // two-level solves since the coarse matrix was last rebuilt
+	double lambda = 0;    // damping of that rebuild
+	long long rebuilds = 0;  // since set_problem (k_pcg5's rebuild log in cInfo)
+	void forget() { valid = false; age = 0; }
+	// the lists of CP (build_coarse_lists run), Ac and Ac^-1 sized for its A; no inverse yet
+	int upload(const CoarsePartition& CP, cudaStream_t s, PinnedArena* arena)
+	{
+		A = CP.A;
+		forget();
+		CUDA_TRY(aggRow.upload(CP.aggRow, s, arena)); CUDA_TRY(naPtr.upload(CP.naPtr, s, arena)); CUDA_TRY(naList.upload(CP.naList, s, arena));
+		CUDA_TRY(needAgg.upload(CP.needAgg, s, arena)); CUDA_TRY(rowOf.upload(CP.rowOf, s, arena));
+		CUDA_TRY(cbPtr.upload(CP.cbPtr, s, arena)); CUDA_TRY(cbList.upload(CP.cbList, s, arena));
+		CUDA_TRY(AcP.alloc((size_t)A * (A + 1) / 2 * 36)); CUDA_TRY(AcInv.alloc(36 * (size_t)A * A));
+		return CUBA_OK;
+	}
+};
+
+// cudaIpc mappings of one device allocation of every rank (ipcExchange); the own entry is the local allocation
+struct PeerMap {
+	void* base[PCG5_MAXWORLD] = { nullptr };
+	void* mappedFor = nullptr;   // local allocation the mappings were exchanged for
+	void close(int rank)
+	{
+		for (int r = 0; r < PCG5_MAXWORLD; r++) { if (base[r] && r != rank) cudaIpcCloseMemHandle(base[r]); base[r] = nullptr; }
+		mappedFor = nullptr;
+	}
 };
 
 // ---- NCCL through dlopen: single-GPU users never need the library ---------------------------------
@@ -307,19 +367,17 @@ struct Engine : EngineBase {
 	DBuf<unsigned long long> llFlags;   // k_pcg3: [wFlag 2*6numP*2 | pFlag 2*2G*2 | abort word]
 	int pcg2Grid = 0, pcg2Cap = 0, pcg2NeedMax = 0, pcg2MaxRows = 0;
 	// two-level PCG (cuba_pcg4.cuh; its coarse level: cuba_coarse.cuh)
+	CoarseLevel coarse4;
 	DBuf<T> cZx, cZhat;
-	DBuf<float> cAcInv;
-	DBuf<double> cAcP, cPart, cU;
+	DBuf<double> cPart, cU;
 	DBuf<double> cdT;               // k_coarse_dense: two copies of the lower 32 x 32 tiles of Ac, sized by setup_pcg2 and setup_pcg5 for
 	                                // the larger of their coarse matrices (DBuf only grows)
-	DBuf<int> cAggRow, cNaPtr, cNaList, cNeedAgg, cInfo, cRowOf, cCbPtr, cCbList;
-	int pcg4A = 0, pcg4Gs = 1, pcg4MaxNeedAgg = 0, pcg4Cap = 0, pcg4SliceInSmem = 0, pcg4ZhInSmem = 0;
+	DBuf<int> cInfo;
+	int pcg4Gs = 1, pcg4MaxNeedAgg = 0, pcg4Cap = 0, pcg4SliceInSmem = 0, pcg4ZhInSmem = 0;
 	size_t pcg4Smem = 0;
 	bool pcg4Ok = false, tlActive = false;
 	PinnedArena arena;
-	bool coarseValid = false;       // cAcInv holds the inverse coarse matrix of an earlier solve of this problem
-	int coarseAge = 0;              // two-level solves since the coarse matrix was last rebuilt
-	double coarseLambda = 0, curLambda = 0;   // damping of that rebuild / of the solve being launched
+	double curLambda = 0;           // damping of the solve being launched
 	bool pcg3Ok = false;
 	size_t pcg2Smem = 0;
 	// reductions
@@ -347,7 +405,7 @@ struct Engine : EngineBase {
 	{
 		DevGuard guard(devOrdinal);
 		if (stream) cudaStreamSynchronize(stream);
-		p5CloseMappings(); uCloseMappings();
+		p5Peer.close(rank); uPeer.close(rank);
 		for (auto& pe : profEvents) { cudaEventDestroy(pe.second.first); cudaEventDestroy(pe.second.second); }
 		for (auto ev : eventPool) cudaEventDestroy(ev);
 		if (hScal) cudaFreeHost(hScal);
@@ -458,7 +516,7 @@ struct Engine : EngineBase {
 			(p->E3 > 0 && (!p->idx3 || !p->meas3 || !p->omega3)))
 			return fail(CUBA_ERR_INVALID, "set_problem: null array with a non-zero count");
 		const auto t0 = std::chrono::steady_clock::now();
-		lastPcgKernel = CUBA_PCG_KERNEL_NONE; p5Rebuilds = 0; bjRetries = 0;
+		lastPcgKernel = CUBA_PCG_KERNEL_NONE; p5.coarse.rebuilds = 0; bjRetries = 0;
 		lvOn = false;      // every level back to 0: both paths below scatter the caller's omega unmasked
 		// Same topology as the problem this engine already holds (sizes, fixed/free split and every (iP, iL) pair identical): only the
 		// numbers changed -- the estimate after a previous optimize(), new measurements -- so every index structure, tile list,
@@ -502,7 +560,7 @@ struct Engine : EngineBase {
 			fprintf(stderr, "setup total %8.3f ms\n", 1e3 * std::chrono::duration<double>(marks.back().second - marks.front().second).count());
 		}
 		cur = 0; trialValid = false;
-		tlActive = false; coarseValid = false; coarseAge = 0; p5CoarseValid = false; p5CoarseAge = 0;
+		forget_solves();
 		resolveProfile();   // drop the events of earlier problems
 		for (int i = 0; i < CUBA_PROF_NUM; i++) prof[i] = 0;
 		const auto t1 = std::chrono::steady_clock::now();
@@ -546,7 +604,7 @@ struct Engine : EngineBase {
 		}
 		CUDA_TRY(cudaStreamSynchronize(stream));      // the caller's buffers are free again
 		cur = 0; trialValid = false;
-		tlActive = false; coarseValid = false; coarseAge = 0; p5CoarseValid = false; p5CoarseAge = 0;
+		forget_solves();
 		resolveProfile();
 		for (int i = 0; i < CUBA_PROF_NUM; i++) prof[i] = 0;
 		return CUBA_OK;
@@ -814,9 +872,9 @@ struct Engine : EngineBase {
 		upperReduce = world > 1 && !schur5Asked && S.numP > 0 && S.numL > 0;
 		if (upperReduce) {
 			uCount = 36 * (size_t)S.nblk + 6 * nP;
-			const size_t need = ((uCount + 1) & ~(size_t)1) + 64;          // + the signal block of the peer all-reduce
+			const size_t need = peer_signal_offset(uCount) + 64;          // + the signal block of the peer all-reduce
 			if (!uVal.p || need > uVal.cap) {
-				if (uMappedFor) { CUDA_TRY(cudaStreamSynchronize(stream)); uCloseMappings(); }
+				if (uPeer.mappedFor) { CUDA_TRY(cudaStreamSynchronize(stream)); uPeer.close(rank); }
 				CUDA_TRY(uVal.alloc(std::max(need, (size_t)1 << 18)));
 				CUDA_TRY(cudaMemsetAsync(uVal.p, 0, sizeof(T) * uVal.cap, stream));
 				uEpoch = 0;
@@ -826,11 +884,11 @@ struct Engine : EngineBase {
 			uPeerOk = false;
 			if (!getenv("CUBA_NCCL_HSC") && comm) {
 				// signals of an earlier problem may sit at another offset: start from a clean block (all ranks do, in lockstep)
-				CUDA_TRY(cudaMemsetAsync(uVal.p + ((uCount + 1) & ~(size_t)1), 0, sizeof(T) * 64, stream));
+				CUDA_TRY(cudaMemsetAsync(uVal.p + peer_signal_offset(uCount), 0, sizeof(T) * 64, stream));
 				uEpoch = 0;
 				int rcx = allreduce(&dScal.p->v[7], 1, false); if (rcx) return rcx;          // nobody signals into a block that is being cleared
 				bool ok = false;
-				rcx = ipcExchange((void*)uVal.p, uPeerBase, uMappedFor, ok); if (rcx) return rcx;
+				rcx = ipcExchange((void*)uVal.p, uPeer, ok); if (rcx) return rcx;
 				uPeerOk = ok;
 				CUDA_TRY(gridBar.alloc(1));
 			}
@@ -1281,8 +1339,8 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_pcg2<T>, PCG2_BLOCK, pcg2Smem));
 		if (perSM < 1) return fail(CUBA_ERR_CUDA, "k_pcg2 cannot be resident with the requested shared memory");
 		arena.reset();
-		CUDA_TRY(ctaRow.upload(rows, stream, arena)); CUDA_TRY(needPtr.upload(nptr, stream, arena)); CUDA_TRY(needCol.upload(ncol, stream, arena));
-		CUDA_TRY(fLocal.upload(local, stream, arena));
+		CUDA_TRY(ctaRow.upload(rows, stream, &arena)); CUDA_TRY(needPtr.upload(nptr, stream, &arena)); CUDA_TRY(needCol.upload(ncol, stream, &arena));
+		CUDA_TRY(fLocal.upload(local, stream, &arena));
 		const size_t n6 = 6 * (size_t)numP;
 		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull)); CUDA_TRY(Linv.alloc(36 * (size_t)numP));
 		CUDA_TRY(vR0.alloc(n6)); CUDA_TRY(vR1.alloc(n6)); CUDA_TRY(vS0.alloc(n6)); CUDA_TRY(vS1.alloc(n6));
@@ -1301,7 +1359,7 @@ struct Engine : EngineBase {
 			CoarsePartition CP;
 			build_coarse_partition(numP, PP, maxAgg, CP);
 			const int gs = CP.gs, A = CP.A, nc = 6 * A;
-			pcg4A = A; pcg4Gs = gs; pcg4MaxNeedAgg = CP.maxNeedAgg;
+			pcg4Gs = gs; pcg4MaxNeedAgg = CP.maxNeedAgg;
 			size_t fixed4 = (size_t)needMax * (12 * sizeof(T) + 8) + (size_t)maxRows * (6 * sizeof(T) + 8) + 8 + 2 * (size_t)nc * sizeof(T)
 				+ (size_t)pcg4MaxNeedAgg * (6 * sizeof(T) + 4) + 64;
 			// shared-memory priorities: all of A^ first, then Z^ of the needed columns, then the CTA's slices of the inverse coarse matrix
@@ -1326,19 +1384,15 @@ struct Engine : EngineBase {
 				if (perSM4 < 1) pcg4Ok = false;
 			}
 			if (pcg4Ok) {
-				CUDA_TRY(cAggRow.upload(CP.aggRow, stream, arena)); CUDA_TRY(cNaPtr.upload(CP.naPtr, stream, arena)); CUDA_TRY(cNaList.upload(CP.naList, stream, arena));
-				CUDA_TRY(cNeedAgg.upload(CP.needAgg, stream, arena));
 				// fine blocks of every coarse block (lower triangle), ascending -> fixed-order sums in k_coarse_assemble
 				build_coarse_lists(numP, S.nfull, S.fRowPtr, S.fColInd, CP);
-				CUDA_TRY(cRowOf.upload(CP.rowOf, stream, arena)); CUDA_TRY(cCbPtr.upload(CP.cbPtr, stream, arena)); CUDA_TRY(cCbList.upload(CP.cbList, stream, arena));
+				int rc = coarse4.upload(CP, stream, &arena); if (rc) return rc;
 				CUDA_TRY(cZx.alloc(36 * (size_t)numP)); CUDA_TRY(cZhat.alloc(36 * (size_t)numP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull));
-				CUDA_TRY(cAcP.alloc((size_t)A * (A + 1) / 2 * 36)); CUDA_TRY(cAcInv.alloc((size_t)nc * nc));
-				if (A > PCG4_MAXAGG1) CUDA_TRY(cdT.alloc(cdense::scratch_doubles(A)));
+				if (coarse_kernel(A) == CUBA_COARSE_KERNEL_DENSE) CUDA_TRY(cdT.alloc(cdense::scratch_doubles(A)));
 				CUDA_TRY(cPart.alloc(2 * (size_t)G * PCG4_PSTRIDE)); CUDA_TRY(cInfo.alloc(1));
 				CUDA_TRY(cudaMemsetAsync(cPart.p, 0, sizeof(double) * cPart.n, stream));
 				// (no synchronisation: the uploads above read the pinned arena, or were staged by the driver before returning)
 			}
-			tlActive = false; coarseValid = false; coarseAge = 0;
 		}
 		return CUBA_OK;
 	}
@@ -1347,25 +1401,13 @@ struct Engine : EngineBase {
 	int launch_pcg4()
 	{
 		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
-		const int numP = S.numP, A = pcg4A;
+		const int numP = S.numP;
 		KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, cZx.p);
-		if (coarse_due(coarseValid, coarseAge, coarseLambda)) {
-			int rc = launch_coarse_setup(A, cCbPtr, cCbList, cAcP, cAcInv, cInfo.p); if (rc) return rc;     // slot 0 of cInfo
-			coarseValid = true; coarseAge = 0; coarseLambda = curLambda;
-		}
-		coarseAge++;
+		int rc = coarse_refresh(coarse4, coarse_scratch(), cInfo.p); if (rc) return rc;     // slot 0 of cInfo
 		Pcg4Args<T> b;
-		Pcg2Args<T>& a = b.base;
-		a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = fLocal; a.fVal = fVal; a.fHat = fHat;
-		a.ctaRow = ctaRow; a.needPtr = needPtr; a.needCol = needCol; a.b = bsc; a.numP = S.numP; a.Linv = Linv;
-		a.R0 = vR0; a.R1 = vR1; a.S0 = vS0; a.S1 = vS1; a.W0 = vW0; a.W1 = vW1; a.P = vP; a.Y = vY; a.x = xp;
-		a.partial = pcg2Partial; a.bar = gridBar; a.capBlocks = pcg4Cap; a.needMax = pcg2NeedMax; a.maxRows = pcg2MaxRows;
-		a.maxIters = cfg.pcg_max_iters > 0 ? cfg.pcg_max_iters : std::max(200, 40 * S.numP);
-		const double tol = cfg.pcg_tol > 0 ? cfg.pcg_tol : (sizeof(T) == 8 ? 1e-11 : 1e-6);
-		a.tol2 = tol * tol;
-		a.status = &dScal.p->pcg;
-		b.Zx = cZx; b.Zhat = cZhat; b.AcInv = cAcInv; b.aggRow = cAggRow; b.naPtr = cNaPtr; b.naList = cNaList; b.needAgg = cNeedAgg;
-		b.A = A; b.gs = pcg4Gs; b.maxNeedAgg = pcg4MaxNeedAgg; b.sliceInSmem = pcg4SliceInSmem; b.zhInSmem = pcg4ZhInSmem; b.cpart = cPart;
+		b.base = pcg2_args(pcg4Cap);
+		b.Zx = cZx; b.Zhat = cZhat; b.AcInv = coarse4.AcInv; b.aggRow = coarse4.aggRow; b.naPtr = coarse4.naPtr; b.naList = coarse4.naList;
+		b.needAgg = coarse4.needAgg; b.A = coarse4.A; b.gs = pcg4Gs; b.maxNeedAgg = pcg4MaxNeedAgg; b.sliceInSmem = pcg4SliceInSmem; b.zhInSmem = pcg4ZhInSmem; b.cpart = cPart;
 		b.timing = nullptr;
 #ifdef CUBA_PCG_TIMING
 		CUDA_TRY(pcgTiming.alloc(8 * (size_t)pcg2Grid));
@@ -1385,18 +1427,31 @@ struct Engine : EngineBase {
 	// as the LM damping falls.  The decision depends on iteration counts only, so runs stay bit-reproducible.
 	void note_pcg_iters(int iters) { if (!lastPcgTwoLevel && iters > (cfg.reserved[5] > 0 ? cfg.reserved[5] : 100)) tlActive = true; }
 
-	int launch_pcg2(bool flagged)
+	// the iteration cap and the squared relative tolerance of every PCG solve
+	int pcg_max_iters() const { return cfg.pcg_max_iters > 0 ? cfg.pcg_max_iters : std::max(200, 40 * S.numP); }
+	double pcg_tol2() const
 	{
-		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
+		const double tol = cfg.pcg_tol > 0 ? cfg.pcg_tol : (sizeof(T) == 8 ? 1e-11 : 1e-6);
+		return tol * tol;
+	}
+
+	// the arguments of k_pcg2 / k_pcg3, and the block-Jacobi part of k_pcg4's, with capBlocks blocks of A^ in shared memory
+	Pcg2Args<T> pcg2_args(int capBlocks)
+	{
 		Pcg2Args<T> a;
 		a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = fLocal; a.fVal = fVal; a.fHat = fHat;
 		a.ctaRow = ctaRow; a.needPtr = needPtr; a.needCol = needCol; a.b = bsc; a.numP = S.numP; a.Linv = Linv;
 		a.R0 = vR0; a.R1 = vR1; a.S0 = vS0; a.S1 = vS1; a.W0 = vW0; a.W1 = vW1; a.P = vP; a.Y = vY; a.x = xp;
-		a.partial = pcg2Partial; a.bar = gridBar; a.capBlocks = pcg2Cap; a.needMax = pcg2NeedMax; a.maxRows = pcg2MaxRows;
-		a.maxIters = cfg.pcg_max_iters > 0 ? cfg.pcg_max_iters : std::max(200, 40 * S.numP);
-		const double tol = cfg.pcg_tol > 0 ? cfg.pcg_tol : (sizeof(T) == 8 ? 1e-11 : 1e-6);
-		a.tol2 = tol * tol;
+		a.partial = pcg2Partial; a.bar = gridBar; a.capBlocks = capBlocks; a.needMax = pcg2NeedMax; a.maxRows = pcg2MaxRows;
+		a.maxIters = pcg_max_iters(); a.tol2 = pcg_tol2();
 		a.status = &dScal.p->pcg;
+		return a;
+	}
+
+	int launch_pcg2(bool flagged)
+	{
+		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
+		const Pcg2Args<T> a = pcg2_args(pcg2Cap);
 		if (flagged) {
 			Pcg3Args<T> b;
 			b.base = a;
@@ -1424,54 +1479,60 @@ struct Engine : EngineBase {
 
 
 	// ---- k_pcg5: two-level, flag-synchronised, rows distributed over the ranks (cuba_pcg5.cuh) --------------------------
-	DBuf<int> p5CtaRow, p5NeedPtr, p5NeedCol, p5Local, p5AggRow, p5NaPtr, p5NaList, p5NeedAgg, p5CbPtr, p5CbList;
-	DBuf<unsigned char> p5RowPeers;
-	DBuf<T> p5Linv, p5R0, p5Zhat, p5RcRow, p5Rc0;
-	DBuf<float> p5AcInv;
-	DBuf<double> p5AcP;
+	// A launch shape of a k_pcg5 plan: k_pcg5 (256 threads, BIG or not: pcg5_legacy_shape) or the tuned one-GPU k_pcg5t
+	// (cuba_pcg5t.cuh), its two-level dimensions (block_jacobi_dims: the block-Jacobi ones), kernel, block and dynamic shared
+	// memory.  perSM: CTAs per SM, 0 when the plan does not fit.
+	struct P5Shape {
+		bool tuned = false, big = false;
+		Pcg5Dims dims{}; p5t::Pcg5Dims tDims{};   // k_pcg5 / k_pcg5t
+		const void* fn = nullptr; int block = PCG5_BLOCK, perSM = 0; size_t smem = 0;
+	};
+	// One rank's boards in 16-byte words: [2 solve halves][2 pass parities] of w, of the per-CTA partials, of the rank summaries
+	// and of the coarse corrections, then the control block at 8-byte word ctl; words: 8-byte words of the whole set.
+	struct P5Boards { size_t w = 0, p = 0, r = 0, c = 0, ctl = 0, words = 0; };
+	// One k_pcg5 solve set up on the device (pcg5_upload): a plan's lists, coarse level and vectors, and its launch shape
+	struct Pcg5Run {
+		int numP = 0, G = 0, W = 1, gs = 1, apc = 1;
+		P5Shape sh;
+		DBuf<int> ctaRow, needPtr, needCol, local;
+		DBuf<unsigned char> rowPeers;
+		CoarseLevel coarse;
+		DBuf<T> Linv, R0, Zhat, rcRow, rc0;
+		P5Boards boards() const
+		{
+			const size_t NR = 3 + 6 * (size_t)(G / gs);
+			P5Boards b;
+			b.w = 4 * 6 * (size_t)numP; b.p = 4 * (size_t)PCG5_REPL * G * p5t::pcg5t_np(apc);
+			b.r = 4 * (size_t)PCG5_REPL * W * NR; b.c = 4 * (size_t)PCG5_REPL * 6 * coarse.A;
+			b.ctl = 2 * (b.w + b.p + b.r + b.c);
+			b.words = b.ctl + (sizeof(Pcg5Ctl) + 7) / 8 + 2;
+			return b;
+		}
+		Pcg5Ctl* ctl(unsigned long long* base) const { return (Pcg5Ctl*)(base + boards().ctl); }
+	};
+	Pcg5Run p5;                                    // the engine's own (setup_pcg5)
 	DBuf<unsigned long long> p5Boards;
-	void* p5PeerBase[PCG5_MAXWORLD] = { nullptr };   // cudaIpc mappings of the peers' boards (own entry: the local allocation)
-	void* p5MappedFor = nullptr;                   // local allocation the mappings were exchanged for
-	size_t p5WWords = 0, p5PWords = 0, p5RWords = 0, p5CWords = 0;
+	P5Boards p5Layout;                             // the layout p5Boards was cleared for
+	PeerMap p5Peer;                                // the peers' boards
 	PcgPartition hostPP;                           // host copy of k_pcg3's row partition of the current system (setup_pcg2)
-	Pcg5Dims p5Dims{}, p5DimsBJ{};
-	size_t p5Smem = 0;
-	int p5G = 0, p5W = 1, p5A = 0, p5Gs = 1;
-	bool p5Ok = false, p5Dist = false, p5Big = false, p5Tuned = false;
-	p5t::Pcg5Dims p5tDims{}, p5tDimsBJ{};            // the tuned one-GPU shape (cuba_pcg5t.cuh), when p5Tuned
-	const void* p5Fn = nullptr;
-	int p5Block = PCG5_BLOCK;
-	bool p5CoarseValid = false; int p5CoarseAge = 0; double p5CoarseLambda = 0;
-	int p5Apc = 1;                                 // aggregates per CTA of the plan (k_pcg5t)
+	bool p5Ok = false, p5Dist = false;
 	// read by cuba_debug_get_pcg_info only: the kernel of the last solve (CUBA_PCG_KERNEL_*), counters since set_problem, and a
 	// log of the cInfo flag of every k_pcg5 coarse rebuild -- rebuild n writes slot 1 + n % P5_INFO_LOG of cInfo (k_pcg4 keeps
 	// slot 0), so no rebuild's outcome is overwritten by the next one and nothing is copied on the solve's path
 	static constexpr int P5_INFO_LOG = 256;
 	int lastPcgKernel = CUBA_PCG_KERNEL_NONE;
-	long long p5Rebuilds = 0, bjRetries = 0;
-	int* p5InfoSlot() const { return cInfo.p + 1 + (int)(p5Rebuilds % P5_INFO_LOG); }
+	long long bjRetries = 0;
+	int* p5InfoSlot() const { return cInfo.p + 1 + (int)(p5.coarse.rebuilds % P5_INFO_LOG); }
 	long long p5TagBound = 0;                      // conservative host-side bound on the device tag base
-
-	Pcg5Ctl* p5Ctl(void* base) const { return (Pcg5Ctl*)((unsigned long long*)base + 2 * (p5WWords + p5PWords + p5RWords + p5CWords)); }
-
-	void p5CloseMappings()
-	{
-		for (int r = 0; r < PCG5_MAXWORLD; r++) {
-			if (p5PeerBase[r] && r != rank) cudaIpcCloseMemHandle(p5PeerBase[r]);
-			p5PeerBase[r] = nullptr;
-		}
-		p5MappedFor = nullptr;
-	}
 
 	// Maps one device allocation of every peer into this process (cudaIpc over NVLink peer access); the 64-byte handles travel by
 	// ncclAllGather.  All ranks agree on the outcome (sum of per-rank success flags), so either everybody uses the peer path or
 	// everybody keeps the NCCL one.
-	int ipcExchange(void* localBase, void** peerBase, void*& mappedFor, bool& ok)
+	int ipcExchange(void* localBase, PeerMap& m, bool& ok)
 	{
 		ok = false;
-		if (mappedFor == localBase) { ok = true; return CUBA_OK; }
-		for (int r = 0; r < PCG5_MAXWORLD; r++) { if (peerBase[r] && r != rank) cudaIpcCloseMemHandle(peerBase[r]); peerBase[r] = nullptr; }
-		mappedFor = nullptr;
+		if (m.mappedFor == localBase) { ok = true; return CUBA_OK; }
+		m.close(rank);
 		cudaIpcMemHandle_t mine;
 		int good = cudaIpcGetMemHandle(&mine, localBase) == cudaSuccess ? 1 : 0;
 		if (!good) cudaGetLastError();
@@ -1484,8 +1545,8 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaMemcpyAsync(all.data(), dh.p, sizeof(cudaIpcMemHandle_t) * (size_t)world, cudaMemcpyDeviceToHost, stream));
 		CUDA_TRY(cudaStreamSynchronize(stream));
 		for (int r = 0; r < world && good; r++) {
-			if (r == rank) { peerBase[r] = localBase; continue; }
-			if (cudaIpcOpenMemHandle(&peerBase[r], all[r], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); peerBase[r] = nullptr; good = 0; }
+			if (r == rank) { m.base[r] = localBase; continue; }
+			if (cudaIpcOpenMemHandle(&m.base[r], all[r], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); m.base[r] = nullptr; good = 0; }
 		}
 		// agreement
 		DBuf<double> flag;
@@ -1496,35 +1557,32 @@ struct Engine : EngineBase {
 		double tot = 0;
 		CUDA_TRY(cudaMemcpyAsync(&tot, flag.p, sizeof(double), cudaMemcpyDeviceToHost, stream));
 		CUDA_TRY(cudaStreamSynchronize(stream));
-		if ((int)(tot + 0.5) != world) {
-			for (int r = 0; r < PCG5_MAXWORLD; r++) { if (peerBase[r] && r != rank) cudaIpcCloseMemHandle(peerBase[r]); peerBase[r] = nullptr; }
-			return CUBA_OK;
-		}
-		mappedFor = localBase;
+		if ((int)(tot + 0.5) != world) { m.close(rank); return CUBA_OK; }
+		m.mappedFor = localBase;
 		ok = true;
 		return CUBA_OK;
 	}
-	int p5Exchange(bool& ok) { return ipcExchange((void*)p5Boards.p, p5PeerBase, p5MappedFor, ok); }
 
 	// ---- the per-trial Hsc | bsc all-reduce over peer memory (cuba_peer_reduce.cuh) ----
-	void* uPeerBase[PCG5_MAXWORLD] = { nullptr };
-	void* uMappedFor = nullptr;
+	PeerMap uPeer;
 	bool uPeerOk = false;
 	unsigned int uEpoch = 0;
 	size_t uCount = 0;             // elements of the all-reduced part of uVal
-	void uCloseMappings()
+	// a buffer of the peer all-reduce holds n elements, then the signal block at this element
+	static size_t peer_signal_offset(size_t n) { return (n + 1) & ~(size_t)1; }
+	// the arguments of rank r of W whose buffers start at bufs[0..W-1]
+	static peer::Args<T> peer_args(void* const* bufs, int r, int W, size_t n, unsigned int epoch, GridBar* bar)
 	{
-		for (int r = 0; r < PCG5_MAXWORLD; r++) { if (uPeerBase[r] && r != rank) cudaIpcCloseMemHandle(uPeerBase[r]); uPeerBase[r] = nullptr; }
-		uMappedFor = nullptr; uPeerOk = false;
+		peer::Args<T> a;
+		const size_t sigOff = peer_signal_offset(n);
+		for (int q = 0; q < peer::MAXW; q++) { a.peers[q] = nullptr; a.sigPeer[q] = nullptr; }
+		for (int q = 0; q < W; q++) { a.peers[q] = (T*)bufs[q]; a.sigPeer[q] = (unsigned int*)((T*)bufs[q] + sigOff); }
+		a.local = a.peers[r]; a.sigLocal = a.sigPeer[r]; a.n = n; a.rank = r; a.world = W; a.epoch = epoch; a.bar = bar;
+		return a;
 	}
 	int launch_peer_allreduce()
 	{
-		peer::Args<T> pa;
-		pa.local = uVal.p; pa.n = uCount; pa.rank = rank; pa.world = world; pa.epoch = ++uEpoch; pa.bar = gridBar;
-		const size_t sigOff = (uCount + 1) & ~(size_t)1;       // the signal block sits behind the data (element units)
-		for (int r = 0; r < peer::MAXW; r++) { pa.peers[r] = nullptr; pa.sigPeer[r] = nullptr; }
-		for (int r = 0; r < world; r++) { pa.peers[r] = (T*)uPeerBase[r]; pa.sigPeer[r] = (unsigned int*)((T*)uPeerBase[r] + sigOff); }
-		pa.sigLocal = (unsigned int*)(uVal.p + sigOff);
+		peer::Args<T> pa = peer_args(uPeer.base, rank, world, uCount, ++uEpoch, gridBar);
 		void* args[] = { (void*)&pa };
 		CUDA_TRY(cudaLaunchCooperativeKernel((void*)peer::k_peer_allreduce<T>, dim3(numSMs), dim3(peer::BLOCK), args, 0, stream));
 		launches++;
@@ -1533,22 +1591,9 @@ struct Engine : EngineBase {
 
 	int pcg5_max_agg() const { return (cfg.reserved[6] > 0 && cfg.reserved[6] < PCG5_MAXAGG) ? cfg.reserved[6] : PCG5_MAXAGG; }
 
-	// The dimensions of a k_pcg5 plan over W ranks that do not depend on the launch shape (capBlocks and zhInSmem stay 0).
-	static Pcg5Dims pcg5_plan_dims(const Pcg5Plan& plan, int W)
-	{
-		const int G = plan.G, nc = 6 * plan.A, NR = 3 + 6 * (G / plan.gs);
-		Pcg5Dims d{};
-		d.needMax = plan.P.needMax; d.maxRows = plan.P.maxRows; d.nc = nc; d.maxNeedAgg = plan.C.maxNeedAgg;
-		d.npv = std::max(std::max(G * p5t::pcg5t_np(plan.apc), W * NR), 6 * plan.C.maxNeedAgg); d.nls = NR;
-		d.sliceRows = (nc + G - 1) / G;
-		return d;
-	}
-
 	// k_pcg5's legacy (256-thread) shape for a plan: the blocks cached in shared memory, Z^ in shared memory or not, BIG or not, the
-	// block-Jacobi dimensions, the dynamic shared memory and the kernel -- k_pcg5, or with `ranks` k_pcg5_ranks (W ranks emulated in
-	// one launch, cuba_debug_pcg5_ranks), so that the emulation runs the shape a W-GPU run would.  perSM: CTAs per SM, 0 when the
-	// plan does not fit.
-	struct P5Shape { Pcg5Dims dims{}, dimsBJ{}; size_t smem = 0; bool big = false; const void* fn = nullptr; int perSM = 0; };
+	// dynamic shared memory and the kernel -- k_pcg5, or with `ranks` k_pcg5_ranks for cuba_debug_pcg5_ranks, whose W ranks emulated
+	// in one launch thus run the shape of a W-GPU run, as they run its upload, board layout and arguments.
 	int pcg5_legacy_shape(const Pcg5Plan& plan, Pcg5Dims d, int W, bool ranks, P5Shape& sh)
 	{
 		sh = P5Shape{};
@@ -1573,22 +1618,21 @@ struct Engine : EngineBase {
 			if ((size_t)d.capBlocks < wantCache) big = true;
 			if (big) d.capBlocks = (int)std::min((size_t)PP.blkMax, (budget - fixed) / per);
 		}
-		Pcg5Dims dBJ = d; dBJ.nc = 0; dBJ.maxNeedAgg = 0; dBJ.zhInSmem = 0; dBJ.sliceRows = 0; dBJ.nls = 3; dBJ.npv = std::max(plan.G * 3, W * 3);
-		const size_t smem = std::max(Pcg5Layout<T>(d).total, Pcg5Layout<T>(dBJ).total);
+		const size_t smem = std::max(Pcg5Layout<T>(d).total, Pcg5Layout<T>(block_jacobi_dims(d, plan.G, W)).total);
 		if (smem > (size_t)smemMax - 1024) return CUBA_OK;
 		const void* fn = ranks ? (big ? (const void*)k_pcg5_ranks<T, true> : (const void*)k_pcg5_ranks<T, false>)
 		                       : (big ? (const void*)k_pcg5<T, true> : (const void*)k_pcg5<T, false>);
 		CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 		int perSM = 0;
 		CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fn, PCG5_BLOCK, smem));
-		sh.dims = d; sh.dimsBJ = dBJ; sh.smem = smem; sh.big = big; sh.fn = fn; sh.perSM = perSM;
+		sh.dims = d; sh.smem = smem; sh.big = big; sh.fn = fn; sh.perSM = perSM;
 		return CUBA_OK;
 	}
 
 	// Partition of the rows over world x G virtual CTAs, aggregates aligned with the ranks, shared-memory budget, boards.
 	int setup_pcg5()
 	{
-		p5Ok = false; p5Dist = false; p5CoarseValid = false; p5CoarseAge = 0;
+		p5Ok = false; p5Dist = false;
 		const int numP = S.numP;
 		if (numP < 1) return CUBA_OK;
 		const int mode = cfg.reserved[0];
@@ -1607,90 +1651,80 @@ struct Engine : EngineBase {
 		const bool tryTuned = W == 1 && !getenv("CUBA_PCG5_LEGACY");
 		int apcTop = p5t::DEFAULT_APC;
 		if (const char* e = getenv("CUBA_PCG5_AGGS_PER_CTA")) apcTop = std::min(3, std::max(1, atoi(e)));
-		p5Tuned = false;
 		Pcg5Plan plan;
-		Pcg5Dims d{};
-		int NR = 0;
-		for (int apc = tryTuned ? apcTop : 1; apc >= 1 && !p5Tuned; apc--) {
+		P5Shape sh;
+		for (int apc = tryTuned ? apcTop : 1; apc >= 1 && !sh.tuned; apc--) {
 			build_pcg5_plan(numP, S.nfull, S.fRowPtr, S.fColInd, W, numSMs, maxAgg, 2 * PCG5_BLOCK / 6, plan, &hostPP, apc);
 			if (!plan.ok) continue;
-			const int G = plan.G;
-			const PcgPartition& PP = plan.P;
-			d = pcg5_plan_dims(plan, W);
-			NR = d.nls;
 			if (!tryTuned) break;
 			using TS = p5t::Pcg5Shape;
 			p5t::Pcg5Dims t = pcg5t_plan_dims(plan);
-			if (PP.maxRows * 6 <= TS::BLOCK && p5t::pcg5t_fit<T>(t, PP.blkMax, apc, budget)) {
-				p5tDims = t;
-				p5tDimsBJ = t; p5tDimsBJ.nc = 0; p5tDimsBJ.maxNeedAgg = 0; p5tDimsBJ.zhInSmem = 0; p5tDimsBJ.sliceRows = 0; p5tDimsBJ.nls = 3; p5tDimsBJ.npv = std::max(G * 3, W * 3);
-				const size_t smemT = std::max(p5t::Pcg5Layout<T>(p5tDims).total, p5t::Pcg5Layout<T>(p5tDimsBJ).total);
+			if (plan.P.maxRows * 6 <= TS::BLOCK && p5t::pcg5t_fit<T>(t, plan.P.blkMax, apc, budget)) {
+				const size_t smemT = std::max(p5t::Pcg5Layout<T>(t).total, p5t::Pcg5Layout<T>(block_jacobi_dims(t, plan.G, W)).total);
 				const void* fn = apc == 3 ? (const void*)p5t::k_pcg5t<T, 3> : apc == 2 ? (const void*)p5t::k_pcg5t<T, 2> : (const void*)p5t::k_pcg5t<T, 1>;
 				int perSM = 0;
 				if (smemT <= (size_t)smemMax - 1024 && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemT) == cudaSuccess &&
 					cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fn, TS::BLOCK, smemT) == cudaSuccess && perSM >= 1) {
-					p5Tuned = true; p5Big = false; p5Fn = fn; p5Block = TS::BLOCK; p5Smem = smemT;
-					p5Dims = Pcg5Dims{}; p5Dims.capBlocks = t.capBlocks;
-					d.capBlocks = t.capBlocks; d.zhInSmem = t.zhInSmem;
+					sh.tuned = true; sh.tDims = t; sh.fn = fn; sh.block = TS::BLOCK; sh.smem = smemT; sh.perSM = perSM;
 				} else cudaGetLastError();
 			}
 			// the other shapes take one aggregate per CTA group
-			if (!p5Tuned && apc == 1) break;
+			if (!sh.tuned && apc == 1) break;
 		}
 		if (!plan.ok) return CUBA_OK;
-		const int G = plan.G, gs = plan.gs, A = plan.A;
-		const PcgPartition& PP = plan.P; const CoarsePartition& CP = plan.C;
-		const std::vector<unsigned char>& peers = plan.rowPeers;
-		const int nc = 6 * A;
-		if (!p5Tuned) {
-			P5Shape sh;
-			int rc = pcg5_legacy_shape(plan, d, W, false, sh); if (rc) return rc;
+		if (!sh.tuned) {
+			int rc = pcg5_legacy_shape(plan, pcg5_plan_dims(plan, W), W, false, sh); if (rc) return rc;
 			if (sh.perSM < 1) return CUBA_OK;
-			d = sh.dims; p5Dims = sh.dims; p5DimsBJ = sh.dimsBJ; p5Smem = sh.smem; p5Big = sh.big; p5Fn = sh.fn;
-			p5Block = PCG5_BLOCK;
 		}
-		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: world %d G %d gs %d A %d aggsPerCta %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceRows %d cap %d smem %zu\n",
-			W, G, gs, A, plan.apc, d.needMax, d.maxRows, PP.blkMax, d.maxNeedAgg, d.zhInSmem, d.sliceRows, d.capBlocks, p5Smem);
-		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg5: shape %s, %d threads\n", p5Big ? "big" : p5Tuned ? "tuned" : "legacy", p5Block);
-		const size_t nblkPz = (size_t)A * (A + 1) / 2;
-		CUDA_TRY(p5CtaRow.upload(PP.rows, stream, arena)); CUDA_TRY(p5NeedPtr.upload(PP.nptr, stream, arena)); CUDA_TRY(p5NeedCol.upload(PP.ncol, stream, arena));
-		CUDA_TRY(p5Local.upload(PP.local, stream, arena)); CUDA_TRY(p5RowPeers.upload(peers, stream, arena));
-		CUDA_TRY(p5AggRow.upload(CP.aggRow, stream, arena)); CUDA_TRY(p5NaPtr.upload(CP.naPtr, stream, arena)); CUDA_TRY(p5NaList.upload(CP.naList, stream, arena));
-		CUDA_TRY(p5NeedAgg.upload(CP.needAgg, stream, arena)); CUDA_TRY(p5CbPtr.upload(CP.cbPtr, stream, arena)); CUDA_TRY(p5CbList.upload(CP.cbList, stream, arena));
-		CUDA_TRY(cRowOf.upload(CP.rowOf, stream, arena));
-		const size_t nP = (size_t)numP;
-		CUDA_TRY(p5Linv.alloc(36 * nP)); CUDA_TRY(p5R0.alloc(6 * nP)); CUDA_TRY(p5Zhat.alloc(36 * nP)); CUDA_TRY(p5RcRow.alloc(6 * nP)); CUDA_TRY(p5Rc0.alloc(std::max(nc, 1)));
-		CUDA_TRY(cZx.alloc(36 * nP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(cInfo.alloc(1 + P5_INFO_LOG));
+		auto show = [&](const auto& d) {
+			fprintf(stderr, "pcg5: world %d G %d gs %d A %d aggsPerCta %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceRows %d cap %d smem %zu\n",
+				W, plan.G, plan.gs, plan.A, plan.apc, d.needMax, d.maxRows, plan.P.blkMax, d.maxNeedAgg, d.zhInSmem, d.sliceRows, d.capBlocks, sh.smem);
+			fprintf(stderr, "pcg5: shape %s, %d threads\n", sh.big ? "big" : sh.tuned ? "tuned" : "legacy", sh.block);
+		};
+		if (getenv("CUBA_PCG_VERBOSE")) { if (sh.tuned) show(sh.tDims); else show(sh.dims); }
+		int rc = pcg5_upload(p5, plan, sh, W, &arena); if (rc) return rc;
+		CUDA_TRY(cZx.alloc(36 * (size_t)numP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(cInfo.alloc(1 + P5_INFO_LOG));
 		CUDA_TRY(cudaMemsetAsync(cInfo.p, 0, sizeof(int) * cInfo.n, stream));
 		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull));
-		CUDA_TRY(p5AcP.alloc(nblkPz * 36)); CUDA_TRY(p5AcInv.alloc((size_t)nc * nc));
-		if (A > PCG4_MAXAGG1) {
-			CUDA_TRY(cdT.alloc(cdense::scratch_doubles(A)));
+		if (coarse_kernel(plan.A) == CUBA_COARSE_KERNEL_DENSE) {
+			CUDA_TRY(cdT.alloc(cdense::scratch_doubles(plan.A)));
 			CUDA_TRY(gridBar.alloc(1));
 		}
-		// boards (16-byte words): [2 solve halves][2 pass parities] of w, of the per-CTA partials and of the rank summaries, then the control block
-		const size_t wW = 4 * 6 * nP, pW = 4 * (size_t)PCG5_REPL * G * p5t::pcg5t_np(plan.apc), rW = 4 * (size_t)PCG5_REPL * W * NR, cW = 4 * (size_t)PCG5_REPL * nc;
-		const size_t words2 = 2 * (wW + pW + rW + cW) + (sizeof(Pcg5Ctl) + 7) / 8 + 2;
-		const bool fresh = !p5Boards.p || words2 > p5Boards.cap || wW != p5WWords || pW != p5PWords || rW != p5RWords || cW != p5CWords;
+		const P5Boards b = p5.boards();
+		const bool fresh = !p5Boards.p || b.words > p5Boards.cap || b.w != p5Layout.w || b.p != p5Layout.p || b.r != p5Layout.r || b.c != p5Layout.c;
 		if (fresh) {
 			// the tag protocol needs boards that start out as zeros; a layout change invalidates every mapping and every tag
-			if (p5MappedFor) { CUDA_TRY(cudaStreamSynchronize(stream)); p5CloseMappings(); }
-			CUDA_TRY(p5Boards.alloc(std::max(words2, (size_t)(1u << 18))));
+			if (p5Peer.mappedFor) { CUDA_TRY(cudaStreamSynchronize(stream)); p5Peer.close(rank); }
+			CUDA_TRY(p5Boards.alloc(std::max(b.words, (size_t)(1u << 18))));
 			CUDA_TRY(cudaMemsetAsync(p5Boards.p, 0, sizeof(unsigned long long) * p5Boards.cap, stream));
-			p5WWords = wW; p5PWords = pW; p5RWords = rW; p5CWords = cW;
+			p5Layout = b;
 			p5TagBound = 0;
 		}
-		p5G = G; p5W = W; p5A = A; p5Gs = gs; p5Apc = plan.apc;
 		if (W > 1) {
 			bool ok = false;
-			int rc = p5Exchange(ok); if (rc) return rc;
+			rc = ipcExchange((void*)p5Boards.p, p5Peer, ok); if (rc) return rc;
 			if (!ok) {
 				if (rank == 0) fprintf(stderr, "cuba_b200: cudaIpc mapping of the peers' PCG boards failed; keeping the replicated PCG\n");
 				return CUBA_OK;
 			}
 			p5Dist = true;
-		} else p5PeerBase[rank] = (void*)p5Boards.p;
+		} else p5Peer.base[rank] = (void*)p5Boards.p;
 		p5Ok = true;
+		return CUBA_OK;
+	}
+
+	// R for a solve of `plan` over W ranks in shape sh: the plan's lists and coarse level (through the pinned arena when one is
+	// given), the vectors of the preparation
+	int pcg5_upload(Pcg5Run& R, const Pcg5Plan& plan, const P5Shape& sh, int W, PinnedArena* arena)
+	{
+		R.numP = S.numP; R.G = plan.G; R.W = W; R.gs = plan.gs; R.apc = plan.apc; R.sh = sh;
+		const PcgPartition& PP = plan.P;
+		CUDA_TRY(R.ctaRow.upload(PP.rows, stream, arena)); CUDA_TRY(R.needPtr.upload(PP.nptr, stream, arena)); CUDA_TRY(R.needCol.upload(PP.ncol, stream, arena));
+		CUDA_TRY(R.local.upload(PP.local, stream, arena)); CUDA_TRY(R.rowPeers.upload(plan.rowPeers, stream, arena));
+		int rc = R.coarse.upload(plan.C, stream, arena); if (rc) return rc;
+		const size_t nP = (size_t)S.numP;
+		CUDA_TRY(R.Linv.alloc(36 * nP)); CUDA_TRY(R.R0.alloc(6 * nP)); CUDA_TRY(R.Zhat.alloc(36 * nP)); CUDA_TRY(R.rcRow.alloc(6 * nP));
+		CUDA_TRY(R.rc0.alloc(std::max(6 * plan.A, 1)));
 		return CUBA_OK;
 	}
 
@@ -1707,22 +1741,20 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// coarse matrix Ac = Z^T S Z of the current system (basis cZx) and its inverse (fp32), for the aggregates behind (cbPtr, cbList);
-	// info: 0 inverted, 1 not positive definite (AcInv zeroed).  The inverse: one CTA while the packed triangle fits its shared
-	// memory (A <= PCG4_MAXAGG1), the blocked sweep on the whole chip above.
-	int launch_coarse_setup(int A, const int* cbPtr, const int* cbList, double* AcP, float* AcInv, int* info)
+	// scratch of a coarse rebuild: the coarse basis Zx of the current state, U [36 nfull], and for k_coarse_dense its tiles and a
+	// zeroed or reused GridBar
+	struct CoarseScratch { T* Zx; double* U; double* tiles; GridBar* bar; };
+	CoarseScratch coarse_scratch() const { return { cZx.p, cU.p, cdT.p, gridBar.p }; }
+
+	// coarse matrix Ac = Z^T S Z of the current system and its inverse (fp32), for the aggregates of L; info: 0 inverted, 1 not
+	// positive definite (AcInv zeroed).  The inverse: coarse_kernel(A).
+	int launch_coarse_setup(const CoarseLevel& L, const CoarseScratch& s, int* info)
 	{
-		return launch_coarse_setup(A, cbPtr, cbList, cRowOf, cZx, cU, cdT, gridBar, AcP, AcInv, info);
-	}
-	// the same on a plan's own aggregate map rowOf and basis Zx, with scratch U [36 nfull], and tiles and bar for A > PCG4_MAXAGG1
-	int launch_coarse_setup(int A, const int* cbPtr, const int* cbList, const int* rowOf, const T* Zx, double* U, double* tiles, GridBar* bar,
-		double* AcP, float* AcInv, int* info)
-	{
-		const int nblkP = A * (A + 1) / 2;
-		KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, rowOf, fColInd.p, S.nfull, Zx, U);
-		KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, cbPtr, cbList, U, nblkP, AcP);
-		if (A > PCG4_MAXAGG1) return launch_coarse_dense(AcP, A, tiles, AcInv, info, bar);
-		k_coarse_invert<T><<<1, 1024, coarse_invert_smem(A), stream>>>(AcP, A, AcInv, info);
+		const int A = L.A, nblkP = A * (A + 1) / 2;
+		KLAUNCH(k_coarse_project<T>, 36LL * S.nfull, fVal.p, L.rowOf.p, fColInd.p, S.nfull, s.Zx, s.U);
+		KLAUNCH(k_coarse_assemble, (long long)nblkP * 36, L.cbPtr.p, L.cbList.p, s.U, nblkP, L.AcP.p);
+		if (coarse_kernel(A) == CUBA_COARSE_KERNEL_DENSE) return launch_coarse_dense(L.AcP, A, s.tiles, L.AcInv, info, s.bar);
+		k_coarse_invert<T><<<1, 1024, coarse_invert_smem(A), stream>>>(L.AcP, A, L.AcInv, info);
 		launches++;
 		CUDA_TRY(cudaGetLastError());
 		return CUBA_OK;
@@ -1734,26 +1766,80 @@ struct Engine : EngineBase {
 	// 26..193 with one that is refreshed every fifth iteration).
 	// Measured limits of that freedom: a coarse inverse from an 81x larger damping costs nothing, one from a 1e5x larger damping
 	// costs 8x the iterations (1 276 vs 149 on kitti00_shaped) -> it is also rebuilt when the damping moved by more than 300x.
-	// valid / age / lambda: whether the solver holds an inverse, its two-level solves since the rebuild, the damping of the rebuild.
-	bool coarse_due(bool valid, int age, double lambda) const
+	bool coarse_due(const CoarseLevel& L) const
 	{
 		const int refreshEvery = cfg.reserved[4] > 0 ? cfg.reserved[4] : 8;
-		const double lamRatio = (valid && lambda > 0 && curLambda > 0) ? std::max(curLambda / lambda, lambda / curLambda) : 1.0;
-		return !valid || age >= refreshEvery || lamRatio > 300.0;
+		const double lamRatio = (L.valid && L.lambda > 0 && curLambda > 0) ? std::max(curLambda / L.lambda, L.lambda / curLambda) : 1.0;
+		return !L.valid || L.age >= refreshEvery || lamRatio > 300.0;
+	}
+	// before a two-level solve: L rebuilt when due, then the solve counted
+	int coarse_refresh(CoarseLevel& L, const CoarseScratch& s, int* info)
+	{
+		if (coarse_due(L)) {
+			int rc = launch_coarse_setup(L, s, info); if (rc) return rc;
+			L.valid = true; L.age = 0; L.lambda = curLambda; L.rebuilds++;
+		}
+		L.age++;
+		return CUBA_OK;
 	}
 
-	int pcg5_max_iters() const { return cfg.pcg_max_iters > 0 ? cfg.pcg_max_iters : std::max(200, 40 * S.numP); }
-	double pcg5_tol2() const
+	// nothing an earlier solve left behind is reused: block-Jacobi first, both coarse inverses rebuilt at their next two-level solve
+	void forget_solves() { tlActive = false; coarse4.forget(); p5.coarse.forget(); }
+
+	// The preparation of a solve of R on the current system: k_pcg5_prep_rows for each of the n control blocks ctl[] (the rows of
+	// Linv, R0, Z^ and rc0 are the same on every rank: computed once, each rank's breakdown counter counted in its own control
+	// block) and, two-level, the coarse basis, rc0 and the coarse level (coarse_refresh).
+	int pcg5_prepare(Pcg5Run& R, bool twoLevel, Pcg5Ctl* const* ctl, int n, const CoarseScratch& s, int* info)
 	{
-		const double tol = cfg.pcg_tol > 0 ? cfg.pcg_tol : (sizeof(T) == 8 ? 1e-11 : 1e-6);
-		return tol * tol;
+		const int numP = R.numP, A = twoLevel ? R.coarse.A : 0;
+		if (twoLevel) KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, s.Zx);
+		Pcg5PrepArgs<T> pa;
+		pa.fRowPtr = fRowPtr; pa.fColInd = fColInd; pa.fVal = fVal; pa.b = bsc; pa.Zx = s.Zx; pa.numP = numP; pa.A = A; pa.aggRow = R.coarse.aggRow;
+		pa.zhatFp32 = R.sh.tuned ? 1 : 0;
+		pa.Linv = R.Linv; pa.R0 = R.R0; pa.Zhat = R.Zhat; pa.rcRow = R.rcRow; pa.rc0 = R.rc0;
+		for (int r = 0; r < n; r++) {
+			pa.ctl = ctl[r];
+			k_pcg5_prep_rows<T><<<(numP + 127) / 128, 128, 0, stream>>>(pa);
+			launches++;
+		}
+		if (twoLevel) {
+			k_pcg5_prep_rc<T><<<(6 * A + 127) / 128, 128, 0, stream>>>(pa);
+			launches++;
+			int rc = coarse_refresh(R.coarse, s, info); if (rc) return rc;
+		}
+		CUDA_TRY(cudaGetLastError());
+		return CUBA_OK;
+	}
+
+	// The arguments of R's solve for its rank r of W: rank q's boards at bases[q] (bases[r]: this rank's own), A^ into hat, x and
+	// status as given.  k_pcg5 (Pcg5Args) and k_pcg5t (p5t::Pcg5Args) differ only in their dims and k_pcg5t's aggRow.
+	template <typename Args>
+	void pcg5_args(Args& a, const Pcg5Run& R, bool twoLevel, int r, int W, unsigned long long* const* bases, T* hat, T* x, PcgStatus* status) const
+	{
+		const P5Boards b = R.boards();
+		a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = R.local; a.fVal = fVal; a.fHat = hat;
+		a.ctaRow = R.ctaRow; a.needPtr = R.needPtr; a.needCol = R.needCol;
+		a.numP = R.numP; a.G = R.G; a.rank = r; a.world = W;
+		a.Linv = R.Linv; a.R0 = R.R0; a.Zhat = R.Zhat; a.rc0 = R.rc0; a.x = x;
+		a.maxIters = pcg_max_iters(); a.tol2 = pcg_tol2();
+		a.status = status;
+		a.AcInv = R.coarse.AcInv; a.naPtr = R.coarse.naPtr; a.naList = R.coarse.naList; a.needAgg = R.coarse.needAgg;
+		a.A = twoLevel ? R.coarse.A : 0; a.gs = R.gs;
+		for (int q = 0; q < PCG5_MAXWORLD; q++) { a.peerW[q] = nullptr; a.peerR[q] = nullptr; a.peerCtl[q] = nullptr; }
+		for (int q = 0; q < W; q++) { a.peerW[q] = bases[q]; a.peerR[q] = bases[q] + 2 * (b.w + b.p); a.peerCtl[q] = (Pcg5Ctl*)(bases[q] + b.ctl); }
+		unsigned long long* own = bases[r];
+		a.wBoard = own; a.pBoard = own + 2 * b.w; a.rBoard = own + 2 * (b.w + b.p); a.cBoard = own + 2 * (b.w + b.p + b.r);
+		a.rowPeers = R.rowPeers; a.ctl = (Pcg5Ctl*)(own + b.ctl);
+		a.timing = nullptr;
+		if constexpr (std::is_same<Args, Pcg5Args<T>>::value) a.dims = R.sh.dims;
+		else { a.dims = R.sh.tDims; a.aggRow = R.coarse.aggRow; }
+		if (!twoLevel) a.dims = block_jacobi_dims(a.dims, R.G, R.W);
 	}
 
 	int launch_pcg5(bool twoLevel)
 	{
 		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
-		const int numP = S.numP, A = twoLevel ? p5A : 0;
-		const int maxIters = pcg5_max_iters();
+		const int maxIters = pcg_max_iters();
 		// tags are 32 bits: long before the device tag base can wrap, every rank (same arithmetic everywhere) clears its boards
 		p5TagBound += (long long)maxIters + 8;
 		if (p5TagBound > (1LL << 31)) {
@@ -1762,75 +1848,32 @@ struct Engine : EngineBase {
 			if (p5Dist) { int rc0 = allreduce(&dScal.p->v[7], 1, false); if (rc0) return rc0; }
 			p5TagBound = (long long)maxIters + 8;
 		}
-		if (twoLevel) KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, cZx.p);
-		Pcg5PrepArgs<T> pa;
-		pa.fRowPtr = fRowPtr; pa.fColInd = fColInd; pa.fVal = fVal; pa.b = bsc; pa.Zx = cZx; pa.numP = numP; pa.A = A; pa.aggRow = p5AggRow; pa.zhatFp32 = p5Tuned ? 1 : 0;
-		pa.Linv = p5Linv; pa.R0 = p5R0; pa.Zhat = p5Zhat; pa.rcRow = p5RcRow; pa.rc0 = p5Rc0; pa.ctl = p5Ctl(p5Boards.p);
-		k_pcg5_prep_rows<T><<<(numP + 127) / 128, 128, 0, stream>>>(pa);
-		launches++;
-		if (twoLevel) {
-			k_pcg5_prep_rc<T><<<(6 * A + 127) / 128, 128, 0, stream>>>(pa);
-			launches++;
-			if (coarse_due(p5CoarseValid, p5CoarseAge, p5CoarseLambda)) {
-				int rc = launch_coarse_setup(A, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5InfoSlot()); if (rc) return rc;
-				p5CoarseValid = true; p5CoarseAge = 0; p5CoarseLambda = curLambda; p5Rebuilds++;
-			}
-			p5CoarseAge++;
-		}
-		CUDA_TRY(cudaGetLastError());
-		// the same arguments for both shapes (cuba_pcg5.cuh / cuba_pcg5t.cuh differ only in their Pcg5Dims)
-		auto fill = [&](auto& a) {
-			using CtlPtr = decltype(a.ctl);
-			a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = p5Local; a.fVal = fVal; a.fHat = fHat;
-			a.ctaRow = p5CtaRow; a.needPtr = p5NeedPtr; a.needCol = p5NeedCol;
-			a.numP = numP; a.G = p5G; a.rank = p5Dist ? rank : 0; a.world = p5W;
-			a.Linv = p5Linv; a.R0 = p5R0; a.Zhat = p5Zhat; a.rc0 = p5Rc0; a.x = xp;
-			a.maxIters = maxIters;
-			a.tol2 = pcg5_tol2();
-			a.status = &dScal.p->pcg;
-			a.AcInv = p5AcInv; a.naPtr = p5NaPtr; a.naList = p5NaList; a.needAgg = p5NeedAgg; a.A = A; a.gs = p5Gs;
-			for (int r = 0; r < PCG5_MAXWORLD; r++) { a.peerW[r] = nullptr; a.peerR[r] = nullptr; a.peerCtl[r] = nullptr; }
-			for (int r = 0; r < p5W; r++) {
-				unsigned long long* base = (unsigned long long*)p5PeerBase[p5Dist ? r : rank];
-				a.peerW[r] = base; a.peerR[r] = base + 2 * (p5WWords + p5PWords); a.peerCtl[r] = reinterpret_cast<CtlPtr>(p5Ctl(base));
-			}
-			a.wBoard = p5Boards.p; a.pBoard = p5Boards.p + 2 * p5WWords; a.rBoard = p5Boards.p + 2 * (p5WWords + p5PWords);
-			a.cBoard = p5Boards.p + 2 * (p5WWords + p5PWords + p5RWords);
-			a.rowPeers = p5RowPeers; a.ctl = reinterpret_cast<CtlPtr>(p5Ctl(p5Boards.p));
-			a.timing = nullptr;
-		};
+		Pcg5Ctl* ctl = p5.ctl(p5Boards.p);
+		int rc = pcg5_prepare(p5, twoLevel, &ctl, 1, coarse_scratch(), p5InfoSlot()); if (rc) return rc;
 #ifdef CUBA_PCG_TIMING
-		CUDA_TRY(pcgTiming.alloc(8 * (size_t)p5G));
+		CUDA_TRY(pcgTiming.alloc(8 * (size_t)p5.G));
 #endif
-		if (p5Dist) CUDA_TRY(cudaMemsetAsync(xp.p, 0, sizeof(T) * 6 * (size_t)numP, stream));     // rows of the other ranks: summed in below
-		Pcg5Args<T> a;
-		p5t::Pcg5Args<T> at;
-		void* args[1];
-		if (p5Tuned) {
-			fill(at);
-			at.aggRow = p5AggRow;
-			at.dims = twoLevel ? p5tDims : p5tDimsBJ;
-			at.dims.capBlocks = p5tDims.capBlocks;
-#ifdef CUBA_PCG_TIMING
-			at.timing = pcgTiming.p;
-#endif
-			args[0] = (void*)&at;
-		} else {
-			fill(a);
-			a.dims = twoLevel ? p5Dims : p5DimsBJ;
-			a.dims.capBlocks = p5Dims.capBlocks;
+		if (p5Dist) CUDA_TRY(cudaMemsetAsync(xp.p, 0, sizeof(T) * 6 * (size_t)S.numP, stream));     // rows of the other ranks: summed in below
+		// a replicated solve (p5.W == 1, also on a multi-rank engine) is rank 0 of one, on this rank's own boards
+		unsigned long long* bases[PCG5_MAXWORLD];
+		for (int r = 0; r < p5.W; r++) bases[r] = (unsigned long long*)p5Peer.base[p5Dist ? r : rank];
+		auto launch = [&](auto& a) {
+			pcg5_args(a, p5, twoLevel, p5Dist ? rank : 0, p5.W, bases, fHat.p, xp.p, &dScal.p->pcg);
 #ifdef CUBA_PCG_TIMING
 			a.timing = pcgTiming.p;
 #endif
-			args[0] = (void*)&a;
-		}
-		CUDA_TRY(cudaLaunchCooperativeKernel(p5Fn, dim3(p5G), dim3(p5Block), args, p5Smem, stream));
-		k_pcg5_commit<<<1, 1, 0, stream>>>(p5Ctl(p5Boards.p));
+			void* args[] = { (void*)&a };
+			return cudaLaunchCooperativeKernel(p5.sh.fn, dim3(p5.G), dim3(p5.sh.block), args, p5.sh.smem, stream);
+		};
+		Pcg5Args<T> a;
+		p5t::Pcg5Args<T> at;
+		CUDA_TRY(p5.sh.tuned ? launch(at) : launch(a));
+		k_pcg5_commit<<<1, 1, 0, stream>>>(ctl);
 		launches += 2;
 		CUDA_TRY(cudaGetLastError());
-		if (p5Dist) { int rc = allreduce(xp.p, 6 * (size_t)numP, true); if (rc) return rc; }
+		if (p5Dist) { rc = allreduce(xp.p, 6 * (size_t)S.numP, true); if (rc) return rc; }
 		lastPcgTwoLevel = twoLevel;
-		lastPcgKernel = p5Tuned ? CUBA_PCG_KERNEL_PCG5T : p5Big ? CUBA_PCG_KERNEL_PCG5_BIG : CUBA_PCG_KERNEL_PCG5;
+		lastPcgKernel = p5.sh.tuned ? CUBA_PCG_KERNEL_PCG5T : p5.sh.big ? CUBA_PCG_KERNEL_PCG5_BIG : CUBA_PCG_KERNEL_PCG5;
 		return CUBA_OK;
 	}
 
@@ -1955,8 +1998,7 @@ struct Engine : EngineBase {
 		const double tau = 1e-5;
 		double nu = 2, lambda = 0, F = 0;
 		int n = 0;
-		tlActive = false; coarseValid = false; coarseAge = 0;     // results never depend on what the engine solved before
-		p5CoarseValid = false; p5CoarseAge = 0; forceBlockJacobi = false;
+		forget_solves(); forceBlockJacobi = false;     // results never depend on what the engine solved before
 		bool haveF = false;
 		for (int it = 0; it < niter; it++) {
 			double chi0 = 0;
@@ -1988,7 +2030,7 @@ struct Engine : EngineBase {
 					const double loose = sizeof(T) == 8 ? 1e-6 : 1e-3;
 					ok = ps.status == 0 || (ps.status == 1 && ps.rz0 > 0 && ps.rz <= loose * loose * ps.rz0);
 					if (ps.status == 2 && lastPcgTwoLevel && attempt == 0) {
-						forceBlockJacobi = true; coarseValid = false; p5CoarseValid = false; bjRetries++;
+						forceBlockJacobi = true; coarse4.valid = false; p5.coarse.valid = false; bjRetries++;
 						rc = stage_commit(0); if (rc) return rc;
 						continue;
 					}
@@ -2116,7 +2158,7 @@ struct Engine : EngineBase {
 		}
 		// the system changed: nothing an earlier solve left behind may be reused (as after refresh_values; the estimate stays)
 		trialValid = false;
-		tlActive = false; coarseValid = false; coarseAge = 0; p5CoarseValid = false; p5CoarseAge = 0;
+		forget_solves();
 		return CUBA_OK;
 	}
 	int set_edge_levels(const uint8_t* levels) override
@@ -2436,42 +2478,43 @@ struct Engine : EngineBase {
 		PcgStatus ps{};
 		CUDA_TRY(cudaMemcpy(&ps, &dScal.p->pcg, sizeof(ps), cudaMemcpyDeviceToHost));
 		int last = -1, bad = 0;
-		if (p5Ok && p5A > 0 && p5Rebuilds > 0) {
-			const int nlog = (int)std::min<long long>(p5Rebuilds, P5_INFO_LOG);
+		if (p5Ok && p5.coarse.A > 0 && p5.coarse.rebuilds > 0) {
+			const int nlog = (int)std::min<long long>(p5.coarse.rebuilds, P5_INFO_LOG);
 			std::vector<int> log(nlog);
 			CUDA_TRY(cudaMemcpy(log.data(), cInfo.p + 1, sizeof(int) * nlog, cudaMemcpyDeviceToHost));
 			for (int v : log) if (v != 0) bad++;
-			last = log[(int)((p5Rebuilds - 1) % P5_INFO_LOG)];
+			last = log[(int)((p5.coarse.rebuilds - 1) % P5_INFO_LOG)];
 		}
-		auto coarseOf = [](int A) { return A > PCG4_MAXAGG1 ? CUBA_COARSE_KERNEL_DENSE : CUBA_COARSE_KERNEL_INVERT; };   // launch_coarse_setup's rule
 		int coarseKernel = CUBA_COARSE_KERNEL_NONE;
-		if (lastPcgTwoLevel && lastPcgKernel == CUBA_PCG_KERNEL_PCG4) coarseKernel = coarseOf(pcg4A);
-		else if (lastPcgTwoLevel && p5Ok) coarseKernel = coarseOf(p5A);
-		const bool tuned = p5Ok && p5Tuned;
+		if (lastPcgTwoLevel && lastPcgKernel == CUBA_PCG_KERNEL_PCG4) coarseKernel = coarse_kernel(coarse4.A);
+		else if (lastPcgTwoLevel && p5Ok) coarseKernel = coarse_kernel(p5.coarse.A);
+		const P5Shape& sh = p5.sh;
+		const bool tuned = p5Ok && sh.tuned;
 		const int32_t v[CUBA_PCG_INFO_LEN] = {
 			lastPcgKernel, lastPcgKernel != CUBA_PCG_KERNEL_NONE && lastPcgTwoLevel ? 1 : 0,
-			p5Ok ? p5Apc : 0, p5Ok ? p5G : 0, p5Ok ? p5Gs : 0, p5Ok ? p5A : 0,
-			p5Ok ? (tuned ? p5tDims.maxRows : p5Dims.maxRows) : 0, p5Ok ? (tuned ? p5tDims.capBlocks : p5Dims.capBlocks) : 0,
-			p5Ok ? (tuned ? p5tDims.zhInSmem : p5Dims.zhInSmem) : 0,
-			coarseKernel, last, ps.status, ps.iters, (int32_t)p5Rebuilds, (int32_t)bjRetries, bad };
+			p5Ok ? p5.apc : 0, p5Ok ? p5.G : 0, p5Ok ? p5.gs : 0, p5Ok ? p5.coarse.A : 0,
+			p5Ok ? (tuned ? sh.tDims.maxRows : sh.dims.maxRows) : 0, p5Ok ? (tuned ? sh.tDims.capBlocks : sh.dims.capBlocks) : 0,
+			p5Ok ? (tuned ? sh.tDims.zhInSmem : sh.dims.zhInSmem) : 0,
+			coarseKernel, last, ps.status, ps.iters, (int32_t)p5.coarse.rebuilds, (int32_t)bjRetries, bad };
 		if (info) memcpy(info, v, sizeof(v));
-		if (coarseLambda) *coarseLambda = p5CoarseValid ? p5CoarseLambda : 0.0;
+		if (coarseLambda) *coarseLambda = p5.coarse.valid ? p5.coarse.lambda : 0.0;
 		return CUBA_OK;
 	}
 	int dbg_coarse(int32_t* rowAgg, double* oAcP, float* oAcInv) override
 	{
 		if (!haveProblem) return fail(CUBA_ERR_STATE, "no problem");
-		if (!p5Ok || p5A < 1 || !p5CoarseValid) return fail(CUBA_ERR_STATE, "debug_get_coarse: no coarse level of k_pcg5 has been built");
-		const int A = p5A, nc = 6 * A;
+		const CoarseLevel& L = p5.coarse;
+		if (!p5Ok || L.A < 1 || !L.valid) return fail(CUBA_ERR_STATE, "debug_get_coarse: no coarse level of k_pcg5 has been built");
+		const int A = L.A, nc = 6 * A;
 		CUDA_TRY(cudaStreamSynchronize(stream));
 		if (rowAgg) {
 			std::vector<int> ptr(A + 1);
-			CUDA_TRY(cudaMemcpy(ptr.data(), p5AggRow.p, sizeof(int) * (A + 1), cudaMemcpyDeviceToHost));
+			CUDA_TRY(cudaMemcpy(ptr.data(), L.aggRow.p, sizeof(int) * (A + 1), cudaMemcpyDeviceToHost));
 			for (int i = 0; i < S.numP; i++) rowAgg[i] = -1;
 			for (int ag = 0; ag < A; ag++) for (int i = ptr[ag]; i < ptr[ag + 1] && i < S.numP; i++) rowAgg[i] = ag;
 		}
-		if (oAcP) CUDA_TRY(cudaMemcpy(oAcP, p5AcP.p, sizeof(double) * 36 * ((size_t)A * (A + 1) / 2), cudaMemcpyDeviceToHost));
-		if (oAcInv) CUDA_TRY(cudaMemcpy(oAcInv, p5AcInv.p, sizeof(float) * (size_t)nc * nc, cudaMemcpyDeviceToHost));
+		if (oAcP) CUDA_TRY(cudaMemcpy(oAcP, L.AcP.p, sizeof(double) * 36 * ((size_t)A * (A + 1) / 2), cudaMemcpyDeviceToHost));
+		if (oAcInv) CUDA_TRY(cudaMemcpy(oAcInv, L.AcInv.p, sizeof(float) * (size_t)nc * nc, cudaMemcpyDeviceToHost));
 		return CUBA_OK;
 	}
 	// include/cuba_b200.h: cuba_debug_coarse_inverse -- k_coarse_dense on a caller's packed matrix, in buffers of its own
@@ -2506,24 +2549,20 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, peer::k_peer_allreduce_ranks<T>, peer::BLOCK, 0));
 		if ((long long)perSM * numSMs < (long long)W * nctas)
 			return fail(CUBA_ERR_INVALID, "debug_peer_allreduce: " + std::to_string(W * nctas) + " CTAs, but only " + std::to_string(perSM * numSMs) + " can be resident at once");
-		// every rank's buffer as launch_peer_allreduce lays it out (n elements, the signal block at the next even element), 16-byte aligned
-		const size_t sigOff = (n + 1) & ~(size_t)1;
+		// every rank's buffer as launch_peer_allreduce lays it out (n elements, then the signal block), 16-byte aligned
 		const size_t sigElems = (2 * peer::MAXW * sizeof(unsigned int) + sizeof(T) - 1) / sizeof(T);
-		const size_t stride = (sigOff + sigElems + 31) / 32 * 32;
+		const size_t stride = (peer_signal_offset(n) + sigElems + 31) / 32 * 32;
 		DBuf<T> buf; DBuf<GridBar> bars; DBuf<peer::Args<T>> dArgs;
 		CUDA_TRY(buf.alloc(stride * W)); CUDA_TRY(bars.alloc(W));
 		CUDA_TRY(cudaMemsetAsync(buf.p, 0, sizeof(T) * stride * W, stream));
 		CUDA_TRY(cudaMemsetAsync(bars.p, 0, sizeof(GridBar) * W, stream));
+		std::vector<void*> bufs(W);
+		for (int r = 0; r < W; r++) bufs[r] = buf.p + stride * r;
 		std::vector<peer::Args<T>> ha(W);
-		for (int r = 0; r < W; r++) {
-			peer::Args<T>& a = ha[r];
-			for (int q = 0; q < peer::MAXW; q++) { a.peers[q] = nullptr; a.sigPeer[q] = nullptr; }
-			for (int q = 0; q < W; q++) { a.peers[q] = buf.p + stride * q; a.sigPeer[q] = (unsigned int*)(buf.p + stride * q + sigOff); }
-			a.local = a.peers[r]; a.sigLocal = a.sigPeer[r]; a.n = n; a.rank = r; a.world = W; a.bar = bars.p + r;
-		}
 		std::vector<T> h((size_t)W * n);
 		for (int c = 0; c < calls; c++) {
-			for (int r = 0; r < W; r++) ha[r].epoch = (unsigned int)c + 1;           // consecutive epochs on the same signal blocks
+			// consecutive epochs on the same signal blocks
+			for (int r = 0; r < W; r++) ha[r] = peer_args(bufs.data(), r, W, n, (unsigned int)c + 1, bars.p + r);
 			CUDA_TRY(dArgs.upload(ha.data(), W, stream));
 			for (size_t i = 0; i < (size_t)W * n; i++) h[i] = (T)parts[(size_t)c * W * n + i];
 			for (int r = 0; r < W; r++) CUDA_TRY(cudaMemcpyAsync(buf.p + stride * r, h.data() + (size_t)r * n, sizeof(T) * n, cudaMemcpyHostToDevice, stream));
@@ -2539,7 +2578,9 @@ struct Engine : EngineBase {
 	}
 
 	// include/cuba_b200.h: cuba_debug_pcg5_ranks -- the row-distributed k_pcg5 of a `world`-rank run on the current reduced system,
-	// every rank's boards in this GPU's memory and all ranks in one cooperative launch of k_pcg5_ranks, in buffers of its own
+	// every rank's boards in this GPU's memory and all ranks in one cooperative launch of k_pcg5_ranks, in buffers of its own.  The
+	// run is uploaded, laid out, prepared and given its arguments by the engine's own k_pcg5 code (pcg5_upload, Pcg5Run::boards,
+	// pcg5_prepare, pcg5_args); only the kernel (k_pcg5_ranks) and where the W board sets live differ from a W-GPU run.
 	int dbg_pcg5_ranks(int W, int twoLevel, int nsolves, double* xOut, int32_t* statusOut, int32_t* planOut, int32_t* aggRowOut, float* acInvOut) override
 	{
 		if (!haveProblem) return fail(CUBA_ERR_STATE, "no problem");
@@ -2552,77 +2593,35 @@ struct Engine : EngineBase {
 		if (!plan.ok) return fail(CUBA_ERR_INVALID, "debug_pcg5_ranks: no k_pcg5 plan for " + std::to_string(W) + " ranks of " + std::to_string(numSMs / W) + " CTAs");
 		P5Shape sh;
 		int rc = pcg5_legacy_shape(plan, pcg5_plan_dims(plan, W), W, true, sh); if (rc) return rc;
-		const int G = plan.G, A = twoLevel ? plan.A : 0, nc = 6 * plan.A;
+		const int G = plan.G, nc = 6 * plan.A;
 		if ((long long)sh.perSM * numSMs < (long long)W * G)
 			return fail(CUBA_ERR_INVALID, "debug_pcg5_ranks: " + std::to_string(W * G) + " CTAs, but only " + std::to_string(sh.perSM * numSMs) + " can be resident at once");
-		const PcgPartition& PP = plan.P; const CoarsePartition& CP = plan.C;
+		Pcg5Run R;
+		rc = pcg5_upload(R, plan, sh, W, nullptr); if (rc) return rc;
 		const size_t nP = (size_t)numP;
-		DBuf<int> dCtaRow, dNeedPtr, dNeedCol, dLocal, dAggRow, dNaPtr, dNaList, dNeedAgg, dCbPtr, dCbList, dRowOf, dInfo;
-		DBuf<unsigned char> dRowPeers;
-		DBuf<T> dLinv, dR0, dZhat, dRcRow, dRc0, dZx, dHat, dx;
-		DBuf<double> dU, dAcP, dTiles;
-		DBuf<float> dAcInv;
+		DBuf<T> dZx, dHat, dx;
+		DBuf<double> dU, dTiles;
+		DBuf<int> dInfo;
 		DBuf<GridBar> dBar;
 		DBuf<PcgStatus> dStatus;
 		DBuf<unsigned long long> boards;
 		DBuf<Pcg5Args<T>> dArgs;
-		CUDA_TRY(dCtaRow.upload(PP.rows, stream)); CUDA_TRY(dNeedPtr.upload(PP.nptr, stream)); CUDA_TRY(dNeedCol.upload(PP.ncol, stream));
-		CUDA_TRY(dLocal.upload(PP.local, stream)); CUDA_TRY(dRowPeers.upload(plan.rowPeers, stream));
-		CUDA_TRY(dAggRow.upload(CP.aggRow, stream)); CUDA_TRY(dNaPtr.upload(CP.naPtr, stream)); CUDA_TRY(dNaList.upload(CP.naList, stream));
-		CUDA_TRY(dNeedAgg.upload(CP.needAgg, stream)); CUDA_TRY(dCbPtr.upload(CP.cbPtr, stream)); CUDA_TRY(dCbList.upload(CP.cbList, stream));
-		CUDA_TRY(dRowOf.upload(CP.rowOf, stream));
-		CUDA_TRY(dLinv.alloc(36 * nP)); CUDA_TRY(dR0.alloc(6 * nP)); CUDA_TRY(dZhat.alloc(36 * nP)); CUDA_TRY(dRcRow.alloc(6 * nP)); CUDA_TRY(dRc0.alloc(std::max(nc, 1)));
 		CUDA_TRY(dZx.alloc(36 * nP)); CUDA_TRY(dU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(dHat.alloc(36 * (size_t)S.nfull)); CUDA_TRY(dx.alloc(6 * nP));
-		CUDA_TRY(dAcP.alloc(36 * ((size_t)plan.A * (plan.A + 1) / 2))); CUDA_TRY(dAcInv.alloc((size_t)nc * nc)); CUDA_TRY(dInfo.alloc(1));
-		CUDA_TRY(dBar.alloc(1)); CUDA_TRY(dStatus.alloc(W));
-		CUDA_TRY(cudaMemsetAsync(dAcInv.p, 0, sizeof(float) * (size_t)nc * nc, stream));
+		if (twoLevel && coarse_kernel(plan.A) == CUBA_COARSE_KERNEL_DENSE) CUDA_TRY(dTiles.alloc(cdense::scratch_doubles(plan.A)));
+		CUDA_TRY(dInfo.alloc(1)); CUDA_TRY(dBar.alloc(1)); CUDA_TRY(dStatus.alloc(W));
+		CUDA_TRY(cudaMemsetAsync(R.coarse.AcInv.p, 0, sizeof(float) * (size_t)nc * nc, stream));
 		CUDA_TRY(cudaMemsetAsync(dInfo.p, 0, sizeof(int), stream));
 		CUDA_TRY(cudaMemsetAsync(dBar.p, 0, sizeof(GridBar), stream));
-		// W board sets laid out as setup_pcg5 lays out one GPU's, zeroed: [2 solve halves][2 pass parities] of w, partials, rank
-		// summaries and coarse corrections, then the control block
-		const int NR = 3 + 6 * (G / plan.gs);
-		const size_t wW = 4 * 6 * nP, pW = 4 * (size_t)PCG5_REPL * G * p5t::pcg5t_np(plan.apc), rW = 4 * (size_t)PCG5_REPL * W * NR, cW = 4 * (size_t)PCG5_REPL * nc;
-		const size_t words2 = 2 * (wW + pW + rW + cW) + (sizeof(Pcg5Ctl) + 7) / 8 + 2;
-		CUDA_TRY(boards.alloc(words2 * W));
-		CUDA_TRY(cudaMemsetAsync(boards.p, 0, sizeof(unsigned long long) * words2 * W, stream));
-		auto base = [&](int r) { return boards.p + words2 * r; };
-		auto ctlOf = [&](int r) { return (Pcg5Ctl*)(base(r) + 2 * (wW + pW + rW + cW)); };
-		// the preparation and the coarse level, as launch_pcg5 runs them on every rank (the rows of Linv, R0, Z^ and rc0 are the
-		// same on every rank: computed once; each rank's breakdown counter gets its own count)
-		if (A > 0) KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, dZx.p);
-		Pcg5PrepArgs<T> pa;
-		pa.fRowPtr = fRowPtr; pa.fColInd = fColInd; pa.fVal = fVal; pa.b = bsc; pa.Zx = dZx; pa.numP = numP; pa.A = A; pa.aggRow = dAggRow; pa.zhatFp32 = 0;
-		pa.Linv = dLinv; pa.R0 = dR0; pa.Zhat = dZhat; pa.rcRow = dRcRow; pa.rc0 = dRc0;
-		for (int r = 0; r < W; r++) {
-			pa.ctl = ctlOf(r);
-			k_pcg5_prep_rows<T><<<(numP + 127) / 128, 128, 0, stream>>>(pa);
-			launches++;
-		}
-		if (A > 0) {
-			k_pcg5_prep_rc<T><<<(6 * A + 127) / 128, 128, 0, stream>>>(pa);
-			launches++;
-			if (A > PCG4_MAXAGG1) CUDA_TRY(dTiles.alloc(cdense::scratch_doubles(A)));
-			rc = launch_coarse_setup(A, dCbPtr, dCbList, dRowOf, dZx, dU, dTiles.p, dBar, dAcP, dAcInv, dInfo); if (rc) return rc;
-		}
-		CUDA_TRY(cudaGetLastError());
+		// W board sets of the engine's layout, zeroed
+		const size_t words = R.boards().words;
+		CUDA_TRY(boards.alloc(words * W));
+		CUDA_TRY(cudaMemsetAsync(boards.p, 0, sizeof(unsigned long long) * words * W, stream));
+		std::vector<unsigned long long*> base(W);
+		std::vector<Pcg5Ctl*> ctl(W);
+		for (int r = 0; r < W; r++) { base[r] = boards.p + words * r; ctl[r] = R.ctl(base[r]); }
+		rc = pcg5_prepare(R, twoLevel != 0, ctl.data(), W, CoarseScratch{ dZx.p, dU.p, dTiles.p, dBar.p }, dInfo.p); if (rc) return rc;
 		std::vector<Pcg5Args<T>> ha(W);
-		for (int r = 0; r < W; r++) {
-			Pcg5Args<T>& a = ha[r];
-			a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = dLocal; a.fVal = fVal; a.fHat = dHat;
-			a.ctaRow = dCtaRow; a.needPtr = dNeedPtr; a.needCol = dNeedCol;
-			a.numP = numP; a.G = G; a.rank = r; a.world = W;
-			a.Linv = dLinv; a.R0 = dR0; a.Zhat = dZhat; a.rc0 = dRc0; a.x = dx;
-			a.dims = A > 0 ? sh.dims : sh.dimsBJ;
-			a.dims.capBlocks = sh.dims.capBlocks;
-			a.maxIters = pcg5_max_iters(); a.tol2 = pcg5_tol2();
-			a.status = dStatus.p + r;
-			a.AcInv = dAcInv; a.naPtr = dNaPtr; a.naList = dNaList; a.needAgg = dNeedAgg; a.A = A; a.gs = plan.gs;
-			for (int q = 0; q < PCG5_MAXWORLD; q++) { a.peerW[q] = nullptr; a.peerR[q] = nullptr; a.peerCtl[q] = nullptr; }
-			for (int q = 0; q < W; q++) { a.peerW[q] = base(q); a.peerR[q] = base(q) + 2 * (wW + pW); a.peerCtl[q] = ctlOf(q); }
-			a.wBoard = base(r); a.pBoard = base(r) + 2 * wW; a.rBoard = base(r) + 2 * (wW + pW); a.cBoard = base(r) + 2 * (wW + pW + rW);
-			a.rowPeers = dRowPeers; a.ctl = ctlOf(r);
-			a.timing = nullptr;
-		}
+		for (int r = 0; r < W; r++) pcg5_args(ha[r], R, twoLevel != 0, r, W, base.data(), dHat.p, dx.p, dStatus.p + r);
 		CUDA_TRY(dArgs.upload(ha.data(), W, stream));
 		std::vector<T> hx(6 * nP);
 		std::vector<PcgStatus> hs(W);
@@ -2632,7 +2631,7 @@ struct Engine : EngineBase {
 			int g = G;
 			void* args[] = { (void*)&pArgs, (void*)&g };
 			CUDA_TRY(cudaLaunchCooperativeKernel(sh.fn, dim3(W * G), dim3(PCG5_BLOCK), args, sh.smem, stream));
-			for (int r = 0; r < W; r++) k_pcg5_commit<<<1, 1, 0, stream>>>(ctlOf(r));
+			for (int r = 0; r < W; r++) k_pcg5_commit<<<1, 1, 0, stream>>>(ctl[r]);
 			launches += 1 + W;
 			CUDA_TRY(cudaGetLastError());
 			CUDA_TRY(cudaMemcpyAsync(hx.data(), dx.p, sizeof(T) * 6 * nP, cudaMemcpyDeviceToHost, stream));
@@ -2645,10 +2644,10 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaMemcpy(&cinfo, dInfo.p, sizeof(int), cudaMemcpyDeviceToHost));
 		int halo = 0;
 		for (unsigned char m : plan.rowPeers) if (m) halo++;
-		const int32_t v[8] = { G, plan.gs, plan.A, PP.needMax, PP.maxRows, halo, sh.big ? 1 : 0, cinfo };
+		const int32_t v[8] = { G, plan.gs, plan.A, plan.P.needMax, plan.P.maxRows, halo, sh.big ? 1 : 0, cinfo };
 		memcpy(planOut, v, sizeof(v));
-		if (aggRowOut) memcpy(aggRowOut, CP.aggRow.data(), sizeof(int) * (plan.A + 1));
-		if (acInvOut) CUDA_TRY(cudaMemcpy(acInvOut, dAcInv.p, sizeof(float) * (size_t)nc * nc, cudaMemcpyDeviceToHost));
+		if (aggRowOut) memcpy(aggRowOut, plan.C.aggRow.data(), sizeof(int) * (plan.A + 1));
+		if (acInvOut) CUDA_TRY(cudaMemcpy(acInvOut, R.coarse.AcInv.p, sizeof(float) * (size_t)nc * nc, cudaMemcpyDeviceToHost));
 		return CUBA_OK;
 	}
 
@@ -2676,8 +2675,8 @@ struct Engine : EngineBase {
 			case 5: rc = launch_backsub(lam); if (!rc) rc = stage_update_nofetch(lam); break;
 			case 6: rc = launch_chi2(cur, 0); break;
 			case 7:   // one rebuild of the coarse inverse of k_pcg5 / k_pcg5t (projection, assembly, inverse) from the current system
-				if (!p5Ok || p5A < 1) rc = fail(CUBA_ERR_STATE, "bench_stage: no two-level k_pcg5 plan");
-				else rc = launch_coarse_setup(p5A, p5CbPtr, p5CbList, p5AcP, p5AcInv, p5InfoSlot());
+				if (!p5Ok || p5.coarse.A < 1) rc = fail(CUBA_ERR_STATE, "bench_stage: no two-level k_pcg5 plan");
+				else rc = launch_coarse_setup(p5.coarse, coarse_scratch(), p5InfoSlot());
 				break;
 			default: rc = fail(CUBA_ERR_INVALID, "bench_stage: unknown stage");
 			}
