@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 #include <string>
 #include <type_traits>
@@ -389,12 +390,10 @@ struct Engine : EngineBase {
 	DBuf<unsigned char> lvLevel;   // [E] in edge-id order; a rank reads and writes its own edges only
 	DBuf<int> lvPartial;
 	DBuf<double> lvCount;
-	// batched pose optimisation (cuba_pose_batch.cuh): the packed batch and the packed results, device and page-locked host copies
-	DBuf<double> pbIn, pbOut;
-	PinnedBuf pbHostIn, pbHostOut;
-	// batched Sim(3) alignment (cuba_sim3_batch.cuh): the same, for its own packed batch
-	DBuf<double> s3In, s3Out;
-	PinnedBuf s3HostIn, s3HostOut;
+	// the batched LM kernels (optimize_poses, optimize_sim3, one after the other on the stream): the packed batch and the packed
+	// results, device and page-locked host copies
+	DBuf<double> batchIn, batchOut;
+	PinnedBuf batchHostIn, batchHostOut;
 	DBuf<Scalars> dScal;
 	Scalars* hScal = nullptr;   // pinned
 	DBuf<double> flushBuf;
@@ -1994,8 +1993,6 @@ struct Engine : EngineBase {
 	{
 		if (!haveProblem) return fail(CUBA_ERR_STATE, "optimize before set_problem");
 		if (lvOn && lvIncluded == 0) { if (nstats) *nstats = 0; return CUBA_OK; }   // every edge at level 1: nothing to optimise
-		const int maxq = 10;
-		const double tau = 1e-5;
 		double nu = 2, lambda = 0, F = 0;
 		int n = 0;
 		forget_solves(); forceBlockJacobi = false;     // results never depend on what the engine solved before
@@ -2009,11 +2006,11 @@ struct Engine : EngineBase {
 			if (it == 0) {
 				double md = 0;
 				rc = stage_max_diagonal(&md); if (rc) return rc;
-				lambda = tau * md;
+				lambda = lm::initial_lambda(md);
 			}
 			int q = 0, trials = 0, pcgIters = 0, pcgFailed = 0;
 			double rho = -1;
-			for (; q < maxq && rho < 0; q++) {
+			for (; q < lm::MAX_TRIALS && rho < 0; q++) {
 				trials++;
 				int iters = 0, ok = 1;
 				double Fhat = 0, scale = 0;
@@ -2039,26 +2036,20 @@ struct Engine : EngineBase {
 				forceBlockJacobi = false;
 				if (S.numP > 0 && S.numL > 0) note_pcg_iters(hScal->pcg.iters);
 				pcgIters += iters; if (!ok) pcgFailed++;
-				scale += 1e-3;
-				rho = ok ? (F - Fhat) / scale : -1;
-				if (!(rho == rho)) rho = -1;   // NaN trial -> reject
-				if (rho > 0) {
-					const double a = 2 * rho - 1;
-					lambda *= std::max(1. / 3, std::min(1 - a * a * a, 2. / 3));
-					nu = 2; F = Fhat;
+				rho = ok ? lm::gain_ratio(F, Fhat, scale) : -1;
+				if (lm::update_damping(rho, lambda, nu)) {
+					F = Fhat;
 					rc = stage_commit(1); if (rc) return rc;
 					break;
-				} else {
-					lambda *= nu; nu *= 2;
-					rc = stage_commit(0); if (rc) return rc;
 				}
+				rc = stage_commit(0); if (rc) return rc;
 			}
 			if (stats) {
 				stats[n].iteration = it; stats[n].trials = trials; stats[n].chi2 = F; stats[n].lambda = lambda;
 				stats[n].pcg_iters = pcgIters; stats[n].pcg_failed = pcgFailed;
 			}
 			n++;
-			if (q == maxq || rho <= 0 || !std::isfinite(lambda)) break;
+			if (lm::stop(q, rho, lambda)) break;
 		}
 		if (nstats) *nstats = n;
 		resolveProfile();   // the stream is idle (every trial ends with a fetch): recycle the profile events instead of hoarding them
@@ -2248,12 +2239,29 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// ---- batched pose optimisation (cuba_pose_batch.cuh): one H2D of the packed batch, one launch, one D2H of the packed results.
-	// Always fp64, on this engine's stream; touches nothing of the engine's problem.  The batch was validated by the caller.
+	// ---- the batched LM kernels: each entry point packs its batch into batchHostIn and unpacks its results from batchHostOut.  Always
+	// fp64, on this engine's stream; they touch nothing of the engine's problem.  The batch was validated by the caller.
+	static_assert(sizeof(lm::IterStat) == sizeof(cuba_iter_stat) && sizeof(lm::IterStat) == 32, "cuba_iter_stat layout");
+
+	// one H2D of the packed batch (nIn doubles), the launch of one CTA per problem, one D2H of the packed results (nOut doubles)
+	template <class Args, class Params>
+	int batch_round_trip(void (*kernel)(Args, Params), const Args& a, const Params& p, size_t nIn, size_t nOut)
+	{
+		CUDA_TRY(cudaMemcpyAsync(batchIn.p, batchHostIn.p, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
+		g_h2dBytes += (long long)(sizeof(double) * nIn);
+		kernel<<<(unsigned)a.B, lm::BLOCK, 0, stream>>>(a, p);
+		launches++;
+		CUDA_TRY(cudaGetLastError());
+		CUDA_TRY(cudaMemcpyAsync(batchHostOut.p, batchOut.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
+		g_d2hBytes += (long long)(sizeof(double) * nOut);
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		return CUBA_OK;
+	}
+
+	// batched pose optimisation (cuba_pose_batch.cuh)
 	int optimize_poses(const cuba_pose_batch* bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
 		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) override
 	{
-		static_assert(sizeof(pb::IterStat) == sizeof(cuba_iter_stat) && sizeof(pb::IterStat) == 32, "cuba_iter_stat layout");
 		const size_t B = (size_t)bt->B, R = (size_t)s.n;
 		if (B == 0) return CUBA_OK;
 		const size_t E2 = (size_t)bt->E2, E3 = (size_t)bt->E3, E = E2 + E3;
@@ -2262,9 +2270,9 @@ struct Engine : EngineBase {
 		const size_t oCam = 8 * B, oEdge = 16 * B, oPtr = oEdge + 8 * E, nIn = oPtr + (B + 1);
 		// results, in doubles: pose [B][8] | stats [nStat] (4 doubles each) | counts [B][R][4], nstats [B][R] as int32 | levels [E] bytes
 		const size_t oStat = 8 * B, oInt = oStat + 4 * nStat, nInt = 5 * B * R, oLev = oInt + (nInt + 1) / 2, nOut = oLev + (E + 7) / 8;
-		CUDA_TRY(pbHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(pbHostOut.grow(sizeof(double) * nOut));
-		CUDA_TRY(pbIn.alloc(nIn)); CUDA_TRY(pbOut.alloc(nOut));
-		double* h = (double*)pbHostIn.p;
+		CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * nOut));
+		CUDA_TRY(batchIn.alloc(nIn)); CUDA_TRY(batchOut.alloc(nOut));
+		double* h = (double*)batchHostIn.p;
 		for (size_t b = 0; b < B; b++) {
 			double* p = h + 8 * b;
 			for (int k = 0; k < 4; k++) p[k] = bt->q[4 * b + k];
@@ -2288,23 +2296,16 @@ struct Engine : EngineBase {
 		int32_t* hp = (int32_t*)(h + oPtr);
 		memcpy(hp, bt->ptr2, sizeof(int32_t) * (B + 1));
 		memcpy(hp + B + 1, bt->ptr3, sizeof(int32_t) * (B + 1));
-		CUDA_TRY(cudaMemcpyAsync(pbIn.p, h, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
-		g_h2dBytes += (long long)(sizeof(double) * nIn);
 		pb::Args a;
 		a.B = (int)B;
-		a.pose = pbIn.p; a.cam = pbIn.p + oCam; a.edge = pbIn.p + oEdge;
-		a.ptr2 = (const int*)(pbIn.p + oPtr); a.ptr3 = a.ptr2 + B + 1;
-		a.poseOut = pbOut.p;
-		a.stats = stats ? (pb::IterStat*)(pbOut.p + oStat) : nullptr;
-		a.counts = (int*)(pbOut.p + oInt); a.nstats = a.counts + 4 * B * R;
-		a.level = (unsigned char*)(pbOut.p + oLev);
-		pb::k_pose_batch<<<(unsigned)B, pb::BLOCK, 0, stream>>>(a, s);
-		launches++;
-		CUDA_TRY(cudaGetLastError());
-		CUDA_TRY(cudaMemcpyAsync(pbHostOut.p, pbOut.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
-		g_d2hBytes += (long long)(sizeof(double) * nOut);
-		CUDA_TRY(cudaStreamSynchronize(stream));
-		const double* o = (const double*)pbHostOut.p;
+		a.pose = batchIn.p; a.cam = batchIn.p + oCam; a.edge = batchIn.p + oEdge;
+		a.ptr2 = (const int*)(batchIn.p + oPtr); a.ptr3 = a.ptr2 + B + 1;
+		a.poseOut = batchOut.p;
+		a.stats = stats ? (lm::IterStat*)(batchOut.p + oStat) : nullptr;
+		a.counts = (int*)(batchOut.p + oInt); a.nstats = a.counts + 4 * B * R;
+		a.level = (unsigned char*)(batchOut.p + oLev);
+		const int rc = batch_round_trip(pb::k_pose_batch, a, s, nIn, nOut); if (rc) return rc;
+		const double* o = (const double*)batchHostOut.p;
 		for (size_t b = 0; b < B; b++) {
 			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
 			for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
@@ -2323,12 +2324,10 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// ---- batched Sim(3) alignment (cuba_sim3_batch.cuh): one H2D of the packed batch, one launch, one D2H of the packed results.
-	// Always fp64, on this engine's stream; touches nothing of the engine's problem.  The batch was validated by the caller.
+	// batched Sim(3) alignment (cuba_sim3_batch.cuh)
 	int optimize_sim3(const cuba_sim3_batch* bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
 		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats) override
 	{
-		static_assert(sizeof(pb::IterStat) == sizeof(cuba_iter_stat) && sizeof(pb::IterStat) == 32, "cuba_iter_stat layout");
 		const size_t B = (size_t)bt->B, N = (size_t)bt->N;
 		if (B == 0) return CUBA_OK;
 		const size_t nStat = stats ? B * (size_t)p.statPer : 0;
@@ -2336,9 +2335,9 @@ struct Engine : EngineBase {
 		const size_t oPair = s3::PROB * B, oPtr = oPair + s3::PAIR * N, nIn = oPtr + (B + 2) / 2;
 		// results, in doubles: S [B][8] | stats [nStat] (4 doubles each) | ninliers [B], nstats [B][2] as int32 | levels [N] bytes
 		const size_t oStat = 8 * B, oInt = oStat + 4 * nStat, oLev = oInt + (3 * B + 1) / 2, nOut = oLev + (N + 7) / 8;
-		CUDA_TRY(s3HostIn.grow(sizeof(double) * nIn)); CUDA_TRY(s3HostOut.grow(sizeof(double) * nOut));
-		CUDA_TRY(s3In.alloc(nIn)); CUDA_TRY(s3Out.alloc(nOut));
-		double* h = (double*)s3HostIn.p;
+		CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * nOut));
+		CUDA_TRY(batchIn.alloc(nIn)); CUDA_TRY(batchOut.alloc(nOut));
+		double* h = (double*)batchHostIn.p;
 		for (size_t b = 0; b < B; b++) {
 			double* d = h + s3::PROB * b;
 			for (int k = 0; k < 4; k++) d[k] = bt->q[4 * b + k];
@@ -2355,22 +2354,15 @@ struct Engine : EngineBase {
 			d[10] = bt->omega1[i]; d[11] = bt->omega2[i];
 		}
 		memcpy(h + oPtr, bt->ptr, sizeof(int32_t) * (B + 1));
-		CUDA_TRY(cudaMemcpyAsync(s3In.p, h, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
-		g_h2dBytes += (long long)(sizeof(double) * nIn);
 		s3::Args a;
 		a.B = (int)B;
-		a.prob = s3In.p; a.pair = s3In.p + oPair; a.ptr = (const int*)(s3In.p + oPtr);
-		a.Sout = s3Out.p;
-		a.stats = stats ? (pb::IterStat*)(s3Out.p + oStat) : nullptr;
-		a.ninliers = (int*)(s3Out.p + oInt); a.nstats = a.ninliers + B;
-		a.level = (unsigned char*)(s3Out.p + oLev);
-		s3::k_sim3_batch<<<(unsigned)B, s3::BLOCK, 0, stream>>>(a, p);
-		launches++;
-		CUDA_TRY(cudaGetLastError());
-		CUDA_TRY(cudaMemcpyAsync(s3HostOut.p, s3Out.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
-		g_d2hBytes += (long long)(sizeof(double) * nOut);
-		CUDA_TRY(cudaStreamSynchronize(stream));
-		const double* o = (const double*)s3HostOut.p;
+		a.prob = batchIn.p; a.pair = batchIn.p + oPair; a.ptr = (const int*)(batchIn.p + oPtr);
+		a.Sout = batchOut.p;
+		a.stats = stats ? (lm::IterStat*)(batchOut.p + oStat) : nullptr;
+		a.ninliers = (int*)(batchOut.p + oInt); a.nstats = a.ninliers + B;
+		a.level = (unsigned char*)(batchOut.p + oLev);
+		const int rc = batch_round_trip(s3::k_sim3_batch, a, p, nIn, nOut); if (rc) return rc;
+		const double* o = (const double*)batchHostOut.p;
 		for (size_t b = 0; b < B; b++) {
 			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
 			for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
@@ -2812,19 +2804,26 @@ int cuba_engine_classify_edges(cuba_engine* e, double chi2_mono, double chi2_ste
 	if (flags & ~(CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE)) return fail(CUBA_ERR_INVALID, "classify_edges: unknown flag");
 	return e->impl->classify_edges(chi2_mono, chi2_stereo, flags, counts);
 }
-// the batch and the schedule come from outside the program: everything the kernel relies on is checked here, before any work
-static int pose_frames_ok(int B, int E, const int32_t* ptr, const double* X, const double* meas, const double* om, const char* what)
+// The batches of the batched LM kernels come from outside the program: everything a kernel relies on is checked before any work.
+// A CSR pointer of B problems over `count` items: present, ptr[0] = 0, non-decreasing and ptr[B] = count (so a negative count
+// fails), and every item array present when there are items.
+static int csr_ok(const std::string& what, int B, int count, const int32_t* ptr, std::initializer_list<const void*> items)
 {
-	if (E < 0) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: negative edge count ") + what);
-	if (!ptr) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: null ptr") + what);
-	if (ptr[0] != 0) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: ptr") + what + "[0] != 0");
+	if (!ptr) return fail(CUBA_ERR_INVALID, what + ": null");
+	if (ptr[0] != 0) return fail(CUBA_ERR_INVALID, what + "[0] != 0");
 	for (int b = 0; b < B; b++)
-		if (ptr[b + 1] < ptr[b]) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: ptr") + what + " decreases");
-	if (ptr[B] != E) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: ptr") + what + "[B] is not the edge count");
-	if (E > 0 && (!X || !meas || !om)) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: null edge array ") + what);
-	for (int i = 0; i < E; i++)
-		if (!std::isfinite(om[i])) return fail(CUBA_ERR_INVALID, std::string("optimize_poses: non-finite omega") + what);
+		if (ptr[b + 1] < ptr[b]) return fail(CUBA_ERR_INVALID, what + " decreases");
+	if (ptr[B] != count) return fail(CUBA_ERR_INVALID, what + "[B] is not the item count");
+	for (const void* p : items)
+		if (count > 0 && !p) return fail(CUBA_ERR_INVALID, what + ": null item array");
 	return CUBA_OK;
+}
+
+static bool all_finite(const double* p, size_t n)
+{
+	for (size_t i = 0; i < n; i++)
+		if (!std::isfinite(p[i])) return false;
+	return true;
 }
 
 int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds,
@@ -2859,16 +2858,10 @@ int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nr
 	if (B == 0) return CUBA_OK;
 	if (!bt->q || !bt->t || !bt->cam || !q_out || !t_out) return fail(CUBA_ERR_INVALID, "optimize_poses: null pose array");
 	if ((long long)bt->E2 + bt->E3 > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many edges");
-	int rc = pose_frames_ok(B, bt->E2, bt->ptr2, bt->X2, bt->meas2, bt->omega2, "2"); if (rc) return rc;
-	rc = pose_frames_ok(B, bt->E3, bt->ptr3, bt->X3, bt->meas3, bt->omega3, "3"); if (rc) return rc;
+	int rc = csr_ok("optimize_poses: ptr2", B, bt->E2, bt->ptr2, { bt->X2, bt->meas2, bt->omega2 }); if (rc) return rc;
+	rc = csr_ok("optimize_poses: ptr3", B, bt->E3, bt->ptr3, { bt->X3, bt->meas3, bt->omega3 }); if (rc) return rc;
+	if (!all_finite(bt->omega2, bt->E2) || !all_finite(bt->omega3, bt->E3)) return fail(CUBA_ERR_INVALID, "optimize_poses: non-finite omega");
 	return e->impl->optimize_poses(bt, s, q_out, t_out, levels_out, counts, stats, nstats);
-}
-
-static bool all_finite(const double* p, size_t n)
-{
-	for (size_t i = 0; i < n; i++)
-		if (!std::isfinite(p[i])) return false;
-	return true;
 }
 
 int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const cuba_sim3_params* params, double* q_out, double* t_out,
@@ -2887,15 +2880,9 @@ int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const c
 	const int B = bt->B;
 	if (B == 0) return CUBA_OK;
 	const size_t nb = (size_t)B, N = (size_t)bt->N;
-	if (!bt->ptr) return fail(CUBA_ERR_INVALID, "optimize_sim3: null ptr");
-	if (bt->ptr[0] != 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: ptr[0] != 0");
-	for (int b = 0; b < B; b++)
-		if (bt->ptr[b + 1] < bt->ptr[b]) return fail(CUBA_ERR_INVALID, "optimize_sim3: ptr decreases");
-	if (bt->ptr[B] != bt->N) return fail(CUBA_ERR_INVALID, "optimize_sim3: ptr[B] is not the pair count");
+	const int rc = csr_ok("optimize_sim3: ptr", B, bt->N, bt->ptr, { bt->X1, bt->X2, bt->obs1, bt->obs2, bt->omega1, bt->omega2 }); if (rc) return rc;
 	if (!bt->q || !bt->t || !bt->s || !bt->cam1 || !bt->cam2 || !q_out || !t_out || !s_out)
 		return fail(CUBA_ERR_INVALID, "optimize_sim3: null problem array");
-	if (N > 0 && (!bt->X1 || !bt->X2 || !bt->obs1 || !bt->obs2 || !bt->omega1 || !bt->omega2))
-		return fail(CUBA_ERR_INVALID, "optimize_sim3: null pair array");
 	if (!all_finite(bt->q, 4 * nb) || !all_finite(bt->t, 3 * nb) || !all_finite(bt->s, nb) || !all_finite(bt->cam1, 4 * nb) ||
 		!all_finite(bt->cam2, 4 * nb))
 		return fail(CUBA_ERR_INVALID, "optimize_sim3: non-finite S12 or intrinsics");

@@ -1,4 +1,4 @@
-// cuba_math.cuh -- per-edge / per-vertex arithmetic of the LM hot path, shared by every kernel.
+// cuba_math.cuh -- per-edge / per-vertex arithmetic of the LM hot path, shared by every kernel, and the LM rules (lm::).
 //
 // Everything here is __host__ __device__ so that tests/test_host_math.py can compile the very same
 // functions with g++ and check them against the oracle without a GPU.
@@ -179,6 +179,90 @@ CUBA_HD bool spd_inverse(T A[N * N])
 }
 template <typename T>
 CUBA_HD bool spd6_inverse(T A[36]) { return spd_inverse<6, T>(A); }
+
+// ---- the Levenberg-Marquardt rules of Engine::optimize (reference src/cuda_bundle_adjustment.cpp:793-857), which the batched
+// kernels' loop (cuba_lm_batch.cuh) follows too.  A small system of N unknowns is packed as sys[0 .. N(N+1)/2): the upper triangle
+// (column n, row l <= n at n (n+1)/2 + l), then b = sys[N(N+1)/2 ..]; the step x solves (H + lambda I) x = b.
+namespace lm {
+
+constexpr int MAX_TRIALS = 10;
+
+// lambda of the first iteration: tau times the largest diagonal entry
+CUBA_HD double initial_lambda(double maxDiagonal)
+{
+	const double tau = 1e-5;
+	return tau * maxDiagonal;
+}
+
+// the largest diagonal entry of a packed system, starting from 0 (k_max_diagonal)
+template <int N>
+CUBA_HD double max_diagonal(const double* sys)
+{
+	double md = 0;
+#pragma unroll
+	for (int d = 0; d < N; d++) { const double v = sys[d * (d + 1) / 2 + d]; md = v > md ? v : md; }
+	return md;
+}
+
+// the damped solve of a packed system (k_solve_poses_only): x = 0 when the Cholesky of H + lambda I fails
+template <int N>
+CUBA_HD void damped_solve(const double* sys, double lambda, double x[N])
+{
+	double M[N * N];
+	for (int e = 0; e < N * N; e++) {
+		const int cn = e / N, l = e - N * cn;
+		const int lo = l < cn ? l : cn, hi = l < cn ? cn : l;
+		M[e] = sys[hi * (hi + 1) / 2 + lo] + ((e % (N + 1)) == 0 ? lambda : 0.0);
+	}
+	if (!spd_inverse<N>(M)) {
+		for (int i = 0; i < N; i++) x[i] = 0;
+	} else {
+		for (int r = 0; r < N; r++) {
+			double sum = 0;
+			for (int c = 0; c < N; c++) sum += M[c * N + r] * sys[N * (N + 1) / 2 + c];
+			x[r] = sum;
+		}
+	}
+}
+
+// the predicted decrease x^T (lambda x + b) of a step
+template <int N>
+CUBA_HD double predicted_decrease(const double* sys, double lambda, const double x[N])
+{
+	double sc = 0;
+	for (int i = 0; i < N; i++) sc += x[i] * (lambda * x[i] + sys[N * (N + 1) / 2 + i]);
+	return sc;
+}
+
+// the gain ratio of a trial that takes chi2 from F to Fhat; a NaN ratio rejects the trial
+CUBA_HD double gain_ratio(double F, double Fhat, double predicted)
+{
+	const double scale = predicted + 1e-3;
+	double rho = (F - Fhat) / scale;
+	if (!(rho == rho)) rho = -1;
+	return rho;
+}
+
+// the lambda / nu update a trial's gain ratio implies; returns whether the trial is accepted
+CUBA_HD bool update_damping(double rho, double& lambda, double& nu)
+{
+	if (rho > 0) {
+		const double x = 2 * rho - 1;
+		lambda *= fmax(1. / 3, fmin(1 - x * x * x, 2. / 3));
+		nu = 2;
+		return true;
+	}
+	lambda *= nu; nu *= 2;
+	return false;
+}
+
+// the end of the iterations: every trial of the iteration rejected, no decrease, or lambda no longer finite
+CUBA_HD bool stop(int rejected, double rho, double lambda)
+{
+	return rejected == MAX_TRIALS || rho <= 0 || !isfinite(lambda);
+}
+
+}  // namespace lm
 
 // pose <- Exp([omega;upsilon]) * pose  (cu:551-592): Rodrigues with the theta<1e-5 Taylor branch,
 // R->quaternion by the trace method (cu:492-521), normalisation with w>=0 (cu:531-539).
