@@ -19,7 +19,7 @@ PROFILE_ITEMS = ("0: Initialize Optimizer", "1: Build Structure", "2: Compute Er
 PCG_INFO_LEN = 16
 PCG_INFO_FIELDS = ("kernel", "two_level", "aggs_per_cta", "G", "gs", "A", "maxRows", "capBlocks", "zhInSmem", "coarse_kernel",
                    "cinfo", "status", "iters", "coarse_rebuilds", "bj_retries", "bad_rebuilds")
-PCG_KERNELS = ("none", "k_pcg", "k_pcg2", "k_pcg3", "k_pcg4", "k_pcg5", "k_pcg5_big", "k_pcg5t")   # "k_pcg" (retired) is never reported
+PCG_KERNELS = ("none", "k_pcg", "k_pcg2", "k_pcg3", "k_pcg4", "k_pcg5", "k_pcg5_big", "k_pcg5t", "k_dense_chol")   # "k_pcg" (retired) is never reported
 COARSE_KERNELS = ("none", "k_coarse_invert", "cluster2<8>", "cluster2<16>", "k_coarse_dense", "k_coarse_chol_cluster")   # the cluster kernels (retired) are never reported
 
 
@@ -118,11 +118,11 @@ _lib = None
 
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
-    "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_flush_l2",
+    "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_linear_solver", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_flush_l2",
     "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
-    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_peer_allreduce", "cuba_debug_pcg5_ranks", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
+    "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_dense_solve", "cuba_debug_peer_allreduce", "cuba_debug_pcg5_ranks", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dense_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
 ]
 
 
@@ -148,6 +148,7 @@ def load_library():
         "cuba_comm_unique_id": [vp],
         "cuba_engine_set_comm": [vp, i, i, vp],
         "cuba_engine_set_problem": [vp, C.POINTER(_Problem)],
+        "cuba_engine_set_linear_solver": [vp, i],
         "cuba_engine_set_structure_reuse": [vp, i],
         "cuba_engine_get_structure_reuses": [vp, C.POINTER(C.c_longlong)],
         "cuba_engine_set_state": [vp, vp, vp, vp],
@@ -180,6 +181,7 @@ def load_library():
         "cuba_debug_get_pcg_info": [vp, vp, C.POINTER(d)],
         "cuba_debug_get_coarse": [vp, vp, vp, vp],
         "cuba_debug_coarse_inverse": [vp, vp, i, vp, vp],
+        "cuba_debug_dense_solve": [vp, vp, vp, i, vp, C.POINTER(i)],
         "cuba_debug_peer_allreduce": [vp, i, C.c_int64, i, vp, vp],
         "cuba_debug_pcg5_ranks": [vp, i, i, i, vp, vp, vp, vp, vp],
         "cuba_debug_build_structure_host": [C.POINTER(_Problem), i, i, C.POINTER(_Sizes), vp, vp, vp, vp, vp, vp, vp, vp],
@@ -187,6 +189,7 @@ def load_library():
         "cuba_debug_pcg5_plan": [C.POINTER(_Problem), i, i, i, vp],
         "cuba_debug_pcg5_plan_apc": [C.POINTER(_Problem), i, i, i, i, vp, C.POINTER(C.c_uint64)],
         "cuba_debug_pcg5t_layout": [C.POINTER(_Problem), i, i, i, C.c_int64, vp],
+        "cuba_debug_dense_layout": [C.POINTER(_Problem), vp, vp],
         "cuba_debug_dropin_problem": [vp, C.POINTER(_Problem)],
         "cuba_debug_dropin_levels": [vp, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_int32)],
         "cuba_bench_stage": [vp, i, i, i, d, C.POINTER(d)],
@@ -276,6 +279,31 @@ def pcg5_plan_apc_host(prob, aggs_per_cta, world=1, num_sms=132, max_aggregates=
     return out
 
 
+LINEAR_SOLVERS = {"pcg": 0, "dense": 1}            # include/cuba_b200.h: CUBA_SOLVER_PCG, CUBA_SOLVER_DENSE_CHOLESKY
+DENSE_MAX_POSES = 2730                             # the direct solver's cap on free poses (n = 6 numP <= 16380)
+DENSE_LAYOUT_FIELDS = ("numP", "n", "nt", "tiles", "tile_mb")
+
+
+def set_linear_solver_raw(value):
+    """cuba_engine_set_linear_solver on no engine: the library checks the value before the engine, so this reaches no device; for
+    tests of that order"""
+    rc = load_library().cuba_engine_set_linear_solver(None, int(value))
+    return rc, load_library().cuba_last_error().decode()
+
+
+def dense_layout_host(prob):
+    """The direct solver's layout for the problem on the CPU (include/cuba_b200.h: cuba_debug_dense_layout): dict of
+    DENSE_LAYOUT_FIELDS and "map", the full-BSR block behind every block (i >= j) of the packed lower block triangle (-1: none)"""
+    L = load_library()
+    P, keep = _problem_struct(prob)
+    info = np.zeros(len(DENSE_LAYOUT_FIELDS), np.int32)
+    m = np.zeros(prob.numP * (prob.numP + 1) // 2, np.int32)
+    _check(L.cuba_debug_dense_layout(C.byref(P), _p(info), _p(m)))
+    out = dict(zip(DENSE_LAYOUT_FIELDS, (int(v) for v in info)))
+    out["map"] = m
+    return out
+
+
 # cuba_debug_pcg5_ranks: plan[] fields
 PCG5_RANKS_PLAN_FIELDS = ("G", "gs", "A", "needMax", "maxRows", "halo", "big", "cinfo")
 PCG5T_LAYOUT_FIELDS = ("ok", "aggs_per_cta", "capBlocks", "streamed_blocks", "zhInSmem", "total_bytes", "blk_bytes", "rsu_bytes",
@@ -358,6 +386,13 @@ class Engine:
         self.sizes = {n: getattr(sz, n) for n, _ in _Sizes._fields_}
         self._stats = []
         return self.sizes
+
+    def set_linear_solver(self, solver):
+        """"pcg" (default: the PCG family of pcg_variant) or "dense" (dense fp64 Cholesky of S, at most DENSE_MAX_POSES free poses);
+        applies from the next initialize()"""
+        if solver not in LINEAR_SOLVERS:
+            raise ValueError("linear solver %r: one of %s" % (solver, ", ".join(LINEAR_SOLVERS)))
+        _check(self.L.cuba_engine_set_linear_solver(self.h, LINEAR_SOLVERS[solver]))
 
     def set_structure_reuse(self, enable):
         _check(self.L.cuba_engine_set_structure_reuse(self.h, int(bool(enable))))
@@ -637,6 +672,18 @@ class Engine:
         info = C.c_int(-1)
         _check(self.L.cuba_debug_coarse_inverse(self.h, _p(AcP), A, _p(AcInv), C.byref(info)))
         return AcInv, info.value
+
+    def debug_dense_solve(self, S, b):
+        """(x, info) of the direct solver's kernel on the dense SPD matrix S [n][n] (its lower triangle is read) and b [n], in buffers
+        of its own; info 1: not positive definite, x zeroed"""
+        S = np.ascontiguousarray(S, dtype=np.float64)
+        b = np.ascontiguousarray(b, dtype=np.float64).reshape(-1)
+        n = b.size
+        assert S.shape == (n, n), (S.shape, n)
+        x = np.zeros(n)
+        info = C.c_int(-1)
+        _check(self.L.cuba_debug_dense_solve(self.h, _p(S), _p(b), n, _p(x), C.byref(info)))
+        return x, info.value
 
     def peer_allreduce(self, parts):
         """the peer all-reduce of a `world`-rank run emulated on this GPU (include/cuba_b200.h: cuba_debug_peer_allreduce): parts

@@ -6,8 +6,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcuba_b200.so")
 SOURCES = ["cuba_engine.cu", "cuba_structure.cpp", "cuba_api.cpp"]
-HEADERS = ["cuba_kernels.cuh", "cuba_jh4.cuh", "cuba_levels.cuh", "cuba_lm_batch.cuh", "cuba_pose_batch.cuh", "cuba_sim3_batch.cuh", "cuba_schur3.cuh", "cuba_schur5.cuh", "cuba_pcg2.cuh", "cuba_pcg3.cuh", "cuba_pcg4.cuh", "cuba_pcg5.cuh", "cuba_pcg5t.cuh", "cuba_coarse.cuh", "cuba_peer_reduce.cuh", "cuba_structure_gpu.cuh", "cuba_math.cuh", "cuba_structure.h",
-           "../../include/cuba_b200.h", "../../include/cuba_b200_levels.h", "../../include/cuba_b200_pose.h", "../../include/cuba_b200_sim3.h", "../../include/cuda_bundle_adjustment.h", "../../include/cuda_bundle_adjustment_types.h"]
+HEADERS = ["cuba_kernels.cuh", "cuba_jh4.cuh", "cuba_levels.cuh", "cuba_lm_batch.cuh", "cuba_pose_batch.cuh", "cuba_sim3_batch.cuh", "cuba_schur3.cuh", "cuba_schur5.cuh", "cuba_pcg2.cuh", "cuba_pcg3.cuh", "cuba_pcg4.cuh", "cuba_pcg5.cuh", "cuba_pcg5t.cuh", "cuba_coarse.cuh", "cuba_dense_chol.cuh", "cuba_peer_reduce.cuh", "cuba_structure_gpu.cuh", "cuba_math.cuh", "cuba_structure.h",
+           "../../include/cuba_b200.h", "../../include/cuba_b200_levels.h", "../../include/cuba_b200_solver.h", "../../include/cuba_b200_pose.h", "../../include/cuba_b200_sim3.h", "../../include/cuda_bundle_adjustment.h", "../../include/cuda_bundle_adjustment_types.h"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = (["-DCUBA_JH4_DEBUG"] if os.environ.get("CUBA_JH4_DEBUG") else []) + ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
          "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared"]

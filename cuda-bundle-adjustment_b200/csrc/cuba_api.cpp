@@ -39,6 +39,7 @@
 #include "../../include/cuba_b200_levels.h"
 #include "../../include/cuba_b200_pose.h"
 #include "../../include/cuba_b200_sim3.h"
+#include "../../include/cuba_b200_solver.h"
 
 namespace cuba
 {
@@ -358,11 +359,15 @@ public:
 		ensureEngine();
 		check(cuba_engine_set_robust_kernel(engine_, CUBA_EDGE_MONOCULAR, kernels_[0].type, kernels_[0].delta));
 		check(cuba_engine_set_robust_kernel(engine_, CUBA_EDGE_STEREO, kernels_[1].type, kernels_[1].delta));
-		if (!uploaded_) {
-			// the reference builds its structure inside the first optimize() iteration (cpp:804-805)
+		if (!uploaded_ || solverChanged_) {
+			// the reference builds its structure inside the first optimize() iteration (cpp:804-805); a new linear solver takes effect
+			// through set_problem too, from the estimate of the last optimize() (the flat arrays hold it), keeping the levels
+			if (uploaded_) levelsFromDevice();
+			check(cuba_engine_set_linear_solver(engine_, solver_ == LinearSolverType::DENSE_CHOLESKY ? CUBA_SOLVER_DENSE_CHOLESKY : CUBA_SOLVER_PCG));
 			cuba_problem p;
 			flatProblem(p);
 			check(cuba_engine_set_problem(engine_, &p));
+			solverChanged_ = false;      // only once the engine holds the problem for the chosen solver: a refused upload is tried again
 			uploaded_ = true;
 			levDevNewer_ = false;
 			// set_problem left every level at 0: lev_ must first take the levels set since initialize() before it is compared with that
@@ -409,6 +414,15 @@ public:
 		p.E3 = static_cast<int32_t>(om3_.size()); p.idx3 = idx3_.data(); p.meas3 = meas3_.data(); p.omega3 = om3_.data();
 		return true;
 	}
+
+	// ---- linear solver (include/cuba_b200_solver.h) ----
+	void setLinearSolver(LinearSolverType type)
+	{
+		if (type == solver_) return;
+		solver_ = type;
+		solverChanged_ = true;
+	}
+	LinearSolverType linearSolver() const { return solver_; }
 
 	// ---- edge levels (include/cuba_b200_levels.h) ----
 	void setEdgeLevel(BaseEdge* e, int level)
@@ -602,6 +616,8 @@ private:
 	HostBuf<int32_t> idx2_, idx3_;
 	HostBuf<unsigned char> lev_;                 // flat levels, order of the flat edge arrays
 	bool initialized_ = false, uploaded_ = false;
+	LinearSolverType solver_ = LinearSolverType::PCG;
+	bool solverChanged_ = false;   // the engine holds the problem for the other solver: the next optimize() uploads it again
 	double initSeconds_ = 0;
 
 	cuba_engine* engine_ = nullptr;
@@ -633,6 +649,10 @@ static Impl& impl_of(const CudaBundleAdjustment& ba)
 void setEdgeLevel(CudaBundleAdjustment& ba, BaseEdge* e, int level) { impl_of(ba).setEdgeLevel(e, level); }
 int edgeLevel(const CudaBundleAdjustment& ba, const BaseEdge* e) { return impl_of(ba).edgeLevel(e); }
 OutlierCounts classifyEdges(CudaBundleAdjustment& ba, const OutlierTest& test) { return impl_of(ba).classifyEdges(test); }
+
+// include/cuba_b200_solver.h
+void setLinearSolver(CudaBundleAdjustment& ba, LinearSolverType type) { impl_of(ba).setLinearSolver(type); }
+LinearSolverType linearSolver(const CudaBundleAdjustment& ba) { return impl_of(ba).linearSolver(); }
 
 // include/cuba_b200_pose.h
 std::vector<PoseRound> orbSlam2PoseSchedule()

@@ -304,6 +304,36 @@ __device__ __forceinline__ void frag_store(double* s, const double (&D)[4][4][2]
 		for (int bj = 0; bj < 4; bj++) *reinterpret_cast<double2*>(s + (8 * bi + r) * TS + 8 * bj + c) = make_double2(sgn * D[bi][bj][0], sgn * D[bi][bj][1]);
 }
 
+// one warp factors the stored tile g = L L^T in registers: lane i loads row i and, on success, holds row i of L (lower, zero above
+// the diagonal) in row and 1 / L(i, i) in rdiag.  Entries above the diagonal of g do not matter.  sRow: NB doubles of shared scratch.  false
+// on a pivot that is not positive (row is then partly factored).  Shared by k_coarse_dense and k_dense_chol (cuba_dense_chol.cuh).
+__device__ __forceinline__ bool pivot_factor(const double* g, double (&row)[NB], double& rdiag, double* sRow, int lane)
+{
+	g += lane * NB;
+#pragma unroll
+	for (int i = 0; i < NB; i += 2) { const double2 v = __ldcg(reinterpret_cast<const double2*>(g + i)); row[i] = v.x; row[i + 1] = v.y; }
+	bool ok = true;
+	rdiag = 0.0;
+#pragma unroll
+	for (int k = 0; k < NB; k++) {
+		sRow[lane] = row[k];
+		__syncwarp();
+		const double d = sRow[k];
+		if (!(d > 0)) { ok = false; break; }
+		const double lkk = sqrt(d), rk = 1.0 / lkk;
+		const double lik = lane > k ? row[k] * rk : lane == k ? lkk : 0.0;      // column k of L
+		if (lane == k) rdiag = rk;
+		__syncwarp();
+		sRow[lane] = lik;
+		__syncwarp();
+#pragma unroll
+		for (int j = k + 1; j < NB; j++) row[j] = fma(-lik, sRow[j], row[j]);
+		row[k] = lik;
+		__syncwarp();
+	}
+	return ok;
+}
+
 // a finished tile in shared memory (element (r, c) = sgn s[r * sr + c * sc]; a diagonal tile mirrored from its lower triangle)
 // -> tile (I, J) of the next copy, or, at the last step, -value in fp32 to both triangles of Ac^-1
 __device__ __forceinline__ void tile_out(const double* s, int sr, int sc, double sgn, bool diag, int I, int J, double* dst, bool last,
@@ -385,28 +415,8 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_coarse_dense(const Args a)
 		if (wid == 0) {
 			// ---- the pivot: every CTA factors A_KK = L L^T in registers (lane i holds row i) and forms L^-1 (lane q: column q) ----
 			double row[NB];
-			const double* g = tile(src, K, K) + lane * NB;
-#pragma unroll
-			for (int i = 0; i < NB; i += 2) { const double2 v = __ldcg(reinterpret_cast<const double2*>(g + i)); row[i] = v.x; row[i + 1] = v.y; }
-			bool ok = true;
-			double rdiag = 0.0;                          // lane i: 1 / L(i, i)
-#pragma unroll
-			for (int k = 0; k < NB; k++) {
-				sRow[lane] = row[k];
-				__syncwarp();
-				const double d = sRow[k];
-				if (!(d > 0)) { ok = false; break; }
-				const double lkk = sqrt(d), rk = 1.0 / lkk;
-				const double lik = lane > k ? row[k] * rk : lane == k ? lkk : 0.0;      // column k of L
-				if (lane == k) rdiag = rk;
-				__syncwarp();
-				sRow[lane] = lik;
-				__syncwarp();
-#pragma unroll
-				for (int j = k + 1; j < NB; j++) row[j] = fma(-lik, sRow[j], row[j]);
-				row[k] = lik;
-				__syncwarp();
-			}
+			double rdiag;                                // lane i: 1 / L(i, i)
+			const bool ok = pivot_factor(tile(src, K, K), row, rdiag, sRow, lane);
 			if (!ok) { if (lane == 0) s_fail = 1; }
 			else {
 				// row = row `lane` of L (lower); column q of L^-1 by forward substitution, x_i = (delta_iq - sum_{k<i} L_ik x_k) / L_ii

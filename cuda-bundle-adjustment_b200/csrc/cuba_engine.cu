@@ -24,6 +24,7 @@
 #include "cuba_pcg5.cuh"
 #include "cuba_pcg5t.cuh"
 #include "cuba_coarse.cuh"
+#include "cuba_dense_chol.cuh"
 #include "cuba_peer_reduce.cuh"
 #include "cuba_jh4.cuh"
 #include "cuba_levels.cuh"
@@ -38,6 +39,12 @@ namespace cuba_b200 {
 
 static thread_local std::string g_err;
 static int fail(int code, const std::string& msg) { g_err = msg; return code; }
+// the direct solver holds the whole reduced camera system in fp64 tiles: at most dchol::MAX_POSES free poses
+static int dense_cap_error(int numP)
+{
+	return fail(CUBA_ERR_INVALID, "set_problem: the dense Cholesky solver takes at most " + std::to_string(dchol::MAX_POSES) + " free poses, this problem has numP = "
+		+ std::to_string(numP) + " (choose CUBA_SOLVER_PCG)");
+}
 
 // fixed shared-memory footprint of k_pcg3 (a superset of k_pcg2's): r,s per needed column, p,y per own row, index lists
 static size_t pcg3_fixed_bytes(int needMax, int maxRows, size_t scalar)
@@ -270,6 +277,7 @@ struct EngineBase {
 	double rk_delta[2] = { 0, 0 };
 	int rank = 0, world = 1;
 	bool structureReuse = true;   // cuba_engine_set_structure_reuse
+	int linSolver = CUBA_SOLVER_PCG;   // cuba_engine_set_linear_solver: applies from the next set_problem
 	long long structureReuses = 0;
 	int devOrdinal = 0;      // CUDA device every call of this engine runs on (set once in init)
 	void* comm = nullptr;
@@ -303,6 +311,7 @@ struct EngineBase {
 	virtual int dbg_pcg_info(int32_t* info, double* coarseLambda) = 0;
 	virtual int dbg_coarse(int32_t* rowAgg, double* AcP, float* AcInv) = 0;
 	virtual int dbg_coarse_inverse(const double* AcP, int A, float* AcInv, int* info) = 0;
+	virtual int dbg_dense_solve(const double* S, const double* b, int n, double* x, int* info) = 0;
 	virtual int dbg_peer_allreduce(int world, size_t n, int calls, const double* parts, double* out) = 0;
 	virtual int dbg_pcg5_ranks(int world, int twoLevel, int nsolves, double* x, int32_t* status, int32_t* plan, int32_t* aggRow, float* AcInv) = 0;
 	virtual int set_edge_levels(const uint8_t* levels) = 0;
@@ -514,13 +523,15 @@ struct Engine : EngineBase {
 		if ((p->Pall > 0 && (!p->q || !p->t || !p->cam)) || (p->Lall > 0 && !p->Xw) || (p->E2 > 0 && (!p->idx2 || !p->meas2 || !p->omega2)) ||
 			(p->E3 > 0 && (!p->idx3 || !p->meas3 || !p->omega3)))
 			return fail(CUBA_ERR_INVALID, "set_problem: null array with a non-zero count");
+		// the cap, before any change; a pose-only system (no free landmark) never reaches the direct solver (k_solve_poses_only)
+		if (linSolver == CUBA_SOLVER_DENSE_CHOLESKY && p->numP > dchol::MAX_POSES && p->numL > 0) return dense_cap_error(p->numP);
 		const auto t0 = std::chrono::steady_clock::now();
 		lastPcgKernel = CUBA_PCG_KERNEL_NONE; p5.coarse.rebuilds = 0; bjRetries = 0;
 		lvOn = false;      // every level back to 0: both paths below scatter the caller's omega unmasked
 		// Same topology as the problem this engine already holds (sizes, fixed/free split and every (iP, iL) pair identical): only the
 		// numbers changed -- the estimate after a previous optimize(), new measurements -- so every index structure, tile list,
 		// product list and PCG partition on the device stays valid.  Upload the values and re-run the three kernels that scatter them.
-		if (structureReuse && reusable && haveProblem && cfg.reserved[1] != 1 && same_topology(p)) {
+		if (structureReuse && reusable && haveProblem && cfg.reserved[1] != 1 && denseSolve == (linSolver == CUBA_SOLVER_DENSE_CHOLESKY) && same_topology(p)) {
 			int rc = refresh_values(p); if (rc) return rc;
 			structureReuses++;
 			prof[CUBA_PROF_BUILD_STRUCTURE] += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
@@ -908,8 +919,18 @@ struct Engine : EngineBase {
 		tmark("alloc + Schur setup queued");
 		if (jhV4) { int rc = setup_jh4(); if (rc) return rc; }
 		tmark("jh4 queued");
-		if (S.numP > 0) { int rc = setup_pcg2(); if (rc) return rc; }        // host-heavy: overlaps the warp-tile kernels queued above
-		if (S.numP > 0 && S.numL > 0) { int rc = setup_pcg5(); if (rc) return rc; }
+		// the solver's setup: no PCG partition or plan for the direct solver (its need lists may not fit, and nothing reads them)
+		denseSolve = linSolver == CUBA_SOLVER_DENSE_CHOLESKY;
+		if (denseSolve) {
+			pcg3Ok = false; pcg4Ok = false; p5Ok = false; p5Dist = false;      // what a PCG structure before this one prepared
+			if (S.numP > 0 && S.numL > 0) { int rc = setup_dense(); if (rc) return rc; }
+			else release_dense();
+		}
+		else {
+			release_dense();                                                   // up to 1 GB of tiles nothing reads any more
+			if (S.numP > 0) { int rc = setup_pcg2(); if (rc) return rc; }        // host-heavy: overlaps the warp-tile kernels queued above
+			if (S.numP > 0 && S.numL > 0) { int rc = setup_pcg5(); if (rc) return rc; }
+		}
 		tmark("pcg partition (host)");
 		if (jhV4) { int rc = setup_jh4_finish(); if (rc) return rc; }
 		tmark("jh4 finish");
@@ -1876,6 +1897,55 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// ---- the direct solver (cuba_dense_chol.cuh) ---------------------------------------------------------------------------
+	bool denseSolve = false;        // the structure was built for the direct solver (set_problem, from linSolver)
+	DBuf<int> dcMap;                // packed lower block triangle -> block of the full BSR (build_dense_block_map)
+	DBuf<double> dcTiles, dcY;
+	DBuf<GridBar> dcBar;
+	// CTAs of k_dense_chol for an n x n system: enough for the widest phase (the first trailing update), at most one per SM
+	int dense_grid(int n) const
+	{
+		const long long nt = dchol::tile_rows(n), widest = std::max(nt * (nt - 1) / 2, nt);
+		return (int)std::max(1LL, std::min<long long>(numSMs, (widest + dchol::WARPS - 1) / dchol::WARPS));
+	}
+	void release_dense() { dcMap.release(); dcTiles.release(); dcY.release(); }
+	int setup_dense()
+	{
+		const int n = 6 * S.numP;
+		std::vector<int> map;
+		build_dense_block_map(S.numP, S.fRowPtr, S.fColInd, map);
+		CUDA_TRY(dcMap.upload(map, stream));
+		CUDA_TRY(dcTiles.alloc(dchol::tile_doubles(n))); CUDA_TRY(dcY.alloc(dchol::rhs_doubles(n)));
+		CUDA_TRY(dcBar.alloc(1));
+		CUDA_TRY(cudaMemsetAsync(dcBar.p, 0, sizeof(GridBar), stream));
+		return CUBA_OK;
+	}
+	template <typename U>
+	int launch_dense_chol(const dchol::Args<U>& a)
+	{
+		CUDA_TRY(cudaFuncSetAttribute(dchol::k_dense_chol<U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dchol::SMEM));
+		void* args[] = { (void*)&a };
+		CUDA_TRY(cudaLaunchCooperativeKernel((void*)dchol::k_dense_chol<U>, dim3(dense_grid(a.n)), dim3(dchol::WARPS * 32), args, dchol::SMEM, stream));
+		launches++;
+		return CUBA_OK;
+	}
+	// S xp = bsc by Cholesky: status slot iters 0, status 0 (2: S not positive definite, xp = 0)
+	int launch_dense()
+	{
+		if (!dcTiles.p) return fail(CUBA_ERR_STATE, "dense solve: the problem has no reduced camera system (no free pose or no free landmark)");
+		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
+		dchol::Args<T> a;
+		a.fVal = fVal; a.blkMap = dcMap; a.dense = nullptr; a.b = bsc; a.n = 6 * S.numP;
+		a.tl = dcTiles; a.y = dcY; a.x = xp; a.status = &dScal.p->pcg; a.info = nullptr; a.bar = dcBar;
+		const int rc = launch_dense_chol(a); if (rc) return rc;
+		lastPcgTwoLevel = false;
+		lastPcgKernel = CUBA_PCG_KERNEL_DENSE;
+		return CUBA_OK;
+	}
+
+	// the reduced-system solve of the structure's solver
+	int launch_solver() { return denseSolve ? launch_dense() : launch_pcg(); }
+
 	int launch_pcg()
 	{
 		lastPcgTwoLevel = false;
@@ -1927,7 +1997,7 @@ struct Engine : EngineBase {
 		int rc = launch_schur(lam); if (rc) return rc;
 		int nScaleL = 0;
 		if (S.numP > 0 && S.numL > 0) {
-			rc = launch_pcg(); if (rc) return rc;
+			rc = launch_solver(); if (rc) return rc;
 			rc = launch_backsub(lam); if (rc) return rc;
 			nScaleL = ntiles;
 		} else if (S.numP > 0) {
@@ -2530,6 +2600,30 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// include/cuba_b200.h: cuba_debug_dense_solve -- k_dense_chol (fp64) on a caller's dense matrix, in buffers of its own
+	int dbg_dense_solve(const double* hS, const double* hb, int n, double* hx, int* hInfo) override
+	{
+		if (n < 1 || !hS || !hb || !hx || !hInfo) return fail(CUBA_ERR_INVALID, "debug_dense_solve: n < 1 or a NULL pointer");
+		if (n > 6 * dchol::MAX_POSES) return fail(CUBA_ERR_INVALID, "debug_dense_solve: n > " + std::to_string(6 * dchol::MAX_POSES));
+		const size_t nn = (size_t)n * n;
+		DBuf<double> dS, db, dx, dT, dY;
+		DBuf<int> dInfo;
+		DBuf<GridBar> dBar;
+		CUDA_TRY(dS.upload(hS, nn, stream)); CUDA_TRY(db.upload(hb, (size_t)n, stream)); CUDA_TRY(dx.alloc((size_t)n));
+		CUDA_TRY(dT.alloc(dchol::tile_doubles(n))); CUDA_TRY(dY.alloc(dchol::rhs_doubles(n)));
+		CUDA_TRY(dInfo.alloc(1)); CUDA_TRY(dBar.alloc(1));
+		CUDA_TRY(cudaMemsetAsync(dBar.p, 0, sizeof(GridBar), stream));
+		CUDA_TRY(cudaMemsetAsync(dInfo.p, 0xff, sizeof(int), stream));          // -1 unless the kernel reports
+		dchol::Args<double> a;
+		a.fVal = nullptr; a.blkMap = nullptr; a.dense = dS; a.b = db; a.n = n;
+		a.tl = dT; a.y = dY; a.x = dx; a.status = nullptr; a.info = dInfo; a.bar = dBar;
+		int rc = launch_dense_chol(a); if (rc) return rc;
+		CUDA_TRY(cudaMemcpyAsync(hx, dx.p, sizeof(double) * n, cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaMemcpyAsync(hInfo, dInfo.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		return CUBA_OK;
+	}
+
 	// include/cuba_b200.h: cuba_debug_peer_allreduce -- `world` ranks of k_peer_allreduce emulated on this GPU by one cooperative
 	// launch of k_peer_allreduce_ranks (numSMs / world CTAs per rank), in buffers of its own
 	int dbg_peer_allreduce(int W, size_t n, int calls, const double* parts, double* out) override
@@ -2663,7 +2757,7 @@ struct Engine : EngineBase {
 			case 1: rc = launch_linearize_landmark(); break;
 			case 2: rc = launch_linearize_pose(); break;
 			case 3: rc = launch_schur(lam); break;
-			case 4: curLambda = lambda; rc = launch_pcg(); break;
+			case 4: curLambda = lambda; rc = launch_solver(); break;
 			case 5: rc = launch_backsub(lam); if (!rc) rc = stage_update_nofetch(lam); break;
 			case 6: rc = launch_chi2(cur, 0); break;
 			case 7:   // one rebuild of the coarse inverse of k_pcg5 / k_pcg5t (projection, assembly, inverse) from the current system
@@ -2776,6 +2870,15 @@ int cuba_engine_set_comm(cuba_engine* e, int rank, int world, const void* uid)
 }
 
 int cuba_engine_set_problem(cuba_engine* e, const cuba_problem* p) { ENGINE_OR_FAIL(e); return e->impl->set_problem(p); }
+int cuba_engine_set_linear_solver(cuba_engine* e, int solver)
+{
+	// the value first: a bad one is refused before anything (a device included) is touched
+	if (solver != CUBA_SOLVER_PCG && solver != CUBA_SOLVER_DENSE_CHOLESKY)
+		return fail(CUBA_ERR_INVALID, "set_linear_solver: " + std::to_string(solver) + " names no solver (0 PCG, 1 dense Cholesky)");
+	ENGINE_OR_FAIL(e);
+	e->impl->linSolver = solver;
+	return CUBA_OK;
+}
 int cuba_engine_set_structure_reuse(cuba_engine* e, int enable) { ENGINE_OR_FAIL(e); e->impl->structureReuse = enable != 0; return CUBA_OK; }
 int cuba_engine_get_structure_reuses(cuba_engine* e, long long* count) { ENGINE_OR_FAIL(e); if (count) *count = e->impl->structureReuses; return CUBA_OK; }
 int cuba_engine_set_state(cuba_engine* e, const double* q, const double* t, const double* Xw)
@@ -2932,6 +3035,7 @@ int cuba_debug_get_delta(cuba_engine* e, double* xp, double* xl) { ENGINE_OR_FAI
 int cuba_debug_get_pcg_info(cuba_engine* e, int32_t* info, double* coarse_lambda) { ENGINE_OR_FAIL(e); return e->impl->dbg_pcg_info(info, coarse_lambda); }
 int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* AcInv) { ENGINE_OR_FAIL(e); return e->impl->dbg_coarse(aggRow, AcP, AcInv); }
 int cuba_debug_coarse_inverse(cuba_engine* e, const double* AcP, int A, float* AcInv, int* info) { ENGINE_OR_FAIL(e); return e->impl->dbg_coarse_inverse(AcP, A, AcInv, info); }
+int cuba_debug_dense_solve(cuba_engine* e, const double* S, const double* b, int n, double* x, int* info) { ENGINE_OR_FAIL(e); return e->impl->dbg_dense_solve(S, b, n, x, info); }
 int cuba_debug_peer_allreduce(cuba_engine* e, int world, int64_t n, int calls, const double* parts, double* out)
 {
 	ENGINE_OR_FAIL(e);
@@ -3076,6 +3180,24 @@ int cuba_debug_pcg5t_layout(const cuba_problem* p, int numSMs, int aggsPerCtaTop
 		else { if (!p5t::pcg5t_fit<float>(t, plan.P.blkMax, apc, (size_t)smemBudget)) continue; report(p5t::Pcg5Layout<float>(t)); }
 		break;
 	}
+	return CUBA_OK;
+}
+
+int cuba_debug_dense_layout(const cuba_problem* p, int32_t* info, int32_t* map)
+{
+	if (!p) return fail(CUBA_ERR_INVALID, "dense_layout: null problem");
+	if (p->numP > dchol::MAX_POSES && p->numL > 0) return dense_cap_error(p->numP);
+	Structure S;
+	const char* err = "";
+	if (!build_structure(p->Pall, p->numP, p->Lall, p->numL, p->E2, p->idx2, p->E3, p->idx3, 0, 1, TILE, S, &err)) return fail(CUBA_ERR_INVALID, err);
+	const int n = 6 * S.numP, nt = dchol::tile_rows(n);
+	std::vector<int> m;
+	build_dense_block_map(S.numP, S.fRowPtr, S.fColInd, m);
+	if (info) {
+		const int64_t v[5] = { S.numP, n, nt, (int64_t)cdense::tiles(nt), (int64_t)(dchol::tile_doubles(n) * sizeof(double) >> 20) };
+		for (int i = 0; i < 5; i++) info[i] = (int32_t)v[i];
+	}
+	if (map && !m.empty()) memcpy(map, m.data(), sizeof(int) * m.size());
 	return CUBA_OK;
 }
 

@@ -307,6 +307,16 @@ void build_coarse_partition(int numP, const PcgPartition& P, int maxAgg, CoarseP
 	C.maxNeedAgg = std::max(maxNA, 1);
 }
 
+void build_dense_block_map(int numP, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, std::vector<int>& map)
+{
+	map.assign((size_t)numP * (numP + 1) / 2, -1);
+	for (int i = 0; i < numP; i++)
+		for (int n = fRowPtr[i]; n < fRowPtr[i + 1]; n++) {
+			const int j = fColInd[n];
+			if (j <= i) map[(size_t)i * (i + 1) / 2 + j] = n;
+		}
+}
+
 void build_coarse_lists(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, CoarsePartition& C)
 {
 	// fine blocks of every coarse block (lower triangle), ascending -> fixed-order sums in k_coarse_assemble

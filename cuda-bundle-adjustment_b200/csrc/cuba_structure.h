@@ -119,6 +119,10 @@ struct Pcg5Plan {
 // `same`: a partition of the same system the caller already has (k_pcg3's); copied instead of rebuilt when its CTA count fits.
 void build_pcg5_plan(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, int world, int numSMs, int maxAgg,
 	int maxRowsPerCta, Pcg5Plan& plan, const PcgPartition* same = nullptr, int apc = 1);
+// The direct solver (cuba_dense_chol.cuh): the block of the symmetric-full BSR behind every block of the packed lower block
+// triangle of S -- block (i >= j) at i (i+1)/2 + j, -1 where S has none.  Built once per structure.
+void build_dense_block_map(int numP, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, std::vector<int>& map);
+
 // invariants of a plan (nullptr when everything holds)
 const char* check_pcg5_plan(int numP, int nfull, const std::vector<int>& fRowPtr, const std::vector<int>& fColInd, const Pcg5Plan& plan);
 

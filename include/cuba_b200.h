@@ -63,7 +63,7 @@ extern "C" {
 #define CUBA_PROF_BUILD_SYSTEM 3
 #define CUBA_PROF_SCHUR_COMPLEMENT 4
 #define CUBA_PROF_DECOMP_SYMBOLIC 5   /* always 0: PCG has no symbolic phase */
-#define CUBA_PROF_DECOMP_NUMERICAL 6  /* the PCG solve                        */
+#define CUBA_PROF_DECOMP_NUMERICAL 6  /* the PCG solve, or the dense Cholesky  */
 #define CUBA_PROF_UPDATE 7
 #define CUBA_PROF_NUM 8
 
@@ -155,6 +155,18 @@ int cuba_engine_set_comm(cuba_engine* e, int rank, int world, const void* nccl_u
 
 /* Upload the problem and build every index structure (initialize + buildStructure). */
 int cuba_engine_set_problem(cuba_engine* e, const cuba_problem* p);
+/* Linear solver of the reduced camera system S xp = bsc (S = Hsc + lambda I), g2o's choice of LinearSolver / Ceres' DENSE_SCHUR
+ * vs ITERATIVE_SCHUR.  CUBA_SOLVER_PCG (default): the PCG family that cuba_config.reserved[0] selects.  CUBA_SOLVER_DENSE_CHOLESKY: a
+ * dense fp64 Cholesky factorisation of S on the tensor pipe (csrc/cuba_dense_chol.cuh; the fp32 engine widens S), with the reference's
+ * semantics: an exact step, and a trial whose factorisation fails (S not positive definite) is rejected.  It needs no PCG partition,
+ * so graphs whose need lists do not fit the PCG's shared memory are accepted, and it takes at most 2730 free poses (n <= 16380,
+ * about 1.1 GB of fp64 tiles): set_problem returns CUBA_ERR_INVALID beyond that, before any allocation, and the engine keeps its
+ * previous problem.  A problem without free landmarks has no reduced camera system (its poses are solved block by block): there
+ * the choice changes nothing, and neither the cap nor the tiles apply.  The choice applies from the next set_problem (a structure-reuse set_problem after a change rebuilds what the new
+ * solver needs); any other value gives CUBA_ERR_INVALID. */
+#define CUBA_SOLVER_PCG 0
+#define CUBA_SOLVER_DENSE_CHOLESKY 1
+int cuba_engine_set_linear_solver(cuba_engine* e, int solver);
 /* Structure reuse (SURVEY.md 8 f-2; on by default): a set_problem whose sizes, fixed/free split and (iP,iL) lists equal those of the
  * problem the engine already holds keeps every device structure (index lists, tiles, product lists, PCG partition) and only
  * uploads the numbers -- repeated local-BA calls on an unchanged graph, e.g. the reference protocol's second initialize()
@@ -347,6 +359,7 @@ int cuba_debug_get_delta(cuba_engine* e, double* xp /*6*numP*/, double* xl /*3*n
 #define CUBA_PCG_KERNEL_PCG5 5            /* k_pcg5<T, false>: the legacy shape */
 #define CUBA_PCG_KERNEL_PCG5_BIG 6        /* k_pcg5<T, true> */
 #define CUBA_PCG_KERNEL_PCG5T 7           /* k_pcg5t<T, K>, K = info[2] */
+#define CUBA_PCG_KERNEL_DENSE 8           /* dchol::k_dense_chol: the direct solver (plan fields 0, status 0 or 2, iterations 0) */
 #define CUBA_COARSE_KERNEL_NONE 0
 #define CUBA_COARSE_KERNEL_INVERT 1       /* k_coarse_invert: one CTA, A <= 37 */
 #define CUBA_COARSE_KERNEL_CLUSTER8 2     /* the retired k_coarse_chol_cluster2<8>: never reported, the number stays taken */
@@ -362,6 +375,10 @@ int cuba_debug_get_coarse(cuba_engine* e, int32_t* aggRow, double* AcP, float* A
  * AcP (layout of cuba_debug_get_coarse, A >= 1 aggregates) in buffers of its own: AcInv [6A][6A] fp32 and info 0 (inverted) or 1
  * (not positive definite: AcInv all zeros).  Needs a GPU, not a problem; no engine state changes. */
 int cuba_debug_coarse_inverse(cuba_engine* e, const double* AcP, int A, float* AcInv, int* info);
+/* Runs the direct solver's kernel k_dense_chol (fp64) on the caller's n x n matrix S (row-major; its lower triangle is read) and b [n],
+ * in buffers of its own: x [n] and info 0 (solved) or 1 (not positive definite: x all zeros).  1 <= n <= 16380.  Needs a GPU, not a
+ * problem; no engine state changes. */
+int cuba_debug_dense_solve(cuba_engine* e, const double* S, const double* b, int n, double* x, int* info);
 /* The two kernels of a landmark-sharded run that exchange through peer memory, with `world` ranks (1..8) emulated on this GPU:
  * the boards of every rank live in this device's memory and ONE cooperative launch runs all ranks, CTA b acting as CTA b % G of
  * rank b / G.  Both use buffers of their own and change no engine state; both fail with CUBA_ERR_INVALID when the world * G CTAs
@@ -413,6 +430,11 @@ int cuba_debug_pcg5_plan_apc(const cuba_problem* p, int world, int numSMs, int m
  * the bytes of the cached blocks, of r / s / u, of the product staging (with the polled words), of rc, of Z^ and of the slice
  * of Ac^-1.  No device needed. */
 int cuba_debug_pcg5t_layout(const cuba_problem* p, int numSMs, int aggsPerCtaTop, int scalarBytes, int64_t smemBudget, int32_t* info);
+/* CPU-only: the layout the direct solver gets for the problem, as set_problem builds it.  info[5] = numP, n = 6 numP, tile rows nt =
+ * ceil(n / 32), lower tiles nt (nt+1) / 2, MB of fp64 tiles; map [numP (numP+1) / 2] (may be NULL): for block (i >= j) of the packed
+ * lower block triangle of S (at i (i+1)/2 + j) its index in the symmetric-full BSR of cuba_debug_build_structure_host, -1 where S has
+ * no block.  CUBA_ERR_INVALID, with the message of set_problem, beyond 2730 free poses when there are free landmarks.  No device needed. */
+int cuba_debug_dense_layout(const cuba_problem* p, int32_t* info, int32_t* map);
 /* The flat arrays the drop-in class (cuba::CudaBundleAdjustment, csrc/cuba_api.cpp) built in its last initialize(): what optimize()
  * hands to cuba_engine_set_problem.  `dropin` is the object's address; the pointers stay valid until the next initialize().
  * Needs no GPU (tests of the graph container: tombstones, re-added edges, fixed vertices, vertices without edges). */
@@ -425,7 +447,7 @@ int cuba_debug_dropin_levels(void* dropin, const uint8_t** levels, int32_t* n);
 /* ---- micro-benchmark hooks for bench.py / profiles (device-resident data, CUDA-event timed) ---- */
 /* Runs the named stage `reps` times back to back and returns the average device milliseconds per
  * repetition.  stage: 0 linearize (landmark pass + pose pass), 1 landmark pass only, 2 pose pass only,
- * 3 schur, 4 pcg, 5 backsub+update+residual, 6 residual only.  flush_l2 != 0 writes a >L2 buffer
+ * 3 schur, 4 the reduced-system solve (PCG or dense Cholesky, as chosen), 5 backsub+update+residual, 6 residual only.  flush_l2 != 0 writes a >L2 buffer
  * between repetitions (outside the timed interval). */
 int cuba_bench_stage(cuba_engine* e, int stage, int reps, int flush_l2, double lambda, double* avg_ms);
 
