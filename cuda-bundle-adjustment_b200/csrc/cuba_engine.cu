@@ -328,6 +328,7 @@ struct Engine : EngineBase {
 	Structure S;
 	cudaStream_t stream = nullptr;
 	int numSMs = 0;
+	int smemMax = 0;        // opt-in dynamic shared memory of one CTA
 	int ntiles = 0, nPoseBlocks = 0, nChiBlocks = 0;
 	int tileSize = TILE;    // 256 or 128, from cfg.reserved[2]
 	int jhMinBlocks = 2;
@@ -368,28 +369,35 @@ struct Engine : EngineBase {
 	bool mixed = false;
 	bool upperReduce = false;   // k_schur3 writes the upper blocks into uVal; one all-reduce of uVal | bsc, then k_expand_upper
 	DBuf<int> prodPtr, prodI, prodJ, prodL, blkRow, blkCol, u2f, u2fT, fRowPtr, fColInd;
-	// pcg v2 (cuba_pcg2.cuh)
-	DBuf<T> fHat, Linv, vR0, vR1, vS0, vS1, vW0, vW1, vP, vY;
-	DBuf<int> fLocal, ctaRow, needPtr, needCol;
-	DBuf<double> pcg2Partial;
-	DBuf<GridBar> gridBar;
-	DBuf<long long> pcgTiming;
-	DBuf<unsigned long long> llFlags;   // k_pcg3: [wFlag 2*6numP*2 | pFlag 2*2G*2 | abort word]
-	int pcg2Grid = 0, pcg2Cap = 0, pcg2NeedMax = 0, pcg2MaxRows = 0;
-	// two-level PCG (cuba_pcg4.cuh; its coarse level: cuba_coarse.cuh)
-	CoarseLevel coarse4;
-	DBuf<T> cZx, cZhat;
-	DBuf<double> cPart, cU;
-	DBuf<double> cdT;               // k_coarse_dense: two copies of the lower 32 x 32 tiles of Ac, sized by setup_pcg2 and setup_pcg5 for
-	                                // the larger of their coarse matrices (DBuf only grows)
+	// One block-Jacobi solve set up on the device (setup_pcg3): the row partition's lists, L^-1, the eight vectors, the partial board
+	// and k_pcg3's flags, and the launch shape of k_pcg3 / k_pcg2 (cuba_pcg3.cuh, cuba_pcg2.cuh), the solve every other one falls back to
+	struct Pcg3Run {
+		int G = 0, cap = 0, needMax = 0, maxRows = 0; size_t smem = 0;   // cap: blocks of A^ cached in shared memory
+		bool pcg3 = false;                               // k_pcg3 fits (one (row, component) pair per thread); k_pcg2 otherwise
+		DBuf<int> ctaRow, needPtr, needCol, local;
+		DBuf<T> Linv, R0, R1, S0, S1, W0, W1, P, Y;
+		DBuf<double> partial;
+		DBuf<unsigned long long> flags;                  // k_pcg3: [wFlag 2*6numP*2 | pFlag 2*2G*2 | abort word]
+	};
+	// One k_pcg4 solve set up on the device (setup_pcg4): its coarse level, Z^, partial board and shape; the rest is p3's
+	struct Pcg4Run {
+		bool ok = false; int gs = 1, maxNeedAgg = 0, cap = 0, sliceInSmem = 0, zhInSmem = 0; size_t smem = 0;
+		CoarseLevel coarse;
+		DBuf<T> Zhat; DBuf<double> part;
+	};
+	Pcg3Run p3;
+	Pcg4Run p4;
+	// Scratch the PCG solves share, each DBuf grown to the largest size asked for: A^ (setup_pcg3, setup_pcg5); the coarse basis Zx,
+	// U [36 nfull] and k_coarse_dense's tiles of a coarse rebuild (setup_pcg4, setup_pcg5); the rebuild flags, slot 0 k_pcg4's, slots
+	// 1..P5_INFO_LOG k_pcg5's log (setup_pcg4: one slot; setup_pcg5: all, zeroed); -DCUBA_PCG_TIMING's per-CTA counters (each launch)
+	DBuf<T> fHat, cZx;
+	DBuf<double> cU, cdT;
 	DBuf<int> cInfo;
-	int pcg4Gs = 1, pcg4MaxNeedAgg = 0, pcg4Cap = 0, pcg4SliceInSmem = 0, pcg4ZhInSmem = 0;
-	size_t pcg4Smem = 0;
-	bool pcg4Ok = false, tlActive = false;
+	DBuf<long long> pcgTiming;
+	// the barrier of every cooperative kernel on the stream (k_pcg2/3/4, k_coarse_dense, k_dense_chol, peer all-reduce), zeroed in init()
+	DBuf<GridBar> gridBar;
 	PinnedArena arena;
 	double curLambda = 0;           // damping of the solve being launched
-	bool pcg3Ok = false;
-	size_t pcg2Smem = 0;
 	// reductions
 	DBuf<double> chiPartial, scalePartialL, scalePartialP, chiSq;
 	// edge levels (cuba_levels.cuh); allocated by the first level call, so that a run without levels keeps its footprint
@@ -434,11 +442,13 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaGetDevice(&dev));
 		devOrdinal = dev;
 		CUDA_TRY(cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev));
+		CUDA_TRY(cudaDeviceGetAttribute(&smemMax, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
 		CUDA_TRY(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
 		CUDA_TRY(cudaMallocHost((void**)&hScal, sizeof(Scalars)));
 		memset(hScal, 0, sizeof(Scalars));
 		CUDA_TRY(dScal.alloc(1));
 		CUDA_TRY(cudaMemsetAsync(dScal.p, 0, sizeof(Scalars), stream));
+		CUDA_TRY(gridBar.alloc(1)); CUDA_TRY(cudaMemsetAsync(gridBar.p, 0, sizeof(GridBar), stream));
 		// for every coarse matrix k_coarse_invert takes (launch_coarse_setup), whichever solver it belongs to
 		CUDA_TRY(cudaFuncSetAttribute(k_coarse_invert<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coarse_invert_smem(PCG4_MAXAGG1)));
 		return CUBA_OK;
@@ -900,7 +910,6 @@ struct Engine : EngineBase {
 				bool ok = false;
 				rcx = ipcExchange((void*)uVal.p, uPeer, ok); if (rcx) return rcx;
 				uPeerOk = ok;
-				CUDA_TRY(gridBar.alloc(1));
 			}
 		}
 		CUDA_TRY(xp.alloc(6 * nP)); CUDA_TRY(xl.alloc(3 * nL));
@@ -921,15 +930,17 @@ struct Engine : EngineBase {
 		tmark("jh4 queued");
 		// the solver's setup: no PCG partition or plan for the direct solver (its need lists may not fit, and nothing reads them)
 		denseSolve = linSolver == CUBA_SOLVER_DENSE_CHOLESKY;
+		p3.pcg3 = false; p4.ok = false; p5Ok = false;          // what a structure before this one prepared
 		if (denseSolve) {
-			pcg3Ok = false; pcg4Ok = false; p5Ok = false; p5Dist = false;      // what a PCG structure before this one prepared
 			if (S.numP > 0 && S.numL > 0) { int rc = setup_dense(); if (rc) return rc; }
 			else release_dense();
 		}
 		else {
 			release_dense();                                                   // up to 1 GB of tiles nothing reads any more
-			if (S.numP > 0) { int rc = setup_pcg2(); if (rc) return rc; }        // host-heavy: overlaps the warp-tile kernels queued above
-			if (S.numP > 0 && S.numL > 0) { int rc = setup_pcg5(); if (rc) return rc; }
+			pick = pcg_choice();
+			if (S.numP > 0) { int rc = setup_pcg3(); if (rc) return rc; }        // host-heavy: overlaps the warp-tile kernels queued above
+			if (S.numP > 0 && pick.p4) { int rc = setup_pcg4(hostPP); if (rc) return rc; }
+			if (S.numP > 0 && S.numL > 0 && pick.p5) { int rc = setup_pcg5(); if (rc) return rc; }
 		}
 		tmark("pcg partition (host)");
 		if (jhV4) { int rc = setup_jh4_finish(); if (rc) return rc; }
@@ -1256,7 +1267,7 @@ struct Engine : EngineBase {
 		}
 		return CUBA_OK;
 	}
-	// second half of the warp-tile setup: the host work of setup_pcg2 runs between the two halves, overlapping the kernels above
+	// second half of the warp-tile setup: the host work of the PCG setups runs between the two halves, overlapping the kernels above
 	int setup_jh4_finish()
 	{
 		if (!jh4Pending) return CUBA_OK;
@@ -1323,20 +1334,45 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// Row partition, need lists and shared-memory budget of k_pcg2.
-	int setup_pcg2()
+	// ---- the PCG kernel of a solve -------------------------------------------------------------------------------------------------
+	// The choice of a structure: the runs to prepare besides the block-Jacobi one, k_pcg5 distributed over the ranks or not, and the
+	// steps of a solve before and after the policy turned two-level (tlActive) and of the block-Jacobi retry of a breakdown.  A step
+	// runs k_pcg5 (two-level or block-Jacobi) when it has a plan, else k_pcg4 when it is prepared, else block-Jacobi k_pcg3 -- k_pcg2
+	// beyond k_pcg3's rows per CTA or when asked for (pcg2).
+	// cfg.reserved[0] (pcg_variant): 0 (also 7: never distributed, 8: distributed at any size) automatic -- block-Jacobi (k_pcg5 when
+	// distributed, k_pcg3 otherwise) until the policy turns two-level, then k_pcg5, or k_pcg4 without a k_pcg5 plan; 5: always
+	// two-level k_pcg5; 6: always block-Jacobi k_pcg5; 3: always k_pcg4; 4: always k_pcg3; 2: k_pcg2.  k_pcg4 is prepared where it can
+	// be asked for: explicitly, by the fp32 engine, or as the fallback for systems beyond k_pcg5's 85 rows per CTA.
+	struct PcgStep { bool p5 = false, twoLevel = false, p4 = false; };
+	struct PcgChoice { bool p4 = false, p5 = false, dist = false, pcg2 = false; PcgStep first, later, retry; };
+	PcgChoice pick;                      // of the current structure (alloc_system)
+	PcgChoice pcg_choice() const
+	{
+		const int m = cfg.reserved[0], numP = S.numP;
+		PcgChoice c;
+		c.p4 = m == 3 || sizeof(T) != 8 || numP > 80 * numSMs * (world > 1 && numP >= 2048 ? world : 1);
+		c.p5 = m != 2 && m != 3 && m != 4;
+		c.dist = c.p5 && world > 1 && comm && m != 7 && (m == 8 || numP >= 2048);
+		c.pcg2 = m == 2;
+		if (m == 0 || m == 7 || m == 8) { c.first = c.retry = { c.dist, false, false }; c.later = { true, true, true }; }
+		else if (m == 5) { c.first = c.later = { true, true, false }; c.retry = { true, false, false }; }
+		else if (m == 6) c.first = c.later = c.retry = { true, false, false };
+		else if (m == 3) c.first = c.later = { false, false, true };
+		return c;
+	}
+	// dynamic shared memory of one CTA of k_pcg2 / k_pcg3 / k_pcg4: leave room for the static arrays (4.4 KB in k_pcg3)
+	size_t pcg3_budget() const { return (size_t)smemMax > 8192 ? (size_t)smemMax - 6144 : 0; }
+	// Row partition, need lists and shared-memory budget of the block-Jacobi solve (p3).
+	int setup_pcg3()
 	{
 		const int numP = S.numP;
-		int smemMax = 0;
-		CUDA_TRY(cudaDeviceGetAttribute(&smemMax, cudaDevAttrMaxSharedMemoryPerBlockOptin, devOrdinal));
-		const size_t budget = (size_t)smemMax > 8192 ? (size_t)smemMax - 6144 : 0;   // leave room for the static arrays (4.4 KB in k_pcg3)
+		const size_t budget = pcg3_budget();
 		const size_t matBytes = (size_t)S.nfull * (36 * sizeof(T) + 4);
 		int G = std::max((numP + 7) / 8, (int)((matBytes + budget - 1) / std::max<size_t>(budget, 1)));
 		G = std::max(1, std::min(G, std::min(numSMs, numP)));
 		// row partition, need lists, block-local column positions: cuba_structure.cpp (CPU-tested)
-		PcgPartition& PP = hostPP;                     // kept: k_pcg5's plan starts from the same partition when its CTA count is the same
+		PcgPartition& PP = hostPP;                     // kept: k_pcg4 and k_pcg5's plan start from the same partition
 		build_pcg_partition(numP, S.nfull, S.fRowPtr, S.fColInd, G, PP);
-		const std::vector<int>& rows = PP.rows; const std::vector<int>& nptr = PP.nptr; const std::vector<int>& ncol = PP.ncol; const std::vector<int>& local = PP.local;
 		const int needMax = PP.needMax, blkMax = PP.blkMax, maxRows = PP.maxRows;
 		const size_t needBytes = pcg3_fixed_bytes(needMax, maxRows, sizeof(T));
 		// k_pcg3 / k_pcg2 keep every needed column in shared memory and are the solver of last resort: without them no solve can run
@@ -1347,73 +1383,72 @@ struct Engine : EngineBase {
 				+ std::to_string(needBytes) + " bytes of shared memory, " + std::to_string(budget) + " available: at most " + std::to_string(fit)
 				+ " columns with " + std::to_string(maxRows) + " rows per CTA); the poses are too densely covisible for this engine");
 		}
-		pcg3Ok =maxRows * 6 <= PCG3_BLOCK && 2 * G <= 2 * PCG3_BLOCK;   // k_pcg3: one (row,component) pair per thread, two partial words per thread
+		p3.pcg3 = maxRows * 6 <= PCG3_BLOCK && 2 * G <= 2 * PCG3_BLOCK;   // k_pcg3: one (row,component) pair per thread, two partial words per thread
 		size_t cap = budget > needBytes ? (budget - needBytes) / (36 * sizeof(T) + 4) : 0;
 		cap = std::min<size_t>(cap, (size_t)blkMax);
-		pcg2Grid = G; pcg2Cap = (int)cap; pcg2NeedMax = needMax; pcg2MaxRows = maxRows;
-		pcg2Smem = (size_t)cap * 36 * sizeof(T) + needBytes + (size_t)cap * 4 + 16;
-		CUDA_TRY(cudaFuncSetAttribute(k_pcg2<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcg2Smem));
-		CUDA_TRY(cudaFuncSetAttribute(k_pcg3<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcg2Smem));
-		CUDA_TRY(llFlags.alloc(2 * (2 * 6 * (size_t)numP) + 2 * (2 * PCG3_REPL * 2 * (size_t)G) + 2));
+		p3.G = G; p3.cap = (int)cap; p3.needMax = needMax; p3.maxRows = maxRows;
+		p3.smem = (size_t)cap * 36 * sizeof(T) + needBytes + (size_t)cap * 4 + 16;
+		CUDA_TRY(cudaFuncSetAttribute(k_pcg2<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p3.smem));
+		CUDA_TRY(cudaFuncSetAttribute(k_pcg3<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p3.smem));
+		CUDA_TRY(p3.flags.alloc(2 * (2 * 6 * (size_t)numP) + 2 * (2 * PCG3_REPL * 2 * (size_t)G) + 2));
 		int perSM = 0;
-		CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_pcg2<T>, PCG2_BLOCK, pcg2Smem));
+		CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_pcg2<T>, PCG2_BLOCK, p3.smem));
 		if (perSM < 1) return fail(CUBA_ERR_CUDA, "k_pcg2 cannot be resident with the requested shared memory");
 		arena.reset();
-		CUDA_TRY(ctaRow.upload(rows, stream, &arena)); CUDA_TRY(needPtr.upload(nptr, stream, &arena)); CUDA_TRY(needCol.upload(ncol, stream, &arena));
-		CUDA_TRY(fLocal.upload(local, stream, &arena));
+		CUDA_TRY(p3.ctaRow.upload(PP.rows, stream, &arena)); CUDA_TRY(p3.needPtr.upload(PP.nptr, stream, &arena)); CUDA_TRY(p3.needCol.upload(PP.ncol, stream, &arena));
+		CUDA_TRY(p3.local.upload(PP.local, stream, &arena));
 		const size_t n6 = 6 * (size_t)numP;
-		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull)); CUDA_TRY(Linv.alloc(36 * (size_t)numP));
-		CUDA_TRY(vR0.alloc(n6)); CUDA_TRY(vR1.alloc(n6)); CUDA_TRY(vS0.alloc(n6)); CUDA_TRY(vS1.alloc(n6));
-		CUDA_TRY(vW0.alloc(n6)); CUDA_TRY(vW1.alloc(n6)); CUDA_TRY(vP.alloc(n6)); CUDA_TRY(vY.alloc(n6));
-		CUDA_TRY(pcg2Partial.alloc(4 * (size_t)G));
-		CUDA_TRY(gridBar.alloc(1));
-		CUDA_TRY(cudaMemsetAsync(gridBar.p, 0, sizeof(GridBar), stream));
+		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull)); CUDA_TRY(p3.Linv.alloc(36 * (size_t)numP));
+		CUDA_TRY(p3.R0.alloc(n6)); CUDA_TRY(p3.R1.alloc(n6)); CUDA_TRY(p3.S0.alloc(n6)); CUDA_TRY(p3.S1.alloc(n6));
+		CUDA_TRY(p3.W0.alloc(n6)); CUDA_TRY(p3.W1.alloc(n6)); CUDA_TRY(p3.P.alloc(n6)); CUDA_TRY(p3.Y.alloc(n6));
+		CUDA_TRY(p3.partial.alloc(4 * (size_t)G));
 		tmark("  pcg2 partition + uploads");
-		// ---- two-level PCG of round 1 (k_pcg4): aggregates = groups of gs consecutive CTAs (at most PCG4_MAXAGG of them).
-		//      Only prepared when it can be asked for: explicitly (reserved[0] == 3), by the fp32 engine, or as the fallback for systems
-		//      beyond k_pcg5's 85 rows per CTA; otherwise its host lists and uploads are skipped (k_pcg5 has its own plan) ----
-		pcg4Ok = false;
-		if (cfg.reserved[0] == 3 || sizeof(T) != 8 || numP > 80 * numSMs * (world > 1 && numP >= 2048 ? world : 1)) {
-			// up to 74 aggregates, fewer with cfg.reserved[6] (37 or fewer: the coarse inverse of one CTA, k_coarse_invert)
-			const int maxAgg = (cfg.reserved[6] > 0 && cfg.reserved[6] < PCG4_MAXAGG) ? cfg.reserved[6] : PCG4_MAXAGG;
-			CoarsePartition CP;
-			build_coarse_partition(numP, PP, maxAgg, CP);
-			const int gs = CP.gs, A = CP.A, nc = 6 * A;
-			pcg4Gs = gs; pcg4MaxNeedAgg = CP.maxNeedAgg;
-			size_t fixed4 = (size_t)needMax * (12 * sizeof(T) + 8) + (size_t)maxRows * (6 * sizeof(T) + 8) + 8 + 2 * (size_t)nc * sizeof(T)
-				+ (size_t)pcg4MaxNeedAgg * (6 * sizeof(T) + 4) + 64;
-			// shared-memory priorities: all of A^ first, then Z^ of the needed columns, then the CTA's slices of the inverse coarse matrix
-			const size_t matAll = (size_t)blkMax * (36 * sizeof(T) + 4);
-			const size_t zhBytes = (size_t)needMax * 36 * sizeof(T);
-			const size_t sliceBytes = (((size_t)pcg4MaxNeedAgg * 6 * nc + 1) & ~(size_t)1) * sizeof(float);
-			pcg4ZhInSmem = budget >= fixed4 + matAll + zhBytes ? 1 : 0;
-			if (pcg4ZhInSmem) fixed4 += zhBytes;
-			pcg4SliceInSmem = budget >= fixed4 + matAll + sliceBytes ? 1 : 0;
-			if (pcg4SliceInSmem) fixed4 += sliceBytes;
-			size_t cap4 = budget > fixed4 ? (budget - fixed4) / (36 * sizeof(T) + 4) : 0;
-			cap4 = std::min<size_t>(cap4, (size_t)blkMax);
-			pcg4Cap = (int)cap4;
-			pcg4Smem = (size_t)cap4 * (36 * sizeof(T) + 4) + fixed4;
-			if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg4: G %d A %d gs %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceInSmem %d cap %d smem %zu\n",
-				G, A, gs, needMax, maxRows, blkMax, pcg4MaxNeedAgg, pcg4ZhInSmem, pcg4SliceInSmem, pcg4Cap, pcg4Smem);
-			pcg4Ok = budget > fixed4 && nc + 64 <= PCG4_BLOCK && numP >= 2 * A;
-			if (pcg4Ok) {
-				CUDA_TRY(cudaFuncSetAttribute(k_pcg4<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcg4Smem));
-				int perSM4 = 0;
-				CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM4, k_pcg4<T>, PCG4_BLOCK, pcg4Smem));
-				if (perSM4 < 1) pcg4Ok = false;
-			}
-			if (pcg4Ok) {
-				// fine blocks of every coarse block (lower triangle), ascending -> fixed-order sums in k_coarse_assemble
-				build_coarse_lists(numP, S.nfull, S.fRowPtr, S.fColInd, CP);
-				int rc = coarse4.upload(CP, stream, &arena); if (rc) return rc;
-				CUDA_TRY(cZx.alloc(36 * (size_t)numP)); CUDA_TRY(cZhat.alloc(36 * (size_t)numP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull));
-				if (coarse_kernel(A) == CUBA_COARSE_KERNEL_DENSE) CUDA_TRY(cdT.alloc(cdense::scratch_doubles(A)));
-				CUDA_TRY(cPart.alloc(2 * (size_t)G * PCG4_PSTRIDE)); CUDA_TRY(cInfo.alloc(1));
-				CUDA_TRY(cudaMemsetAsync(cPart.p, 0, sizeof(double) * cPart.n, stream));
-				// (no synchronisation: the uploads above read the pinned arena, or were staged by the driver before returning)
-			}
+		return CUBA_OK;
+	}
+
+	// k_pcg4 (p4) on the block-Jacobi partition PP: aggregates = groups of gs consecutive CTAs (at most PCG4_MAXAGG of them)
+	int setup_pcg4(const PcgPartition& PP)
+	{
+		const int numP = S.numP, G = PP.G, needMax = PP.needMax, blkMax = PP.blkMax, maxRows = PP.maxRows;
+		const size_t budget = pcg3_budget();
+		// up to 74 aggregates, fewer with cfg.reserved[6] (37 or fewer: the coarse inverse of one CTA, k_coarse_invert)
+		const int maxAgg = (cfg.reserved[6] > 0 && cfg.reserved[6] < PCG4_MAXAGG) ? cfg.reserved[6] : PCG4_MAXAGG;
+		CoarsePartition CP;
+		build_coarse_partition(numP, PP, maxAgg, CP);
+		const int gs = CP.gs, A = CP.A, nc = 6 * A;
+		p4.gs = gs; p4.maxNeedAgg = CP.maxNeedAgg;
+		size_t fixed4 = (size_t)needMax * (12 * sizeof(T) + 8) + (size_t)maxRows * (6 * sizeof(T) + 8) + 8 + 2 * (size_t)nc * sizeof(T)
+			+ (size_t)p4.maxNeedAgg * (6 * sizeof(T) + 4) + 64;
+		// shared-memory priorities: all of A^ first, then Z^ of the needed columns, then the CTA's slices of the inverse coarse matrix
+		const size_t matAll = (size_t)blkMax * (36 * sizeof(T) + 4);
+		const size_t zhBytes = (size_t)needMax * 36 * sizeof(T);
+		const size_t sliceBytes = (((size_t)p4.maxNeedAgg * 6 * nc + 1) & ~(size_t)1) * sizeof(float);
+		p4.zhInSmem = budget >= fixed4 + matAll + zhBytes ? 1 : 0;
+		if (p4.zhInSmem) fixed4 += zhBytes;
+		p4.sliceInSmem = budget >= fixed4 + matAll + sliceBytes ? 1 : 0;
+		if (p4.sliceInSmem) fixed4 += sliceBytes;
+		size_t cap4 = budget > fixed4 ? (budget - fixed4) / (36 * sizeof(T) + 4) : 0;
+		cap4 = std::min<size_t>(cap4, (size_t)blkMax);
+		p4.cap = (int)cap4;
+		p4.smem = (size_t)cap4 * (36 * sizeof(T) + 4) + fixed4;
+		if (getenv("CUBA_PCG_VERBOSE")) fprintf(stderr, "pcg4: G %d A %d gs %d needMax %d maxRows %d blkMax %d maxNeedAgg %d zhInSmem %d sliceInSmem %d cap %d smem %zu\n",
+			G, A, gs, needMax, maxRows, blkMax, p4.maxNeedAgg, p4.zhInSmem, p4.sliceInSmem, p4.cap, p4.smem);
+		p4.ok = budget > fixed4 && nc + 64 <= PCG4_BLOCK && numP >= 2 * A;
+		if (p4.ok) {
+			CUDA_TRY(cudaFuncSetAttribute(k_pcg4<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p4.smem));
+			int perSM4 = 0;
+			CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM4, k_pcg4<T>, PCG4_BLOCK, p4.smem));
+			if (perSM4 < 1) p4.ok = false;
 		}
+		if (!p4.ok) return CUBA_OK;
+		// fine blocks of every coarse block (lower triangle), ascending -> fixed-order sums in k_coarse_assemble
+		build_coarse_lists(numP, S.nfull, S.fRowPtr, S.fColInd, CP);
+		int rc = p4.coarse.upload(CP, stream, &arena); if (rc) return rc;
+		CUDA_TRY(cZx.alloc(36 * (size_t)numP)); CUDA_TRY(p4.Zhat.alloc(36 * (size_t)numP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull));
+		if (coarse_kernel(A) == CUBA_COARSE_KERNEL_DENSE) CUDA_TRY(cdT.alloc(cdense::scratch_doubles(A)));
+		CUDA_TRY(p4.part.alloc(2 * (size_t)G * PCG4_PSTRIDE)); CUDA_TRY(cInfo.alloc(1));
+		CUDA_TRY(cudaMemsetAsync(p4.part.p, 0, sizeof(double) * p4.part.n, stream));
+		// (no synchronisation: the uploads above read the pinned arena, or were staged by the driver before returning)
 		return CUBA_OK;
 	}
 
@@ -1421,26 +1456,26 @@ struct Engine : EngineBase {
 	int launch_pcg4()
 	{
 		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
-		const int numP = S.numP;
-		KLAUNCH(k_coarse_basis<T>, numP, pose[cur].p, numP, cZx.p);
-		int rc = coarse_refresh(coarse4, coarse_scratch(), cInfo.p); if (rc) return rc;     // slot 0 of cInfo
+		KLAUNCH(k_coarse_basis<T>, S.numP, pose[cur].p, S.numP, cZx.p);
+		const CoarseLevel& L = p4.coarse;
+		int rc = coarse_refresh(p4.coarse, coarse_scratch(), cInfo.p); if (rc) return rc;     // slot 0 of cInfo
 		Pcg4Args<T> b;
-		b.base = pcg2_args(pcg4Cap);
-		b.Zx = cZx; b.Zhat = cZhat; b.AcInv = coarse4.AcInv; b.aggRow = coarse4.aggRow; b.naPtr = coarse4.naPtr; b.naList = coarse4.naList;
-		b.needAgg = coarse4.needAgg; b.A = coarse4.A; b.gs = pcg4Gs; b.maxNeedAgg = pcg4MaxNeedAgg; b.sliceInSmem = pcg4SliceInSmem; b.zhInSmem = pcg4ZhInSmem; b.cpart = cPart;
+		b.base = pcg2_args(p3, p4.cap);
+		b.Zx = cZx; b.Zhat = p4.Zhat; b.AcInv = L.AcInv; b.aggRow = L.aggRow; b.naPtr = L.naPtr; b.naList = L.naList;
+		b.needAgg = L.needAgg; b.A = L.A; b.gs = p4.gs; b.maxNeedAgg = p4.maxNeedAgg; b.sliceInSmem = p4.sliceInSmem; b.zhInSmem = p4.zhInSmem; b.cpart = p4.part;
 		b.timing = nullptr;
 #ifdef CUBA_PCG_TIMING
-		CUDA_TRY(pcgTiming.alloc(8 * (size_t)pcg2Grid));
+		CUDA_TRY(pcgTiming.alloc(8 * (size_t)p3.G));
 		b.timing = pcgTiming.p;
 #endif
 		void* args[] = { (void*)&b };
-		CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg4<T>, dim3(pcg2Grid), dim3(PCG4_BLOCK), args, pcg4Smem, stream));
+		CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg4<T>, dim3(p3.G), dim3(PCG4_BLOCK), args, p4.smem, stream));
 		launches++;
 		lastPcgTwoLevel = true;
 		lastPcgKernel = CUBA_PCG_KERNEL_PCG4;
 		return CUBA_OK;
 	}
-	bool lastPcgTwoLevel = false;
+	bool lastPcgTwoLevel = false, tlActive = false;   // tlActive: the default solver's policy turned two-level (note_pcg_iters)
 	bool forceBlockJacobi = false;   // retry of a trial whose two-level solve broke down
 	// policy of the default solver: block-Jacobi (k_pcg3, the cheaper iteration) while it converges quickly, two-level (k_pcg4,
 	// a dearer iteration but 2-8x fewer of them) once a block-Jacobi solve needed more than 100 iterations -- the count grows
@@ -1455,48 +1490,39 @@ struct Engine : EngineBase {
 		return tol * tol;
 	}
 
-	// the arguments of k_pcg2 / k_pcg3, and the block-Jacobi part of k_pcg4's, with capBlocks blocks of A^ in shared memory
-	Pcg2Args<T> pcg2_args(int capBlocks)
+	// the arguments of k_pcg2 / k_pcg3, and the block-Jacobi part of k_pcg4's, on R with capBlocks blocks of A^ in shared memory
+	Pcg2Args<T> pcg2_args(const Pcg3Run& R, int capBlocks)
 	{
 		Pcg2Args<T> a;
-		a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = fLocal; a.fVal = fVal; a.fHat = fHat;
-		a.ctaRow = ctaRow; a.needPtr = needPtr; a.needCol = needCol; a.b = bsc; a.numP = S.numP; a.Linv = Linv;
-		a.R0 = vR0; a.R1 = vR1; a.S0 = vS0; a.S1 = vS1; a.W0 = vW0; a.W1 = vW1; a.P = vP; a.Y = vY; a.x = xp;
-		a.partial = pcg2Partial; a.bar = gridBar; a.capBlocks = capBlocks; a.needMax = pcg2NeedMax; a.maxRows = pcg2MaxRows;
+		a.fRowPtr = fRowPtr; a.fColInd = fColInd; a.fLocal = R.local; a.fVal = fVal; a.fHat = fHat;
+		a.ctaRow = R.ctaRow; a.needPtr = R.needPtr; a.needCol = R.needCol; a.b = bsc; a.numP = S.numP; a.Linv = R.Linv;
+		a.R0 = R.R0; a.R1 = R.R1; a.S0 = R.S0; a.S1 = R.S1; a.W0 = R.W0; a.W1 = R.W1; a.P = R.P; a.Y = R.Y; a.x = xp;
+		a.partial = R.partial; a.bar = gridBar; a.capBlocks = capBlocks; a.needMax = R.needMax; a.maxRows = R.maxRows;
 		a.maxIters = pcg_max_iters(); a.tol2 = pcg_tol2();
 		a.status = &dScal.p->pcg;
 		return a;
 	}
 
-	int launch_pcg2(bool flagged)
+	// the block-Jacobi solve on p3: k_pcg3 (flag-synchronised exchange) or k_pcg2 (one grid barrier per iteration)
+	int launch_pcg3()
 	{
 		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
-		const Pcg2Args<T> a = pcg2_args(pcg2Cap);
-		if (flagged) {
-			Pcg3Args<T> b;
-			b.base = a;
-			b.wFlag = llFlags.p;
-			b.pFlag = llFlags.p + 2 * (2 * 6 * (size_t)S.numP);
-			b.abortFlag = (int*)(b.pFlag + 2 * (2 * PCG3_REPL * 2 * (size_t)pcg2Grid));
-			b.timing = nullptr;
+		const bool flagged = p3.pcg3 && !pick.pcg2;
+		Pcg3Args<T> b{};
+		b.base = pcg2_args(p3, p3.cap);
+		b.wFlag = p3.flags.p;
+		b.pFlag = p3.flags.p + 2 * (2 * 6 * (size_t)S.numP);
+		b.abortFlag = (int*)(b.pFlag + 2 * (2 * PCG3_REPL * 2 * (size_t)p3.G));
 #ifdef CUBA_PCG_TIMING
-			CUDA_TRY(pcgTiming.alloc(8 * (size_t)pcg2Grid));
-			b.timing = pcgTiming.p;
+		if (flagged) { CUDA_TRY(pcgTiming.alloc(8 * (size_t)p3.G)); b.timing = pcgTiming.p; }
 #endif
-			CUDA_TRY(cudaMemsetAsync(llFlags.p, 0, sizeof(unsigned long long) * llFlags.n, stream));
-			void* args3[] = { (void*)&b };
-			CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg3<T>, dim3(pcg2Grid), dim3(PCG3_BLOCK), args3, pcg2Smem, stream));
-			launches++;
-			lastPcgKernel = CUBA_PCG_KERNEL_PCG3;
-			return CUBA_OK;
-		}
-		void* args[] = { (void*)&a };
-		CUDA_TRY(cudaLaunchCooperativeKernel((void*)k_pcg2<T>, dim3(pcg2Grid), dim3(PCG2_BLOCK), args, pcg2Smem, stream));
+		if (flagged) CUDA_TRY(cudaMemsetAsync(p3.flags.p, 0, sizeof(unsigned long long) * p3.flags.n, stream));
+		void* args[] = { flagged ? (void*)&b : (void*)&b.base };
+		CUDA_TRY(cudaLaunchCooperativeKernel(flagged ? (void*)k_pcg3<T> : (void*)k_pcg2<T>, dim3(p3.G), dim3(flagged ? PCG3_BLOCK : PCG2_BLOCK), args, p3.smem, stream));
 		launches++;
-		lastPcgKernel = CUBA_PCG_KERNEL_PCG2;
+		lastPcgKernel = flagged ? CUBA_PCG_KERNEL_PCG3 : CUBA_PCG_KERNEL_PCG2;
 		return CUBA_OK;
 	}
-
 
 	// ---- k_pcg5: two-level, flag-synchronised, rows distributed over the ranks (cuba_pcg5.cuh) --------------------------
 	// A launch shape of a k_pcg5 plan: k_pcg5 (256 threads, BIG or not: pcg5_legacy_shape) or the tuned one-GPU k_pcg5t
@@ -1534,8 +1560,8 @@ struct Engine : EngineBase {
 	DBuf<unsigned long long> p5Boards;
 	P5Boards p5Layout;                             // the layout p5Boards was cleared for
 	PeerMap p5Peer;                                // the peers' boards
-	PcgPartition hostPP;                           // host copy of k_pcg3's row partition of the current system (setup_pcg2)
-	bool p5Ok = false, p5Dist = false;
+	PcgPartition hostPP;                           // host copy of k_pcg3's row partition of the current system (setup_pcg3)
+	bool p5Ok = false;
 	// read by cuba_debug_get_pcg_info only: the kernel of the last solve (CUBA_PCG_KERNEL_*), counters since set_problem, and a
 	// log of the cInfo flag of every k_pcg5 coarse rebuild -- rebuild n writes slot 1 + n % P5_INFO_LOG of cInfo (k_pcg4 keeps
 	// slot 0), so no rebuild's outcome is overwritten by the next one and nothing is copied on the solve's path
@@ -1617,8 +1643,6 @@ struct Engine : EngineBase {
 	int pcg5_legacy_shape(const Pcg5Plan& plan, Pcg5Dims d, int W, bool ranks, P5Shape& sh)
 	{
 		sh = P5Shape{};
-		int smemMax = 0;
-		CUDA_TRY(cudaDeviceGetAttribute(&smemMax, cudaDevAttrMaxSharedMemoryPerBlockOptin, devOrdinal));
 		const size_t budget = (size_t)smemMax > 4096 ? (size_t)smemMax - 2048 : 0;   // static arrays of k_pcg5: < 1 KB
 		const PcgPartition& PP = plan.P;
 		const size_t per = 36 * sizeof(T) + 4;
@@ -1652,15 +1676,7 @@ struct Engine : EngineBase {
 	// Partition of the rows over world x G virtual CTAs, aggregates aligned with the ranks, shared-memory budget, boards.
 	int setup_pcg5()
 	{
-		p5Ok = false; p5Dist = false;
-		const int numP = S.numP;
-		if (numP < 1) return CUBA_OK;
-		const int mode = cfg.reserved[0];
-		if (mode == 2 || mode == 3 || mode == 4) return CUBA_OK;          // an older kernel was asked for explicitly
-		const bool wantDist = world > 1 && comm && mode != 7 && (mode == 8 || numP >= 2048);
-		const int W = wantDist ? world : 1;
-		int smemMax = 0;
-		CUDA_TRY(cudaDeviceGetAttribute(&smemMax, cudaDevAttrMaxSharedMemoryPerBlockOptin, devOrdinal));
+		const int numP = S.numP, W = pick.dist ? world : 1;
 		const size_t budget = (size_t)smemMax > 4096 ? (size_t)smemMax - 2048 : 0;   // static arrays of k_pcg5: < 1 KB
 		// rows over world x G virtual CTAs (about eight rows each, never more than 42: one thread per (row, component) pair in the
 		// row sums), rank-aligned aggregates, halo masks: cuba_structure.cpp (CPU-tested through cuba_debug_pcg5_plan)
@@ -1706,10 +1722,7 @@ struct Engine : EngineBase {
 		CUDA_TRY(cZx.alloc(36 * (size_t)numP)); CUDA_TRY(cU.alloc(36 * (size_t)S.nfull)); CUDA_TRY(cInfo.alloc(1 + P5_INFO_LOG));
 		CUDA_TRY(cudaMemsetAsync(cInfo.p, 0, sizeof(int) * cInfo.n, stream));
 		CUDA_TRY(fHat.alloc(36 * (size_t)S.nfull));
-		if (coarse_kernel(plan.A) == CUBA_COARSE_KERNEL_DENSE) {
-			CUDA_TRY(cdT.alloc(cdense::scratch_doubles(plan.A)));
-			CUDA_TRY(gridBar.alloc(1));
-		}
+		if (coarse_kernel(plan.A) == CUBA_COARSE_KERNEL_DENSE) CUDA_TRY(cdT.alloc(cdense::scratch_doubles(plan.A)));
 		const P5Boards b = p5.boards();
 		const bool fresh = !p5Boards.p || b.words > p5Boards.cap || b.w != p5Layout.w || b.p != p5Layout.p || b.r != p5Layout.r || b.c != p5Layout.c;
 		if (fresh) {
@@ -1727,7 +1740,6 @@ struct Engine : EngineBase {
 				if (rank == 0) fprintf(stderr, "cuba_b200: cudaIpc mapping of the peers' PCG boards failed; keeping the replicated PCG\n");
 				return CUBA_OK;
 			}
-			p5Dist = true;
 		} else p5Peer.base[rank] = (void*)p5Boards.p;
 		p5Ok = true;
 		return CUBA_OK;
@@ -1804,7 +1816,7 @@ struct Engine : EngineBase {
 	}
 
 	// nothing an earlier solve left behind is reused: block-Jacobi first, both coarse inverses rebuilt at their next two-level solve
-	void forget_solves() { tlActive = false; coarse4.forget(); p5.coarse.forget(); }
+	void forget_solves() { tlActive = false; p4.coarse.forget(); p5.coarse.forget(); }
 
 	// The preparation of a solve of R on the current system: k_pcg5_prep_rows for each of the n control blocks ctl[] (the rows of
 	// Linv, R0, Z^ and rc0 are the same on every rank: computed once, each rank's breakdown counter counted in its own control
@@ -1863,9 +1875,9 @@ struct Engine : EngineBase {
 		// tags are 32 bits: long before the device tag base can wrap, every rank (same arithmetic everywhere) clears its boards
 		p5TagBound += (long long)maxIters + 8;
 		if (p5TagBound > (1LL << 31)) {
-			if (p5Dist) { int rc0 = allreduce(&dScal.p->v[7], 1, false); if (rc0) return rc0; }   // nobody still writes into a peer's boards
+			if (pick.dist) { int rc0 = allreduce(&dScal.p->v[7], 1, false); if (rc0) return rc0; }   // nobody still writes into a peer's boards
 			CUDA_TRY(cudaMemsetAsync(p5Boards.p, 0, sizeof(unsigned long long) * p5Boards.cap, stream));
-			if (p5Dist) { int rc0 = allreduce(&dScal.p->v[7], 1, false); if (rc0) return rc0; }
+			if (pick.dist) { int rc0 = allreduce(&dScal.p->v[7], 1, false); if (rc0) return rc0; }
 			p5TagBound = (long long)maxIters + 8;
 		}
 		Pcg5Ctl* ctl = p5.ctl(p5Boards.p);
@@ -1873,12 +1885,12 @@ struct Engine : EngineBase {
 #ifdef CUBA_PCG_TIMING
 		CUDA_TRY(pcgTiming.alloc(8 * (size_t)p5.G));
 #endif
-		if (p5Dist) CUDA_TRY(cudaMemsetAsync(xp.p, 0, sizeof(T) * 6 * (size_t)S.numP, stream));     // rows of the other ranks: summed in below
+		if (pick.dist) CUDA_TRY(cudaMemsetAsync(xp.p, 0, sizeof(T) * 6 * (size_t)S.numP, stream));     // rows of the other ranks: summed in below
 		// a replicated solve (p5.W == 1, also on a multi-rank engine) is rank 0 of one, on this rank's own boards
 		unsigned long long* bases[PCG5_MAXWORLD];
-		for (int r = 0; r < p5.W; r++) bases[r] = (unsigned long long*)p5Peer.base[p5Dist ? r : rank];
+		for (int r = 0; r < p5.W; r++) bases[r] = (unsigned long long*)p5Peer.base[pick.dist ? r : rank];
 		auto launch = [&](auto& a) {
-			pcg5_args(a, p5, twoLevel, p5Dist ? rank : 0, p5.W, bases, fHat.p, xp.p, &dScal.p->pcg);
+			pcg5_args(a, p5, twoLevel, pick.dist ? rank : 0, p5.W, bases, fHat.p, xp.p, &dScal.p->pcg);
 #ifdef CUBA_PCG_TIMING
 			a.timing = pcgTiming.p;
 #endif
@@ -1891,7 +1903,7 @@ struct Engine : EngineBase {
 		k_pcg5_commit<<<1, 1, 0, stream>>>(ctl);
 		launches += 2;
 		CUDA_TRY(cudaGetLastError());
-		if (p5Dist) { rc = allreduce(xp.p, 6 * (size_t)S.numP, true); if (rc) return rc; }
+		if (pick.dist) { rc = allreduce(xp.p, 6 * (size_t)S.numP, true); if (rc) return rc; }
 		lastPcgTwoLevel = twoLevel;
 		lastPcgKernel = p5.sh.tuned ? CUBA_PCG_KERNEL_PCG5T : p5.sh.big ? CUBA_PCG_KERNEL_PCG5_BIG : CUBA_PCG_KERNEL_PCG5;
 		return CUBA_OK;
@@ -1901,7 +1913,6 @@ struct Engine : EngineBase {
 	bool denseSolve = false;        // the structure was built for the direct solver (set_problem, from linSolver)
 	DBuf<int> dcMap;                // packed lower block triangle -> block of the full BSR (build_dense_block_map)
 	DBuf<double> dcTiles, dcY;
-	DBuf<GridBar> dcBar;
 	// CTAs of k_dense_chol for an n x n system: enough for the widest phase (the first trailing update), at most one per SM
 	int dense_grid(int n) const
 	{
@@ -1916,8 +1927,6 @@ struct Engine : EngineBase {
 		build_dense_block_map(S.numP, S.fRowPtr, S.fColInd, map);
 		CUDA_TRY(dcMap.upload(map, stream));
 		CUDA_TRY(dcTiles.alloc(dchol::tile_doubles(n))); CUDA_TRY(dcY.alloc(dchol::rhs_doubles(n)));
-		CUDA_TRY(dcBar.alloc(1));
-		CUDA_TRY(cudaMemsetAsync(dcBar.p, 0, sizeof(GridBar), stream));
 		return CUBA_OK;
 	}
 	template <typename U>
@@ -1936,7 +1945,7 @@ struct Engine : EngineBase {
 		ProfScope ps(this, CUBA_PROF_DECOMP_NUMERICAL);
 		dchol::Args<T> a;
 		a.fVal = fVal; a.blkMap = dcMap; a.dense = nullptr; a.b = bsc; a.n = 6 * S.numP;
-		a.tl = dcTiles; a.y = dcY; a.x = xp; a.status = &dScal.p->pcg; a.info = nullptr; a.bar = dcBar;
+		a.tl = dcTiles; a.y = dcY; a.x = xp; a.status = &dScal.p->pcg; a.info = nullptr; a.bar = gridBar;
 		const int rc = launch_dense_chol(a); if (rc) return rc;
 		lastPcgTwoLevel = false;
 		lastPcgKernel = CUBA_PCG_KERNEL_DENSE;
@@ -1949,19 +1958,10 @@ struct Engine : EngineBase {
 	int launch_pcg()
 	{
 		lastPcgTwoLevel = false;
-		// 0 (also 7, 8): automatic = block-Jacobi while a solve converges quickly, two-level afterwards -- k_pcg5 for the two-level solves
-		// (and, when the rows are distributed over the ranks, for every solve), k_pcg3 for the quick block-Jacobi ones on one GPU;
-		// 5: always two-level k_pcg5; 6: always block-Jacobi k_pcg5; 3: always k_pcg4; 4: always k_pcg3; 2: k_pcg2.
-		// Whatever was asked for, a solve the chosen kernel cannot take (no k_pcg5 plan, no k_pcg4 partition) is block-Jacobi
-		// k_pcg3 -- k_pcg2 beyond k_pcg3's rows per CTA.
-		const int m = cfg.reserved[0];
-		const bool automatic = m == 0 || m == 7 || m == 8;
-		const bool two = tlActive && !forceBlockJacobi;
-		if (p5Ok && (m == 5 || m == 6)) return launch_pcg5(m == 5 && !forceBlockJacobi);
-		if (p5Ok && automatic && (p5Dist || two)) return launch_pcg5(two);
-		if (pcg4Ok && ((automatic && two) || (m == 3 && !forceBlockJacobi))) return launch_pcg4();
-		if (m == 2) return launch_pcg2(false);   // k_pcg2: one grid barrier per iteration
-		return launch_pcg2(pcg3Ok);              // k_pcg3: flag-synchronised exchange
+		const PcgStep& s = forceBlockJacobi ? pick.retry : tlActive ? pick.later : pick.first;
+		if (s.p5 && p5Ok) return launch_pcg5(s.twoLevel);
+		if (s.p4 && p4.ok) return launch_pcg4();
+		return launch_pcg3();
 	}
 
 	int launch_backsub(T lambda)
@@ -2097,7 +2097,7 @@ struct Engine : EngineBase {
 					const double loose = sizeof(T) == 8 ? 1e-6 : 1e-3;
 					ok = ps.status == 0 || (ps.status == 1 && ps.rz0 > 0 && ps.rz <= loose * loose * ps.rz0);
 					if (ps.status == 2 && lastPcgTwoLevel && attempt == 0) {
-						forceBlockJacobi = true; coarse4.valid = false; p5.coarse.valid = false; bjRetries++;
+						forceBlockJacobi = true; p4.coarse.valid = false; p5.coarse.valid = false; bjRetries++;
 						rc = stage_commit(0); if (rc) return rc;
 						continue;
 					}
@@ -2525,10 +2525,10 @@ struct Engine : EngineBase {
 
 	int dbg_pcg_timing(long long* out, int maxCtas) override
 	{
-		const int n = std::min(maxCtas, pcg2Grid);
+		const int n = std::min(maxCtas, (int)(pcgTiming.n / 8));     // the last launch sized pcgTiming for its grid
 		if (!pcgTiming.p || n <= 0) return 0;
-		cudaMemcpyAsync(out, pcgTiming.p, sizeof(long long) * 8 * (size_t)n, cudaMemcpyDeviceToHost, stream);
-		cudaStreamSynchronize(stream);
+		CUDA_TRY(cudaMemcpyAsync(out, pcgTiming.p, sizeof(long long) * 8 * (size_t)n, cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaStreamSynchronize(stream));
 		return n;
 	}
 
@@ -2548,7 +2548,7 @@ struct Engine : EngineBase {
 			last = log[(int)((p5.coarse.rebuilds - 1) % P5_INFO_LOG)];
 		}
 		int coarseKernel = CUBA_COARSE_KERNEL_NONE;
-		if (lastPcgTwoLevel && lastPcgKernel == CUBA_PCG_KERNEL_PCG4) coarseKernel = coarse_kernel(coarse4.A);
+		if (lastPcgTwoLevel && lastPcgKernel == CUBA_PCG_KERNEL_PCG4) coarseKernel = coarse_kernel(p4.coarse.A);
 		else if (lastPcgTwoLevel && p5Ok) coarseKernel = coarse_kernel(p5.coarse.A);
 		const P5Shape& sh = p5.sh;
 		const bool tuned = p5Ok && sh.tuned;
@@ -3002,7 +3002,7 @@ int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const c
 }
 
 int cuba_engine_get_profile(cuba_engine* e, double* sec) { ENGINE_OR_FAIL(e); if (!sec) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_profile(sec); }
-// debug: per-CTA phase timings of the last k_pcg3 launch (library built with -DCUBA_PCG_TIMING); returns the CTA count
+// debug: per-CTA phase timings of the last PCG launch (library built with -DCUBA_PCG_TIMING); returns the CTA count
 int cuba_debug_get_pcg_timing(cuba_engine* e, long long* out, int maxCtas)
 {
 	if (!e || !e->impl) return -1;

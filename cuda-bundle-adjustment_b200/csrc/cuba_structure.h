@@ -69,7 +69,8 @@ bool build_structure(int Pall, int numP, int Lall, int numL, int E2, const int32
 	int rank, int world, int tileEdges, Structure& S, const char** err);
 
 // ---- host side of the PCG setup (pure C++, tested on the CPU through cuba_debug_pcg_partition) --------------------
-// (Engine::setup_pcg2 in cuba_engine.cu calls these functions: one implementation for the engine and for the CPU tests.)
+// (Engine::setup_pcg3, setup_pcg4 and setup_pcg5 in cuba_engine.cu call these functions: one implementation for the engine and for
+// the CPU tests.)
 // Row partition of the reduced pose system over G persistent CTAs: contiguous row ranges balanced by block count, the sorted
 // list of block columns every CTA needs, and the position of each block's column in that list (diagonal blocks: -1-pos).
 struct PcgPartition {

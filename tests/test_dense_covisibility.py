@@ -25,7 +25,7 @@ sla = pytest.importorskip("scipy.linalg")
 DENSE = ("orbit_600", "covis_1000", "covis_2000", "local_ba")
 H100_SMS = 132
 H100_SMEM_OPTIN = 232448                      # cudaDevAttrMaxSharedMemoryPerBlockOptin of an H100
-PCG3_BUDGET = H100_SMEM_OPTIN - 6144          # setup_pcg2's budget: the opt-in limit less k_pcg3's static arrays
+PCG3_BUDGET = H100_SMEM_OPTIN - 6144          # Engine::pcg3_budget: the opt-in limit less k_pcg3's static arrays
 STAGE_TOL = 1e-11
 TOL = 1e-10
 
