@@ -7,6 +7,8 @@ import os
 
 import numpy as np
 
+from . import graphio
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROBUST_NONE, ROBUST_HUBER, ROBUST_TUKEY = 0, 1, 2
 EDGE_MONOCULAR, EDGE_STEREO = 0, 1
@@ -29,6 +31,28 @@ PCG5_PLAN_FIELDS = ("ok", "G", "gs", "A", "needMax", "maxRows", "maxNeedAgg", "h
 
 class CubaError(RuntimeError):
     pass
+
+
+# the status word of the device-resident batches (include/cuba_b200.h: CUBA_BATCH_*): a bit per failed check
+BATCH_STATUS = {1: "ptr does not start at 0", 2: "ptr decreases", 4: "ptr does not end at the item count",
+                8: "non-finite omega or pair value", 16: "non-finite S12 or intrinsics", 32: "s <= 0"}
+
+
+ITER_STAT_DTYPE = np.dtype([("iteration", "<i4"), ("trials", "<i4"), ("chi2", "<f8"), ("lambda_", "<f8"), ("pcg_iters", "<i4"),
+                            ("pcg_failed", "<i4")])
+
+
+def stats_view(stats):
+    """the stats tensor of optimize_poses_device / optimize_sim3_device ([B, S, 4] float64 words) as the structured [B, S] array
+    the _flat methods return; copies to the host, so it waits for the call"""
+    a = np.ascontiguousarray(stats.cpu().numpy())
+    return a.view(ITER_STAT_DTYPE).reshape(a.shape[:2])
+
+
+def batch_status_message(status):
+    """the checks a status word of optimize_poses_device / optimize_sim3_device reports as failed, as text ("ok" for 0)"""
+    status = int(status)
+    return "; ".join(m for bit, m in BATCH_STATUS.items() if status & bit) or ("ok" if status == 0 else "unknown status %d" % status)
 
 
 def library_path():
@@ -118,8 +142,8 @@ _lib = None
 
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
-    "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_linear_solver", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_flush_l2",
-    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_engine_get_profile",
+    "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_linear_solver", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_get_device", "cuba_engine_flush_l2",
+    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_pose_batch_workspace_bytes", "cuba_engine_optimize_poses_device", "cuba_sim3_batch_workspace_bytes", "cuba_engine_optimize_sim3_device", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
     "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_dense_solve", "cuba_debug_peer_allreduce", "cuba_debug_pcg5_ranks", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dense_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
@@ -155,6 +179,7 @@ def load_library():
         "cuba_engine_get_sizes": [vp, C.POINTER(_Sizes)],
         "cuba_engine_reset_state": [vp],
         "cuba_engine_get_stream": [vp, C.POINTER(vp)],
+        "cuba_engine_get_device": [vp, C.POINTER(i)],
         "cuba_engine_flush_l2": [vp],
         "cuba_engine_optimize": [vp, i, vp, C.POINTER(i)],
         "cuba_engine_get_state": [vp, vp, vp, vp],
@@ -164,6 +189,9 @@ def load_library():
         "cuba_engine_classify_edges": [vp, d, d, i, vp],
         "cuba_engine_optimize_poses": [vp, C.POINTER(_PoseBatch), i, vp, vp, vp, vp, vp, vp, vp],
         "cuba_engine_optimize_sim3": [vp, C.POINTER(_Sim3Batch), C.POINTER(_Sim3Params), vp, vp, vp, vp, vp, vp, vp],
+        "cuba_engine_optimize_poses_device": [vp, C.POINTER(_PoseBatch), i, vp, vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp, vp],
+        "cuba_engine_optimize_sim3_device": [vp, C.POINTER(_Sim3Batch), C.POINTER(_Sim3Params), vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp,
+                                             vp, vp],
         "cuba_engine_get_profile": [vp, vp],
         "cuba_engine_get_launch_count": [vp, C.POINTER(C.c_longlong)],
         "cuba_get_transfer_bytes": [C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)],
@@ -198,6 +226,10 @@ def load_library():
         fn = getattr(L, name)
         fn.argtypes = args
         fn.restype = C.c_int
+    L.cuba_pose_batch_workspace_bytes.argtypes = [i, i, i, i, vp, i]
+    L.cuba_pose_batch_workspace_bytes.restype = C.c_size_t
+    L.cuba_sim3_batch_workspace_bytes.argtypes = [i, i, C.POINTER(_Sim3Params), i]
+    L.cuba_sim3_batch_workspace_bytes.restype = C.c_size_t
     _lib = L
     return L
 
@@ -348,6 +380,9 @@ class Engine:
         h = C.c_void_p()
         _check(self.L.cuba_engine_create(C.byref(cfg), C.byref(h)))
         self.h = h
+        d = C.c_int(-1)
+        _check(self.L.cuba_engine_get_device(h, C.byref(d)))
+        self._device = d.value          # the device the engine runs on, device=-1 resolved
         self.sizes = None
         self._stats = []
 
@@ -506,11 +541,9 @@ class Engine:
         graphio.PoseFrame objects.  Returns, per frame, a dict of q [4], t [3], levels (the frame's mono edges then its stereo edges),
         counts [R,4] (included mono, included stereo, newly excluded, re-included after each round) and stats (per round, the
         iteration statistics as optimize() returns them)."""
-        n2 = np.array([len(f.omega2) for f in frames], np.int64); n3 = np.array([len(f.omega3) for f in frames], np.int64)
-        ptr2 = np.concatenate([[0], np.cumsum(n2)]); ptr3 = np.concatenate([[0], np.cumsum(n3)])
-        cat = lambda name, w: np.concatenate([np.asarray(getattr(f, name), np.float64).reshape(-1, w) for f in frames]) if frames else np.zeros((0, w))
-        r = self.optimize_poses_flat(cat("q", 4), cat("t", 3), cat("cam", 5), ptr2, cat("X2", 3), cat("meas2", 2), cat("omega2", 1).ravel(),
-                                     ptr3, cat("X3", 3), cat("meas3", 3), cat("omega3", 1).ravel(), rounds)
+        a = graphio.pose_batch_arrays(frames)
+        ptr2, ptr3 = a["ptr2"], a["ptr3"]
+        r = self.optimize_poses_flat(rounds=rounds, **a)
         off = np.concatenate([[0], np.cumsum([int(x.iterations) for x in rounds])])
         E2 = int(ptr2[-1])
         res = []
@@ -557,12 +590,9 @@ class Engine:
         problem, a dict of q [4], t [3], s, levels (0/1 per pair), ninliers and stats (the iteration statistics of the first and of
         the second optimize, as optimize() returns them)."""
         params = Sim3Params() if params is None else params
-        n = np.array([len(p.omega1) for p in problems], np.int64)
-        ptr = np.concatenate([[0], np.cumsum(n)])
-        cat = lambda name, w: np.concatenate([np.asarray(getattr(p, name), np.float64).reshape(-1, w) for p in problems]) if problems else np.zeros((0, w))
-        r = self.optimize_sim3_flat(ptr, cat("q", 4), cat("t", 3), cat("s", 1).ravel(), cat("cam1", 4), cat("cam2", 4),
-                                    np.array([int(bool(p.fix_scale)) for p in problems], np.int32), cat("X1", 3), cat("X2", 3),
-                                    cat("obs1", 2), cat("obs2", 2), cat("omega1", 1).ravel(), cat("omega2", 1).ravel(), params)
+        a = graphio.sim3_batch_arrays(problems)
+        ptr = a["ptr"]
+        r = self.optimize_sim3_flat(params=params, **a)
         off = (0, int(params.iterations))
         res = []
         for b in range(len(problems)):
@@ -574,6 +604,149 @@ class Engine:
             res.append(dict(q=r["q"][b], t=r["t"][b], s=float(r["s"][b]), levels=r["levels"][ptr[b]:ptr[b + 1]].copy(),
                             ninliers=int(r["ninliers"][b]), stats=stats))
         return res
+
+    # --- the two batches on device-resident data (include/cuba_b200.h: cuba_engine_optimize_*_device) --------------------------------
+    # Every tensor whose address reaches the library -- inputs, outputs (fresh or reused through out=) and the workspace -- is checked
+    # here first: the library cannot see the size or the device of a device buffer.
+    @staticmethod
+    def _check_tensors(what, arrays):
+        """arrays: (name, tensor or None, torch dtype, shape or None).  Type, dtype, contiguity and, where given, shape."""
+        import torch
+        for name, a, dt, shape in arrays:
+            if a is None:
+                continue
+            if not isinstance(a, torch.Tensor):
+                raise TypeError("%s: %s must be a torch tensor, got %s" % (what, name, type(a).__name__))
+            if a.dtype != dt:
+                raise TypeError("%s: %s is %s, must be %s" % (what, name, a.dtype, dt))
+            if not a.is_contiguous():
+                raise ValueError("%s: %s is not contiguous" % (what, name))
+            if shape is not None and tuple(a.shape) != tuple(shape):
+                raise ValueError("%s: %s has shape %s, must be %s" % (what, name, tuple(a.shape), tuple(shape)))
+
+    def _check_devices(self, what, arrays):
+        for name, a in arrays:
+            if a is not None and (a.device.type != "cuda" or a.device.index != self._device):
+                raise ValueError("%s: %s is on %s, the engine on cuda:%d" % (what, name, a.device, self._device))
+
+    @staticmethod
+    def _count(what, name, a, width, n=None):
+        """a.numel() / width, checked against n when given"""
+        k = a.numel() // width
+        if a.numel() != k * width or (n is not None and k != n):
+            raise ValueError("%s: %s has %d elements, expected %s x %d" % (what, name, a.numel(), "a multiple" if n is None else n, width))
+        return k
+
+    def _device_call(self, what, inputs, out_spec, with_stats, out, workspace):
+        """the host-side checks and allocations of a device call.  inputs: (name, tensor) already checked for dtype and shape;
+        out_spec: {name: (shape, dtype)} of every output.  A reused `out` must hold exactly those tensors (stats absent or None
+        without with_stats); a reused workspace must be a float64 CUDA tensor (the library checks its size).  Returns (out,
+        workspace or None, torch)."""
+        import torch
+        if out is not None:
+            if not isinstance(out, dict):
+                raise TypeError("%s: out must be the dict an earlier call returned" % what)
+            if (out.get("stats") is not None) != bool(with_stats):
+                raise ValueError("%s: out%s stats, with_stats is %s" % (what, " has" if out.get("stats") is not None else " has no", with_stats))
+            missing = [k for k in out_spec if k != "stats" and k not in out]
+            if missing:
+                raise ValueError("%s: out lacks %s" % (what, ", ".join(missing)))
+            self._check_tensors(what, [("out[%r]" % k, out.get(k), dt, shape) for k, (shape, dt) in out_spec.items()])
+        self._check_tensors(what, [("workspace", workspace, torch.float64, None)])
+        if workspace is not None and workspace.dim() != 1:
+            raise ValueError("%s: workspace must be one-dimensional" % what)
+        self._check_devices(what, [("workspace", workspace)] + ([("out[%r]" % k, out.get(k)) for k in out_spec] if out is not None else []) +
+                            list(inputs))
+        if out is None:
+            dev = torch.device("cuda", self._device)
+            out = {k: None if (k == "stats" and not with_stats) else torch.empty(shape, dtype=dt, device=dev) for k, (shape, dt) in out_spec.items()}
+        return out, workspace, torch
+
+    def _workspace(self, torch, workspace, need):
+        return torch.empty((need + 7) // 8, dtype=torch.float64, device=torch.device("cuda", self._device)) if workspace is None else workspace
+
+    def _torch_stream(self):
+        """torch.cuda.current_stream() of the engine's device as the C ABI takes it"""
+        import torch
+        h = torch.cuda.current_stream(self._device).cuda_stream
+        return h if h else 1          # handle 0 is the legacy default stream: cudaStreamLegacy, not "the engine's stream"
+
+    def optimize_poses_device(self, q, t, cam, ptr2, X2, meas2, omega2, ptr3, X3, meas3, omega3, rounds, with_stats=True, out=None,
+                              workspace=None):
+        """cuba_engine_optimize_poses_device: optimize_poses_flat on torch CUDA tensors of the engine's device (float64, ptr2 / ptr3
+        int32, all contiguous), on torch.cuda.current_stream(); no host synchronisation, no host<->device copy.  Returns a dict of CUDA
+        tensors with optimize_poses_flat's keys and shapes, except stats: [B, sum of iterations, 4] float64 words holding
+        cuba_iter_stat, which stats_view() turns into the structured array; plus "status" (int32 [1], 0 = ok, else the bits of
+        BATCH_STATUS; no output is written then) and "workspace".  out / workspace: an earlier result dict and its "workspace" entry,
+        to run again into the same tensors (a CUDA graph replays into them); they must fit this batch exactly."""
+        what = "optimize_poses_device"
+        import torch
+        f64, i32 = torch.float64, torch.int32
+        inputs = [("q", q, f64), ("t", t, f64), ("cam", cam, f64), ("ptr2", ptr2, i32), ("X2", X2, f64), ("meas2", meas2, f64),
+                  ("omega2", omega2, f64), ("ptr3", ptr3, i32), ("X3", X3, f64), ("meas3", meas3, f64), ("omega3", omega3, f64)]
+        self._check_tensors(what, [(n, a, dt, None) for n, a, dt in inputs])
+        B = self._count(what, "q", q, 4)
+        for name, a, w in (("t", t, 3), ("cam", cam, 5)):
+            self._count(what, name, a, w, B)
+        for name, a in (("ptr2", ptr2), ("ptr3", ptr3)):
+            self._count(what, name, a, 1, B + 1)
+        E2, E3 = omega2.numel(), omega3.numel()
+        for name, a, w, n in (("X2", X2, 3, E2), ("meas2", meas2, 2, E2), ("X3", X3, 3, E3), ("meas3", meas3, 3, E3)):
+            self._count(what, name, a, w, n)
+        R = len(rounds)
+        S = sum(max(int(r.iterations), 0) for r in rounds)
+        spec = dict(q=((B, 4), f64), t=((B, 3), f64), levels=((E2 + E3,), torch.uint8), counts=((B, R, 4), i32), stats=((B, S, 4), f64),
+                    nstats=((B, R), i32), status=((1,), i32))
+        out, workspace, torch = self._device_call(what, [(n, a) for n, a, _ in inputs], spec, with_stats, out, workspace)
+        rs = self._rounds_struct(rounds)
+        workspace = self._workspace(torch, workspace, int(self.L.cuba_pose_batch_workspace_bytes(B, E2, E3, R, rs, int(bool(with_stats)))))
+        ptr = lambda a: None if a is None else a.data_ptr()
+        batch = _PoseBatch(B, E2, E3, ptr(q), ptr(t), ptr(cam), ptr(ptr2), ptr(X2), ptr(meas2), ptr(omega2), ptr(ptr3), ptr(X3), ptr(meas3),
+                           ptr(omega3))
+        _check(self.L.cuba_engine_optimize_poses_device(self.h, C.byref(batch), R, rs, ptr(workspace), workspace.numel() * workspace.element_size(),
+                                                        ptr(out["q"]), ptr(out["t"]), ptr(out["levels"]), ptr(out["counts"]),
+                                                        ptr(out["stats"]), ptr(out["nstats"]), ptr(out["status"]), C.c_void_p(self._torch_stream())))
+        out["workspace"] = workspace
+        return out
+
+    def optimize_sim3_device(self, ptr, q, t, s, cam1, cam2, fix_scale, X1, X2, obs1, obs2, omega1, omega2, params=None, with_stats=True,
+                             out=None, workspace=None):
+        """cuba_engine_optimize_sim3_device: optimize_sim3_flat on torch CUDA tensors of the engine's device (float64, ptr and
+        fix_scale int32, fix_scale may be None; all contiguous), on torch.cuda.current_stream(); no host synchronisation, no
+        host<->device copy.  Returns a dict of CUDA tensors with optimize_sim3_flat's keys and shapes, except stats: [B, iterations +
+        max(bad, good), 4] float64 words (stats_view()); plus "status" (int32 [1]; BATCH_STATUS) and "workspace".  out / workspace as
+        for optimize_poses_device."""
+        what = "optimize_sim3_device"
+        params = Sim3Params() if params is None else params
+        import torch
+        f64, i32 = torch.float64, torch.int32
+        inputs = [("ptr", ptr, i32), ("q", q, f64), ("t", t, f64), ("s", s, f64), ("cam1", cam1, f64), ("cam2", cam2, f64),
+                  ("fix_scale", fix_scale, i32), ("X1", X1, f64), ("X2", X2, f64), ("obs1", obs1, f64), ("obs2", obs2, f64),
+                  ("omega1", omega1, f64), ("omega2", omega2, f64)]
+        self._check_tensors(what, [(n, a, dt, None) for n, a, dt in inputs])
+        B = s.numel()
+        for name, a, w, n in (("q", q, 4, B), ("t", t, 3, B), ("cam1", cam1, 4, B), ("cam2", cam2, 4, B), ("ptr", ptr, 1, B + 1)):
+            self._count(what, name, a, w, n)
+        if fix_scale is not None:
+            self._count(what, "fix_scale", fix_scale, 1, B)
+        N = omega1.numel()
+        for name, a, w in (("X1", X1, 3), ("X2", X2, 3), ("obs1", obs1, 2), ("obs2", obs2, 2), ("omega2", omega2, 1)):
+            self._count(what, name, a, w, N)
+        S = max(int(params.iterations), 0) + max(int(params.iterations_bad), int(params.iterations_good), 0)
+        spec = dict(q=((B, 4), f64), t=((B, 3), f64), s=((B,), f64), levels=((N,), torch.uint8), ninliers=((B,), i32), stats=((B, S, 4), f64),
+                    nstats=((B, 2), i32), status=((1,), i32))
+        out, workspace, torch = self._device_call(what, [(n, a) for n, a, _ in inputs], spec, with_stats, out, workspace)
+        prm = _Sim3Params(float(params.chi2), int(params.iterations), int(params.iterations_bad), int(params.iterations_good),
+                          int(params.min_pairs))
+        workspace = self._workspace(torch, workspace, int(self.L.cuba_sim3_batch_workspace_bytes(B, N, C.byref(prm), int(bool(with_stats)))))
+        p = lambda a: None if a is None else a.data_ptr()
+        batch = _Sim3Batch(B, N, p(ptr), p(q), p(t), p(s), p(cam1), p(cam2), p(fix_scale), p(X1), p(X2), p(obs1), p(obs2), p(omega1), p(omega2))
+        _check(self.L.cuba_engine_optimize_sim3_device(self.h, C.byref(batch), C.byref(prm), p(workspace),
+                                                       workspace.numel() * workspace.element_size(), p(out["q"]), p(out["t"]), p(out["s"]),
+                                                       p(out["levels"]), p(out["ninliers"]), p(out["stats"]), p(out["nstats"]), p(out["status"]),
+                                                       C.c_void_p(self._torch_stream())))
+        out["workspace"] = workspace
+        return out
 
     def launch_count(self):
         n = C.c_longlong(0)

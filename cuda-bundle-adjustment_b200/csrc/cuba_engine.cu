@@ -30,6 +30,7 @@
 #include "cuba_levels.cuh"
 #include "cuba_pose_batch.cuh"
 #include "cuba_sim3_batch.cuh"
+#include "cuba_batch_io.cuh"
 #include "cuba_schur3.cuh"
 #include "cuba_schur5.cuh"
 #include "cuba_structure.h"
@@ -2309,8 +2310,8 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// ---- the batched LM kernels: each entry point packs its batch into batchHostIn and unpacks its results from batchHostOut.  Always
-	// fp64, on this engine's stream; they touch nothing of the engine's problem.  The batch was validated by the caller.
+	// ---- the batched LM kernels: each entry point packs its batch into batchHostIn (layouts of cuba_batch_io.cuh) and unpacks its
+	// results from batchHostOut.  Always fp64, on this engine's stream; they touch nothing of the engine's problem.  The batch was validated by the caller.
 	static_assert(sizeof(lm::IterStat) == sizeof(cuba_iter_stat) && sizeof(lm::IterStat) == 32, "cuba_iter_stat layout");
 
 	// one H2D of the packed batch (nIn doubles), the launch of one CTA per problem, one D2H of the packed results (nOut doubles)
@@ -2336,10 +2337,8 @@ struct Engine : EngineBase {
 		if (B == 0) return CUBA_OK;
 		const size_t E2 = (size_t)bt->E2, E3 = (size_t)bt->E3, E = E2 + E3;
 		const size_t nStat = stats ? B * (size_t)s.statOff[s.n] : 0;
-		// input, in doubles: pose [B][8] | cam [B][8] | edges [E][8] | ptr2, ptr3 as int32 [B+1] each
-		const size_t oCam = 8 * B, oEdge = 16 * B, oPtr = oEdge + 8 * E, nIn = oPtr + (B + 1);
-		// results, in doubles: pose [B][8] | stats [nStat] (4 doubles each) | counts [B][R][4], nstats [B][R] as int32 | levels [E] bytes
-		const size_t oStat = 8 * B, oInt = oStat + 4 * nStat, nInt = 5 * B * R, oLev = oInt + (nInt + 1) / 2, nOut = oLev + (E + 7) / 8;
+		const bio::PoseLayout L(B, E, R, nStat);
+		const size_t oCam = L.oCam, oEdge = L.oEdge, oPtr = L.oPtr, nIn = L.nIn, oStat = L.oStat, oInt = L.oInt, oLev = L.oLev, nOut = L.nOut;
 		CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * nOut));
 		CUDA_TRY(batchIn.alloc(nIn)); CUDA_TRY(batchOut.alloc(nOut));
 		double* h = (double*)batchHostIn.p;
@@ -2401,10 +2400,8 @@ struct Engine : EngineBase {
 		const size_t B = (size_t)bt->B, N = (size_t)bt->N;
 		if (B == 0) return CUBA_OK;
 		const size_t nStat = stats ? B * (size_t)p.statPer : 0;
-		// input, in doubles: problems [B][PROB] | pairs [N][PAIR] | ptr as int32 [B+1]
-		const size_t oPair = s3::PROB * B, oPtr = oPair + s3::PAIR * N, nIn = oPtr + (B + 2) / 2;
-		// results, in doubles: S [B][8] | stats [nStat] (4 doubles each) | ninliers [B], nstats [B][2] as int32 | levels [N] bytes
-		const size_t oStat = 8 * B, oInt = oStat + 4 * nStat, oLev = oInt + (3 * B + 1) / 2, nOut = oLev + (N + 7) / 8;
+		const bio::Sim3Layout L(B, N, nStat);
+		const size_t oPair = L.oPair, oPtr = L.oPtr, nIn = L.nIn, oStat = L.oStat, oInt = L.oInt, oLev = L.oLev, nOut = L.nOut;
 		CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * nOut));
 		CUDA_TRY(batchIn.alloc(nIn)); CUDA_TRY(batchOut.alloc(nOut));
 		double* h = (double*)batchHostIn.p;
@@ -2888,6 +2885,7 @@ int cuba_engine_set_state(cuba_engine* e, const double* q, const double* t, cons
 	return e->impl->set_state(q, t, Xw);
 }
 int cuba_engine_reset_state(cuba_engine* e) { ENGINE_OR_FAIL(e); return e->impl->reset_state(); }
+int cuba_engine_get_device(const cuba_engine* e, int* device) { ENGINE_OR_FAIL(e); if (!device) return fail(CUBA_ERR_INVALID, "null out"); *device = e->impl->devOrdinal; return CUBA_OK; }
 int cuba_engine_get_stream(cuba_engine* e, void** s) { ENGINE_OR_FAIL(e); if (!s) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_stream(s); }
 int cuba_engine_flush_l2(cuba_engine* e) { ENGINE_OR_FAIL(e); return e->impl->flush_l2(); }
 int cuba_engine_get_sizes(const cuba_engine* e, cuba_sizes* out) { ENGINE_OR_FAIL(e); if (!out) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_sizes(out); }
@@ -2929,15 +2927,11 @@ static bool all_finite(const double* p, size_t n)
 	return true;
 }
 
-int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds,
-	double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats)
+// the schedule of optimize_poses, checked: everything a host can see without the batch
+static int pose_schedule(int nrounds, const cuba_pose_round* rounds, pb::Schedule& s)
 {
-	ENGINE_OR_FAIL(e);
-	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_poses: null batch");
-	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: B < 0");
 	if (nrounds < 1 || nrounds > CUBA_POSE_MAX_ROUNDS || !rounds) return fail(CUBA_ERR_INVALID, "optimize_poses: nrounds outside 1..CUBA_POSE_MAX_ROUNDS");
 	static_assert(CUBA_POSE_MAX_ROUNDS == pb::MAX_ROUNDS, "round limit");
-	pb::Schedule s;
 	memset(&s, 0, sizeof(s));
 	s.n = nrounds;
 	long long off = 0;
@@ -2957,6 +2951,17 @@ int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nr
 		if (off > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many iterations");
 	}
 	s.statOff[nrounds] = (int)off;
+	return CUBA_OK;
+}
+
+int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds,
+	double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats)
+{
+	ENGINE_OR_FAIL(e);
+	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_poses: null batch");
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: B < 0");
+	pb::Schedule s;
+	{ const int rc0 = pose_schedule(nrounds, rounds, s); if (rc0) return rc0; }
 	const int B = bt->B;
 	if (B == 0) return CUBA_OK;
 	if (!bt->q || !bt->t || !bt->cam || !q_out || !t_out) return fail(CUBA_ERR_INVALID, "optimize_poses: null pose array");
@@ -2967,17 +2972,27 @@ int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nr
 	return e->impl->optimize_poses(bt, s, q_out, t_out, levels_out, counts, stats, nstats);
 }
 
-int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const cuba_sim3_params* params, double* q_out, double* t_out,
-	double* s_out, uint8_t* levels_out, int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats)
+// the parameters of optimize_sim3, checked
+static int sim3_params(const cuba_sim3_params& P, s3::Params& p)
 {
-	ENGINE_OR_FAIL(e);
-	if (!bt || !params) return fail(CUBA_ERR_INVALID, "optimize_sim3: null batch or params");
-	const cuba_sim3_params& P = *params;
 	if (!std::isfinite(P.chi2) || !(P.chi2 > 0)) return fail(CUBA_ERR_INVALID, "optimize_sim3: chi2 not finite and positive");
 	if (P.iterations < 0 || P.iterations_bad < 0 || P.iterations_good < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: negative iterations");
 	if (P.min_pairs < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: negative min_pairs");
 	if ((long long)P.iterations + std::max(P.iterations_bad, P.iterations_good) > INT32_MAX)
 		return fail(CUBA_ERR_INVALID, "optimize_sim3: too many iterations");
+	p.chi2 = P.chi2; p.delta = std::sqrt(P.chi2);
+	p.iterations = P.iterations; p.iterationsBad = P.iterations_bad; p.iterationsGood = P.iterations_good; p.minPairs = P.min_pairs;
+	p.statPer = P.iterations + std::max(P.iterations_bad, P.iterations_good);
+	return CUBA_OK;
+}
+
+int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const cuba_sim3_params* params, double* q_out, double* t_out,
+	double* s_out, uint8_t* levels_out, int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats)
+{
+	ENGINE_OR_FAIL(e);
+	if (!bt || !params) return fail(CUBA_ERR_INVALID, "optimize_sim3: null batch or params");
+	s3::Params p;
+	{ const int rc0 = sim3_params(*params, p); if (rc0) return rc0; }
 	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: B < 0");
 	if (bt->N < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: N < 0");
 	const int B = bt->B;
@@ -2994,11 +3009,151 @@ int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const c
 	if (!all_finite(bt->X1, 3 * N) || !all_finite(bt->X2, 3 * N) || !all_finite(bt->obs1, 2 * N) || !all_finite(bt->obs2, 2 * N) ||
 		!all_finite(bt->omega1, N) || !all_finite(bt->omega2, N))
 		return fail(CUBA_ERR_INVALID, "optimize_sim3: non-finite pair");
-	s3::Params p;
-	p.chi2 = P.chi2; p.delta = std::sqrt(P.chi2);
-	p.iterations = P.iterations; p.iterationsBad = P.iterations_bad; p.iterationsGood = P.iterations_good; p.minPairs = P.min_pairs;
-	p.statPer = P.iterations + std::max(P.iterations_bad, P.iterations_good);
 	return e->impl->optimize_sim3(bt, p, q_out, t_out, s_out, levels_out, ninliers, stats, nstats);
+}
+
+// ---- the batches on device-resident data (cuba_batch_io.cuh).  Host-side checks come first and touch neither the engine nor a
+// device; the data checks run on the device into *status.
+
+// csr_ok's checks that need no element of ptr
+static int csr_present(const std::string& what, int count, const int32_t* ptr, std::initializer_list<const void*> items)
+{
+	if (!ptr) return fail(CUBA_ERR_INVALID, what + ": null");
+	if (count < 0) return fail(CUBA_ERR_INVALID, what + "[B] is not the item count");
+	for (const void* p : items)
+		if (count > 0 && !p) return fail(CUBA_ERR_INVALID, what + ": null item array");
+	return CUBA_OK;
+}
+
+static int workspace_ok(const char* what, const void* ws, size_t bytes, size_t need)
+{
+	if (bytes < need || (need > 0 && !ws))
+		return fail(CUBA_ERR_INVALID, std::string(what) + ": workspace of " + std::to_string(bytes) + " bytes, " + std::to_string(need) + " needed");
+	if ((uintptr_t)ws % alignof(double)) return fail(CUBA_ERR_INVALID, std::string(what) + ": workspace not 8-byte aligned");
+	return CUBA_OK;
+}
+
+static cudaStream_t batch_stream(cuba_engine* e, void* stream)
+{
+	if (stream) return (cudaStream_t)stream;
+	void* s = nullptr;
+	e->impl->get_stream(&s);
+	return (cudaStream_t)s;
+}
+
+static size_t pose_workspace(int B, int E2, int E3, const pb::Schedule& s, bool withStats)
+{
+	const size_t nb = (size_t)B;
+	const bio::PoseLayout L(nb, (size_t)E2 + (size_t)E3, (size_t)s.n, withStats ? nb * (size_t)s.statOff[s.n] : 0);
+	return sizeof(double) * (L.nIn + L.nOut);
+}
+
+size_t cuba_pose_batch_workspace_bytes(int B, int E2, int E3, int nrounds, const cuba_pose_round* rounds, int with_stats)
+{
+	pb::Schedule s;
+	if (B <= 0 || E2 < 0 || E3 < 0 || (long long)E2 + E3 > INT32_MAX) return 0;
+	const std::string err = g_err;
+	const int rc = pose_schedule(nrounds, rounds, s);
+	g_err = err;       // a size query leaves the last error alone
+	return rc ? 0 : pose_workspace(B, E2, E3, s, with_stats != 0);
+}
+
+int cuba_engine_optimize_poses_device(cuba_engine* e, const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds,
+	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats,
+	int32_t* nstats, int32_t* status, void* stream)
+{
+	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_poses: null batch");
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: B < 0");
+	pb::Schedule s;
+	{ const int rc0 = pose_schedule(nrounds, rounds, s); if (rc0) return rc0; }
+	if (!status) return fail(CUBA_ERR_INVALID, "optimize_poses_device: null status");
+	const int B = bt->B;
+	if (B > 0) {
+		if (!bt->q || !bt->t || !bt->cam || !q_out || !t_out) return fail(CUBA_ERR_INVALID, "optimize_poses: null pose array");
+		if ((long long)bt->E2 + bt->E3 > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many edges");
+		int rc = csr_present("optimize_poses: ptr2", bt->E2, bt->ptr2, { bt->X2, bt->meas2, bt->omega2 }); if (rc) return rc;
+		rc = csr_present("optimize_poses: ptr3", bt->E3, bt->ptr3, { bt->X3, bt->meas3, bt->omega3 }); if (rc) return rc;
+		rc = workspace_ok("optimize_poses_device", workspace, workspace_bytes, pose_workspace(B, bt->E2, bt->E3, s, stats != nullptr)); if (rc) return rc;
+	}
+	ENGINE_OR_FAIL(e);
+	const cudaStream_t st = batch_stream(e, stream);
+	CUDA_TRY(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+	if (B == 0) return CUBA_OK;
+	const size_t nb = (size_t)B, E = (size_t)bt->E2 + (size_t)bt->E3, statPer = (size_t)s.statOff[s.n];
+	const bio::PoseLayout L(nb, E, (size_t)s.n, stats ? nb * statPer : 0);
+	double* in = (double*)workspace;
+	bio::k_validate_poses<<<bio::grid_for(std::max(nb + 1, E)), bio::BLOCK, 0, st>>>(*bt, status);
+	bio::k_pack_poses<<<(unsigned)B, bio::BLOCK, 0, st>>>(*bt, L, in, status);
+	pb::Args a;
+	a.B = B;
+	a.pose = in; a.cam = in + L.oCam; a.edge = in + L.oEdge;
+	a.ptr2 = (const int*)(in + L.oPtr); a.ptr3 = a.ptr2 + nb + 1;
+	double* o = in + L.nIn;
+	a.poseOut = o;
+	a.stats = stats ? (lm::IterStat*)(o + L.oStat) : nullptr;
+	a.counts = (int*)(o + L.oInt); a.nstats = a.counts + 4 * nb * (size_t)s.n;
+	a.level = (unsigned char*)(o + L.oLev);
+	pb::k_pose_batch<<<(unsigned)B, lm::BLOCK, 0, st>>>(a, s);
+	bio::k_unpack_poses<<<(unsigned)B, bio::BLOCK, 0, st>>>(L, B, s.n, bt->E2, (int)statPer, in, q_out, t_out, levels_out, counts, stats, nstats, status);
+	CUDA_TRY(cudaGetLastError());
+	return CUBA_OK;
+}
+
+static size_t sim3_workspace(int B, int N, const s3::Params& p, bool withStats)
+{
+	const bio::Sim3Layout L((size_t)B, (size_t)N, withStats ? (size_t)B * (size_t)p.statPer : 0);
+	return sizeof(double) * (L.nIn + L.nOut);
+}
+
+size_t cuba_sim3_batch_workspace_bytes(int B, int N, const cuba_sim3_params* params, int with_stats)
+{
+	s3::Params p;
+	if (B <= 0 || N < 0 || !params) return 0;
+	const std::string err = g_err;
+	const int rc = sim3_params(*params, p);
+	g_err = err;
+	return rc ? 0 : sim3_workspace(B, N, p, with_stats != 0);
+}
+
+int cuba_engine_optimize_sim3_device(cuba_engine* e, const cuba_sim3_batch* bt, const cuba_sim3_params* params,
+	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, double* s_out, uint8_t* levels_out, int32_t* ninliers,
+	cuba_iter_stat* stats, int32_t* nstats, int32_t* status, void* stream)
+{
+	if (!bt || !params) return fail(CUBA_ERR_INVALID, "optimize_sim3: null batch or params");
+	s3::Params p;
+	{ const int rc0 = sim3_params(*params, p); if (rc0) return rc0; }
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: B < 0");
+	if (bt->N < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: N < 0");
+	if (!status) return fail(CUBA_ERR_INVALID, "optimize_sim3_device: null status");
+	const int B = bt->B;
+	if (B > 0) {
+		int rc = csr_present("optimize_sim3: ptr", bt->N, bt->ptr, { bt->X1, bt->X2, bt->obs1, bt->obs2, bt->omega1, bt->omega2 }); if (rc) return rc;
+		if (!bt->q || !bt->t || !bt->s || !bt->cam1 || !bt->cam2 || !q_out || !t_out || !s_out)
+			return fail(CUBA_ERR_INVALID, "optimize_sim3: null problem array");
+		rc = workspace_ok("optimize_sim3_device", workspace, workspace_bytes, sim3_workspace(B, bt->N, p, stats != nullptr)); if (rc) return rc;
+	}
+	ENGINE_OR_FAIL(e);
+	const cudaStream_t st = batch_stream(e, stream);
+	CUDA_TRY(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+	if (B == 0) return CUBA_OK;
+	const size_t nb = (size_t)B, N = (size_t)bt->N, nStat = stats ? nb * (size_t)p.statPer : 0;
+	const bio::Sim3Layout L(nb, N, nStat);
+	double* in = (double*)workspace;
+	bio::k_validate_sim3<<<bio::grid_for(std::max(4 * nb + 1, 3 * N)), bio::BLOCK, 0, st>>>(*bt, status);
+	bio::k_pack_sim3<<<bio::grid_for(s3::PROB * nb + s3::PAIR * N + nb + 1), bio::BLOCK, 0, st>>>(*bt, L, in, status);
+	s3::Args a;
+	a.B = B;
+	a.prob = in; a.pair = in + L.oPair; a.ptr = (const int*)(in + L.oPtr);
+	double* o = in + L.nIn;
+	a.Sout = o;
+	a.stats = stats ? (lm::IterStat*)(o + L.oStat) : nullptr;
+	a.ninliers = (int*)(o + L.oInt); a.nstats = a.ninliers + nb;
+	a.level = (unsigned char*)(o + L.oLev);
+	s3::k_sim3_batch<<<(unsigned)B, lm::BLOCK, 0, st>>>(a, p);
+	bio::k_unpack_sim3<<<bio::grid_for(std::max(8 * nb, std::max(4 * nStat, N))), bio::BLOCK, 0, st>>>(L, B, bt->N, nStat, in, q_out, t_out,
+		s_out, levels_out, ninliers, stats, nstats, status);
+	CUDA_TRY(cudaGetLastError());
+	return CUBA_OK;
 }
 
 int cuba_engine_get_profile(cuba_engine* e, double* sec) { ENGINE_OR_FAIL(e); if (!sec) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_profile(sec); }

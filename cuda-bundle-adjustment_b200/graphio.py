@@ -194,6 +194,25 @@ def pose_frames(prob: FlatProblem, rows):
     return out
 
 
+def _cat(items, name, w):
+    """the field `name` of every item as one contiguous float64 array [n, w] ([n] for w = 1)"""
+    a = np.concatenate([np.asarray(getattr(x, name), np.float64).reshape(-1, w) for x in items]) if items else np.zeros((0, w))
+    return np.ascontiguousarray(a.ravel() if w == 1 else a)
+
+
+def _ptr(counts):
+    return np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64))]).astype(np.int32)
+
+
+def pose_batch_arrays(frames):
+    """the flat arrays of cuba_pose_batch for a list of PoseFrame: the keyword arguments of Engine.optimize_poses_flat (numpy) and,
+    moved to the GPU, of Engine.optimize_poses_device"""
+    return dict(q=_cat(frames, "q", 4), t=_cat(frames, "t", 3), cam=_cat(frames, "cam", 5), ptr2=_ptr([len(f.omega2) for f in frames]),
+                X2=_cat(frames, "X2", 3), meas2=_cat(frames, "meas2", 2), omega2=_cat(frames, "omega2", 1),
+                ptr3=_ptr([len(f.omega3) for f in frames]), X3=_cat(frames, "X3", 3), meas3=_cat(frames, "meas3", 3),
+                omega3=_cat(frames, "omega3", 1))
+
+
 @dataclasses.dataclass
 class Sim3Problem:
     """One problem of Engine.optimize_sim3 (ORB-SLAM2's OptimizeSim3): S12 = (q, t, s), S12 X = s R(q) X + t, from camera 2 into
@@ -261,6 +280,16 @@ def sim3_problems(prob: FlatProblem, pairs, scale=1.0, fix_scale=False):
             cam2=np.array(prob.cam[j][:4], dtype=np.float64), X1=X @ Ri.T + prob.t[i], X2=(X @ Rj.T + prob.t[j]) / s0[k],
             obs1=uv[a].copy(), obs2=uv[b].copy(), omega1=om[a].copy(), omega2=om[b].copy(), fix_scale=bool(fix_scale), landmarks=common))
     return out
+
+
+def sim3_batch_arrays(problems):
+    """the flat arrays of cuba_sim3_batch for a list of Sim3Problem, fix_scale from each problem: the keyword arguments of
+    Engine.optimize_sim3_flat (numpy) and, moved to the GPU, of Engine.optimize_sim3_device"""
+    return dict(ptr=_ptr([len(p.omega1) for p in problems]), q=_cat(problems, "q", 4), t=_cat(problems, "t", 3),
+                s=_cat(problems, "s", 1), cam1=_cat(problems, "cam1", 4), cam2=_cat(problems, "cam2", 4),
+                fix_scale=np.array([int(bool(p.fix_scale)) for p in problems], np.int32), X1=_cat(problems, "X1", 3),
+                X2=_cat(problems, "X2", 3), obs1=_cat(problems, "obs1", 2), obs2=_cat(problems, "obs2", 2), omega1=_cat(problems, "omega1", 1),
+                omega2=_cat(problems, "omega2", 1))
 
 
 def write_back(g, prob: FlatProblem, q, t, Xw):

@@ -181,6 +181,8 @@ int cuba_engine_set_state(cuba_engine* e, const double* q, const double* t, cons
 int cuba_engine_reset_state(cuba_engine* e);
 
 int cuba_engine_get_sizes(const cuba_engine* e, cuba_sizes* out);
+/* The CUDA device ordinal the engine runs on (the current device at create time when cuba_config.device was -1). */
+int cuba_engine_get_device(const cuba_engine* e, int* device);
 /* The CUDA stream (cudaStream_t) every kernel of this engine is launched on -- for CUDA-event timing. */
 int cuba_engine_get_stream(cuba_engine* e, void** stream);
 /* Overwrite a buffer larger than L2 on the engine's stream (benchmark hygiene between timed steps). */
@@ -307,6 +309,39 @@ typedef struct cuba_sim3_params {
  * chi2 that is not finite and positive. */
 int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* batch, const cuba_sim3_params* params, double* q_out, double* t_out,
 	double* s_out, uint8_t* levels_out, int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats);
+
+/* ---- the same two batches on device-resident data (csrc/cuba_batch_io.cuh) ----
+ * Every array pointer of the batch and every output is a DEVICE pointer on the engine's device; the schedule / parameters stay host
+ * structs.  The call validates, packs, runs the batch's kernel and unpacks on `stream` (NULL = the engine's stream; the legacy default
+ * stream is cudaStreamLegacy): it copies nothing between host and device, never synchronises, allocates nothing and neither reads nor
+ * changes any engine state (the engine's buffers, its launch count included), so it can be captured into a CUDA graph, and two calls
+ * with two workspaces on two streams are independent.  The results are bit for bit those of cuba_engine_optimize_poses /
+ * _optimize_sim3: the same packed records go to the same kernel.  Output layouts are theirs.
+ *
+ * The workspace is the caller's: at least *_workspace_bytes(...) bytes of device memory, 8-byte aligned, used only during the call's
+ * work on `stream`.  The size functions are host-only; they return 0 for B <= 0 and for arguments the call itself refuses.  with_stats:
+ * whether `stats` will be non-NULL.
+ *
+ * Host-side checks (CUBA_ERR_INVALID before any launch, with the messages of the host entry points where they check the same thing,
+ * and before the engine is looked at): a NULL batch, B < 0, N < 0 or a negative edge count, the schedule / parameters, NULL pointers
+ * the host entry points refuse, a NULL status, a workspace that is too small or misaligned.
+ * Data-dependent checks run on the device and land in *status (a device int32, written on the stream by every call that returns
+ * CUBA_OK, B = 0 included; a call refused on the host writes nothing): 0 when the batch is valid, else the OR of the CUBA_BATCH_* bits of every check that failed.  When *status != 0 no output array is written. */
+#define CUBA_BATCH_OK 0
+#define CUBA_BATCH_PTR_START 1           /* a CSR pointer does not start at 0 (ptr2 / ptr3 / ptr)                       */
+#define CUBA_BATCH_PTR_DECREASES 2       /* a CSR pointer decreases                                                   */
+#define CUBA_BATCH_PTR_END 4             /* a CSR pointer does not end at the item count (E2 / E3 / N)                */
+#define CUBA_BATCH_NONFINITE_ITEM 8      /* a non-finite omega (pose batch) or pair value (X1, X2, obs1, obs2, omega) */
+#define CUBA_BATCH_NONFINITE_PROBLEM 16  /* Sim3: a non-finite q, t, s or intrinsic                                   */
+#define CUBA_BATCH_SCALE 32              /* Sim3: a finite s <= 0                                                     */
+size_t cuba_pose_batch_workspace_bytes(int B, int E2, int E3, int nrounds, const cuba_pose_round* rounds, int with_stats);
+int cuba_engine_optimize_poses_device(cuba_engine* e, const cuba_pose_batch* batch_dev, int nrounds, const cuba_pose_round* rounds,
+	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats,
+	int32_t* nstats, int32_t* status, void* stream);
+size_t cuba_sim3_batch_workspace_bytes(int B, int N, const cuba_sim3_params* params, int with_stats);
+int cuba_engine_optimize_sim3_device(cuba_engine* e, const cuba_sim3_batch* batch_dev, const cuba_sim3_params* params,
+	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, double* s_out, uint8_t* levels_out, int32_t* ninliers,
+	cuba_iter_stat* stats, int32_t* nstats, int32_t* status, void* stream);
 
 /* seconds per profile bucket accumulated since set_problem, [CUBA_PROF_NUM] */
 int cuba_engine_get_profile(cuba_engine* e, double* seconds);
