@@ -143,7 +143,7 @@ _lib = None
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
     "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_linear_solver", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_get_device", "cuba_engine_flush_l2",
-    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_pose_batch_workspace_bytes", "cuba_engine_optimize_poses_device", "cuba_sim3_batch_workspace_bytes", "cuba_engine_optimize_sim3_device", "cuba_engine_get_profile",
+    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_set_problem_device", "cuba_engine_set_state_device", "cuba_engine_get_state_device", "cuba_engine_get_chi2_device", "cuba_engine_set_edge_levels_device", "cuba_engine_get_edge_levels_device", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_pose_batch_workspace_bytes", "cuba_engine_optimize_poses_device", "cuba_sim3_batch_workspace_bytes", "cuba_engine_optimize_sim3_device", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
     "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_dense_solve", "cuba_debug_peer_allreduce", "cuba_debug_pcg5_ranks", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dense_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
@@ -187,6 +187,12 @@ def load_library():
         "cuba_engine_set_edge_levels": [vp, vp],
         "cuba_engine_get_edge_levels": [vp, vp],
         "cuba_engine_classify_edges": [vp, d, d, i, vp],
+        "cuba_engine_set_problem_device": [vp, C.POINTER(_Problem), vp],
+        "cuba_engine_set_state_device": [vp, vp, vp, vp, vp],
+        "cuba_engine_get_state_device": [vp, vp, vp, vp, vp],
+        "cuba_engine_get_chi2_device": [vp, vp, vp],
+        "cuba_engine_set_edge_levels_device": [vp, vp, vp],
+        "cuba_engine_get_edge_levels_device": [vp, vp, vp],
         "cuba_engine_optimize_poses": [vp, C.POINTER(_PoseBatch), i, vp, vp, vp, vp, vp, vp, vp],
         "cuba_engine_optimize_sim3": [vp, C.POINTER(_Sim3Batch), C.POINTER(_Sim3Params), vp, vp, vp, vp, vp, vp, vp],
         "cuba_engine_optimize_poses_device": [vp, C.POINTER(_PoseBatch), i, vp, vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp, vp],
@@ -746,6 +752,106 @@ class Engine:
                                                        p(out["levels"]), p(out["ninliers"]), p(out["stats"]), p(out["nstats"]), p(out["status"]),
                                                        C.c_void_p(self._torch_stream())))
         out["workspace"] = workspace
+        return out
+
+    # --- the engine's own problem on device-resident data (include/cuba_b200.h: cuba_engine_set_problem_device etc.) ----------------
+    # Torch CUDA tensors of the engine's device, checked like the batches' (dtype, contiguity, exact shape, device) before any library
+    # call; the work runs on torch.cuda.current_stream(), ordered after what is queued there, and torch's later work after it.
+    def _problem_sizes(self, what):
+        if self.sizes is None:
+            raise CubaError("%s before initialize / initialize_device" % what)
+        s = self.sizes
+        return s["Pall"], s["Lall"], s["E2"] + s["E3"]
+
+    def _tensors(self, what, arrays):
+        """arrays: (name, tensor or None, torch dtype, exact shape)"""
+        self._check_tensors(what, arrays)
+        self._check_devices(what, [(n, a) for n, a, _, _ in arrays])
+
+    def _empty(self, shape, dtype):
+        import torch
+        return torch.empty(shape, dtype=dtype, device=torch.device("cuda", self._device))
+
+    def initialize_device(self, prob):
+        """initialize() on device-resident arrays: prob is a dict or an object with initialize()'s fields (Pall, numP, Lall, numL and
+        q [Pall,4], t [Pall,3], cam [Pall,5], Xw [Lall,3], idx2 [E2,2] int32, meas2 [E2,2], omega2 [E2], idx3 [E3,2] int32, meas3 [E3,3],
+        omega3 [E3] as torch CUDA tensors, float64 unless noted; E2 / E3 default to the lengths of omega2 / omega3).  Synchronous like
+        initialize(); no bulk host<->device copy.  Returns sizes."""
+        what = "initialize_device"
+        import torch
+        get = (lambda k, d=None: prob.get(k, d)) if isinstance(prob, dict) else (lambda k, d=None: getattr(prob, k, d))
+        Pall, numP, Lall, numL = (int(get(k)) for k in ("Pall", "numP", "Lall", "numL"))
+        names = ("q", "t", "cam", "Xw", "idx2", "meas2", "omega2", "idx3", "meas3", "omega3")
+        a = {n: get(n) for n in names}
+        missing = [n for n in names if a[n] is None]
+        if missing:
+            raise TypeError("%s: prob lacks %s" % (what, ", ".join(missing)))
+        f64, i32 = torch.float64, torch.int32
+        self._check_tensors(what, [("omega2", a["omega2"], f64, None), ("omega3", a["omega3"], f64, None)])
+        E2 = int(get("E2", a["omega2"].shape[0] if a["omega2"].dim() else -1))
+        E3 = int(get("E3", a["omega3"].shape[0] if a["omega3"].dim() else -1))
+        spec = [("q", f64, (Pall, 4)), ("t", f64, (Pall, 3)), ("cam", f64, (Pall, 5)), ("Xw", f64, (Lall, 3)), ("idx2", i32, (E2, 2)),
+                ("meas2", f64, (E2, 2)), ("omega2", f64, (E2,)), ("idx3", i32, (E3, 2)), ("meas3", f64, (E3, 3)), ("omega3", f64, (E3,))]
+        self._tensors(what, [(n, a[n], dt, shape) for n, dt, shape in spec])
+        p = {n: a[n].data_ptr() for n in a}
+        P = _Problem(Pall, numP, Lall, numL, p["q"], p["t"], p["cam"], p["Xw"], E2, p["idx2"], p["meas2"], p["omega2"], E3, p["idx3"],
+                     p["meas3"], p["omega3"])
+        _check(self.L.cuba_engine_set_problem_device(self.h, C.byref(P), C.c_void_p(self._torch_stream())))
+        sz = _Sizes()
+        _check(self.L.cuba_engine_get_sizes(self.h, C.byref(sz)))
+        self.sizes = {n: getattr(sz, n) for n, _ in _Sizes._fields_}
+        self._stats = []
+        return self.sizes
+
+    def set_state_device(self, q, t, Xw):
+        """set_state() from CUDA tensors q [Pall,4], t [Pall,3], Xw [Lall,3] (float64); no synchronisation"""
+        what = "set_state_device"
+        import torch
+        Pall, Lall, _ = self._problem_sizes(what)
+        self._tensors(what, [("q", q, torch.float64, (Pall, 4)), ("t", t, torch.float64, (Pall, 3)), ("Xw", Xw, torch.float64, (Lall, 3))])
+        _check(self.L.cuba_engine_set_state_device(self.h, q.data_ptr(), t.data_ptr(), Xw.data_ptr(), C.c_void_p(self._torch_stream())))
+
+    def state_device(self, out=None):
+        """state() into CUDA tensors (q [Pall,4], t [Pall,3], Xw [Lall,3], float64), fresh or the tuple `out`; no synchronisation"""
+        what = "state_device"
+        import torch
+        Pall, Lall, _ = self._problem_sizes(what)
+        shapes = ((Pall, 4), (Pall, 3), (Lall, 3))
+        if out is None:
+            out = tuple(self._empty(sh, torch.float64) for sh in shapes)
+        elif not isinstance(out, tuple) or len(out) != 3:
+            raise TypeError("%s: out must be a tuple (q, t, Xw)" % what)
+        self._tensors(what, [(n, a, torch.float64, sh) for n, a, sh in zip(("q", "t", "Xw"), out, shapes)])
+        _check(self.L.cuba_engine_get_state_device(self.h, *(a.data_ptr() for a in out), C.c_void_p(self._torch_stream())))
+        return out
+
+    def chi_squared_device(self, out=None):
+        """chi_squared() into a CUDA tensor [E2+E3] float64 (fresh or `out`); no synchronisation"""
+        what = "chi_squared_device"
+        import torch
+        _, _, E = self._problem_sizes(what)
+        out = self._empty((E,), torch.float64) if out is None else out
+        self._tensors(what, [("out", out, torch.float64, (E,))])
+        _check(self.L.cuba_engine_get_chi2_device(self.h, out.data_ptr(), C.c_void_p(self._torch_stream())))
+        return out
+
+    def set_edge_levels_device(self, levels):
+        """set_edge_levels() from a CUDA tensor [E2+E3] uint8 (0 = optimised, non-zero = left out), or None = all 0; waits for one
+        8-byte count"""
+        what = "set_edge_levels_device"
+        import torch
+        _, _, E = self._problem_sizes(what)
+        self._tensors(what, [("levels", levels, torch.uint8, (E,))])
+        _check(self.L.cuba_engine_set_edge_levels_device(self.h, None if levels is None else levels.data_ptr(), C.c_void_p(self._torch_stream())))
+
+    def edge_levels_device(self, out=None):
+        """edge_levels() into a CUDA tensor [E2+E3] uint8 (fresh or `out`); no synchronisation"""
+        what = "edge_levels_device"
+        import torch
+        _, _, E = self._problem_sizes(what)
+        out = self._empty((E,), torch.uint8) if out is None else out
+        self._tensors(what, [("out", out, torch.uint8, (E,))])
+        _check(self.L.cuba_engine_get_edge_levels_device(self.h, out.data_ptr(), C.c_void_p(self._torch_stream())))
         return out
 
     def launch_count(self):

@@ -31,6 +31,7 @@
 #include "cuba_pose_batch.cuh"
 #include "cuba_sim3_batch.cuh"
 #include "cuba_batch_io.cuh"
+#include "cuba_problem_io.cuh"
 #include "cuba_schur3.cuh"
 #include "cuba_schur5.cuh"
 #include "cuba_structure.h"
@@ -181,6 +182,13 @@ struct DBuf {
 		return cudaMemcpyAsync(p, h, sizeof(U) * count, cudaMemcpyHostToDevice, s);
 	}
 	cudaError_t upload(const std::vector<U>& h, cudaStream_t s) { return upload(h.data(), h.size(), s); }
+	// from a caller's device array on the same device: no host traffic, nothing counted
+	cudaError_t copy(const U* d, size_t count, cudaStream_t s)
+	{
+		cudaError_t e = alloc(count);
+		if (e != cudaSuccess || !count) return e;
+		return cudaMemcpyAsync(p, d, sizeof(U) * count, cudaMemcpyDeviceToDevice, s);
+	}
 	// through the pinned arena when one is given
 	cudaError_t upload(const std::vector<U>& h, cudaStream_t s, PinnedArena* arena)
 	{
@@ -318,6 +326,13 @@ struct EngineBase {
 	virtual int set_edge_levels(const uint8_t* levels) = 0;
 	virtual int get_edge_levels(uint8_t* levels) = 0;
 	virtual int classify_edges(double chi2Mono, double chi2Stereo, int flags, int32_t* counts) = 0;
+	// the problem on device-resident arrays, ordered after `caller`'s work (NULL: the engine's stream)
+	virtual int set_problem_device(const cuba_problem* p, cudaStream_t caller) = 0;
+	virtual int set_state_device(const double* q, const double* t, const double* Xw, cudaStream_t caller) = 0;
+	virtual int get_state_device(double* q, double* t, double* Xw, cudaStream_t caller) = 0;
+	virtual int get_chi2_device(double* out, cudaStream_t caller) = 0;
+	virtual int set_edge_levels_device(const uint8_t* levels, cudaStream_t caller) = 0;
+	virtual int get_edge_levels_device(uint8_t* levels, cudaStream_t caller) = 0;
 	virtual int optimize_poses(const cuba_pose_batch* bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
 		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) = 0;
 	virtual int optimize_sim3(const cuba_sim3_batch* bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
@@ -417,6 +432,7 @@ struct Engine : EngineBase {
 	DBuf<double> flushBuf;
 	std::vector<std::pair<int, std::pair<cudaEvent_t, cudaEvent_t>>> profEvents;
 	std::vector<cudaEvent_t> eventPool;
+	cudaEvent_t joinIn = nullptr, joinOut = nullptr;   // the caller's stream -> the engine's, and back (on_caller_stream)
 
 	~Engine() override
 	{
@@ -425,6 +441,8 @@ struct Engine : EngineBase {
 		p5Peer.close(rank); uPeer.close(rank);
 		for (auto& pe : profEvents) { cudaEventDestroy(pe.second.first); cudaEventDestroy(pe.second.second); }
 		for (auto ev : eventPool) cudaEventDestroy(ev);
+		if (joinIn) cudaEventDestroy(joinIn);
+		if (joinOut) cudaEventDestroy(joinOut);
 		if (hScal) cudaFreeHost(hScal);
 		if (hMeta) cudaFreeHost(hMeta);
 		if (jh4Host) cudaFreeHost(jh4Host);
@@ -445,6 +463,7 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev));
 		CUDA_TRY(cudaDeviceGetAttribute(&smemMax, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
 		CUDA_TRY(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+		CUDA_TRY(cudaEventCreateWithFlags(&joinIn, cudaEventDisableTiming)); CUDA_TRY(cudaEventCreateWithFlags(&joinOut, cudaEventDisableTiming));
 		CUDA_TRY(cudaMallocHost((void**)&hScal, sizeof(Scalars)));
 		memset(hScal, 0, sizeof(Scalars));
 		CUDA_TRY(dScal.alloc(1));
@@ -486,6 +505,19 @@ struct Engine : EngineBase {
 		return r;
 	}
 
+	// Runs f on the engine's stream after the work the caller has queued on `caller` so far, and orders the caller's later work after
+	// f's: an event each way (none for NULL or the engine's own stream).  Neither synchronises, so a capture of `caller` takes the
+	// engine's work as a fork and a join of the graph.
+	template <class F>
+	int on_caller_stream(cudaStream_t caller, F&& f)
+	{
+		const bool join = caller && caller != stream;
+		if (join) { CUDA_TRY(cudaEventRecord(joinIn, caller)); CUDA_TRY(cudaStreamWaitEvent(stream, joinIn, 0)); }
+		const int rc = f();
+		if (join) { CUDA_TRY(cudaEventRecord(joinOut, stream)); CUDA_TRY(cudaStreamWaitEvent(caller, joinOut, 0)); }
+		return rc;
+	}
+
 	// ---- collectives (landmark-sharded runs) ----------------------------------------------------------
 	int allreduce(void* buf, size_t count, bool isT)
 	{
@@ -507,12 +539,19 @@ struct Engine : EngineBase {
 		CUDA_TRY(rawQ.upload(q, 4 * (size_t)Pall, stream)); CUDA_TRY(rawT.upload(t, 3 * (size_t)Pall, stream));
 		CUDA_TRY(rawX.upload(X, 3 * (size_t)Lall, stream));
 		if (c) CUDA_TRY(rawC.upload(c, 5 * (size_t)Pall, stream));
+		return pack_state(rawQ.p, rawT.p, c ? rawC.p : nullptr, rawX.p);
+	}
+	// the padded records from flat fp64 arrays on the device, the engine's or the caller's (read in place); c == NULL keeps cam.
+	// Allocates nothing once set_problem has sized the buffers.
+	int pack_state(const double* q, const double* t, const double* c, const double* X)
+	{
+		const int Pall = S.Pall, Lall = S.Lall;
 		CUDA_TRY(pose0.alloc(8 * (size_t)Pall)); CUDA_TRY(Xw0.alloc(4 * (size_t)Lall));
 		for (int b = 0; b < 2; b++) { CUDA_TRY(pose[b].alloc(8 * (size_t)Pall)); CUDA_TRY(Xw[b].alloc(4 * (size_t)Lall)); }
 		if (c) CUDA_TRY(cam.alloc(8 * (size_t)Pall));
 		const int n = std::max(Pall, Lall);
 		if (n > 0) {
-			k_pack_state<T><<<(n + 255) / 256, 256, 0, stream>>>(rawQ.p, rawT.p, c ? rawC.p : nullptr, rawX.p, Pall, Lall,
+			k_pack_state<T><<<(n + 255) / 256, 256, 0, stream>>>(q, t, c, X, Pall, Lall,
 				pose0.p, pose[0].p, pose[1].p, c ? cam.p : nullptr, Xw0.p, Xw[0].p, Xw[1].p);
 			launches++;
 			CUDA_TRY(cudaGetLastError());
@@ -525,7 +564,14 @@ struct Engine : EngineBase {
 	std::vector<std::pair<const char*, std::chrono::steady_clock::time_point>> marks;
 	void tmark(const char* name) { if (markOn) marks.push_back({ name, std::chrono::steady_clock::now() }); }
 	bool markOn = false;
-	int set_problem(const cuba_problem* p) override
+	int set_problem(const cuba_problem* p) override { return load_problem(p, false); }
+	int set_problem_device(const cuba_problem* p, cudaStream_t caller) override
+	{
+		return on_caller_stream(caller, [&] { return load_problem(p, true); });
+	}
+	// set_problem from host arrays (dev = false) or from device arrays on the engine's device (dev = true: copied device to device,
+	// the state read in place); everything else, structure reuse across both included, is one path
+	int load_problem(const cuba_problem* p, bool dev)
 	{
 		markOn = getenv("CUBA_SETUP_TIMING") != nullptr; marks.clear(); tmark("start");
 		if (!p) return fail(CUBA_ERR_INVALID, "set_problem: null problem");
@@ -536,17 +582,29 @@ struct Engine : EngineBase {
 			return fail(CUBA_ERR_INVALID, "set_problem: null array with a non-zero count");
 		// the cap, before any change; a pose-only system (no free landmark) never reaches the direct solver (k_solve_poses_only)
 		if (linSolver == CUBA_SOLVER_DENSE_CHOLESKY && p->numP > dchol::MAX_POSES && p->numL > 0) return dense_cap_error(p->numP);
+		if (dev && cfg.reserved[1] == 1)
+			return fail(CUBA_ERR_INVALID, "set_problem_device: the host structure builder (reserved[1] = 1) reads host arrays; use set_problem");
 		const auto t0 = std::chrono::steady_clock::now();
 		lastPcgKernel = CUBA_PCG_KERNEL_NONE; p5.coarse.rebuilds = 0; bjRetries = 0;
 		lvOn = false;      // every level back to 0: both paths below scatter the caller's omega unmasked
 		// Same topology as the problem this engine already holds (sizes, fixed/free split and every (iP, iL) pair identical): only the
 		// numbers changed -- the estimate after a previous optimize(), new measurements -- so every index structure, tile list,
 		// product list and PCG partition on the device stays valid.  Upload the values and re-run the three kernels that scatter them.
-		if (structureReuse && reusable && haveProblem && cfg.reserved[1] != 1 && denseSolve == (linSolver == CUBA_SOLVER_DENSE_CHOLESKY) && same_topology(p)) {
-			int rc = refresh_values(p); if (rc) return rc;
-			structureReuses++;
-			prof[CUBA_PROF_BUILD_STRUCTURE] += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-			return CUBA_OK;
+		// Host lists are compared with the host copy of the held ones; device lists, or host lists after a device problem (no host
+		// copy), on the device against g_idx2 / g_idx3, the flag read back with refresh_values' synchronisation -- when they differ,
+		// the rebuild below overwrites everything the refresh wrote.
+		if (structureReuse && reusable && haveProblem && cfg.reserved[1] != 1 && denseSolve == (linSolver == CUBA_SOLVER_DENSE_CHOLESKY) && same_sizes(p)) {
+			const bool onDevice = dev || !lastIdxOnHost;
+			bool same = onDevice || same_lists(p);
+			if (same) {
+				int rc = refresh_values(p, dev, onDevice, same); if (rc) return rc;
+			}
+			if (same) {
+				if (!lastIdxOnHost && !dev) { keep_lists(p); lastIdxOnHost = true; }
+				structureReuses++;
+				prof[CUBA_PROF_BUILD_STRUCTURE] += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+				return CUBA_OK;
+			}
 		}
 		haveProblem = false;
 		reusable = false;
@@ -567,10 +625,10 @@ struct Engine : EngineBase {
 		jh4MinB = cfg.reserved[2] == 8 ? 5 : (cfg.reserved[2] == 9 ? 6 : 4);
 		// (the bulk copy needs 16-byte multiples: 144-byte fp64 blocks qualify, 72-byte fp32 blocks do not)
 		if (cfg.reserved[2] == 0 && sizeof(T) != 8) { tileSize = 128; jhMinBlocks = 6; }
-		int rc = (cfg.reserved[1] == 1) ? build_on_host(p) : build_on_gpu(p);
+		int rc = (cfg.reserved[1] == 1) ? build_on_host(p) : build_on_gpu(p, dev);
 		if (rc) return rc;
 		tmark("structure built");
-		rc = upload_state(p->q, p->t, p->cam, p->Xw); if (rc) return rc;
+		rc = dev ? pack_state(p->q, p->t, p->cam, p->Xw) : upload_state(p->q, p->t, p->cam, p->Xw); if (rc) return rc;
 		tmark("state uploaded");
 		rc = alloc_system(); if (rc) return rc;
 		CUDA_TRY(cudaStreamSynchronize(stream));
@@ -588,7 +646,9 @@ struct Engine : EngineBase {
 		prof[CUBA_PROF_BUILD_STRUCTURE] += std::chrono::duration<double>(t1 - t0).count();
 		haveProblem = true;
 		if (cfg.reserved[1] != 1 && structureReuse) {
-			lastIdx2.assign(p->idx2, p->idx2 + 2 * (size_t)p->E2); lastIdx3.assign(p->idx3, p->idx3 + 2 * (size_t)p->E3);
+			if (dev) { lastIdx2.clear(); lastIdx3.clear(); }
+			else keep_lists(p);
+			lastIdxOnHost = !dev;
 			const int sz[6] = { p->Pall, p->numP, p->Lall, p->numL, p->E2, p->E3 };
 			memcpy(lastSizes, sz, sizeof(sz));
 			reusable = true;
@@ -596,23 +656,47 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	bool same_topology(const cuba_problem* p) const
+	bool same_sizes(const cuba_problem* p) const
 	{
 		const int sz[6] = { p->Pall, p->numP, p->Lall, p->numL, p->E2, p->E3 };
-		if (memcmp(sz, lastSizes, sizeof(sz)) != 0) return false;
+		return memcmp(sz, lastSizes, sizeof(sz)) == 0;
+	}
+	bool same_lists(const cuba_problem* p) const
+	{
 		if (p->E2 > 0 && memcmp(p->idx2, lastIdx2.data(), sizeof(int32_t) * 2 * (size_t)p->E2) != 0) return false;
 		if (p->E3 > 0 && memcmp(p->idx3, lastIdx3.data(), sizeof(int32_t) * 2 * (size_t)p->E3) != 0) return false;
 		return true;
 	}
+	void keep_lists(const cuba_problem* p)
+	{
+		lastIdx2.assign(p->idx2, p->idx2 + 2 * (size_t)p->E2); lastIdx3.assign(p->idx3, p->idx3 + 2 * (size_t)p->E3);
+	}
 
-	// set_problem on an unchanged topology: measurements, information values and the estimate go up, the edge streams are re-scattered
-	int refresh_values(const cuba_problem* p)
+	// a raw problem array into the engine's buffer: uploaded from the host, or copied from the caller's device array
+	template <typename U>
+	cudaError_t put(DBuf<U>& b, const U* src, size_t n, bool dev) { return dev ? b.copy(src, n, stream) : b.upload(src, n, stream); }
+
+	// set_problem on an unchanged topology: measurements, information values and the estimate go up (or across, dev), the edge streams
+	// are re-scattered.  compare: the lists are first compared with the held ones on the device (host lists go up once for that);
+	// same = false when they differ, and then nothing of the refresh counts (the caller rebuilds).
+	int refresh_values(const cuba_problem* p, bool dev, bool compare, bool& same)
 	{
 		using namespace sgpu;
 		const int E2 = p->E2, E3 = p->E3, eL = S.eLocal;
-		CUDA_TRY(g_meas2.upload(p->meas2, 2 * (size_t)E2, stream)); CUDA_TRY(g_meas3.upload(p->meas3, 3 * (size_t)E3, stream));
-		CUDA_TRY(g_om2.upload(p->omega2, (size_t)E2, stream)); CUDA_TRY(g_om3.upload(p->omega3, (size_t)E3, stream));
-		int rc = upload_state(p->q, p->t, p->cam, p->Xw); if (rc) return rc;
+		if (compare) {
+			const int32_t* i2 = p->idx2;
+			const int32_t* i3 = p->idx3;
+			if (!dev) {
+				CUDA_TRY(cmpIdx2.upload(i2, 2 * (size_t)E2, stream)); CUDA_TRY(cmpIdx3.upload(i3, 2 * (size_t)E3, stream));
+				i2 = cmpIdx2.p; i3 = cmpIdx3.p;
+			}
+			CUDA_TRY(cmpFlag.alloc(1));
+			CUDA_TRY(cudaMemsetAsync(cmpFlag.p, 0, sizeof(int), stream));
+			KLAUNCH(pio::k_idx_differ, 2 * ((long long)E2 + E3), i2, g_idx2.p, 2 * (long long)E2, i3, g_idx3.p, 2 * (long long)E3, cmpFlag.p);
+		}
+		CUDA_TRY(put(g_meas2, p->meas2, 2 * (size_t)E2, dev)); CUDA_TRY(put(g_meas3, p->meas3, 3 * (size_t)E3, dev));
+		CUDA_TRY(put(g_om2, p->omega2, (size_t)E2, dev)); CUDA_TRY(put(g_om3, p->omega3, (size_t)E3, dev));
+		int rc = dev ? pack_state(p->q, p->t, p->cam, p->Xw) : upload_state(p->q, p->t, p->cam, p->Xw); if (rc) return rc;
 		KLAUNCH(k_edge_stream<T>, eL, g_keyS.p, g_valS.p, g_ff.p, g_hplG.p, savedKBeg, eL, S.hplBase, E2, g_meas2.p, g_om2.p, g_meas3.p, g_om3.p,
 			e_user.p, e_ip.p, e_il.p, e_hpl.p, e_mx.p, e_my.p, e_mz.p, e_om.p);
 		KLAUNCH(k_pose_stream<T>, eL, g_psrc.p, posePtr.p, S.numP, eL, e_ip.p, e_il.p, e_mx.p, e_my.p, e_mz.p, e_om.p, p_il.p, p_mx.p, p_my.p, p_mz.p, p_om.p);
@@ -623,7 +707,14 @@ struct Engine : EngineBase {
 					e_mx.p, e_my.p, e_mz.p, e_om.p, e_ip.p, e_il.p, e_hpl.p, w_tile.p, w_rec.p, w_tilePose.p, w_tilePieces.p);
 			}
 		}
+		int differ = 0;
+		if (compare) {
+			g_d2hBytes += (long long)sizeof(differ);
+			CUDA_TRY(cudaMemcpyAsync(&differ, cmpFlag.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
+		}
 		CUDA_TRY(cudaStreamSynchronize(stream));      // the caller's buffers are free again
+		same = differ == 0;
+		if (!same) return CUBA_OK;
 		cur = 0; trialValid = false;
 		forget_solves();
 		resolveProfile();
@@ -676,6 +767,8 @@ struct Engine : EngineBase {
 	bool hostStructureValid = false;
 	// structure reuse across set_problem calls (repeated local BA on an unchanged graph): the last problem's index lists
 	std::vector<int32_t> lastIdx2, lastIdx3;
+	bool lastIdxOnHost = true;    // lastIdx2 / lastIdx3 hold the lists (false after a set_problem_device: g_idx2 / g_idx3 only)
+	DBuf<int> cmpIdx2, cmpIdx3, cmpFlag;   // the device comparison of refresh_values: host lists, "some word differs"
 	int lastSizes[6] = { -1, -1, -1, -1, -1, -1 };
 	int savedKBeg = 0;
 	bool reusable = false;      // the device structures of the last problem are complete and were built on the device
@@ -714,16 +807,16 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	int build_on_gpu(const cuba_problem* p)
+	int build_on_gpu(const cuba_problem* p, bool dev)
 	{
 		using namespace sgpu;
 		S = Structure();
 		const int Pall = p->Pall, numP = p->numP, Lall = p->Lall, numL = p->numL, E2 = p->E2, E3 = p->E3, E = E2 + E3;
 		S.Pall = Pall; S.numP = numP; S.Lall = Lall; S.numL = numL; S.E2 = E2; S.E3 = E3; S.E = E;
-		// raw problem -> device (the only bulk H2D traffic of set_problem besides the state)
-		CUDA_TRY(g_idx2.upload(p->idx2, 2 * (size_t)E2, stream)); CUDA_TRY(g_idx3.upload(p->idx3, 2 * (size_t)E3, stream));
-		CUDA_TRY(g_meas2.upload(p->meas2, 2 * (size_t)E2, stream)); CUDA_TRY(g_meas3.upload(p->meas3, 3 * (size_t)E3, stream));
-		CUDA_TRY(g_om2.upload(p->omega2, (size_t)E2, stream)); CUDA_TRY(g_om3.upload(p->omega3, (size_t)E3, stream));
+		// raw problem -> device (the only bulk H2D traffic of set_problem besides the state; none from device arrays)
+		CUDA_TRY(put(g_idx2, p->idx2, 2 * (size_t)E2, dev)); CUDA_TRY(put(g_idx3, p->idx3, 2 * (size_t)E3, dev));
+		CUDA_TRY(put(g_meas2, p->meas2, 2 * (size_t)E2, dev)); CUDA_TRY(put(g_meas3, p->meas3, 3 * (size_t)E3, dev));
+		CUDA_TRY(put(g_om2, p->omega2, (size_t)E2, dev)); CUDA_TRY(put(g_om3, p->omega3, (size_t)E3, dev));
 		CUDA_TRY(g_meta.alloc(1));
 		CUDA_TRY(cudaMemsetAsync(g_meta.p, 0, sizeof(Meta), stream));
 		// 1. canonical (iL, iP, edge id) order
@@ -963,6 +1056,12 @@ struct Engine : EngineBase {
 		CUDA_TRY(cudaStreamSynchronize(stream));      // the caller's buffers are free again
 		trialValid = false;
 		return CUBA_OK;
+	}
+
+	int set_state_device(const double* q, const double* t, const double* X, cudaStream_t caller) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "set_state before set_problem");
+		return on_caller_stream(caller, [&] { trialValid = false; return pack_state(q, t, nullptr, X); });
 	}
 
 	int reset_state() override
@@ -2127,42 +2226,48 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// The landmarks get_state returns: Xw[cur], or in landmark-sharded runs every rank's own range all-gathered into the trial
+	// buffer, which is free between LM iterations.  (!comm: a CUBA_DRY_SHARD engine returns its own buffer -- its landmarks updated,
+	// the others as uploaded.)
+	int gather_landmarks(const T*& xw)
+	{
+		xw = Xw[cur].p;
+		if (!(world > 1 && comm && S.numL > 0)) return CUBA_OK;
+		// all-gather of the sharded landmarks: every rank broadcasts its own range in place (one grouped NCCL call)
+		T* tmp = Xw[cur ^ 1].p;
+		trialValid = false;
+		CUDA_TRY(cudaMemcpyAsync(tmp, Xw[cur].p, sizeof(T) * 4 * (size_t)S.Lall, cudaMemcpyDeviceToDevice, stream));
+		if (shardBoundValid) {
+			const int dt = sizeof(T) == 8 ? NCCL_FLOAT64 : NCCL_FLOAT32;
+			g_nccl.GroupStart();
+			int rcn = 0;
+			for (int r = 0; r < world; r++) {
+				const int b0 = std::min(shardBound[r], S.numL), b1 = std::min(shardBound[r + 1], S.numL);     // fixed landmarks never change
+				if (b1 > b0) rcn |= g_nccl.Broadcast(tmp + 4 * (size_t)b0, tmp + 4 * (size_t)b0, 4 * (size_t)(b1 - b0), dt, r, comm, stream);
+			}
+			rcn |= g_nccl.GroupEnd();
+			if (rcn != 0) return fail(CUBA_ERR_COMM, "ncclBroadcast (landmark gather) failed");
+		} else {
+			// host-built structure (debug path): zero the foreign entries, sum over ranks
+			CUDA_TRY(cudaMemsetAsync(tmp, 0, sizeof(T) * 4 * (size_t)S.Lall, stream));
+			if (S.lmEnd > S.lmBeg)
+				CUDA_TRY(cudaMemcpyAsync(tmp + 4 * (size_t)S.lmBeg, Xw[cur].p + 4 * (size_t)S.lmBeg, sizeof(T) * 4 * (size_t)(S.lmEnd - S.lmBeg), cudaMemcpyDeviceToDevice, stream));
+			int rc = allreduce(tmp, 4 * (size_t)S.Lall, true); if (rc) return rc;
+		}
+		xw = tmp;
+		return CUBA_OK;
+	}
+
 	int get_state(double* q, double* t, double* X) override
 	{
 		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_state before set_problem");
 		std::vector<T> hp((size_t)S.Pall * 8), hx((size_t)S.Lall * 4);
 		g_d2hBytes += (long long)(sizeof(T) * (hp.size() + hx.size()));
 		CUDA_TRY(cudaMemcpyAsync(hp.data(), pose[cur].p, sizeof(T) * hp.size(), cudaMemcpyDeviceToHost, stream));
-		if (world > 1 && comm && S.numL > 0) {
-			// all-gather of the sharded landmarks: every rank broadcasts its own range in place (one grouped NCCL call).
-			// The trial buffer is free between LM iterations and serves as the gather target.
-			// (!comm: a CUBA_DRY_SHARD engine returns its own buffer -- its landmarks updated, the others as uploaded)
-			T* tmp = Xw[cur ^ 1].p;
-			trialValid = false;
-			CUDA_TRY(cudaMemcpyAsync(tmp, Xw[cur].p, sizeof(T) * 4 * (size_t)S.Lall, cudaMemcpyDeviceToDevice, stream));
-			if (shardBoundValid) {
-				const int dt = sizeof(T) == 8 ? NCCL_FLOAT64 : NCCL_FLOAT32;
-				g_nccl.GroupStart();
-				int rcn = 0;
-				for (int r = 0; r < world; r++) {
-					const int b0 = std::min(shardBound[r], S.numL), b1 = std::min(shardBound[r + 1], S.numL);     // fixed landmarks never change
-					if (b1 > b0) rcn |= g_nccl.Broadcast(tmp + 4 * (size_t)b0, tmp + 4 * (size_t)b0, 4 * (size_t)(b1 - b0), dt, r, comm, stream);
-				}
-				rcn |= g_nccl.GroupEnd();
-				if (rcn != 0) return fail(CUBA_ERR_COMM, "ncclBroadcast (landmark gather) failed");
-			} else {
-				// host-built structure (debug path): zero the foreign entries, sum over ranks
-				CUDA_TRY(cudaMemsetAsync(tmp, 0, sizeof(T) * 4 * (size_t)S.Lall, stream));
-				if (S.lmEnd > S.lmBeg)
-					CUDA_TRY(cudaMemcpyAsync(tmp + 4 * (size_t)S.lmBeg, Xw[cur].p + 4 * (size_t)S.lmBeg, sizeof(T) * 4 * (size_t)(S.lmEnd - S.lmBeg), cudaMemcpyDeviceToDevice, stream));
-				int rc = allreduce(tmp, 4 * (size_t)S.Lall, true); if (rc) return rc;
-			}
-			CUDA_TRY(cudaMemcpyAsync(hx.data(), tmp, sizeof(T) * hx.size(), cudaMemcpyDeviceToHost, stream));
-			CUDA_TRY(cudaStreamSynchronize(stream));
-		} else {
-			CUDA_TRY(cudaMemcpyAsync(hx.data(), Xw[cur].p, sizeof(T) * hx.size(), cudaMemcpyDeviceToHost, stream));
-			CUDA_TRY(cudaStreamSynchronize(stream));
-		}
+		const T* xw = nullptr;
+		int rc = gather_landmarks(xw); if (rc) return rc;
+		CUDA_TRY(cudaMemcpyAsync(hx.data(), xw, sizeof(T) * hx.size(), cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaStreamSynchronize(stream));
 		for (int i = 0; i < S.Pall; i++) {
 			if (q) for (int k = 0; k < 4; k++) q[4 * (size_t)i + k] = (double)hp[8 * (size_t)i + k];
 			if (t) for (int k = 0; k < 3; k++) t[3 * (size_t)i + k] = (double)hp[8 * (size_t)i + 4 + k];
@@ -2170,23 +2275,44 @@ struct Engine : EngineBase {
 		if (X) for (int i = 0; i < S.Lall; i++) for (int k = 0; k < 3; k++) X[3 * (size_t)i + k] = (double)hx[4 * (size_t)i + k];
 		return CUBA_OK;
 	}
-
-	int get_chi2(double* out) override
+	int get_state_device(double* q, double* t, double* X, cudaStream_t caller) override
 	{
-		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_chi2 before set_problem");
-		CUDA_TRY(cudaMemsetAsync(chiSq.p, 0, sizeof(double) * (size_t)std::max(S.E, 1), stream));
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_state before set_problem");
+		return on_caller_stream(caller, [&] {
+			const T* xw = nullptr;
+			int rc = gather_landmarks(xw); if (rc) return rc;
+			KLAUNCH(pio::k_unpack_state<T>, std::max(S.Pall, S.Lall), pose[cur].p, xw, S.Pall, S.Lall, q, t, X);
+			return CUBA_OK;
+		});
+	}
+
+	// per-edge chi2 into out[E] on the device (chiSq, or the caller's array), summed over the ranks of a landmark-sharded run
+	int chi_sqs_into(double* out)
+	{
+		if (S.E > 0) CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(double) * (size_t)S.E, stream));
 		if (S.eLocal > 0) {
 			ChiArgs<T> a = chiArgs(cur);
 			if (lvOn) a.om = e_om0;      // edges at level 1 report omega |r|^2 with the caller's omega
-			k_chi_sqs<T><<<(S.eLocal + 255) / 256, 256, 0, stream>>>(a, e_user, chiSq);
+			k_chi_sqs<T><<<(S.eLocal + 255) / 256, 256, 0, stream>>>(a, e_user, out);
 			launches++;
 			CUDA_TRY(cudaGetLastError());
 		}
-		if (world > 1) { int rc = allreduce(chiSq.p, (size_t)S.E, false); if (rc) return rc; }
+		if (world > 1) { int rc = allreduce(out, (size_t)S.E, false); if (rc) return rc; }
+		return CUBA_OK;
+	}
+	int get_chi2(double* out) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_chi2 before set_problem");
+		int rc = chi_sqs_into(chiSq.p); if (rc) return rc;
 		g_d2hBytes += (long long)(sizeof(double) * (size_t)S.E);
 		CUDA_TRY(cudaMemcpyAsync(out, chiSq.p, sizeof(double) * (size_t)S.E, cudaMemcpyDeviceToHost, stream));
 		CUDA_TRY(cudaStreamSynchronize(stream));
 		return CUBA_OK;
+	}
+	int get_chi2_device(double* out, cudaStream_t caller) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_chi2 before set_problem");
+		return on_caller_stream(caller, [&] { return chi_sqs_into(out); });
 	}
 
 	// ---- edge levels (cuba_levels.cuh) ----------------------------------------------------------------
@@ -2247,6 +2373,32 @@ struct Engine : EngineBase {
 		lvIncluded = included;
 		return CUBA_OK;
 	}
+	// The levels from a device array: normalised and counted on the device; one read-back of the count, which optimize() decides on.
+	// Every rank has the whole array: lvIncluded counts all ranks' edges, a CUBA_DRY_SHARD rank its own (as own_included).
+	int set_edge_levels_device(const uint8_t* levels, cudaStream_t caller) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "set_edge_levels before set_problem");
+		return on_caller_stream(caller, [&] {
+			int rc = levels_init(); if (rc) return rc;
+			const int E = S.E, eL = S.eLocal, n = std::max(E, eL), nb = (n + RED_BLOCK - 1) / RED_BLOCK;
+			CUDA_TRY(lvPartial.alloc(4 * (size_t)std::max(nb, 1))); CUDA_TRY(lvCount.alloc(4));
+			if (n > 0) {
+				pio::k_levels_in<<<nb, RED_BLOCK, 0, stream>>>(levels, E, e_user.p, eL, lvLevel.p, lvPartial.p);
+				launches++;
+				CUDA_TRY(cudaGetLastError());
+			}
+			rc = levels_scatter(); if (rc) return rc;
+			lv::k_sum_counts<<<1, RED_BLOCK, 0, stream>>>(lvPartial.p, n > 0 ? nb : 0, lvCount.p);
+			launches++;
+			CUDA_TRY(cudaGetLastError());
+			double included = 0;
+			g_d2hBytes += (long long)sizeof(included);
+			CUDA_TRY(cudaMemcpyAsync(&included, lvCount.p + (world > 1 && !comm ? 1 : 0), sizeof(included), cudaMemcpyDeviceToHost, stream));
+			CUDA_TRY(cudaStreamSynchronize(stream));
+			lvIncluded = (long long)included;
+			return CUBA_OK;
+		});
+	}
 	// CUBA_DRY_SHARD (no communicator): optimize() and classify_edges see this rank's edges only, so "no edge included" is judged on
 	// them alone, on every path.  One read-back of the shard's edge ids, on this diagnostic path only; -1 when it fails.
 	long long own_included(const unsigned char* h)
@@ -2269,16 +2421,35 @@ struct Engine : EngineBase {
 			g_d2hBytes += (long long)E;
 			return CUBA_OK;
 		}
-		// landmark-sharded: every rank holds its own edges' levels; the per-edge chi2 path collects them
-		CUDA_TRY(cudaMemsetAsync(chiSq.p, 0, sizeof(double) * E, stream));
-		KLAUNCH(lv::k_levels_out, S.eLocal, e_user.p, lvLevel.p, S.eLocal, chiSq.p);
-		int rc = allreduce(chiSq.p, E, false); if (rc) return rc;
+		int rc = collect_levels(); if (rc) return rc;
 		std::vector<double> h(E);
 		g_d2hBytes += (long long)(sizeof(double) * E);
 		CUDA_TRY(cudaMemcpyAsync(h.data(), chiSq.p, sizeof(double) * E, cudaMemcpyDeviceToHost, stream));
 		CUDA_TRY(cudaStreamSynchronize(stream));
 		for (size_t i = 0; i < E; i++) out[i] = h[i] != 0.0;
 		return CUBA_OK;
+	}
+	// landmark-sharded: every rank holds its own edges' levels; the per-edge chi2 path collects them into chiSq (fp64, edge-id order)
+	int collect_levels()
+	{
+		CUDA_TRY(cudaMemsetAsync(chiSq.p, 0, sizeof(double) * (size_t)S.E, stream));
+		KLAUNCH(lv::k_levels_out, S.eLocal, e_user.p, lvLevel.p, S.eLocal, chiSq.p);
+		return allreduce(chiSq.p, (size_t)S.E, false);
+	}
+	int get_edge_levels_device(uint8_t* out, cudaStream_t caller) override
+	{
+		if (!haveProblem) return fail(CUBA_ERR_STATE, "get_edge_levels before set_problem");
+		const size_t E = (size_t)S.E;
+		if (E == 0) return CUBA_OK;
+		return on_caller_stream(caller, [&] {
+			if (!lvOn) CUDA_TRY(cudaMemsetAsync(out, 0, E, stream));
+			else if (world <= 1) CUDA_TRY(cudaMemcpyAsync(out, lvLevel.p, E, cudaMemcpyDeviceToDevice, stream));
+			else {
+				int rc = collect_levels(); if (rc) return rc;
+				KLAUNCH(pio::k_levels_narrow, E, chiSq.p, (int)E, out);
+			}
+			return CUBA_OK;
+		});
 	}
 	int classify_edges(double chi2Mono, double chi2Stereo, int flags, int32_t* counts) override
 	{
@@ -2905,6 +3076,42 @@ int cuba_engine_classify_edges(cuba_engine* e, double chi2_mono, double chi2_ste
 	if (flags & ~(CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE)) return fail(CUBA_ERR_INVALID, "classify_edges: unknown flag");
 	return e->impl->classify_edges(chi2_mono, chi2_stereo, flags, counts);
 }
+// ---- the engine's problem on device-resident arrays: the host entry points' checks and messages, then the work on the engine's
+// stream ordered after `stream`'s (NULL: the engine's stream)
+int cuba_engine_set_problem_device(cuba_engine* e, const cuba_problem* p_dev, void* stream)
+{
+	ENGINE_OR_FAIL(e);
+	return e->impl->set_problem_device(p_dev, (cudaStream_t)stream);
+}
+int cuba_engine_set_state_device(cuba_engine* e, const double* q, const double* t, const double* Xw, void* stream)
+{
+	ENGINE_OR_FAIL(e);
+	if (!q || !t || !Xw) return fail(CUBA_ERR_INVALID, "set_state: null array");
+	return e->impl->set_state_device(q, t, Xw, (cudaStream_t)stream);
+}
+int cuba_engine_get_state_device(cuba_engine* e, double* q, double* t, double* Xw, void* stream)
+{
+	ENGINE_OR_FAIL(e);
+	return e->impl->get_state_device(q, t, Xw, (cudaStream_t)stream);
+}
+int cuba_engine_get_chi2_device(cuba_engine* e, double* per_edge, void* stream)
+{
+	ENGINE_OR_FAIL(e);
+	if (!per_edge) return fail(CUBA_ERR_INVALID, "null out");
+	return e->impl->get_chi2_device(per_edge, (cudaStream_t)stream);
+}
+int cuba_engine_set_edge_levels_device(cuba_engine* e, const uint8_t* levels, void* stream)
+{
+	ENGINE_OR_FAIL(e);
+	return e->impl->set_edge_levels_device(levels, (cudaStream_t)stream);
+}
+int cuba_engine_get_edge_levels_device(cuba_engine* e, uint8_t* levels, void* stream)
+{
+	ENGINE_OR_FAIL(e);
+	if (!levels) return fail(CUBA_ERR_INVALID, "null out");
+	return e->impl->get_edge_levels_device(levels, (cudaStream_t)stream);
+}
+
 // The batches of the batched LM kernels come from outside the program: everything a kernel relies on is checked before any work.
 // A CSR pointer of B problems over `count` items: present, ptr[0] = 0, non-decreasing and ptr[B] = count (so a negative count
 // fails), and every item array present when there are items.

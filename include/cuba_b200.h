@@ -214,6 +214,49 @@ int cuba_engine_get_edge_levels(cuba_engine* e, uint8_t* levels);          /* 0 
 #define CUBA_CLASSIFY_REINCLUDE 2
 int cuba_engine_classify_edges(cuba_engine* e, double chi2_mono, double chi2_stereo, int flags, int32_t* counts);
 
+/* ---- the engine's problem on device-resident data (csrc/cuba_problem_io.cuh) ----
+ * The same calls as set_problem / set_state / get_state / get_chi2 / set_edge_levels / get_edge_levels with every array a DEVICE
+ * pointer on the engine's device (sizes and counts stay host values), for callers that keep their map on the GPU (a torch front end,
+ * a SLAM back end whose pose and Sim3 steps already run on device data).  Each result is bit for bit that of the host entry point of
+ * the same name, in every precision, with either linear solver and every robust kernel.  Each call first makes the engine's stream
+ * wait for the work queued so far on `stream` (an event; NULL = the engine's stream, the legacy default stream is cudaStreamLegacy),
+ * and makes `stream` wait for the call's work; the caller's arrays are read or written in that window.  Each returns CUBA_ERR_STATE
+ * before a problem exists where the host call does, and makes the host call's argument checks with its messages.
+ *
+ * set_problem_device: the problem of cuba_engine_set_problem; returns once it is in place (it reads the builder's counts back, as
+ * set_problem does).  Raw arrays are copied device to device and the state is read in place: no bulk host<->device traffic, only
+ * what set_problem moves besides them (the builder's small read-backs, the block pattern the PCG partition is built from on the host,
+ * and the partition's uploads).  The index checks (an index out of range, an edge with both ends fixed, a free landmark without
+ * edges) fail as in set_problem, and a refused problem leaves the engine as a refused set_problem does.  Structure reuse works
+ * across both calls: a problem whose sizes and (iP, iL) lists equal the held one's only refreshes the values, whichever call gave
+ * either; lists the host cannot memcmp are compared on the device (one kernel).  CUBA_ERR_INVALID, nothing changed, on an engine
+ * with the host structure builder (cuba_config.reserved[1] = 1), which reads host arrays.
+ * set_state_device: q [4*Pall], t [3*Pall], Xw [3*Lall]; one kernel reads them; no synchronisation, no allocation.
+ * get_state_device: as get_state (any pointer may be NULL; fp32 engines widen); one kernel writes them.  Landmark-sharded runs
+ * all-gather the landmarks first, as get_state does.  No host<->device copy, no synchronisation, no allocation.
+ * get_chi2_device: per_edge [E2+E3] as get_chi2 (summed over the ranks of a sharded run).  No copy to the host, no synchronisation.
+ * set_edge_levels_device: levels [E2+E3] as set_edge_levels (NULL = all 0); normalised and counted on the device; synchronises once,
+ * on an 8-byte read-back of the count of included edges that optimize() decides on.
+ * get_edge_levels_device: 0 or 1 per edge into levels [E2+E3].  No copy to the host, no synchronisation.
+ * set_state_device, get_state_device and get_chi2_device never synchronise and, once set_problem has sized the engine, allocate
+ * nothing: they can be captured into a CUDA graph on `stream` (not set_problem_device / set_edge_levels_device, which synchronise).
+ * A graph holds the engine's buffers as they are at capture.  set_state_device writes the initial state and both working buffers,
+ * so a graph of it stays valid until the next set_problem / set_problem_device.  get_state_device and get_chi2_device read the
+ * CURRENT working buffer, which every accepted LM step swaps, and get_chi2_device the omega of the edge levels at capture; in
+ * landmark-sharded runs get_state_device's all-gather also writes the other working buffer.  A graph holding either is therefore
+ * valid only until the next optimize, cuba_stage_update, cuba_stage_commit, set_problem / set_problem_device, set_edge_levels /
+ * set_edge_levels_device or classify_edges: capture it again after those.  Replayed later, it reads the buffer that was current
+ * at capture, which then holds a trial or an older estimate.
+ * cuba_get_transfer_bytes counts what the calls move between host and device: what set_problem counts besides the raw arrays and
+ * the state (the block pattern and the partition's uploads; the builder's small read-backs are counted by neither call), the
+ * 4-byte flag of a structure comparison on the device, and the 8-byte count of set_edge_levels_device. */
+int cuba_engine_set_problem_device(cuba_engine* e, const cuba_problem* p_dev, void* stream);
+int cuba_engine_set_state_device(cuba_engine* e, const double* q, const double* t, const double* Xw, void* stream);
+int cuba_engine_get_state_device(cuba_engine* e, double* q, double* t, double* Xw, void* stream);
+int cuba_engine_get_chi2_device(cuba_engine* e, double* per_edge, void* stream);
+int cuba_engine_set_edge_levels_device(cuba_engine* e, const uint8_t* levels, void* stream);
+int cuba_engine_get_edge_levels_device(cuba_engine* e, uint8_t* levels, void* stream);
+
 /* Pose optimisation of many frames (ORB-SLAM2's Optimizer::PoseOptimization, batched).  A frame is one free SE(3) pose and its
  * edges, each carrying its own world point, which is held fixed.  Host arrays, fp64; the edges of frame b are [ptr2[b], ptr2[b+1])
  * and [ptr3[b], ptr3[b+1]), ptr2[0] = ptr3[0] = 0, ptr2[B] = E2, ptr3[B] = E3.  Array pointers of an empty edge type may be NULL. */
