@@ -93,6 +93,38 @@ static D block_jacobi_dims(D d, int G, int W)
 // sweep on the whole chip above
 static int coarse_kernel(int A) { return A > PCG4_MAXAGG1 ? CUBA_COARSE_KERNEL_DENSE : CUBA_COARSE_KERNEL_INVERT; }
 
+// The J+H and Schur kernels of an engine (stage_choice)
+struct StageChoice {
+	bool jh4 = false;                        // the warp-tile pass k_linearize_landmark4 (cuba_jh4.cuh), fp64 only
+	int jh4Stages = 2, jh4MinB = 4;          // its pipeline stages and CTAs per SM (the grid's, also under mixed precision)
+	int tileSize = LM_TILE, minBlocks = 4;   // first-generation landmark tiles: edges, CTAs per SM (k_backsub runs on them too)
+	bool mixed = false;                      // Hpl in fp32: k_linearize_landmark4<4, 2, 0, true> whatever the shape
+	bool schur5 = false;                     // the tensor-pipe Schur is asked for and the engine can run it (alloc_system: useSchur5)
+};
+// The only reader of cfg.reserved[2] (J+H kernel), reserved[3] (Schur kernel) and use_fp32 == 2; refuses a value that names no kernel.
+// reserved[2]: 0 = k_linearize_landmark4, two stages, 4 CTAs of 4 warps per SM; 7 = three stages; 8 / 9 = 5 / 6 CTAs per SM; 1..4 = the
+// first generation (tileOf x minBOf).  The fp32 engine's default is 128 x 6 first-generation tiles: the warp tiles' bulk copy needs
+// 16-byte multiples, which 144-byte fp64 blocks are and 72-byte fp32 blocks are not.  reserved[3] = 5, the tensor-pipe Schur
+// (cuba_schur5.cuh), is opt-in: 12 % faster than k_schur3 on the banded 5 M-edge graph, on par on kitti00_shaped, 2x slower on the real
+// ba_kitti_00 whose loop closures leave 4.4 products per (tile, destination) segment.
+static int stage_choice(const cuba_config& c, bool fp64, StageChoice& s)
+{
+	const int r2 = c.reserved[2], r3 = c.reserved[3];
+	if (r2 < 0 || r2 == 5 || r2 == 6 || r2 > 9)
+		return fail(CUBA_ERR_INVALID, "create: reserved[2] = " + std::to_string(r2) + " names no J+H kernel (0..4, 7..9)");
+	if (r3 != 0 && r3 != 3 && r3 != 5)
+		return fail(CUBA_ERR_INVALID, "create: reserved[3] = " + std::to_string(r3) + " names no Schur kernel (0, 3, 5)");
+	static const int tileOf[10] = { LM_TILE, 256, 256, 128, 128, 0, 0, LM_TILE, LM_TILE, LM_TILE }, minBOf[10] = { 4, 2, 3, 4, 6, 0, 0, 4, 4, 4 };
+	s.jh4 = (r2 == 0 || r2 >= 7) && fp64;
+	s.jh4Stages = r2 == 7 ? 3 : 2;
+	s.jh4MinB = r2 == 8 ? 5 : (r2 == 9 ? 6 : 4);
+	s.tileSize = r2 == 0 && !fp64 ? 128 : tileOf[r2];
+	s.minBlocks = r2 == 0 && !fp64 ? 6 : minBOf[r2];
+	s.mixed = c.use_fp32 == 2 && s.jh4;
+	s.schur5 = r3 == 5 && c.reserved[1] != 1 && c.use_fp32 != 2 && fp64;
+	return CUBA_OK;
+}
+
 #define CUDA_TRY(expr)                                                                                      \
 	do {                                                                                                    \
 		cudaError_t _e = (expr);                                                                            \
@@ -346,30 +378,27 @@ struct Engine : EngineBase {
 	int numSMs = 0;
 	int smemMax = 0;        // opt-in dynamic shared memory of one CTA
 	int ntiles = 0, nPoseBlocks = 0, nChiBlocks = 0;
-	int tileSize = TILE;    // 256 or 128, from cfg.reserved[2]
-	int jhMinBlocks = 2;
-	int nChiLin = 0;
-	// warp-tile J+H landmark pass (cuba_jh4.cuh)
-	bool jhV4 = true;
-	int ntW = 0, jh4Grid = 0, jh4HasBig = 0, jh4MinB = 4, jh4Nst = 2;
-	const void* jh4AttrSet = nullptr;
-	int* jh4Host = nullptr;      // pinned: {number of warp tiles, any cut landmark}
-	bool jh4Pending = false;
-	DBuf<int> w_levels, w_start, w_pieces, w_base, w_tilePose, w_tilePieces, w_pieceCount, w_flag;
-	DBuf<jh4::WTile> w_tile;
-	DBuf<jh4::Rec> w_rec;
-	DBuf<double> w_bigPartial;
-	// landmark-tile Schur complement on the tensor pipe (cuba_schur5.cuh), fp64 only; k_schur3 (cuba_schur3.cuh) otherwise
-	bool useSchur5 = false;
-	int s5Ntiles = 0;
-	DBuf<int> s5TileLm;
-	DBuf<TileInfo> s5TileInfo;
-	DBuf<int4> s5SegRec;
-	DBuf<unsigned int> s5Off;
-	DBuf<unsigned long long> s5_key, s5_keyS, s5_key3, s5_key3S;
-	DBuf<int> s5_val, s5_valS, s5_head, s5_segId, s5_segStart, s5_segTile, s5_segDest, s5_val3, s5_val3S, s5_segRank, s5_rankDest, s5_tileSegPtr, s5_destSegPtr, s5_p2i, s5_p2j;
-	DBuf<schur5::Counts> s5_counts;
-	DBuf<T> s5_partial;
+	StageChoice stages;     // of cfg (init)
+	// The warp-tile J+H pass of a structure (setup_jh4, setup_jh4_finish), and its kernel of the choice (init sets the attribute once)
+	struct Jh4Run {
+		int ntiles = 0, grid = 0; const void* fn = nullptr; size_t smem = 0;
+		int* host = nullptr;         // pinned: {number of warp tiles, any cut landmark}
+		bool pending = false;        // setup_jh4 queued the read-back of `host`
+		DBuf<int> levels, start, pieces, base, tilePose, tilePieces, pieceCount, flag;
+		DBuf<jh4::WTile> tile; DBuf<jh4::Rec> rec; DBuf<double> bigPartial;
+	};
+	Jh4Run wt;
+	// The landmark-tile Schur complement on the tensor pipe of a structure (setup_schur5)
+	struct Schur5Run {
+		int ntiles = 0;
+		DBuf<TileInfo> tileInfo; DBuf<int4> segRec; DBuf<unsigned int> off;
+		DBuf<unsigned long long> key, keyS, key3, key3S;
+		DBuf<int> tileLm, val, valS, head, segId, segStart, segTile, segDest, val3, val3S, segRank, rankDest, tileSegPtr, destSegPtr, p2i, p2j;
+		DBuf<schur5::Counts> counts;
+		DBuf<T> partial;
+	};
+	Schur5Run s5;
+	bool useSchur5 = false;   // this structure's Schur runs on the tensor pipe; k_schur3 (cuba_schur3.cuh) otherwise
 	int cur = 0;            // current state buffer
 	bool trialValid = false;
 	// state
@@ -381,8 +410,7 @@ struct Engine : EngineBase {
 	// system
 	DBuf<T> Hpp, bp, Hll, bl, Hpl, invHll, fVal, bsc, xp, xl;
 	DBuf<T> uVal;            // landmark-sharded runs: upper Hsc blocks | bsc, the buffer of the per-trial all-reduce
-	DBuf<float> HplF;        // mixed precision (cfg.use_fp32 == 2, fp64 engine): the Hpl blocks in fp32, 20 floats per block
-	bool mixed = false;
+	DBuf<float> HplF;        // mixed precision (stages.mixed): the Hpl blocks in fp32, 20 floats per block
 	bool upperReduce = false;   // k_schur3 writes the upper blocks into uVal; one all-reduce of uVal | bsc, then k_expand_upper
 	DBuf<int> prodPtr, prodI, prodJ, prodL, blkRow, blkCol, u2f, u2fT, fRowPtr, fColInd;
 	// One block-Jacobi solve set up on the device (setup_pcg3): the row partition's lists, L^-1, the eight vectors, the partial board
@@ -445,7 +473,7 @@ struct Engine : EngineBase {
 		if (joinOut) cudaEventDestroy(joinOut);
 		if (hScal) cudaFreeHost(hScal);
 		if (hMeta) cudaFreeHost(hMeta);
-		if (jh4Host) cudaFreeHost(jh4Host);
+		if (wt.host) cudaFreeHost(wt.host);
 		if (stream) cudaStreamDestroy(stream);
 		if (comm && g_nccl.CommDestroy) g_nccl.CommDestroy(comm);
 	}
@@ -471,6 +499,17 @@ struct Engine : EngineBase {
 		CUDA_TRY(gridBar.alloc(1)); CUDA_TRY(cudaMemsetAsync(gridBar.p, 0, sizeof(GridBar), stream));
 		// for every coarse matrix k_coarse_invert takes (launch_coarse_setup), whichever solver it belongs to
 		CUDA_TRY(cudaFuncSetAttribute(k_coarse_invert<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coarse_invert_smem(PCG4_MAXAGG1)));
+		int rc = stage_choice(cfg, sizeof(T) == 8, stages); if (rc) return rc;
+		if (stages.jh4) {
+			const void*& fn = wt.fn; size_t& smem = wt.smem;
+#define JH4_PICK(MB, NS, ...) { fn = (const void*)jh4::k_linearize_landmark4<MB, NS, __VA_ARGS__>; smem = (size_t)NS * jh4::WARPS * sizeof(jh4::StageOf<MB, NS>); }
+			if (stages.mixed) JH4_PICK(4, 2, 0, true)
+			else if (stages.jh4Stages == 3) JH4_PICK(4, 3, 0)
+			else if (stages.jh4MinB == 4) JH4_PICK(4, 2, 0)
+			else if (stages.jh4MinB == 5) JH4_PICK(5, 2, 0)
+			else JH4_PICK(6, 2, 0)
+			CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+		}
 		return CUBA_OK;
 	}
 
@@ -610,21 +649,6 @@ struct Engine : EngineBase {
 		reusable = false;
 		hostStructureValid = false;
 		shardBoundValid = false;
-		// landmark-tile shape of the first-generation kernel: 1 = 256 edges, 2 CTAs/SM; 2 = 256, 3 CTAs/SM; 3 = 128, 4 CTAs/SM;
-		// 4 = 128, 6 CTAs/SM; otherwise LM_TILE edges, 4 CTAs/SM
-		switch (cfg.reserved[2]) {
-		case 2: tileSize = 256; jhMinBlocks = 3; break;
-		case 3: tileSize = 128; jhMinBlocks = 4; break;
-		case 4: tileSize = 128; jhMinBlocks = 6; break;
-		case 1: tileSize = 256; jhMinBlocks = 2; break;
-		default: tileSize = LM_TILE; jhMinBlocks = 4; break;
-		}
-		// k_linearize_landmark4: 0 = two-stage pipeline, 4 CTAs of 4 warps per SM (default); 8/9 = 5/6 CTAs per SM; 7 = three stages
-		jhV4 = (cfg.reserved[2] == 0 || (cfg.reserved[2] >= 7 && cfg.reserved[2] <= 9)) && sizeof(T) == 8;
-		jh4Nst = cfg.reserved[2] == 7 ? 3 : 2;
-		jh4MinB = cfg.reserved[2] == 8 ? 5 : (cfg.reserved[2] == 9 ? 6 : 4);
-		// (the bulk copy needs 16-byte multiples: 144-byte fp64 blocks qualify, 72-byte fp32 blocks do not)
-		if (cfg.reserved[2] == 0 && sizeof(T) != 8) { tileSize = 128; jhMinBlocks = 6; }
 		int rc = (cfg.reserved[1] == 1) ? build_on_host(p) : build_on_gpu(p, dev);
 		if (rc) return rc;
 		tmark("structure built");
@@ -700,13 +724,7 @@ struct Engine : EngineBase {
 		KLAUNCH(k_edge_stream<T>, eL, g_keyS.p, g_valS.p, g_ff.p, g_hplG.p, savedKBeg, eL, S.hplBase, E2, g_meas2.p, g_om2.p, g_meas3.p, g_om3.p,
 			e_user.p, e_ip.p, e_il.p, e_hpl.p, e_mx.p, e_my.p, e_mz.p, e_om.p);
 		KLAUNCH(k_pose_stream<T>, eL, g_psrc.p, posePtr.p, S.numP, eL, e_ip.p, e_il.p, e_mx.p, e_my.p, e_mz.p, e_om.p, p_il.p, p_mx.p, p_my.p, p_mz.p, p_om.p);
-		if constexpr (sizeof(T) == 8) {
-			if (jhV4 && ntW > 0) {
-				const int lb = S.lmBeg, N = S.lmEnd - S.lmBeg;
-				KLAUNCH(jh4::k_emit, (long long)N * 32, w_start.p, w_pieces.p, w_base.p, N, lmPtr.p, lb, w_levels.p,
-					e_mx.p, e_my.p, e_mz.p, e_om.p, e_ip.p, e_il.p, e_hpl.p, w_tile.p, w_rec.p, w_tilePose.p, w_tilePieces.p);
-			}
-		}
+		rc = jh4_emit(); if (rc) return rc;
 		int differ = 0;
 		if (compare) {
 			g_d2hBytes += (long long)sizeof(differ);
@@ -726,7 +744,7 @@ struct Engine : EngineBase {
 	int build_on_host(const cuba_problem* p)
 	{
 		const char* err = "";
-		if (!build_structure(p->Pall, p->numP, p->Lall, p->numL, p->E2, p->idx2, p->E3, p->idx3, rank, world, tileSize, S, &err))
+		if (!build_structure(p->Pall, p->numP, p->Lall, p->numL, p->E2, p->idx2, p->E3, p->idx3, rank, world, stages.tileSize, S, &err))
 			return fail(CUBA_ERR_INVALID, err);
 		hostStructureValid = true;
 		const int eL = S.eLocal;
@@ -858,7 +876,7 @@ struct Engine : EngineBase {
 		KLAUNCH(k_tile_ptr, numL + 2, lmPtr.p, numL, eL, tilePtr.p);
 		const int tb = std::min(S.lmBeg, numL), te = std::min(S.lmEnd, numL) + (S.lmEnd > numL ? 1 : 0);
 		// windows a little shorter than the CTA so that the tail of a tile's last landmark usually still fits one chunk
-		const int window = tileSize - 16;
+		const int window = stages.tileSize - 16;
 		const int nt = (eL + window - 1) / window;
 		CUDA_TRY(tileLm.alloc((size_t)nt + 1));
 		KLAUNCH(k_tiles, nt + 1, tilePtr.p, tb, te, window, nt, tileLm.p);
@@ -970,20 +988,14 @@ struct Engine : EngineBase {
 		// Hpp | bp | (chi2 slot) and Hsc | bsc are single allocations: one collective each in landmark-sharded runs
 		CUDA_TRY(Hpp.alloc(42 * nP + 2)); bp.alias(Hpp.p + 36 * nP, 6 * nP);
 		CUDA_TRY(Hll.alloc(9 * nL)); CUDA_TRY(bl.alloc(3 * nL));
-		mixed = cfg.use_fp32 == 2 && sizeof(T) == 8 && jhV4;
-		if (mixed) { CUDA_TRY(HplF.alloc(20 * (size_t)std::max(S.nhplLocal, 1))); CUDA_TRY(Hpl.alloc(1)); }
+		if (stages.mixed) { CUDA_TRY(HplF.alloc(20 * (size_t)std::max(S.nhplLocal, 1))); CUDA_TRY(Hpl.alloc(1)); }
 		else CUDA_TRY(Hpl.alloc(18 * (size_t)S.nhplLocal));
 		CUDA_TRY(invHll.alloc(9 * nL));
 		CUDA_TRY(fVal.alloc(36 * (size_t)S.nfull + 6 * nP)); bsc.alias(fVal.p + 36 * (size_t)S.nfull, 6 * nP);
-		// Schur kernel: 0 / 3 = k_schur3 (destination-sorted products, six lanes per product; default), 5 = landmark tiles on the fp64
-		// tensor pipe (k_schur_tiles_mma + k_schur_reduce, cuba_schur5.cuh: 12 % faster on the banded 5 M-edge graph, on par on
-		// kitti00_shaped, 2x slower on the real ba_kitti_00 whose loop closures leave 4.4 products per (tile, destination) segment ->
-		// opt-in).  A request for 5 that schur5 cannot serve (host-built structure, fp32 or mixed precision, no products on this rank,
-		// a repeated (pose, landmark) pair anywhere in the graph: its bsc term rides on every product of a diagonal destination)
-		// runs k_schur3.  upperReduce depends on the request only, so that every rank of a sharded run joins the same collective.
-		const bool schur5Asked = cfg.reserved[3] == 5 && cfg.reserved[1] != 1 && cfg.use_fp32 != 2 && sizeof(T) == 8;
-		useSchur5 = schur5Asked && S.numP > 0 && S.numL > 0 && ntiles > 0 && S.eLocal > 0 && S.nmulLocal > 0 && !S.repeatedPairs;
-		upperReduce = world > 1 && !schur5Asked && S.numP > 0 && S.numL > 0;
+		// k_schur3 serves a tensor-pipe request the structure cannot (no products on this rank; a repeated (pose, landmark) pair: its bsc
+		// term rides on every product of a diagonal destination).  upperReduce follows the request, so every rank joins one collective.
+		useSchur5 = stages.schur5 && S.numP > 0 && S.numL > 0 && ntiles > 0 && S.eLocal > 0 && S.nmulLocal > 0 && !S.repeatedPairs;
+		upperReduce = world > 1 && !stages.schur5 && S.numP > 0 && S.numL > 0;
 		if (upperReduce) {
 			uCount = 36 * (size_t)S.nblk + 6 * nP;
 			const size_t need = peer_signal_offset(uCount) + 64;          // + the signal block of the peer all-reduce
@@ -1014,13 +1026,13 @@ struct Engine : EngineBase {
 		if (nP) CUDA_TRY(cudaMemsetAsync(xp.p, 0, sizeof(T) * 6 * nP, stream));
 		if (nP) CUDA_TRY(cudaMemsetAsync(Hpp.p, 0, sizeof(T) * 36 * nP, stream));
 		if (nP) CUDA_TRY(cudaMemsetAsync(bp.p, 0, sizeof(T) * 6 * nP, stream));
-		if (!useSchur5 && S.nmulLocal > 0) {
+		if (useSchur5) { int rc = setup_schur5(); if (rc) return rc; }
+		else if (S.nmulLocal > 0) {
 			CUDA_TRY(prodL.alloc((size_t)S.nmulLocal));
 			KLAUNCH(schur3::k_prod_landmark, S.nmulLocal, prodI.p, hplLm.p, (int)S.nmulLocal, prodL.p);
 		}
-		if (useSchur5) { int rc = setup_schur5(); if (rc) return rc; }
 		tmark("alloc + Schur setup queued");
-		if (jhV4) { int rc = setup_jh4(); if (rc) return rc; }
+		if (stages.jh4) { int rc = setup_jh4(); if (rc) return rc; }
 		tmark("jh4 queued");
 		// the solver's setup: no PCG partition or plan for the direct solver (its need lists may not fit, and nothing reads them)
 		denseSolve = linSolver == CUBA_SOLVER_DENSE_CHOLESKY;
@@ -1037,12 +1049,11 @@ struct Engine : EngineBase {
 			if (S.numP > 0 && S.numL > 0 && pick.p5) { int rc = setup_pcg5(); if (rc) return rc; }
 		}
 		tmark("pcg partition (host)");
-		if (jhV4) { int rc = setup_jh4_finish(); if (rc) return rc; }
+		if (stages.jh4) { int rc = setup_jh4_finish(); if (rc) return rc; }
 		tmark("jh4 finish");
-		nChiLin = jhV4 ? jh4Grid : ntiles;
 		nPoseBlocks = (S.numP + RED_BLOCK - 1) / RED_BLOCK;
 		nChiBlocks = std::max(1, std::min((eL + RED_BLOCK - 1) / RED_BLOCK, numSMs * 8));
-		CUDA_TRY(chiPartial.alloc((size_t)std::max(std::max(ntiles, nChiBlocks), jh4Grid) + 1));
+		CUDA_TRY(chiPartial.alloc((size_t)std::max(std::max(ntiles, nChiBlocks), wt.grid) + 1));
 		CUDA_TRY(scalePartialL.alloc((size_t)std::max(ntiles, (S.numL + RED_BLOCK - 1) / RED_BLOCK) + 1));
 		CUDA_TRY(scalePartialP.alloc((size_t)nPoseBlocks + 1));
 		CUDA_TRY(chiSq.alloc((size_t)S.E));
@@ -1106,68 +1117,67 @@ struct Engine : EngineBase {
 	int launch_linearize_landmark()
 	{
 		if (ntiles <= 0) return CUBA_OK;
+		if (stages.jh4) return launch_jh4();
 		LinLmArgs<T> a;
 		a.pose = pose[cur]; a.cam = cam; a.Xw = Xw[cur];
 		a.mx = e_mx; a.my = e_my; a.mz = e_mz; a.om = e_om; a.ip = e_ip; a.il = e_il; a.hpl = e_hpl;
 		a.lmPtr = tilePtr; a.tileLm = tileLm; a.numP = S.numP; a.numL = S.numL;
 		a.Hpl = Hpl; a.Hll = Hll; a.bl = bl; a.chiPartial = chiPartial; a.rk = rkParams();
-		if (jhV4) {
-			if constexpr (sizeof(T) == 8) {
-				if (ntW <= 0) return CUBA_OK;
-				jh4::Args b;
-				b.pose = pose[cur]; b.cam = cam; b.Xw = Xw[cur];
-				b.rec = w_rec; b.tile = w_tile; b.tilePose = w_tilePose; b.tilePieces = w_tilePieces; b.pieceCount = w_pieceCount; b.ntiles = ntW; b.numL = S.numL;
-				b.Hpl = Hpl; b.HplF = mixed ? HplF.p : nullptr; b.Hll = Hll; b.bl = bl; b.bigPartial = w_bigPartial; b.chiPartial = chiPartial; b.rk = rkParams();
-				const void* fn = nullptr; size_t smem = 0;
-#define JH4_PICK(MB, NS, DB) { fn = (const void*)jh4::k_linearize_landmark4<MB, NS, DB>; smem = (size_t)NS * jh4::WARPS * sizeof(jh4::StageOf<MB, NS>); }
-				int dbg = 0;
-#ifdef CUBA_JH4_DEBUG
-				dbg = getenv("CUBA_JH4_DBG") ? atoi(getenv("CUBA_JH4_DBG")) : 0;
-				if (jh4Nst == 3) { switch (dbg) { case 1: JH4_PICK(4, 3, 1) break; case 2: JH4_PICK(4, 3, 2) break; case 4: JH4_PICK(4, 3, 4) break; case 6: JH4_PICK(4, 3, 6) break;
-					case 7: JH4_PICK(4, 3, 7) break; case 8: JH4_PICK(4, 3, 8) break; case 15: JH4_PICK(4, 3, 15) break; default: dbg = 0; } }
-				else { switch (dbg) { case 8: JH4_PICK(5, 2, 8) break; case 7: JH4_PICK(5, 2, 7) break; default: dbg = 0; } }
-#endif
-				if (mixed) { fn = (const void*)jh4::k_linearize_landmark4<4, 2, 0, true>; smem = (size_t)2 * jh4::WARPS * sizeof(jh4::StageOf<4, 2>); }
-				if (!fn) {
-					if (jh4Nst == 3) JH4_PICK(4, 3, 0)
-					else if (jh4MinB == 4) JH4_PICK(4, 2, 0)
-					else if (jh4MinB == 5) JH4_PICK(5, 2, 0)
-					else JH4_PICK(6, 2, 0)
-				}
-				if (fn != jh4AttrSet) { CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); jh4AttrSet = fn; }   // once per kernel, not per launch
-				void* kargs[] = { (void*)&b };
-				CUDA_TRY(cudaLaunchKernel(fn, dim3(jh4Grid), dim3(jh4::WARPS * 32), kargs, smem, stream));
-#ifdef CUBA_JH4_DEBUG
-				if (dbg & 8) {
-					const int nw = jh4Grid * jh4::WARPS;
-					std::vector<double> h(11 * (size_t)nw);
-					cudaMemcpyAsync(h.data(), w_bigPartial.p, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, stream);
-					cudaStreamSynchronize(stream);
-					double acc[8] = { 0 };
-					for (int w = 0; w < nw; w++) for (int i = 0; i < 8; i++) acc[i] += h[8 * (size_t)w + i];
-					static int once = 0;
-					if (once++ == 3) {
-						const char* nm[8] = { "cpasync_wait", "mbar_wait", "lds_inputs", "math+hpl_staging", "fence+bulk_store", "wait_read+issue", "reduce+stores", "rotate(descr)" };
-						double tot = 0; for (int i = 0; i < 8; i++) tot += acc[i];
-						for (int i = 0; i < 8; i++) fprintf(stderr, "jh4 phase %-18s %9.0f cycles/warp  %5.1f %%\n", nm[i], acc[i] / nw, 100 * acc[i] / tot);
-						fprintf(stderr, "jh4 total %9.0f cycles/warp, %d warps, %d tiles\n", tot / nw, nw, ntW);
-						double s0 = 1e300, s1 = 0, l0 = 1e300, l1 = 0, e0 = 1e300, e1 = 0;
-						for (int w = 0; w < nw; w++) {
-							const double* g = h.data() + 8 * (size_t)nw + 3 * (size_t)w;
-							s0 = std::min(s0, g[0]); s1 = std::max(s1, g[0]); l0 = std::min(l0, g[1]); l1 = std::max(l1, g[1]); e0 = std::min(e0, g[2]); e1 = std::max(e1, g[2]);
-						}
-						fprintf(stderr, "jh4 globaltimer (ns, rel. first start): start %.0f..%.0f  loop entry %.0f..%.0f  loop exit %.0f..%.0f\n", 0.0, s1 - s0, l0 - s0, l1 - s0, e0 - s0, e1 - s0);
-					}
-				}
-#endif
-			}
-		}
-		else if (tileSize == 128 && jhMinBlocks >= 6) k_linearize_landmark<T, 128, 6><<<ntiles, 128, 0, stream>>>(a);
-		else if (tileSize == 128) k_linearize_landmark<T, 128, 4><<<ntiles, 128, 0, stream>>>(a);
-		else if (jhMinBlocks >= 3) k_linearize_landmark<T, 256, 3><<<ntiles, 256, 0, stream>>>(a);
+		if (stages.tileSize == 128 && stages.minBlocks >= 6) k_linearize_landmark<T, 128, 6><<<ntiles, 128, 0, stream>>>(a);
+		else if (stages.tileSize == 128) k_linearize_landmark<T, 128, 4><<<ntiles, 128, 0, stream>>>(a);
+		else if (stages.minBlocks >= 3) k_linearize_landmark<T, 256, 3><<<ntiles, 256, 0, stream>>>(a);
 		else k_linearize_landmark<T, 256, 2><<<ntiles, 256, 0, stream>>>(a);
 		launches++;
 		CUDA_TRY(cudaGetLastError());
+		return CUBA_OK;
+	}
+	// The warp-tile pass over wt.  -DCUBA_JH4_DEBUG (tools/jh4_dbg.sh): CUBA_JH4_DBG launches an instrumented instance of the shape
+	// instead of wt.fn, except under mixed precision; with bit 3 the phase counters of the fourth launch go to stderr.
+	int launch_jh4()
+	{
+		if constexpr (sizeof(T) == 8) {
+			if (wt.ntiles <= 0) return CUBA_OK;
+			jh4::Args b;
+			b.pose = pose[cur]; b.cam = cam; b.Xw = Xw[cur];
+			b.rec = wt.rec; b.tile = wt.tile; b.tilePose = wt.tilePose; b.tilePieces = wt.tilePieces; b.pieceCount = wt.pieceCount; b.ntiles = wt.ntiles; b.numL = S.numL;
+			b.Hpl = Hpl; b.HplF = stages.mixed ? HplF.p : nullptr; b.Hll = Hll; b.bl = bl; b.bigPartial = wt.bigPartial; b.chiPartial = chiPartial; b.rk = rkParams();
+			const void* fn = wt.fn; size_t smem = wt.smem;
+#ifdef CUBA_JH4_DEBUG
+			int dbg = getenv("CUBA_JH4_DBG") ? atoi(getenv("CUBA_JH4_DBG")) : 0;
+			if (stages.jh4Stages == 3) { switch (dbg) { case 1: JH4_PICK(4, 3, 1) break; case 2: JH4_PICK(4, 3, 2) break; case 4: JH4_PICK(4, 3, 4) break; case 6: JH4_PICK(4, 3, 6) break;
+				case 7: JH4_PICK(4, 3, 7) break; case 8: JH4_PICK(4, 3, 8) break; case 15: JH4_PICK(4, 3, 15) break; default: dbg = 0; } }
+			else { switch (dbg) { case 8: JH4_PICK(5, 2, 8) break; case 7: JH4_PICK(5, 2, 7) break; default: dbg = 0; } }
+			if (stages.mixed) { fn = wt.fn; smem = wt.smem; }
+			if (fn != wt.fn) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+#endif
+			void* kargs[] = { (void*)&b };
+			CUDA_TRY(cudaLaunchKernel(fn, dim3(wt.grid), dim3(jh4::WARPS * 32), kargs, smem, stream));
+#ifdef CUBA_JH4_DEBUG
+			if (dbg & 8) {
+				const int nw = wt.grid * jh4::WARPS;
+				std::vector<double> h(11 * (size_t)nw);
+				cudaMemcpyAsync(h.data(), wt.bigPartial.p, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, stream);
+				cudaStreamSynchronize(stream);
+				double acc[8] = { 0 };
+				for (int w = 0; w < nw; w++) for (int i = 0; i < 8; i++) acc[i] += h[8 * (size_t)w + i];
+				static int once = 0;
+				if (once++ == 3) {
+					const char* nm[8] = { "cpasync_wait", "mbar_wait", "lds_inputs", "math+hpl_staging", "fence+bulk_store", "wait_read+issue", "reduce+stores", "rotate(descr)" };
+					double tot = 0; for (int i = 0; i < 8; i++) tot += acc[i];
+					for (int i = 0; i < 8; i++) fprintf(stderr, "jh4 phase %-18s %9.0f cycles/warp  %5.1f %%\n", nm[i], acc[i] / nw, 100 * acc[i] / tot);
+					fprintf(stderr, "jh4 total %9.0f cycles/warp, %d warps, %d tiles\n", tot / nw, nw, wt.ntiles);
+					double s0 = 1e300, s1 = 0, l0 = 1e300, l1 = 0, e0 = 1e300, e1 = 0;
+					for (int w = 0; w < nw; w++) {
+						const double* g = h.data() + 8 * (size_t)nw + 3 * (size_t)w;
+						s0 = std::min(s0, g[0]); s1 = std::max(s1, g[0]); l0 = std::min(l0, g[1]); l1 = std::max(l1, g[1]); e0 = std::min(e0, g[2]); e1 = std::max(e1, g[2]);
+					}
+					fprintf(stderr, "jh4 globaltimer (ns, rel. first start): start %.0f..%.0f  loop entry %.0f..%.0f  loop exit %.0f..%.0f\n", 0.0, s1 - s0, l0 - s0, l1 - s0, e0 - s0, e1 - s0);
+				}
+			}
+#endif
+			launches++;
+			CUDA_TRY(cudaGetLastError());
+		}
 		return CUBA_OK;
 	}
 	int launch_linearize_pose()
@@ -1205,7 +1215,7 @@ struct Engine : EngineBase {
 			ProfScope ps(this, CUBA_PROF_BUILD_SYSTEM);
 			int rc = launch_linearize_landmark(); if (rc) return rc;
 			rc = launch_linearize_pose(); if (rc) return rc;
-			rc = launch_sum(chiPartial, ntiles > 0 ? nChiLin : 0, nullptr, 0, nullptr, 0, 0); if (rc) return rc;
+			rc = launch_sum(chiPartial, ntiles <= 0 ? 0 : stages.jh4 ? wt.grid : ntiles, nullptr, 0, nullptr, 0, 0); if (rc) return rc;
 			if (world > 1) {
 				// ONE collective: Hpp | bp | chi2 are contiguous (the chi2 partial rides in the slot behind bp)
 				if constexpr (sizeof(T) == 8) {
@@ -1271,27 +1281,7 @@ struct Engine : EngineBase {
 	int launch_schur(T lambda)
 	{
 		ProfScope ps(this, CUBA_PROF_SCHUR_COMPLEMENT);
-		if (useSchur5) {
-			if constexpr (sizeof(T) == 8) {
-				schur5::Args sa;
-				sa.Hpl = Hpl; sa.Hll = Hll; sa.bl = bl; sa.info = s5TileInfo; sa.hplLm = hplLm; sa.tileSegPtr = s5_tileSegPtr; sa.segRec = s5SegRec; sa.off = s5Off;
-				sa.p2i = s5_p2i; sa.p2j = s5_p2j; sa.numL = S.numL; sa.lambda = lambda; sa.invHll = invHll; sa.partial = s5_partial;
-				schur5::k_schur_tiles_mma<<<s5Ntiles, schur5::WARPS * 32, sizeof(schur5::Smem), stream>>>(sa);
-				launches++;
-				CUDA_TRY(cudaGetLastError());
-				schur5::ReduceArgs<T> ra;
-				ra.partial = s5_partial; ra.destSegPtr = s5_destSegPtr; ra.Hpp = Hpp; ra.bp = bp;
-				ra.blkRow = blkRow; ra.blkCol = blkCol; ra.u2f = u2f; ra.u2fT = u2fT; ra.nblk = S.nblk; ra.lambda = lambda;
-				ra.addDiag = rank == 0 ? 1 : 0; ra.fVal = fVal; ra.bsc = bsc;
-				schur5::k_schur_reduce<T><<<(S.nblk + 3) / 4, 128, 0, stream>>>(ra);
-				launches++;
-				CUDA_TRY(cudaGetLastError());
-				if (world > 1) {
-					int rc = allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true); if (rc) return rc;   // Hsc | bsc: one buffer
-				}
-			}
-			return CUBA_OK;
-		}
+		if (useSchur5) return launch_schur5(lambda);
 		{
 			// the inverses of this rank's landmarks only (nobody reads the others here)
 			const int l0 = std::min(S.lmBeg, S.numL), l1 = std::min(S.lmEnd, S.numL);
@@ -1302,28 +1292,13 @@ struct Engine : EngineBase {
 			}
 		}
 		if (S.numP > 0 && S.numL > 0) {
-			schur3::Args<T> a;
-			a.Hpl = Hpl; a.invHll = invHll; a.bl = bl; a.Hpp = Hpp; a.bp = bp;
-			a.prodPtr = prodPtr; a.prodI = prodI; a.prodJ = prodJ; a.prodL = prodL;
-			a.blkRow = blkRow; a.blkCol = blkCol; a.u2f = u2f; a.u2fT = u2fT; a.nblk = S.nblk;
-			a.lambda = lambda; a.addDiag = rank == 0 ? 1 : 0; a.fVal = fVal; a.bsc = bsc; a.uVal = upperReduce ? uVal.p : nullptr;
-			if (mixed) {
-				if constexpr (sizeof(T) == 8) {
-					schur3::Args<double, float> m;
-					m.Hpl = HplF; m.invHll = invHll; m.bl = bl; m.Hpp = Hpp; m.bp = bp; m.prodPtr = prodPtr; m.prodI = prodI; m.prodJ = prodJ; m.prodL = prodL;
-					m.blkRow = blkRow; m.blkCol = blkCol; m.u2f = u2f; m.u2fT = u2fT; m.nblk = S.nblk; m.lambda = lambda; m.addDiag = a.addDiag; m.fVal = fVal; m.bsc = bsc; m.uVal = a.uVal;
-					schur3::k_schur3<double, float><<<(S.nblk + schur3::WARPS - 1) / schur3::WARPS, schur3::WARPS * 32, 0, stream>>>(m);
-				}
-			}
-			else schur3::k_schur3<T><<<(S.nblk + schur3::WARPS - 1) / schur3::WARPS, schur3::WARPS * 32, 0, stream>>>(a);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
+			int rc = stages.mixed ? launch_schur3(HplF.p, lambda) : launch_schur3(Hpl.p, lambda); if (rc) return rc;
 			if (upperReduce) {
 				// upper blocks | bsc: one collective of half the bytes, then both triangles are filled locally
 				static const bool timing = getenv("CUBA_SCHUR_TIMING") != nullptr;      // diagnosis: split of the stage, printed by rank 0
 				cudaEvent_t ev[3];
 				if (timing) { for (auto& e : ev) cudaEventCreate(&e); cudaEventRecord(ev[0], stream); }
-				int rc = uPeerOk ? launch_peer_allreduce() : allreduce(uVal.p, 36 * (size_t)S.nblk + 6 * (size_t)S.numP, true); if (rc) return rc;
+				rc = uPeerOk ? launch_peer_allreduce() : allreduce(uVal.p, 36 * (size_t)S.nblk + 6 * (size_t)S.numP, true); if (rc) return rc;
 				if (timing) cudaEventRecord(ev[1], stream);
 				KLAUNCH(schur3::k_expand_upper<T>, 36LL * S.nblk, uVal.p, u2f.p, u2fT.p, blkRow.p, blkCol.p, S.nblk, fVal.p);
 				if (timing) {
@@ -1335,8 +1310,43 @@ struct Engine : EngineBase {
 				}
 			}
 			else if (world > 1) {
-				int rc = allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true); if (rc) return rc;   // Hsc | bsc: one buffer
+				rc = allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true); if (rc) return rc;   // Hsc | bsc: one buffer
 			}
+		}
+		return CUBA_OK;
+	}
+	// k_schur3 on Hpl blocks of type HT: T, or float under mixed precision
+	template <typename HT>
+	int launch_schur3(const HT* hpl, T lambda)
+	{
+		schur3::Args<T, HT> a;
+		a.Hpl = hpl; a.invHll = invHll; a.bl = bl; a.Hpp = Hpp; a.bp = bp;
+		a.prodPtr = prodPtr; a.prodI = prodI; a.prodJ = prodJ; a.prodL = prodL;
+		a.blkRow = blkRow; a.blkCol = blkCol; a.u2f = u2f; a.u2fT = u2fT; a.nblk = S.nblk;
+		a.lambda = lambda; a.addDiag = rank == 0 ? 1 : 0; a.fVal = fVal; a.bsc = bsc; a.uVal = upperReduce ? uVal.p : nullptr;
+		schur3::k_schur3<T, HT><<<(S.nblk + schur3::WARPS - 1) / schur3::WARPS, schur3::WARPS * 32, 0, stream>>>(a);
+		launches++;
+		CUDA_TRY(cudaGetLastError());
+		return CUBA_OK;
+	}
+	// the Schur complement on the tensor pipe (s5): the products of each (tile, destination) segment, then one reduction per block
+	int launch_schur5(T lambda)
+	{
+		if constexpr (sizeof(T) == 8) {
+			schur5::Args sa;
+			sa.Hpl = Hpl; sa.Hll = Hll; sa.bl = bl; sa.info = s5.tileInfo; sa.hplLm = hplLm; sa.tileSegPtr = s5.tileSegPtr; sa.segRec = s5.segRec; sa.off = s5.off;
+			sa.p2i = s5.p2i; sa.p2j = s5.p2j; sa.numL = S.numL; sa.lambda = lambda; sa.invHll = invHll; sa.partial = s5.partial;
+			schur5::k_schur_tiles_mma<<<s5.ntiles, schur5::WARPS * 32, sizeof(schur5::Smem), stream>>>(sa);
+			launches++;
+			CUDA_TRY(cudaGetLastError());
+			schur5::ReduceArgs<T> ra;
+			ra.partial = s5.partial; ra.destSegPtr = s5.destSegPtr; ra.Hpp = Hpp; ra.bp = bp;
+			ra.blkRow = blkRow; ra.blkCol = blkCol; ra.u2f = u2f; ra.u2fT = u2fT; ra.nblk = S.nblk; ra.lambda = lambda;
+			ra.addDiag = rank == 0 ? 1 : 0; ra.fVal = fVal; ra.bsc = bsc;
+			schur5::k_schur_reduce<T><<<(S.nblk + 3) / 4, 128, 0, stream>>>(ra);
+			launches++;
+			CUDA_TRY(cudaGetLastError());
+			if (world > 1) return allreduce(fVal.p, 36 * (size_t)S.nfull + 6 * (size_t)S.numP, true);   // Hsc | bsc: one buffer
 		}
 		return CUBA_OK;
 	}
@@ -1344,47 +1354,49 @@ struct Engine : EngineBase {
 	// warp tiles of the J+H landmark pass (cuba_jh4.cuh): greedy packing by binary lifting, padded records, pose lists
 	int setup_jh4()
 	{
-		ntW = 0; jh4Grid = 0; jh4HasBig = 0;
-		if constexpr (sizeof(T) == 8) {
-			using namespace jh4;
-			const int lb = S.lmBeg, N = S.lmEnd - S.lmBeg;
-			if (N <= 0 || S.eLocal <= 0) return CUBA_OK;
-			int K = 1;
-			while ((1LL << K) <= (long long)N) K++;
-			CUDA_TRY(w_levels.alloc((size_t)K * ((size_t)N + 1)));
-			CUDA_TRY(w_start.alloc((size_t)N + 1)); CUDA_TRY(w_pieces.alloc((size_t)N + 1)); CUDA_TRY(w_base.alloc((size_t)N + 1));
-			CUDA_TRY(w_flag.alloc(1));
-			CUDA_TRY(cudaMemsetAsync(w_flag.p, 0, sizeof(int), stream));
-			KLAUNCH(jh4::k_next, N + 1, lmPtr.p, lb, N, w_levels.p);
-			for (int k = 1; k < K; k++)
-				KLAUNCH(jh4::k_lift, N + 1, w_levels.p + (size_t)(k - 1) * ((size_t)N + 1), N, w_levels.p + (size_t)k * ((size_t)N + 1));
-			KLAUNCH(jh4::k_starts, N + 1, w_levels.p, K, N, lmPtr.p, lb, w_start.p, w_pieces.p, w_flag.p);
-			int rc = exclusiveSum(w_pieces.p, w_base.p, N + 1); if (rc) return rc;
-			if (!jh4Host) CUDA_TRY(cudaMallocHost((void**)&jh4Host, 2 * sizeof(int)));
-			CUDA_TRY(cudaMemcpyAsync(&jh4Host[0], w_base.p + N, sizeof(int), cudaMemcpyDeviceToHost, stream));
-			CUDA_TRY(cudaMemcpyAsync(&jh4Host[1], w_flag.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
-			jh4Pending = true;
-		}
+		wt.ntiles = 0; wt.grid = 0;
+		const int lb = S.lmBeg, N = S.lmEnd - S.lmBeg;
+		if (N <= 0 || S.eLocal <= 0) return CUBA_OK;
+		int K = 1;
+		while ((1LL << K) <= (long long)N) K++;
+		CUDA_TRY(wt.levels.alloc((size_t)K * ((size_t)N + 1)));
+		CUDA_TRY(wt.start.alloc((size_t)N + 1)); CUDA_TRY(wt.pieces.alloc((size_t)N + 1)); CUDA_TRY(wt.base.alloc((size_t)N + 1));
+		CUDA_TRY(wt.flag.alloc(1));
+		CUDA_TRY(cudaMemsetAsync(wt.flag.p, 0, sizeof(int), stream));
+		KLAUNCH(jh4::k_next, N + 1, lmPtr.p, lb, N, wt.levels.p);
+		for (int k = 1; k < K; k++)
+			KLAUNCH(jh4::k_lift, N + 1, wt.levels.p + (size_t)(k - 1) * ((size_t)N + 1), N, wt.levels.p + (size_t)k * ((size_t)N + 1));
+		KLAUNCH(jh4::k_starts, N + 1, wt.levels.p, K, N, lmPtr.p, lb, wt.start.p, wt.pieces.p, wt.flag.p);
+		int rc = exclusiveSum(wt.pieces.p, wt.base.p, N + 1); if (rc) return rc;
+		if (!wt.host) CUDA_TRY(cudaMallocHost((void**)&wt.host, 2 * sizeof(int)));
+		CUDA_TRY(cudaMemcpyAsync(&wt.host[0], wt.base.p + N, sizeof(int), cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaMemcpyAsync(&wt.host[1], wt.flag.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
+		wt.pending = true;
 		return CUBA_OK;
 	}
 	// second half of the warp-tile setup: the host work of the PCG setups runs between the two halves, overlapping the kernels above
 	int setup_jh4_finish()
 	{
-		if (!jh4Pending) return CUBA_OK;
-		jh4Pending = false;
+		if (!wt.pending) return CUBA_OK;
+		wt.pending = false;
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		const int big = wt.host[1], nt = wt.ntiles = wt.host[0];
+		if (nt <= 0) return CUBA_OK;
+		CUDA_TRY(wt.tile.alloc(nt)); CUDA_TRY(wt.rec.alloc(nt)); CUDA_TRY(wt.tilePose.alloc(32 * (size_t)nt)); CUDA_TRY(wt.tilePieces.alloc(nt)); CUDA_TRY(wt.pieceCount.alloc(nt));
+		CUDA_TRY(cudaMemsetAsync(wt.pieceCount.p, 0, sizeof(int) * (size_t)nt, stream));
+		CUDA_TRY(wt.bigPartial.alloc(std::max<size_t>(big ? 12 * (size_t)nt : 12, 11 * (size_t)numSMs * 6 * jh4::WARPS)));
+		int rc = jh4_emit(); if (rc) return rc;
+		wt.grid = std::max(1, std::min((nt + jh4::WARPS - 1) / jh4::WARPS, numSMs * stages.jh4MinB));
+		return CUBA_OK;
+	}
+	// the warp-tile records from the landmark-major edge streams: at setup, and whenever a refresh or the level mask rewrites them
+	int jh4_emit()
+	{
 		if constexpr (sizeof(T) == 8) {
-			using namespace jh4;
+			if (wt.ntiles <= 0) return CUBA_OK;
 			const int lb = S.lmBeg, N = S.lmEnd - S.lmBeg;
-			CUDA_TRY(cudaStreamSynchronize(stream));
-			const int big = jh4Host[1];
-			ntW = jh4Host[0]; jh4HasBig = big;
-			if (ntW <= 0) return CUBA_OK;
-			CUDA_TRY(w_tile.alloc(ntW)); CUDA_TRY(w_rec.alloc(ntW)); CUDA_TRY(w_tilePose.alloc(32 * (size_t)ntW)); CUDA_TRY(w_tilePieces.alloc(ntW)); CUDA_TRY(w_pieceCount.alloc(ntW));
-			CUDA_TRY(cudaMemsetAsync(w_pieceCount.p, 0, sizeof(int) * (size_t)ntW, stream));
-			CUDA_TRY(w_bigPartial.alloc(std::max<size_t>(big ? 12 * (size_t)ntW : 12, 11 * (size_t)numSMs * 6 * jh4::WARPS)));
-			KLAUNCH(jh4::k_emit, (long long)N * 32, w_start.p, w_pieces.p, w_base.p, N, lmPtr.p, lb, w_levels.p,
-				e_mx.p, e_my.p, e_mz.p, e_om.p, e_ip.p, e_il.p, e_hpl.p, w_tile.p, w_rec.p, w_tilePose.p, w_tilePieces.p);
-			jh4Grid = std::max(1, std::min((ntW + WARPS - 1) / WARPS, numSMs * jh4MinB));
+			KLAUNCH(jh4::k_emit, (long long)N * 32, wt.start.p, wt.pieces.p, wt.base.p, N, lmPtr.p, lb, wt.levels.p,
+				e_mx.p, e_my.p, e_mz.p, e_om.p, e_ip.p, e_il.p, e_hpl.p, wt.tile.p, wt.rec.p, wt.tilePose.p, wt.tilePieces.p);
 		}
 		return CUBA_OK;
 	}
@@ -1396,40 +1408,40 @@ struct Engine : EngineBase {
 		using namespace schur5;
 		const int N = (int)S.nmulLocal, nblk = S.nblk;
 		const int tb5 = std::min(S.lmBeg, S.numL), te5 = std::min(S.lmEnd, S.numL) + (S.lmEnd > S.numL ? 1 : 0);
-		const int nt = s5Ntiles = (S.eLocal + WINDOW - 1) / WINDOW;
-		CUDA_TRY(s5TileLm.alloc((size_t)nt + 1)); CUDA_TRY(s5TileInfo.alloc((size_t)nt));
-		KLAUNCH(sgpu::k_tiles, nt + 1, tilePtr.p, tb5, te5, WINDOW, nt, s5TileLm.p);
-		k_tile_info3<<<nt, 128, 0, stream>>>(tilePtr.p, s5TileLm.p, e_ip.p, e_hpl.p, S.eLocal, S.nhplLocal, nt, s5TileInfo.p);
+		const int nt = s5.ntiles = (S.eLocal + WINDOW - 1) / WINDOW;
+		CUDA_TRY(s5.tileLm.alloc((size_t)nt + 1)); CUDA_TRY(s5.tileInfo.alloc((size_t)nt));
+		KLAUNCH(sgpu::k_tiles, nt + 1, tilePtr.p, tb5, te5, WINDOW, nt, s5.tileLm.p);
+		k_tile_info3<<<nt, 128, 0, stream>>>(tilePtr.p, s5.tileLm.p, e_ip.p, e_hpl.p, S.eLocal, S.nhplLocal, nt, s5.tileInfo.p);
 		launches++;
 		CUDA_TRY(cudaGetLastError());
-		CUDA_TRY(s5_key.alloc(N)); CUDA_TRY(s5_keyS.alloc(N)); CUDA_TRY(s5_val.alloc(N)); CUDA_TRY(s5_valS.alloc(N));
-		CUDA_TRY(s5_head.alloc(N)); CUDA_TRY(s5_segId.alloc(N)); CUDA_TRY(s5_counts.alloc(1));
-		KLAUNCH(k_keys, N, prodPtr.p, nblk, prodI.p, N, s5TileInfo.p, nt, s5_key.p, s5_val.p);
-		int rc = sortPairs(s5_key.p, s5_keyS.p, s5_val.p, s5_valS.p, N, 64); if (rc) return rc;
-		KLAUNCH(k_heads, N, s5_keyS.p, N, s5_head.p);
-		rc = exclusiveSum(s5_head.p, s5_segId.p, N); if (rc) return rc;
-		k_counts<<<1, 32, 0, stream>>>(s5_keyS.p, s5_head.p, s5_segId.p, N, s5_counts.p);
+		CUDA_TRY(s5.key.alloc(N)); CUDA_TRY(s5.keyS.alloc(N)); CUDA_TRY(s5.val.alloc(N)); CUDA_TRY(s5.valS.alloc(N));
+		CUDA_TRY(s5.head.alloc(N)); CUDA_TRY(s5.segId.alloc(N)); CUDA_TRY(s5.counts.alloc(1));
+		KLAUNCH(k_keys, N, prodPtr.p, nblk, prodI.p, N, s5.tileInfo.p, nt, s5.key.p, s5.val.p);
+		int rc = sortPairs(s5.key.p, s5.keyS.p, s5.val.p, s5.valS.p, N, 64); if (rc) return rc;
+		KLAUNCH(k_heads, N, s5.keyS.p, N, s5.head.p);
+		rc = exclusiveSum(s5.head.p, s5.segId.p, N); if (rc) return rc;
+		k_counts<<<1, 32, 0, stream>>>(s5.keyS.p, s5.head.p, s5.segId.p, N, s5.counts.p);
 		launches++;
 		Counts hc;
-		CUDA_TRY(cudaMemcpyAsync(&hc, s5_counts.p, sizeof(hc), cudaMemcpyDeviceToHost, stream));
+		CUDA_TRY(cudaMemcpyAsync(&hc, s5.counts.p, sizeof(hc), cudaMemcpyDeviceToHost, stream));
 		CUDA_TRY(cudaStreamSynchronize(stream));
 		const int nseg = hc.nseg, nvalid = hc.nvalid;
-		CUDA_TRY(s5_segStart.alloc((size_t)nseg + 1)); CUDA_TRY(s5_segTile.alloc(nseg)); CUDA_TRY(s5_segDest.alloc(nseg));
-		CUDA_TRY(s5_key3.alloc(nseg)); CUDA_TRY(s5_key3S.alloc(nseg)); CUDA_TRY(s5_val3.alloc(nseg)); CUDA_TRY(s5_val3S.alloc(nseg));
-		CUDA_TRY(s5_segRank.alloc(nseg)); CUDA_TRY(s5_rankDest.alloc(nseg));
-		CUDA_TRY(s5_tileSegPtr.alloc((size_t)nt + 1)); CUDA_TRY(s5_destSegPtr.alloc((size_t)nblk + 1));
-		CUDA_TRY(s5_p2i.alloc(N)); CUDA_TRY(s5_p2j.alloc(N));
-		KLAUNCH(k_segments, N + 1, s5_keyS.p, s5_valS.p, s5_head.p, s5_segId.p, prodI.p, prodJ.p, N, nseg, nvalid,
-			s5_segStart.p, s5_segTile.p, s5_segDest.p, s5_p2i.p, s5_p2j.p, s5_key3.p, s5_val3.p);
-		KLAUNCH(k_ptr_from_field, nt + 1, s5_segTile.p, nseg, nt, s5_tileSegPtr.p);
-		rc = sortPairs(s5_key3.p, s5_key3S.p, s5_val3.p, s5_val3S.p, nseg, 32 + sgpu::bits_for((unsigned long long)std::max(nblk, 1))); if (rc) return rc;
-		KLAUNCH(k_rank, nseg, s5_key3S.p, s5_val3S.p, nseg, s5_segRank.p, s5_rankDest.p);
-		KLAUNCH(k_ptr_from_field, nblk + 1, s5_rankDest.p, nseg, nblk, s5_destSegPtr.p);
-		CUDA_TRY(s5_partial.alloc((size_t)PW * std::max(nseg, 1)));
-		CUDA_TRY(s5SegRec.alloc((size_t)std::max(nseg, 1)));
-		KLAUNCH(k_seg_records, nseg, s5_segStart.p, s5_segDest.p, s5_segRank.p, s5_segTile.p, blkRow.p, blkCol.p, s5TileInfo.p, s5_p2i.p, s5_p2j.p, nseg, s5SegRec.p);
-		CUDA_TRY(s5Off.alloc((size_t)std::max(nvalid, 1)));
-		KLAUNCH(k_prod_offsets, nvalid, s5_segStart.p, s5_segTile.p, s5TileInfo.p, s5_p2i.p, s5_p2j.p, nseg, nvalid, s5Off.p);
+		CUDA_TRY(s5.segStart.alloc((size_t)nseg + 1)); CUDA_TRY(s5.segTile.alloc(nseg)); CUDA_TRY(s5.segDest.alloc(nseg));
+		CUDA_TRY(s5.key3.alloc(nseg)); CUDA_TRY(s5.key3S.alloc(nseg)); CUDA_TRY(s5.val3.alloc(nseg)); CUDA_TRY(s5.val3S.alloc(nseg));
+		CUDA_TRY(s5.segRank.alloc(nseg)); CUDA_TRY(s5.rankDest.alloc(nseg));
+		CUDA_TRY(s5.tileSegPtr.alloc((size_t)nt + 1)); CUDA_TRY(s5.destSegPtr.alloc((size_t)nblk + 1));
+		CUDA_TRY(s5.p2i.alloc(N)); CUDA_TRY(s5.p2j.alloc(N));
+		KLAUNCH(k_segments, N + 1, s5.keyS.p, s5.valS.p, s5.head.p, s5.segId.p, prodI.p, prodJ.p, N, nseg, nvalid,
+			s5.segStart.p, s5.segTile.p, s5.segDest.p, s5.p2i.p, s5.p2j.p, s5.key3.p, s5.val3.p);
+		KLAUNCH(k_ptr_from_field, nt + 1, s5.segTile.p, nseg, nt, s5.tileSegPtr.p);
+		rc = sortPairs(s5.key3.p, s5.key3S.p, s5.val3.p, s5.val3S.p, nseg, 32 + sgpu::bits_for((unsigned long long)std::max(nblk, 1))); if (rc) return rc;
+		KLAUNCH(k_rank, nseg, s5.key3S.p, s5.val3S.p, nseg, s5.segRank.p, s5.rankDest.p);
+		KLAUNCH(k_ptr_from_field, nblk + 1, s5.rankDest.p, nseg, nblk, s5.destSegPtr.p);
+		CUDA_TRY(s5.partial.alloc((size_t)PW * std::max(nseg, 1)));
+		CUDA_TRY(s5.segRec.alloc((size_t)std::max(nseg, 1)));
+		KLAUNCH(k_seg_records, nseg, s5.segStart.p, s5.segDest.p, s5.segRank.p, s5.segTile.p, blkRow.p, blkCol.p, s5.tileInfo.p, s5.p2i.p, s5.p2j.p, nseg, s5.segRec.p);
+		CUDA_TRY(s5.off.alloc((size_t)std::max(nvalid, 1)));
+		KLAUNCH(k_prod_offsets, nvalid, s5.segStart.p, s5.segTile.p, s5.tileInfo.p, s5.p2i.p, s5.p2j.p, nseg, nvalid, s5.off.p);
 		CUDA_TRY(cudaFuncSetAttribute(k_schur_tiles_mma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)));
 		return CUBA_OK;
 	}
@@ -2067,24 +2079,20 @@ struct Engine : EngineBase {
 	int launch_backsub(T lambda)
 	{
 		ProfScope ps(this, CUBA_PROF_SCHUR_COMPLEMENT);
-		if (ntiles > 0 && S.numL > 0) {
-			BacksubArgs<T> a;
-			a.Hpl = Hpl; a.invHll = invHll; a.bl = bl; a.xp = xp; a.ip = e_ip; a.hpl = e_hpl; a.lmPtr = tilePtr; a.tileLm = tileLm;
-			a.numL = S.numL; a.lambda = lambda; a.XwCur = Xw[cur]; a.XwTrial = Xw[cur ^ 1]; a.xl = xl; a.scalePartial = scalePartialL;
-			if (mixed) {
-				if constexpr (sizeof(T) == 8) {
-					BacksubArgs<double, float> m;
-					m.Hpl = HplF; m.invHll = invHll; m.bl = bl; m.xp = xp; m.ip = e_ip; m.hpl = e_hpl; m.lmPtr = tilePtr; m.tileLm = tileLm;
-					m.numL = S.numL; m.lambda = lambda; m.XwCur = Xw[cur]; m.XwTrial = Xw[cur ^ 1]; m.xl = xl; m.scalePartial = scalePartialL;
-					if (tileSize == 128) k_backsub<double, 128, float><<<ntiles, 128, 0, stream>>>(m);
-					else k_backsub<double, 256, float><<<ntiles, 256, 0, stream>>>(m);
-				}
-			}
-			else if (tileSize == 128) k_backsub<T, 128><<<ntiles, 128, 0, stream>>>(a);
-			else k_backsub<T, 256><<<ntiles, 256, 0, stream>>>(a);
-			launches++;
-			CUDA_TRY(cudaGetLastError());
-		}
+		if (ntiles > 0 && S.numL > 0) return stages.mixed ? launch_backsub(HplF.p, lambda) : launch_backsub(Hpl.p, lambda);
+		return CUBA_OK;
+	}
+	// k_backsub on Hpl blocks of type HT: T, or float under mixed precision
+	template <typename HT>
+	int launch_backsub(const HT* hpl, T lambda)
+	{
+		BacksubArgs<T, HT> a;
+		a.Hpl = hpl; a.invHll = invHll; a.bl = bl; a.xp = xp; a.ip = e_ip; a.hpl = e_hpl; a.lmPtr = tilePtr; a.tileLm = tileLm;
+		a.numL = S.numL; a.lambda = lambda; a.XwCur = Xw[cur]; a.XwTrial = Xw[cur ^ 1]; a.xl = xl; a.scalePartial = scalePartialL;
+		if (stages.tileSize == 128) k_backsub<T, 128, HT><<<ntiles, 128, 0, stream>>>(a);
+		else k_backsub<T, 256, HT><<<ntiles, 256, 0, stream>>>(a);
+		launches++;
+		CUDA_TRY(cudaGetLastError());
 		return CUBA_OK;
 	}
 
@@ -2337,13 +2345,7 @@ struct Engine : EngineBase {
 		const int eL = S.eLocal;
 		KLAUNCH(lv::k_mask_omega<T>, eL, e_om0.p, e_user.p, lvLevel.p, eL, e_om.p);
 		KLAUNCH(lv::k_pose_omega<T>, eL, g_psrc.p, posePtr.p, S.numP, eL, e_om.p, p_om.p);
-		if constexpr (sizeof(T) == 8) {
-			if (jhV4 && ntW > 0) {
-				const int lb = S.lmBeg, N = S.lmEnd - S.lmBeg;
-				KLAUNCH(jh4::k_emit, (long long)N * 32, w_start.p, w_pieces.p, w_base.p, N, lmPtr.p, lb, w_levels.p,
-					e_mx.p, e_my.p, e_mz.p, e_om.p, e_ip.p, e_il.p, e_hpl.p, w_tile.p, w_rec.p, w_tilePose.p, w_tilePieces.p);
-			}
-		}
+		int rc = jh4_emit(); if (rc) return rc;
 		// the system changed: nothing an earlier solve left behind may be reused (as after refresh_values; the estimate stays)
 		trialValid = false;
 		forget_solves();
@@ -2658,7 +2660,7 @@ struct Engine : EngineBase {
 		if (oHpl) {
 			// local blocks land at their global positions; foreign blocks read as zero
 			memset(oHpl, 0, sizeof(double) * 18 * (size_t)S.nhpl);
-			if (mixed) {
+			if (stages.mixed) {
 				std::vector<float> hf(20 * (size_t)S.nhplLocal);
 				CUDA_TRY(cudaMemcpyAsync(hf.data(), HplF.p, sizeof(float) * hf.size(), cudaMemcpyDeviceToHost, stream));
 				CUDA_TRY(cudaStreamSynchronize(stream));
@@ -2979,15 +2981,12 @@ int cuba_engine_create(const cuba_config* cfg, cuba_engine** out)
 	c.device = -1; c.deterministic = 1;
 	if (cfg) c = *cfg;
 	// kernel-selecting slots: a value that names no kernel is an error, not a silent default
-	const int r0 = c.reserved[0], r2 = c.reserved[2], r3 = c.reserved[3];
+	const int r0 = c.reserved[0];
 	if (r0 != 0 && (r0 < 2 || r0 > 8))
 		return fail(CUBA_ERR_INVALID, "create: reserved[0] = " + std::to_string(r0) + " names no PCG kernel (0, 2..8)");
-	if (r2 < 0 || r2 == 5 || r2 == 6 || r2 > 9)
-		return fail(CUBA_ERR_INVALID, "create: reserved[2] = " + std::to_string(r2) + " names no J+H kernel (0..4, 7..9)");
-	if (r3 != 0 && r3 != 3 && r3 != 5)
-		return fail(CUBA_ERR_INVALID, "create: reserved[3] = " + std::to_string(r3) + " names no Schur kernel (0, 3, 5)");
+	StageChoice stages;
+	int rc = stage_choice(c, c.use_fp32 != 1, stages); if (rc) return rc;
 	std::unique_ptr<EngineBase> impl;
-	int rc;
 	if (c.use_fp32 == 1) { auto* e = new Engine<float>(); e->cfg = c; impl.reset(e); rc = e->init(); }
 	else { auto* e = new Engine<double>(); e->cfg = c; impl.reset(e); rc = e->init(); }
 	if (rc) return rc;
