@@ -35,7 +35,7 @@ class CubaError(RuntimeError):
 
 # the status word of the device-resident batches (include/cuba_b200.h: CUBA_BATCH_*): a bit per failed check
 BATCH_STATUS = {1: "ptr does not start at 0", 2: "ptr decreases", 4: "ptr does not end at the item count",
-                8: "non-finite omega or pair value", 16: "non-finite S12 or intrinsics", 32: "s <= 0"}
+                8: "non-finite omega or pair value", 16: "non-finite S12 or intrinsics", 32: "s <= 0", 64: "iP outside [0, P)"}
 
 
 ITER_STAT_DTYPE = np.dtype([("iteration", "<i4"), ("trials", "<i4"), ("chi2", "<f8"), ("lambda_", "<f8"), ("pcg_iters", "<i4"),
@@ -43,14 +43,15 @@ ITER_STAT_DTYPE = np.dtype([("iteration", "<i4"), ("trials", "<i4"), ("chi2", "<
 
 
 def stats_view(stats):
-    """the stats tensor of optimize_poses_device / optimize_sim3_device ([B, S, 4] float64 words) as the structured [B, S] array
-    the _flat methods return; copies to the host, so it waits for the call"""
+    """the stats tensor of optimize_poses_device / optimize_sim3_device / optimize_points_device ([B, S, 4] float64 words) as the
+    structured [B, S] array the _flat methods return; copies to the host, so it waits for the call"""
     a = np.ascontiguousarray(stats.cpu().numpy())
     return a.view(ITER_STAT_DTYPE).reshape(a.shape[:2])
 
 
 def batch_status_message(status):
-    """the checks a status word of optimize_poses_device / optimize_sim3_device reports as failed, as text ("ok" for 0)"""
+    """the checks a status word of optimize_poses_device / optimize_sim3_device / optimize_points_device reports as failed, as text
+    ("ok" for 0)"""
     status = int(status)
     return "; ".join(m for bit, m in BATCH_STATUS.items() if status & bit) or ("ok" if status == 0 else "unknown status %d" % status)
 
@@ -115,6 +116,12 @@ def orbslam2_pose_schedule():
     return [PoseRound(**(huber if r < 2 else {})) for r in range(4)]
 
 
+class _PointBatch(C.Structure):
+    _fields_ = [("B", C.c_int32), ("P", C.c_int32), ("E2", C.c_int32), ("E3", C.c_int32), ("Xw", C.c_void_p), ("q", C.c_void_p),
+                ("t", C.c_void_p), ("cam", C.c_void_p), ("ptr2", C.c_void_p), ("iP2", C.c_void_p), ("meas2", C.c_void_p),
+                ("omega2", C.c_void_p), ("ptr3", C.c_void_p), ("iP3", C.c_void_p), ("meas3", C.c_void_p), ("omega3", C.c_void_p)]
+
+
 class _Sim3Batch(C.Structure):
     _fields_ = [("B", C.c_int32), ("N", C.c_int32), ("ptr", C.c_void_p), ("q", C.c_void_p), ("t", C.c_void_p), ("s", C.c_void_p),
                 ("cam1", C.c_void_p), ("cam2", C.c_void_p), ("fix_scale", C.c_void_p), ("X1", C.c_void_p), ("X2", C.c_void_p),
@@ -143,7 +150,7 @@ _lib = None
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
     "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_linear_solver", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_get_device", "cuba_engine_flush_l2",
-    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_set_problem_device", "cuba_engine_set_state_device", "cuba_engine_get_state_device", "cuba_engine_get_chi2_device", "cuba_engine_set_edge_levels_device", "cuba_engine_get_edge_levels_device", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_pose_batch_workspace_bytes", "cuba_engine_optimize_poses_device", "cuba_sim3_batch_workspace_bytes", "cuba_engine_optimize_sim3_device", "cuba_engine_get_profile",
+    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_set_problem_device", "cuba_engine_set_state_device", "cuba_engine_get_state_device", "cuba_engine_get_chi2_device", "cuba_engine_set_edge_levels_device", "cuba_engine_get_edge_levels_device", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_pose_batch_workspace_bytes", "cuba_engine_optimize_poses_device", "cuba_sim3_batch_workspace_bytes", "cuba_engine_optimize_sim3_device", "cuba_engine_optimize_points", "cuba_point_batch_workspace_bytes", "cuba_engine_optimize_points_device", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
     "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_dense_solve", "cuba_debug_peer_allreduce", "cuba_debug_pcg5_ranks", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dense_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
@@ -198,6 +205,8 @@ def load_library():
         "cuba_engine_optimize_poses_device": [vp, C.POINTER(_PoseBatch), i, vp, vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp, vp],
         "cuba_engine_optimize_sim3_device": [vp, C.POINTER(_Sim3Batch), C.POINTER(_Sim3Params), vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp,
                                              vp, vp],
+        "cuba_engine_optimize_points": [vp, C.POINTER(_PointBatch), i, vp, vp, vp, vp, vp, vp],
+        "cuba_engine_optimize_points_device": [vp, C.POINTER(_PointBatch), i, vp, vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp],
         "cuba_engine_get_profile": [vp, vp],
         "cuba_engine_get_launch_count": [vp, C.POINTER(C.c_longlong)],
         "cuba_get_transfer_bytes": [C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)],
@@ -236,6 +245,8 @@ def load_library():
     L.cuba_pose_batch_workspace_bytes.restype = C.c_size_t
     L.cuba_sim3_batch_workspace_bytes.argtypes = [i, i, C.POINTER(_Sim3Params), i]
     L.cuba_sim3_batch_workspace_bytes.restype = C.c_size_t
+    L.cuba_point_batch_workspace_bytes.argtypes = [i, i, i, i, i, vp, i]
+    L.cuba_point_batch_workspace_bytes.restype = C.c_size_t
     _lib = L
     return L
 
@@ -520,6 +531,14 @@ class Engine:
             rs[k].flags = (1 if r.depth else 0) | (2 if r.reinclude else 0)
         return rs
 
+    @staticmethod
+    def _round_stats(stats, nstats, rounds):
+        """one problem's structured stats [sum of iterations] and nstats [R] as, per round, the list optimize() returns"""
+        off = np.concatenate([[0], np.cumsum([int(x.iterations) for x in rounds])])
+        return [[dict(iteration=int(s["iteration"]), trials=int(s["trials"]), chi2=float(s["chi2"]), lambda_=float(s["lambda_"]),
+                      pcg_iters=int(s["pcg_iters"]), pcg_failed=int(s["pcg_failed"])) for s in stats[off[k]:off[k] + nstats[k]]]
+                for k in range(len(rounds))]
+
     def optimize_poses_flat(self, q, t, cam, ptr2, X2, meas2, omega2, ptr3, X3, meas3, omega3, rounds, B=None, E2=None, E3=None):
         """cuba_engine_optimize_poses on flat arrays (include/cuba_b200.h); B / E2 / E3 default to the array sizes.  Returns a dict of
         q [B,4], t [B,3], levels [E2+E3] (mono then stereo), counts [B,R,4], stats [B,sum of iterations] (structured) and nstats [B,R]."""
@@ -550,18 +569,46 @@ class Engine:
         a = graphio.pose_batch_arrays(frames)
         ptr2, ptr3 = a["ptr2"], a["ptr3"]
         r = self.optimize_poses_flat(rounds=rounds, **a)
-        off = np.concatenate([[0], np.cumsum([int(x.iterations) for x in rounds])])
         E2 = int(ptr2[-1])
-        res = []
-        for b in range(len(frames)):
-            stats = []
-            for k in range(len(rounds)):
-                rows = r["stats"][b, off[k]:off[k] + r["nstats"][b, k]]
-                stats.append([dict(iteration=int(s["iteration"]), trials=int(s["trials"]), chi2=float(s["chi2"]), lambda_=float(s["lambda_"]),
-                                   pcg_iters=int(s["pcg_iters"]), pcg_failed=int(s["pcg_failed"])) for s in rows])
-            res.append(dict(q=r["q"][b], t=r["t"][b], counts=r["counts"][b], stats=stats,
-                            levels=np.concatenate([r["levels"][ptr2[b]:ptr2[b + 1]], r["levels"][E2 + ptr3[b]:E2 + ptr3[b + 1]]])))
-        return res
+        return [dict(q=r["q"][b], t=r["t"][b], counts=r["counts"][b], stats=self._round_stats(r["stats"][b], r["nstats"][b], rounds),
+                     levels=np.concatenate([r["levels"][ptr2[b]:ptr2[b + 1]], r["levels"][E2 + ptr3[b]:E2 + ptr3[b + 1]]]))
+                for b in range(len(frames))]
+
+    # --- batched structure-only refinement (many map points against fixed poses in one launch) ----------------------------------------
+    def optimize_points_flat(self, Xw, q, t, cam, ptr2, iP2, meas2, omega2, ptr3, iP3, meas3, omega3, rounds, B=None, P=None, E2=None,
+                             E3=None):
+        """cuba_engine_optimize_points on flat arrays (include/cuba_b200.h); B / P / E2 / E3 default to the array sizes.  Returns a dict
+        of Xw [B,3], levels [E2+E3] (mono then stereo), counts [B,R,4], stats [B,sum of iterations] (structured) and nstats [B,R]."""
+        f64 = lambda a, w: np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1, w) if w > 1 else np.asarray(a, dtype=np.float64).reshape(-1))
+        i32 = lambda a: np.ascontiguousarray(np.asarray(a).reshape(-1), dtype=np.int32)
+        Xw, q, t, cam = f64(Xw, 3), f64(q, 4), f64(t, 3), f64(cam, 5)
+        meas2, omega2, meas3, omega3 = f64(meas2, 2), f64(omega2, 1), f64(meas3, 3), f64(omega3, 1)
+        ptr2, iP2, ptr3, iP3 = i32(ptr2), i32(iP2), i32(ptr3), i32(iP3)
+        B = len(Xw) if B is None else int(B)
+        P = len(q) if P is None else int(P)
+        E2 = len(omega2) if E2 is None else int(E2)
+        E3 = len(omega3) if E3 is None else int(E3)
+        nb, R = max(B, 0), len(rounds)
+        S = sum(max(int(r.iterations), 0) for r in rounds)
+        out = dict(Xw=np.zeros((nb, 3)), levels=np.zeros(max(E2, 0) + max(E3, 0), np.uint8), counts=np.zeros((nb, R, 4), np.int32),
+                   stats=(_IterStat * max(nb * S, 1))(), nstats=np.zeros((nb, R), np.int32))
+        batch = _PointBatch(B, P, E2, E3, _p(Xw), _p(q), _p(t), _p(cam), _p(ptr2), _p(iP2), _p(meas2), _p(omega2), _p(ptr3), _p(iP3),
+                            _p(meas3), _p(omega3))
+        _check(self.L.cuba_engine_optimize_points(self.h, C.byref(batch), R, self._rounds_struct(rounds), _p(out["Xw"]), _p(out["levels"]),
+                                                  _p(out["counts"]), out["stats"], _p(out["nstats"])))
+        out["stats"] = np.frombuffer(out["stats"], dtype=ITER_STAT_DTYPE)[:nb * S].reshape(nb, S).copy()
+        return out
+
+    def optimize_points(self, batch, rounds):
+        """Refines every point of a graphio.PointBatch against its fixed poses under the round schedule (list of PoseRound; restart =
+        from the point's input position) in one launch.  Returns, per point, a dict of Xw [3], levels (the point's mono edges then its
+        stereo edges), counts [R,4] (included mono, included stereo, newly excluded, re-included after each round) and stats (per round,
+        the iteration statistics as optimize() returns them)."""
+        r = self.optimize_points_flat(rounds=rounds, **batch.arrays())
+        ptr2, ptr3, E2 = batch.ptr2, batch.ptr3, int(batch.ptr2[-1])
+        return [dict(Xw=r["Xw"][b], counts=r["counts"][b], stats=self._round_stats(r["stats"][b], r["nstats"][b], rounds),
+                     levels=np.concatenate([r["levels"][ptr2[b]:ptr2[b + 1]], r["levels"][E2 + ptr3[b]:E2 + ptr3[b + 1]]]))
+                for b in range(batch.B)]
 
     # --- batched Sim(3) alignment (ORB-SLAM2's OptimizeSim3 over many keyframe pairs in one launch) ------------------------------------
     def optimize_sim3_flat(self, ptr, q, t, s, cam1, cam2, fix_scale, X1, X2, obs1, obs2, omega1, omega2, params=None, B=None, N=None):
@@ -751,6 +798,44 @@ class Engine:
                                                        workspace.numel() * workspace.element_size(), p(out["q"]), p(out["t"]), p(out["s"]),
                                                        p(out["levels"]), p(out["ninliers"]), p(out["stats"]), p(out["nstats"]), p(out["status"]),
                                                        C.c_void_p(self._torch_stream())))
+        out["workspace"] = workspace
+        return out
+
+    def optimize_points_device(self, Xw, q, t, cam, ptr2, iP2, meas2, omega2, ptr3, iP3, meas3, omega3, rounds, with_stats=True, out=None,
+                               workspace=None):
+        """cuba_engine_optimize_points_device: optimize_points_flat on torch CUDA tensors of the engine's device (float64, ptr2 / ptr3 /
+        iP2 / iP3 int32, all contiguous), on torch.cuda.current_stream(); no host synchronisation, no host<->device copy.  Returns a
+        dict of CUDA tensors with optimize_points_flat's keys and shapes, except stats: [B, sum of iterations, 4] float64 words
+        (stats_view()); plus "status" (int32 [1]; BATCH_STATUS) and "workspace".  out / workspace as for optimize_poses_device."""
+        what = "optimize_points_device"
+        import torch
+        f64, i32 = torch.float64, torch.int32
+        inputs = [("Xw", Xw, f64), ("q", q, f64), ("t", t, f64), ("cam", cam, f64), ("ptr2", ptr2, i32), ("iP2", iP2, i32),
+                  ("meas2", meas2, f64), ("omega2", omega2, f64), ("ptr3", ptr3, i32), ("iP3", iP3, i32), ("meas3", meas3, f64),
+                  ("omega3", omega3, f64)]
+        self._check_tensors(what, [(n, a, dt, None) for n, a, dt in inputs])
+        B = self._count(what, "Xw", Xw, 3)
+        P = self._count(what, "q", q, 4)
+        for name, a, w in (("t", t, 3), ("cam", cam, 5)):
+            self._count(what, name, a, w, P)
+        for name, a in (("ptr2", ptr2), ("ptr3", ptr3)):
+            self._count(what, name, a, 1, B + 1)
+        E2, E3 = omega2.numel(), omega3.numel()
+        for name, a, w, n in (("iP2", iP2, 1, E2), ("meas2", meas2, 2, E2), ("iP3", iP3, 1, E3), ("meas3", meas3, 3, E3)):
+            self._count(what, name, a, w, n)
+        R = len(rounds)
+        S = sum(max(int(r.iterations), 0) for r in rounds)
+        spec = dict(Xw=((B, 3), f64), levels=((E2 + E3,), torch.uint8), counts=((B, R, 4), i32), stats=((B, S, 4), f64), nstats=((B, R), i32),
+                    status=((1,), i32))
+        out, workspace, torch = self._device_call(what, [(n, a) for n, a, _ in inputs], spec, with_stats, out, workspace)
+        rs = self._rounds_struct(rounds)
+        workspace = self._workspace(torch, workspace, int(self.L.cuba_point_batch_workspace_bytes(B, P, E2, E3, R, rs, int(bool(with_stats)))))
+        ptr = lambda a: None if a is None else a.data_ptr()
+        batch = _PointBatch(B, P, E2, E3, ptr(Xw), ptr(q), ptr(t), ptr(cam), ptr(ptr2), ptr(iP2), ptr(meas2), ptr(omega2), ptr(ptr3), ptr(iP3),
+                            ptr(meas3), ptr(omega3))
+        _check(self.L.cuba_engine_optimize_points_device(self.h, C.byref(batch), R, rs, ptr(workspace), workspace.numel() * workspace.element_size(),
+                                                         ptr(out["Xw"]), ptr(out["levels"]), ptr(out["counts"]), ptr(out["stats"]),
+                                                         ptr(out["nstats"]), ptr(out["status"]), C.c_void_p(self._torch_stream())))
         out["workspace"] = workspace
         return out
 

@@ -38,6 +38,7 @@
 #include "../../include/cuda_bundle_adjustment.h"
 #include "../../include/cuba_b200_levels.h"
 #include "../../include/cuba_b200_pose.h"
+#include "../../include/cuba_b200_points.h"
 #include "../../include/cuba_b200_sim3.h"
 #include "../../include/cuba_b200_solver.h"
 
@@ -669,6 +670,44 @@ std::vector<PoseRound> orbSlam2PoseSchedule()
 	return s;
 }
 
+// the C ABI's rounds of a drop-in schedule; perProblem = the stat slots of one problem
+static std::vector<cuba_pose_round> c_rounds(const std::vector<PoseRound>& schedule, size_t& perProblem)
+{
+	std::vector<cuba_pose_round> rounds(schedule.size());
+	perProblem = 0;
+	for (size_t r = 0; r < schedule.size(); r++) {
+		const PoseRound& s = schedule[r];
+		cuba_pose_round& c = rounds[r];
+		c.iterations = s.iterations;
+		c.kernel_type[0] = static_cast<int32_t>(s.kernelMono); c.kernel_type[1] = static_cast<int32_t>(s.kernelStereo);
+		c.delta[0] = s.deltaMono; c.delta[1] = s.deltaStereo;
+		c.restart = s.restart ? 1 : 0;
+		c.chi2_mono = s.test.chi2Mono; c.chi2_stereo = s.test.chi2Stereo;
+		c.flags = (s.test.requirePositiveDepth ? CUBA_CLASSIFY_DEPTH : 0) | (s.test.reinclude ? CUBA_CLASSIFY_REINCLUDE : 0);
+		perProblem += static_cast<size_t>(std::max(s.iterations, 0));
+	}
+	return rounds;
+}
+
+// problem b's BatchStatistics per round
+static std::vector<BatchStatistics> round_stats(const std::vector<cuba_pose_round>& rounds, const std::vector<cuba_iter_stat>& stats,
+	const std::vector<int32_t>& nstats, size_t b, size_t perProblem)
+{
+	const size_t R = rounds.size();
+	std::vector<BatchStatistics> out;
+	size_t off = 0;
+	for (size_t r = 0; r < R; r++) {
+		BatchStatistics st;
+		for (int i = 0; i < nstats[b * R + r]; i++) {
+			const cuba_iter_stat& s = stats[b * perProblem + off + i];
+			st.push_back(BatchInfo{ s.iteration, s.chi2 });
+		}
+		out.push_back(st);
+		off += static_cast<size_t>(rounds[r].iterations);
+	}
+	return out;
+}
+
 std::vector<PoseResult> optimizePoses(CudaBundleAdjustment& ba, const std::vector<PoseFrame>& frames, const std::vector<PoseRound>& schedule)
 {
 	Impl& impl = impl_of(ba);
@@ -703,19 +742,8 @@ std::vector<PoseResult> optimizePoses(CudaBundleAdjustment& ba, const std::vecto
 		if (om2.size() + om3.size() > static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizePoses: too many edges");
 		ptr2[b + 1] = static_cast<int32_t>(om2.size()); ptr3[b + 1] = static_cast<int32_t>(om3.size());
 	}
-	std::vector<cuba_pose_round> rounds(schedule.size());
 	size_t perFrame = 0;
-	for (size_t r = 0; r < schedule.size(); r++) {
-		const PoseRound& s = schedule[r];
-		cuba_pose_round& c = rounds[r];
-		c.iterations = s.iterations;
-		c.kernel_type[0] = static_cast<int32_t>(s.kernelMono); c.kernel_type[1] = static_cast<int32_t>(s.kernelStereo);
-		c.delta[0] = s.deltaMono; c.delta[1] = s.deltaStereo;
-		c.restart = s.restart ? 1 : 0;
-		c.chi2_mono = s.test.chi2Mono; c.chi2_stereo = s.test.chi2Stereo;
-		c.flags = (s.test.requirePositiveDepth ? CUBA_CLASSIFY_DEPTH : 0) | (s.test.reinclude ? CUBA_CLASSIFY_REINCLUDE : 0);
-		perFrame += static_cast<size_t>(std::max(s.iterations, 0));
-	}
+	const std::vector<cuba_pose_round> rounds = c_rounds(schedule, perFrame);
 	const size_t R = rounds.size();
 	cuba_pose_batch bt;
 	bt.B = static_cast<int32_t>(B); bt.E2 = static_cast<int32_t>(om2.size()); bt.E3 = static_cast<int32_t>(om3.size());
@@ -744,16 +772,84 @@ std::vector<PoseResult> optimizePoses(CudaBundleAdjustment& ba, const std::vecto
 			res.levels.push_back(lv);
 			res.inliers += lv == 0;
 		}
-		size_t off = 0;
-		for (size_t r = 0; r < R; r++) {
-			BatchStatistics st;
-			for (int i = 0; i < nstats[b * R + r]; i++) {
-				const cuba_iter_stat& s = stats[b * perFrame + off + i];
-				st.push_back(BatchInfo{ s.iteration, s.chi2 });
+		res.rounds = round_stats(rounds, stats, nstats, b, perFrame);
+	}
+	return out;
+}
+
+// include/cuba_b200_points.h
+std::vector<PointResult> optimizePoints(CudaBundleAdjustment& ba, const std::vector<PointProblem>& points, const std::vector<PoseRound>& schedule)
+{
+	Impl& impl = impl_of(ba);
+	if (points.size() > static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizePoints: too many points");
+	const size_t B = points.size();
+	std::vector<double> Xw(3 * B), q, t, cam, m2, om2, m3, om3;
+	std::vector<int32_t> ptr2(B + 1, 0), ptr3(B + 1, 0), iP2, iP3;
+	std::unordered_map<const PoseVertex*, int32_t> table;    // each pose once, shared by every point that observes it
+	for (size_t b = 0; b < B; b++) {
+		const PointProblem& pt = points[b];
+		if (!pt.landmark) throw std::invalid_argument("cuba::optimizePoints: point without a landmark");
+		for (int k = 0; k < 3; k++) Xw[3 * b + k] = pt.landmark->Xw.data()[k];
+		for (const BaseEdge* e : pt.edges) {
+			if (!e) throw std::invalid_argument("cuba::optimizePoints: null edge");
+			if (e->landmarkVertex() != pt.landmark) throw std::invalid_argument("cuba::optimizePoints: an edge's landmark vertex is not the point's landmark");
+			const PoseVertex* p = e->poseVertex();
+			if (!p) throw std::invalid_argument("cuba::optimizePoints: an edge without a pose");
+			auto it = table.find(p);
+			if (it == table.end()) {
+				if (table.size() >= static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizePoints: too many poses");
+				it = table.emplace(p, static_cast<int32_t>(table.size())).first;
+				for (int k = 0; k < 4; k++) q.push_back(p->q.coeffs().data()[k]);
+				for (int k = 0; k < 3; k++) t.push_back(p->t.data()[k]);
+				const CameraParams& c = p->camera;
+				cam.push_back(c.fx); cam.push_back(c.fy); cam.push_back(c.cx); cam.push_back(c.cy); cam.push_back(c.bf);
 			}
-			res.rounds.push_back(st);
-			off += static_cast<size_t>(rounds[r].iterations);
+			if (e->dim() == 2) {
+				const MonoEdge* me = static_cast<const MonoEdge*>(e);
+				m2.push_back(me->measurement.data()[0]); m2.push_back(me->measurement.data()[1]);
+				om2.push_back(me->information);
+				iP2.push_back(it->second);
+			} else if (e->dim() == 3) {
+				const StereoEdge* se = static_cast<const StereoEdge*>(e);
+				for (int k = 0; k < 3; k++) m3.push_back(se->measurement.data()[k]);
+				om3.push_back(se->information);
+				iP3.push_back(it->second);
+			} else throw std::invalid_argument("cuba::optimizePoints: an edge that is neither monocular nor stereo");
 		}
+		if (om2.size() + om3.size() > static_cast<size_t>(INT32_MAX)) throw std::invalid_argument("cuba::optimizePoints: too many edges");
+		ptr2[b + 1] = static_cast<int32_t>(om2.size()); ptr3[b + 1] = static_cast<int32_t>(om3.size());
+	}
+	size_t perPoint = 0;
+	const std::vector<cuba_pose_round> rounds = c_rounds(schedule, perPoint);
+	const size_t R = rounds.size();
+	cuba_point_batch bt;
+	bt.B = static_cast<int32_t>(B); bt.P = static_cast<int32_t>(table.size());
+	bt.E2 = static_cast<int32_t>(om2.size()); bt.E3 = static_cast<int32_t>(om3.size());
+	bt.Xw = Xw.data(); bt.q = q.data(); bt.t = t.data(); bt.cam = cam.data();
+	bt.ptr2 = ptr2.data(); bt.iP2 = iP2.data(); bt.meas2 = m2.data(); bt.omega2 = om2.data();
+	bt.ptr3 = ptr3.data(); bt.iP3 = iP3.data(); bt.meas3 = m3.data(); bt.omega3 = om3.data();
+	std::vector<double> Xo(3 * B);
+	std::vector<uint8_t> lev(om2.size() + om3.size());
+	std::vector<int32_t> counts(4 * B * std::max<size_t>(R, 1)), nstats(B * std::max<size_t>(R, 1));
+	std::vector<cuba_iter_stat> stats(std::max<size_t>(B * perPoint, 1));
+	// the schedule and the batch are checked by the engine before anything runs: a refusal is the caller's input
+	const int rc = cuba_engine_optimize_points(impl.poseEngine(), &bt, static_cast<int>(R), rounds.data(), Xo.data(), lev.data(), counts.data(),
+		stats.data(), nstats.data());
+	if (rc == CUBA_ERR_INVALID) throw std::invalid_argument(std::string("cuba::optimizePoints: ") + cuba_last_error());
+	if (rc != CUBA_OK) throw std::runtime_error(std::string("cuba_b200: ") + cuba_last_error());
+	std::vector<PointResult> out(B);
+	const size_t E2 = om2.size();
+	for (size_t b = 0; b < B; b++) {
+		LandmarkVertex* l = points[b].landmark;
+		for (int k = 0; k < 3; k++) l->Xw.data()[k] = Xo[3 * b + k];
+		PointResult& res = out[b];
+		size_t i2 = static_cast<size_t>(ptr2[b]), i3 = E2 + static_cast<size_t>(ptr3[b]);
+		for (const BaseEdge* e : points[b].edges) {
+			const int lv = e->dim() == 2 ? lev[i2++] : lev[i3++];
+			res.levels.push_back(lv);
+			res.inliers += lv == 0;
+		}
+		res.rounds = round_stats(rounds, stats, nstats, b, perPoint);
 	}
 	return out;
 }

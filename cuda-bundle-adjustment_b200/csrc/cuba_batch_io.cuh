@@ -1,8 +1,9 @@
-// cuba_batch_io.cuh -- the packed layouts of the batched LM kernels (k_pose_batch, k_sim3_batch) and the kernels that validate, pack
-// and unpack a batch whose arrays are already in device memory (cuba_engine_optimize_poses_device / _sim3_device).
+// cuba_batch_io.cuh -- the packed layouts of the batched LM kernels (k_pose_batch, k_sim3_batch, k_point_batch) and the kernels that
+// validate, pack and unpack a batch whose arrays are already in device memory (cuba_engine_optimize_poses_device / _sim3_device /
+// _points_device).
 //
-// PoseLayout and Sim3Layout are the one definition of the packed records: the host round trip (Engine::optimize_poses /
-// optimize_sim3) packs into them, the device path packs into them, and cuba_*_batch_workspace_bytes sizes them.  The records are
+// PoseLayout, Sim3Layout and PointLayout are the one definition of the packed records: the host round trip (Engine::optimize_poses /
+// optimize_sim3 / optimize_points) packs into them, the device path packs into them, and cuba_*_batch_workspace_bytes sizes them.  The records are
 // those the LM kernels read: an input area (nIn doubles) followed, in the device path's workspace, by the results (nOut doubles).
 //
 // The device path runs, on one stream:
@@ -16,6 +17,7 @@
 
 #include "cuba_pose_batch.cuh"
 #include "cuba_sim3_batch.cuh"
+#include "cuba_point_batch.cuh"
 
 namespace cuba_b200 {
 namespace bio {
@@ -44,8 +46,21 @@ struct Sim3Layout {
 	}
 };
 
+// point batch, in doubles.  input: Xw [B][4] | pose [P][8] | cam [P][8] | edges [E][4] | iP [E], ptr2, ptr3 [B+1] each as int32.
+// results: Xw [B][4] | stats [nStat] (4 doubles each) | counts [B][R][4], nstats [B][R] as int32 | levels [E] bytes
+struct PointLayout {
+	size_t oPose, oCam, oEdge, oIdx, nIn;
+	size_t oStat, oInt, oLev, nOut;
+	__host__ __device__ PointLayout(size_t B, size_t P, size_t E, size_t R, size_t nStat)
+	{
+		oPose = 4 * B; oCam = oPose + 8 * P; oEdge = oCam + 8 * P; oIdx = oEdge + 4 * E; nIn = oIdx + (E + 2 * (B + 1) + 1) / 2;
+		oStat = 4 * B; oInt = oStat + 4 * nStat; oLev = oInt + (5 * B * R + 1) / 2; nOut = oLev + (E + 7) / 8;
+	}
+};
+
 constexpr int BLOCK = 256;
 constexpr unsigned MAX_GRID = 4096;   // the grid-stride kernels
+constexpr int POINTS_PER_BLOCK = BLOCK / 32;   // k_pack_points / k_unpack_points: one warp per point
 
 __device__ __forceinline__ size_t gtid() { return (size_t)blockIdx.x * blockDim.x + threadIdx.x; }
 __device__ __forceinline__ size_t gstride() { return (size_t)gridDim.x * blockDim.x; }
@@ -209,6 +224,86 @@ __global__ void __launch_bounds__(BLOCK) k_unpack_sim3(const Sim3Layout L, int B
 	if (levelsOut) {
 		const uint8_t* lv = (const uint8_t*)(o + L.oLev);
 		for (size_t k = gtid(); k < N; k += gstride()) levelsOut[k] = lv[k];
+	}
+}
+
+__global__ void __launch_bounds__(BLOCK) k_validate_points(const cuba_point_batch bt, int32_t* status)
+{
+	int bad = 0;
+	for (size_t i = gtid(); i <= (size_t)bt.B; i += gstride()) bad |= ptr_bits(bt.ptr2, bt.B, bt.E2, i) | ptr_bits(bt.ptr3, bt.B, bt.E3, i);
+	bad |= finite_bits(bt.omega2, (size_t)bt.E2, CUBA_BATCH_NONFINITE_ITEM) | finite_bits(bt.omega3, (size_t)bt.E3, CUBA_BATCH_NONFINITE_ITEM);
+	for (size_t i = gtid(); i < (size_t)bt.E2; i += gstride())
+		if (bt.iP2[i] < 0 || bt.iP2[i] >= bt.P) bad |= CUBA_BATCH_INDEX;
+	for (size_t i = gtid(); i < (size_t)bt.E3; i += gstride())
+		if (bt.iP3[i] < 0 || bt.iP3[i] >= bt.P) bad |= CUBA_BATCH_INDEX;
+	report(bad, status);
+}
+
+// one warp per point, and the pose table grid-stride: the records of Engine::optimize_points' host loop; a point's mono edge i at
+// ptr3[b] + i, its stereo edge j at ptr2[b+1] + j
+__global__ void __launch_bounds__(BLOCK) k_pack_points(const cuba_point_batch bt, const PointLayout L, double* in, const int32_t* status)
+{
+	const int B = bt.B, b = blockIdx.x * POINTS_PER_BLOCK + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+	int32_t* ip = (int32_t*)(in + L.oIdx);
+	const size_t E = (size_t)bt.E2 + (size_t)bt.E3;
+	int32_t* p2 = ip + E;
+	int32_t* p3 = p2 + B + 1;
+	const bool ok = *status == 0;
+	if (b < B && lane == 0) {
+		p2[b] = ok ? bt.ptr2[b] : 0; p3[b] = ok ? bt.ptr3[b] : 0;
+		if (b == B - 1) { p2[B] = ok ? bt.ptr2[B] : 0; p3[B] = ok ? bt.ptr3[B] : 0; }
+	}
+	if (!ok) return;
+	const size_t P = (size_t)bt.P;
+	for (size_t k = gtid(); k < 16 * P; k += gstride()) {
+		const size_t p = (k % (8 * P)) / 8;
+		const int c = (int)(k & 7);
+		in[L.oPose + k] = k < 8 * P ? (c < 4 ? bt.q[4 * p + c] : c < 7 ? bt.t[3 * p + c - 4] : 0.0) : (c < 5 ? bt.cam[5 * p + c] : 0.0);
+	}
+	if (b >= B) return;
+	if (lane < 4) in[4 * (size_t)b + lane] = lane < 3 ? bt.Xw[3 * (size_t)b + lane] : 0.0;
+	const size_t i0 = (size_t)bt.ptr2[b], n2 = (size_t)bt.ptr2[b + 1] - i0, j0 = (size_t)bt.ptr3[b], n3 = (size_t)bt.ptr3[b + 1] - j0;
+	const size_t m0 = i0 + j0, s0 = (size_t)bt.ptr2[b + 1] + j0;
+	for (size_t k = lane; k < 4 * n2; k += 32) {
+		const size_t i = i0 + k / 4;
+		const int c = (int)(k & 3);
+		in[L.oEdge + 4 * m0 + k] = c < 2 ? bt.meas2[2 * i + c] : c == 3 ? bt.omega2[i] : 0.0;
+	}
+	for (size_t k = lane; k < n2; k += 32) ip[m0 + k] = bt.iP2[i0 + k];
+	for (size_t k = lane; k < 4 * n3; k += 32) {
+		const size_t j = j0 + k / 4;
+		const int c = (int)(k & 3);
+		in[L.oEdge + 4 * s0 + k] = c < 3 ? bt.meas3[3 * j + c] : bt.omega3[j];
+	}
+	for (size_t k = lane; k < n3; k += 32) ip[s0 + k] = bt.iP3[j0 + k];
+}
+
+// one warp per point: Xw, stats, counts, nstats and the levels back in mono-then-stereo order.  statPer: stat slots per point
+__global__ void __launch_bounds__(BLOCK) k_unpack_points(const PointLayout L, int B, int R, int E2, int E3, int statPer, const double* in,
+	double* XwOut, uint8_t* levelsOut, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats, const int32_t* status)
+{
+	if (*status) return;
+	const int b = blockIdx.x * POINTS_PER_BLOCK + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+	if (b >= B) return;
+	const double* o = in + L.nIn;
+	if (lane < 3) XwOut[3 * (size_t)b + lane] = o[4 * (size_t)b + lane];
+	if (stats) {
+		const size_t n = 4 * (size_t)statPer, k0 = n * b;
+		const unsigned long long* s = (const unsigned long long*)(o + L.oStat);
+		unsigned long long* d = (unsigned long long*)stats;
+		for (size_t k = lane; k < n; k += 32) d[k0 + k] = s[k0 + k];
+	}
+	const int32_t* oi = (const int32_t*)(o + L.oInt);
+	if (counts)
+		for (int k = lane; k < 4 * R; k += 32) counts[(size_t)b * 4 * R + k] = oi[(size_t)b * 4 * R + k];
+	if (nstats)
+		for (int k = lane; k < R; k += 32) nstats[(size_t)b * R + k] = oi[4 * (size_t)B * R + (size_t)b * R + k];
+	if (levelsOut) {
+		const int32_t* p2 = (const int32_t*)(in + L.oIdx) + (size_t)E2 + (size_t)E3;
+		const int32_t* p3 = p2 + B + 1;
+		const uint8_t* lv = (const uint8_t*)(o + L.oLev);
+		for (size_t i = (size_t)p2[b] + lane; i < (size_t)p2[b + 1]; i += 32) levelsOut[i] = lv[(size_t)p3[b] + i];
+		for (size_t j = (size_t)p3[b] + lane; j < (size_t)p3[b + 1]; j += 32) levelsOut[(size_t)E2 + j] = lv[(size_t)p2[b + 1] + j];
 	}
 }
 

@@ -30,6 +30,7 @@
 #include "cuba_levels.cuh"
 #include "cuba_pose_batch.cuh"
 #include "cuba_sim3_batch.cuh"
+#include "cuba_point_batch.cuh"
 #include "cuba_batch_io.cuh"
 #include "cuba_problem_io.cuh"
 #include "cuba_schur3.cuh"
@@ -369,6 +370,8 @@ struct EngineBase {
 		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) = 0;
 	virtual int optimize_sim3(const cuba_sim3_batch* bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
 		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats) = 0;
+	virtual int optimize_points(const cuba_point_batch* bt, const pb::Schedule& s, double* XwOut, uint8_t* levelsOut, int32_t* counts,
+		cuba_iter_stat* stats, int32_t* nstats) = 0;
 };
 
 template <typename T>
@@ -451,8 +454,8 @@ struct Engine : EngineBase {
 	DBuf<unsigned char> lvLevel;   // [E] in edge-id order; a rank reads and writes its own edges only
 	DBuf<int> lvPartial;
 	DBuf<double> lvCount;
-	// the batched LM kernels (optimize_poses, optimize_sim3, one after the other on the stream): the packed batch and the packed
-	// results, device and page-locked host copies
+	// the batched LM kernels (optimize_poses, optimize_sim3, optimize_points, one after the other on the stream): the packed batch
+	// and the packed results, device and page-locked host copies
 	DBuf<double> batchIn, batchOut;
 	PinnedBuf batchHostIn, batchHostOut;
 	DBuf<Scalars> dScal;
@@ -2487,13 +2490,14 @@ struct Engine : EngineBase {
 	// results from batchHostOut.  Always fp64, on this engine's stream; they touch nothing of the engine's problem.  The batch was validated by the caller.
 	static_assert(sizeof(lm::IterStat) == sizeof(cuba_iter_stat) && sizeof(lm::IterStat) == 32, "cuba_iter_stat layout");
 
-	// one H2D of the packed batch (nIn doubles), the launch of one CTA per problem, one D2H of the packed results (nOut doubles)
+	// one H2D of the packed batch (nIn doubles), the launch of `grid` CTAs of lm::BLOCK threads, one D2H of the packed results (nOut
+	// doubles)
 	template <class Args, class Params>
-	int batch_round_trip(void (*kernel)(Args, Params), const Args& a, const Params& p, size_t nIn, size_t nOut)
+	int batch_round_trip(void (*kernel)(Args, Params), unsigned grid, const Args& a, const Params& p, size_t nIn, size_t nOut)
 	{
 		CUDA_TRY(cudaMemcpyAsync(batchIn.p, batchHostIn.p, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
 		g_h2dBytes += (long long)(sizeof(double) * nIn);
-		kernel<<<(unsigned)a.B, lm::BLOCK, 0, stream>>>(a, p);
+		kernel<<<grid, lm::BLOCK, 0, stream>>>(a, p);
 		launches++;
 		CUDA_TRY(cudaGetLastError());
 		CUDA_TRY(cudaMemcpyAsync(batchHostOut.p, batchOut.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
@@ -2546,7 +2550,7 @@ struct Engine : EngineBase {
 		a.stats = stats ? (lm::IterStat*)(batchOut.p + oStat) : nullptr;
 		a.counts = (int*)(batchOut.p + oInt); a.nstats = a.counts + 4 * B * R;
 		a.level = (unsigned char*)(batchOut.p + oLev);
-		const int rc = batch_round_trip(pb::k_pose_batch, a, s, nIn, nOut); if (rc) return rc;
+		const int rc = batch_round_trip(pb::k_pose_batch, (unsigned)B, a, s, nIn, nOut); if (rc) return rc;
 		const double* o = (const double*)batchHostOut.p;
 		for (size_t b = 0; b < B; b++) {
 			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
@@ -2601,7 +2605,7 @@ struct Engine : EngineBase {
 		a.stats = stats ? (lm::IterStat*)(batchOut.p + oStat) : nullptr;
 		a.ninliers = (int*)(batchOut.p + oInt); a.nstats = a.ninliers + B;
 		a.level = (unsigned char*)(batchOut.p + oLev);
-		const int rc = batch_round_trip(s3::k_sim3_batch, a, p, nIn, nOut); if (rc) return rc;
+		const int rc = batch_round_trip(s3::k_sim3_batch, (unsigned)B, a, p, nIn, nOut); if (rc) return rc;
 		const double* o = (const double*)batchHostOut.p;
 		for (size_t b = 0; b < B; b++) {
 			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
@@ -2613,6 +2617,74 @@ struct Engine : EngineBase {
 		if (ninliers) memcpy(ninliers, oi, sizeof(int32_t) * B);
 		if (nstats) memcpy(nstats, oi + B, sizeof(int32_t) * 2 * B);
 		if (levelsOut && N) memcpy(levelsOut, (const unsigned char*)(o + oLev), N);
+		return CUBA_OK;
+	}
+
+	// batched structure-only refinement (cuba_point_batch.cuh)
+	int optimize_points(const cuba_point_batch* bt, const pb::Schedule& s, double* XwOut, uint8_t* levelsOut, int32_t* counts,
+		cuba_iter_stat* stats, int32_t* nstats) override
+	{
+		const size_t B = (size_t)bt->B, P = (size_t)bt->P, R = (size_t)s.n;
+		if (B == 0) return CUBA_OK;
+		const size_t E2 = (size_t)bt->E2, E3 = (size_t)bt->E3, E = E2 + E3;
+		const size_t nStat = stats ? B * (size_t)s.statOff[s.n] : 0;
+		const bio::PointLayout L(B, P, E, R, nStat);
+		CUDA_TRY(batchHostIn.grow(sizeof(double) * L.nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * L.nOut));
+		CUDA_TRY(batchIn.alloc(L.nIn)); CUDA_TRY(batchOut.alloc(L.nOut));
+		double* h = (double*)batchHostIn.p;
+		for (size_t p = 0; p < P; p++) {
+			double* d = h + L.oPose + 8 * p;
+			for (int k = 0; k < 4; k++) d[k] = bt->q[4 * p + k];
+			for (int k = 0; k < 3; k++) d[4 + k] = bt->t[3 * p + k];
+			d[7] = 0;
+			double* c = h + L.oCam + 8 * p;
+			for (int k = 0; k < 5; k++) c[k] = bt->cam[5 * p + k];
+			c[5] = c[6] = c[7] = 0;
+		}
+		int32_t* hi = (int32_t*)(h + L.oIdx);
+		for (size_t b = 0; b < B; b++) {
+			double* x = h + 4 * b;
+			for (int k = 0; k < 3; k++) x[k] = bt->Xw[3 * b + k];
+			x[3] = 0;
+			// a point's edges are contiguous, its mono edges first: mono i at ptr3[b] + i, stereo j at ptr2[b+1] + j
+			for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) {
+				const size_t k = (size_t)bt->ptr3[b] + i;
+				double* d = h + L.oEdge + 4 * k;
+				d[0] = bt->meas2[2 * i]; d[1] = bt->meas2[2 * i + 1]; d[2] = 0; d[3] = bt->omega2[i];
+				hi[k] = bt->iP2[i];
+			}
+			for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) {
+				const size_t k = (size_t)bt->ptr2[b + 1] + j;
+				double* d = h + L.oEdge + 4 * k;
+				d[0] = bt->meas3[3 * j]; d[1] = bt->meas3[3 * j + 1]; d[2] = bt->meas3[3 * j + 2]; d[3] = bt->omega3[j];
+				hi[k] = bt->iP3[j];
+			}
+		}
+		memcpy(hi + E, bt->ptr2, sizeof(int32_t) * (B + 1));
+		memcpy(hi + E + B + 1, bt->ptr3, sizeof(int32_t) * (B + 1));
+		ptb::Args a;
+		a.B = (int)B;
+		a.Xw = batchIn.p; a.pose = batchIn.p + L.oPose; a.cam = batchIn.p + L.oCam; a.edge = batchIn.p + L.oEdge;
+		a.iP = (const int*)(batchIn.p + L.oIdx); a.ptr2 = a.iP + E; a.ptr3 = a.ptr2 + B + 1;
+		a.XwOut = batchOut.p;
+		a.stats = stats ? (lm::IterStat*)(batchOut.p + L.oStat) : nullptr;
+		a.counts = (int*)(batchOut.p + L.oInt); a.nstats = a.counts + 4 * B * R;
+		a.level = (unsigned char*)(batchOut.p + L.oLev);
+		const int rc = batch_round_trip(ptb::k_point_batch, (unsigned)((B + ptb::WARPS - 1) / ptb::WARPS), a, s, L.nIn, L.nOut); if (rc) return rc;
+		const double* o = (const double*)batchHostOut.p;
+		for (size_t b = 0; b < B; b++)
+			for (int k = 0; k < 3; k++) XwOut[3 * b + k] = o[4 * b + k];
+		if (stats && nStat) memcpy(stats, o + L.oStat, sizeof(cuba_iter_stat) * nStat);
+		const int32_t* oi = (const int32_t*)(o + L.oInt);
+		if (counts) memcpy(counts, oi, sizeof(int32_t) * 4 * B * R);
+		if (nstats) memcpy(nstats, oi + 4 * B * R, sizeof(int32_t) * B * R);
+		if (levelsOut) {
+			const unsigned char* lv = (const unsigned char*)(o + L.oLev);
+			for (size_t b = 0; b < B; b++) {
+				for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) levelsOut[i] = lv[(size_t)bt->ptr3[b] + i];
+				for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) levelsOut[E2 + j] = lv[(size_t)bt->ptr2[b + 1] + j];
+			}
+		}
 		return CUBA_OK;
 	}
 
@@ -3133,28 +3205,28 @@ static bool all_finite(const double* p, size_t n)
 	return true;
 }
 
-// the schedule of optimize_poses, checked: everything a host can see without the batch
-static int pose_schedule(int nrounds, const cuba_pose_round* rounds, pb::Schedule& s)
+// the schedule of optimize_poses / optimize_points (`what`), checked: everything a host can see without the batch
+static int pose_schedule(int nrounds, const cuba_pose_round* rounds, pb::Schedule& s, const char* what = "optimize_poses")
 {
-	if (nrounds < 1 || nrounds > CUBA_POSE_MAX_ROUNDS || !rounds) return fail(CUBA_ERR_INVALID, "optimize_poses: nrounds outside 1..CUBA_POSE_MAX_ROUNDS");
+	if (nrounds < 1 || nrounds > CUBA_POSE_MAX_ROUNDS || !rounds) return fail(CUBA_ERR_INVALID, std::string(what) + ": nrounds outside 1..CUBA_POSE_MAX_ROUNDS");
 	static_assert(CUBA_POSE_MAX_ROUNDS == pb::MAX_ROUNDS, "round limit");
 	memset(&s, 0, sizeof(s));
 	s.n = nrounds;
 	long long off = 0;
 	for (int r = 0; r < nrounds; r++) {
 		const cuba_pose_round& R = rounds[r];
-		if (R.iterations < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: negative iterations");
-		if (R.flags & ~(CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE)) return fail(CUBA_ERR_INVALID, "optimize_poses: unknown flag");
+		if (R.iterations < 0) return fail(CUBA_ERR_INVALID, std::string(what) + ": negative iterations");
+		if (R.flags & ~(CUBA_CLASSIFY_DEPTH | CUBA_CLASSIFY_REINCLUDE)) return fail(CUBA_ERR_INVALID, std::string(what) + ": unknown flag");
 		for (int k = 0; k < 2; k++) {
-			if (R.kernel_type[k] < CUBA_ROBUST_NONE || R.kernel_type[k] > CUBA_ROBUST_TUKEY) return fail(CUBA_ERR_INVALID, "optimize_poses: unknown kernel type");
-			if (!std::isfinite(R.delta[k])) return fail(CUBA_ERR_INVALID, "optimize_poses: non-finite delta");
+			if (R.kernel_type[k] < CUBA_ROBUST_NONE || R.kernel_type[k] > CUBA_ROBUST_TUKEY) return fail(CUBA_ERR_INVALID, std::string(what) + ": unknown kernel type");
+			if (!std::isfinite(R.delta[k])) return fail(CUBA_ERR_INVALID, std::string(what) + ": non-finite delta");
 			s.rk[r].type[k] = R.kernel_type[k]; s.rk[r].delta[k] = R.delta[k];
 		}
 		s.r[r].iterations = R.iterations; s.r[r].restart = R.restart != 0; s.r[r].flags = R.flags;
 		s.r[r].chi2[0] = R.chi2_mono; s.r[r].chi2[1] = R.chi2_stereo;
 		s.statOff[r] = (int)off;
 		off += R.iterations;
-		if (off > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many iterations");
+		if (off > INT32_MAX) return fail(CUBA_ERR_INVALID, std::string(what) + ": too many iterations");
 	}
 	s.statOff[nrounds] = (int)off;
 	return CUBA_OK;
@@ -3176,6 +3248,51 @@ int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nr
 	rc = csr_ok("optimize_poses: ptr3", B, bt->E3, bt->ptr3, { bt->X3, bt->meas3, bt->omega3 }); if (rc) return rc;
 	if (!all_finite(bt->omega2, bt->E2) || !all_finite(bt->omega3, bt->E3)) return fail(CUBA_ERR_INVALID, "optimize_poses: non-finite omega");
 	return e->impl->optimize_poses(bt, s, q_out, t_out, levels_out, counts, stats, nstats);
+}
+
+// host arrays of a point batch: a pose index outside [0, P)
+static bool poses_in_range(const int32_t* iP, int n, int P)
+{
+	for (int i = 0; i < n; i++)
+		if (iP[i] < 0 || iP[i] >= P) return false;
+	return true;
+}
+
+// the checks of optimize_points and optimize_points_device that need no element of the batch's arrays
+static int point_batch_args(const cuba_point_batch* bt, int nrounds, const cuba_pose_round* rounds, pb::Schedule& s)
+{
+	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_points: null batch");
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_points: B < 0");
+	if (bt->P < 0) return fail(CUBA_ERR_INVALID, "optimize_points: P < 0");
+	if (bt->E2 < 0) return fail(CUBA_ERR_INVALID, "optimize_points: E2 < 0");
+	if (bt->E3 < 0) return fail(CUBA_ERR_INVALID, "optimize_points: E3 < 0");
+	return pose_schedule(nrounds, rounds, s, "optimize_points");
+}
+
+// point_batch_args' checks of the pointers, for B > 0
+static int point_batch_pointers(const cuba_point_batch* bt, const double* XwOut)
+{
+	if (!bt->Xw || !XwOut) return fail(CUBA_ERR_INVALID, "optimize_points: null Xw");
+	if (bt->P > 0 && (!bt->q || !bt->t || !bt->cam)) return fail(CUBA_ERR_INVALID, "optimize_points: null pose array");
+	if ((long long)bt->E2 + bt->E3 > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_points: too many edges");
+	return CUBA_OK;
+}
+
+int cuba_engine_optimize_points(cuba_engine* e, const cuba_point_batch* bt, int nrounds, const cuba_pose_round* rounds, double* Xw_out,
+	uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats)
+{
+	ENGINE_OR_FAIL(e);
+	pb::Schedule s;
+	{ const int rc0 = point_batch_args(bt, nrounds, rounds, s); if (rc0) return rc0; }
+	const int B = bt->B;
+	if (B == 0) return CUBA_OK;
+	int rc = point_batch_pointers(bt, Xw_out); if (rc) return rc;
+	rc = csr_ok("optimize_points: ptr2", B, bt->E2, bt->ptr2, { bt->iP2, bt->meas2, bt->omega2 }); if (rc) return rc;
+	rc = csr_ok("optimize_points: ptr3", B, bt->E3, bt->ptr3, { bt->iP3, bt->meas3, bt->omega3 }); if (rc) return rc;
+	if (!poses_in_range(bt->iP2, bt->E2, bt->P)) return fail(CUBA_ERR_INVALID, "optimize_points: iP2 outside [0, P)");
+	if (!poses_in_range(bt->iP3, bt->E3, bt->P)) return fail(CUBA_ERR_INVALID, "optimize_points: iP3 outside [0, P)");
+	if (!all_finite(bt->omega2, bt->E2) || !all_finite(bt->omega3, bt->E3)) return fail(CUBA_ERR_INVALID, "optimize_points: non-finite omega");
+	return e->impl->optimize_points(bt, s, Xw_out, levels_out, counts, stats, nstats);
 }
 
 // the parameters of optimize_sim3, checked
@@ -3358,6 +3475,62 @@ int cuba_engine_optimize_sim3_device(cuba_engine* e, const cuba_sim3_batch* bt, 
 	s3::k_sim3_batch<<<(unsigned)B, lm::BLOCK, 0, st>>>(a, p);
 	bio::k_unpack_sim3<<<bio::grid_for(std::max(8 * nb, std::max(4 * nStat, N))), bio::BLOCK, 0, st>>>(L, B, bt->N, nStat, in, q_out, t_out,
 		s_out, levels_out, ninliers, stats, nstats, status);
+	CUDA_TRY(cudaGetLastError());
+	return CUBA_OK;
+}
+
+static size_t point_workspace(int B, int P, int E2, int E3, const pb::Schedule& s, bool withStats)
+{
+	const size_t nb = (size_t)B;
+	const bio::PointLayout L(nb, (size_t)P, (size_t)E2 + (size_t)E3, (size_t)s.n, withStats ? nb * (size_t)s.statOff[s.n] : 0);
+	return sizeof(double) * (L.nIn + L.nOut);
+}
+
+size_t cuba_point_batch_workspace_bytes(int B, int P, int E2, int E3, int nrounds, const cuba_pose_round* rounds, int with_stats)
+{
+	pb::Schedule s;
+	if (B <= 0 || P < 0 || E2 < 0 || E3 < 0 || (long long)E2 + E3 > INT32_MAX) return 0;
+	const std::string err = g_err;
+	const int rc = pose_schedule(nrounds, rounds, s);
+	g_err = err;       // a size query leaves the last error alone
+	return rc ? 0 : point_workspace(B, P, E2, E3, s, with_stats != 0);
+}
+
+int cuba_engine_optimize_points_device(cuba_engine* e, const cuba_point_batch* bt, int nrounds, const cuba_pose_round* rounds,
+	void* workspace, size_t workspace_bytes, double* Xw_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats,
+	int32_t* nstats, int32_t* status, void* stream)
+{
+	pb::Schedule s;
+	{ const int rc0 = point_batch_args(bt, nrounds, rounds, s); if (rc0) return rc0; }
+	if (!status) return fail(CUBA_ERR_INVALID, "optimize_points_device: null status");
+	const int B = bt->B;
+	if (B > 0) {
+		int rc = point_batch_pointers(bt, Xw_out); if (rc) return rc;
+		rc = csr_present("optimize_points: ptr2", bt->E2, bt->ptr2, { bt->iP2, bt->meas2, bt->omega2 }); if (rc) return rc;
+		rc = csr_present("optimize_points: ptr3", bt->E3, bt->ptr3, { bt->iP3, bt->meas3, bt->omega3 }); if (rc) return rc;
+		rc = workspace_ok("optimize_points_device", workspace, workspace_bytes, point_workspace(B, bt->P, bt->E2, bt->E3, s, stats != nullptr)); if (rc) return rc;
+	}
+	ENGINE_OR_FAIL(e);
+	const cudaStream_t st = batch_stream(e, stream);
+	CUDA_TRY(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+	if (B == 0) return CUBA_OK;
+	const size_t nb = (size_t)B, E = (size_t)bt->E2 + (size_t)bt->E3, statPer = (size_t)s.statOff[s.n];
+	const bio::PointLayout L(nb, (size_t)bt->P, E, (size_t)s.n, stats ? nb * statPer : 0);
+	double* in = (double*)workspace;
+	const unsigned gridIo = (unsigned)((nb + bio::POINTS_PER_BLOCK - 1) / bio::POINTS_PER_BLOCK);
+	bio::k_validate_points<<<bio::grid_for(std::max(nb + 1, E)), bio::BLOCK, 0, st>>>(*bt, status);
+	bio::k_pack_points<<<gridIo, bio::BLOCK, 0, st>>>(*bt, L, in, status);
+	ptb::Args a;
+	a.B = B;
+	a.Xw = in; a.pose = in + L.oPose; a.cam = in + L.oCam; a.edge = in + L.oEdge;
+	a.iP = (const int*)(in + L.oIdx); a.ptr2 = a.iP + E; a.ptr3 = a.ptr2 + nb + 1;
+	double* o = in + L.nIn;
+	a.XwOut = o;
+	a.stats = stats ? (lm::IterStat*)(o + L.oStat) : nullptr;
+	a.counts = (int*)(o + L.oInt); a.nstats = a.counts + 4 * nb * (size_t)s.n;
+	a.level = (unsigned char*)(o + L.oLev);
+	ptb::k_point_batch<<<(unsigned)((nb + ptb::WARPS - 1) / ptb::WARPS), lm::BLOCK, 0, st>>>(a, s);
+	bio::k_unpack_points<<<gridIo, bio::BLOCK, 0, st>>>(L, B, s.n, bt->E2, bt->E3, (int)statPer, in, Xw_out, levels_out, counts, stats, nstats, status);
 	CUDA_TRY(cudaGetLastError());
 	return CUBA_OK;
 }

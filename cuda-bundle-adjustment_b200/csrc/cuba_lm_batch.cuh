@@ -6,6 +6,8 @@
 // trial state from there.  All sums are fixed-order warp trees followed by a fixed-order sum over the warps, so a problem's result is
 // bit-reproducible and depends neither on the other problems of the batch nor on its position.  The sums over warps are done by every
 // thread, which therefore holds the same F, lambda and nu and follows the same control flow without a broadcast.
+//
+// optimize_warp is the same loop for one small problem per warp (k_point_batch), for problems of a few items each.
 #pragma once
 
 #include "cuba_kernels.cuh"
@@ -116,6 +118,57 @@ __device__ __forceinline__ int optimize(const Problem& P, Shared<Problem::N>& sh
 			st.iteration = it; st.trials = trials; st.chi2 = F; st.lambda = lambda; st.pcg_iters = 0; st.pcg_failed = 0;
 		}
 		__syncthreads();     // sys and the trial state are rewritten by the next iteration
+		if (stop(q, rho, lambda)) return it + 1;
+	}
+	return iterations;
+}
+
+// optimize(iterations) of one problem per WARP (k_point_batch): the loop of optimize above with the state X[N] in registers.  Every
+// entry of the packed system and every chi2 is a warp_sum, whose xor butterfly leaves bitwise the same value in every lane, so every
+// lane solves, updates and decides identically: no shared memory, no broadcast, no barrier.  The problem type supplies
+//   N                   the number of unknowns, and the size of the state
+//   linearize(acc, X)   per lane: adds its items' share of the packed system and of the robust chi2 at state X to acc[NSYS]
+//   chi2(X)             per lane: its items' robust chi2 at state X
+//   solve(sys, lambda, x)   x solves (H + lambda I) x = b
+//   update(x, X, Xt)    Xt = X moved by the step x
+// Lane 0 writes one IterStat per iteration to stats[0 ..] unless stats is null; returns the number written.  With no item included:
+// no iteration, X untouched.
+template <class Problem>
+__device__ __forceinline__ int optimize_warp(const Problem& P, double X[Problem::N], int included, int iterations, IterStat* stats)
+{
+	constexpr int N = Problem::N, NSYS = N * (N + 1) / 2 + N + 1;
+	if (included == 0) return 0;
+	double nu = 2, lambda = 0, F = 0;
+	for (int it = 0; it < iterations; it++) {
+		double sys[NSYS];
+#pragma unroll
+		for (int i = 0; i < NSYS; i++) sys[i] = 0;
+		P.linearize(sys, X);
+#pragma unroll
+		for (int i = 0; i < NSYS; i++) sys[i] = warp_sum(sys[i]);
+		F = sys[NSYS - 1];
+		if (it == 0) lambda = initial_lambda(max_diagonal<N>(sys));
+		int q = 0, trials = 0;
+		double rho = -1;
+		for (; q < MAX_TRIALS && rho < 0; q++) {
+			trials++;
+			double x[N], Xt[N];
+			P.solve(sys, lambda, x);
+			P.update(x, X, Xt);
+			const double predicted = predicted_decrease<N>(sys, lambda, x);
+			const double Fhat = warp_sum(P.chi2(Xt));
+			rho = gain_ratio(F, Fhat, predicted);
+			if (update_damping(rho, lambda, nu)) {
+				F = Fhat;
+#pragma unroll
+				for (int i = 0; i < N; i++) X[i] = Xt[i];
+				break;
+			}
+		}
+		if ((threadIdx.x & 31) == 0 && stats) {
+			IterStat& st = stats[it];
+			st.iteration = it; st.trials = trials; st.chi2 = F; st.lambda = lambda; st.pcg_iters = 0; st.pcg_failed = 0;
+		}
 		if (stop(q, rho, lambda)) return it + 1;
 	}
 	return iterations;

@@ -214,6 +214,73 @@ def pose_batch_arrays(frames):
 
 
 @dataclasses.dataclass
+class PointBatch:
+    """The points of Engine.optimize_points: a table of P poses, held fixed, and B points, each an initial position and its edges
+    (mono [ptr2[b], ptr2[b+1]), stereo [ptr3[b], ptr3[b+1])), each edge naming its pose by index in the table."""
+    q: np.ndarray       # [P,4] x,y,z,w
+    t: np.ndarray       # [P,3]
+    cam: np.ndarray     # [P,5]
+    Xw: np.ndarray      # [B,3]
+    ptr2: np.ndarray    # [B+1] int32
+    iP2: np.ndarray     # [E2] int32
+    meas2: np.ndarray   # [E2,2]
+    omega2: np.ndarray  # [E2]
+    ptr3: np.ndarray    # [B+1] int32
+    iP3: np.ndarray     # [E3] int32
+    meas3: np.ndarray   # [E3,3]
+    omega3: np.ndarray  # [E3]
+    landmarks: np.ndarray = None    # [B] landmark ids (iL) of the flat problem the points were cut from
+    mono_ids: np.ndarray = None     # [E2] edge ids (0..E2-1) of that flat problem
+    stereo_ids: np.ndarray = None   # [E3] ids among its stereo edges
+
+    @property
+    def B(self):
+        return len(self.ptr2) - 1
+
+    def arrays(self):
+        """the keyword arguments of Engine.optimize_points_flat (numpy) and, moved to the GPU, of Engine.optimize_points_device"""
+        return {k: getattr(self, k) for k in ("Xw", "q", "t", "cam", "ptr2", "iP2", "meas2", "omega2", "ptr3", "iP3", "meas3", "omega3")}
+
+    def sub_problem(self, b, Xw=None, keep=None) -> FlatProblem:
+        """The engine's sub-problem of point b: the poses its kept edges name (ascending table index) as fixed vertices, the point at Xw
+        (default: its input position) as the only free landmark, and the edges where keep[mono + stereo] is true (default: all)."""
+        m = np.arange(self.ptr2[b], self.ptr2[b + 1]); s = np.arange(self.ptr3[b], self.ptr3[b + 1])
+        keep = np.ones(len(m) + len(s), bool) if keep is None else np.asarray(keep, bool)
+        m, s = m[keep[:len(m)]], s[keep[len(m):]]
+        poses, inv = np.unique(np.concatenate([self.iP2[m], self.iP3[s]]), return_inverse=True)
+        ip = inv.astype(np.int32)
+        X = self.Xw[b] if Xw is None else Xw
+        return FlatProblem(
+            Pall=len(poses), numP=0, Lall=1, numL=1, q=self.q[poses].reshape(-1, 4).copy(), t=self.t[poses].reshape(-1, 3).copy(),
+            cam=self.cam[poses].reshape(-1, 5).copy(), Xw=np.array(X, dtype=np.float64).reshape(1, 3),
+            idx2=np.stack([ip[:len(m)], np.zeros(len(m), np.int32)], 1).astype(np.int32), meas2=self.meas2[m].reshape(-1, 2),
+            omega2=self.omega2[m].copy(), idx3=np.stack([ip[len(m):], np.zeros(len(s), np.int32)], 1).astype(np.int32),
+            meas3=self.meas3[s].reshape(-1, 3), omega3=self.omega3[s].copy())
+
+
+def point_batch(prob: FlatProblem, landmarks) -> PointBatch:
+    """The points of the landmarks (indices iL of prob) against prob's whole pose table: each landmark at prob.Xw with all of its
+    edges in edge-id order.  Point b's sub_problem is what flatten() gives for the graph of that one landmark, free, with its edges
+    and their poses, fixed."""
+    def groups(idx):
+        order = np.argsort(idx[:, 1], kind="stable")
+        return order, np.searchsorted(idx[order, 1], np.arange(prob.Lall + 1))
+    o2, p2 = groups(prob.idx2)
+    o3, p3 = groups(prob.idx3)
+    L = np.asarray(landmarks, np.int64).reshape(-1)
+    m = np.concatenate([o2[p2[l]:p2[l + 1]] for l in L]).astype(np.int64) if len(L) else np.zeros(0, np.int64)
+    s = np.concatenate([o3[p3[l]:p3[l + 1]] for l in L]).astype(np.int64) if len(L) else np.zeros(0, np.int64)
+    return PointBatch(
+        q=np.ascontiguousarray(prob.q, dtype=np.float64).reshape(-1, 4), t=np.ascontiguousarray(prob.t, dtype=np.float64).reshape(-1, 3),
+        cam=np.ascontiguousarray(prob.cam, dtype=np.float64).reshape(-1, 5), Xw=np.ascontiguousarray(prob.Xw[L], dtype=np.float64).reshape(-1, 3),
+        ptr2=_ptr(p2[L + 1] - p2[L]), iP2=np.ascontiguousarray(prob.idx2[m, 0], dtype=np.int32),
+        meas2=np.ascontiguousarray(prob.meas2[m], dtype=np.float64).reshape(-1, 2), omega2=np.ascontiguousarray(prob.omega2[m], dtype=np.float64),
+        ptr3=_ptr(p3[L + 1] - p3[L]), iP3=np.ascontiguousarray(prob.idx3[s, 0], dtype=np.int32),
+        meas3=np.ascontiguousarray(prob.meas3[s], dtype=np.float64).reshape(-1, 3), omega3=np.ascontiguousarray(prob.omega3[s], dtype=np.float64),
+        landmarks=L, mono_ids=m, stereo_ids=s)
+
+
+@dataclasses.dataclass
 class Sim3Problem:
     """One problem of Engine.optimize_sim3 (ORB-SLAM2's OptimizeSim3): S12 = (q, t, s), S12 X = s R(q) X + t, from camera 2 into
     camera 1, and N matched pairs: X1 / X2 the point in camera-1 / camera-2 coordinates, obs1 / obs2 its keypoints, omega1 / omega2

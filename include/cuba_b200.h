@@ -353,20 +353,58 @@ typedef struct cuba_sim3_params {
 int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* batch, const cuba_sim3_params* params, double* q_out, double* t_out,
 	double* s_out, uint8_t* levels_out, int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats);
 
-/* ---- the same two batches on device-resident data (csrc/cuba_batch_io.cuh) ----
+/* Structure-only refinement of many map points (g2o's StructureOnlySolver; the refinement of newly triangulated points, or of the
+ * points after their keyframes moved).  Point b is one free world position Xw[b] and its edges: monocular [ptr2[b], ptr2[b+1]) and
+ * stereo [ptr3[b], ptr3[b+1]), ptr2[0] = ptr3[0] = 0, ptr2[B] = E2, ptr3[B] = E3.  Edge k names its pose iP in a table of P poses
+ * (q, t, cam; Xc = R(q) Xw + t as in cuba_problem), which are held fixed and shared by index.  Host arrays, fp64.  Array pointers
+ * of an empty edge type, and the pose table when P = 0, may be NULL. */
+typedef struct cuba_point_batch {
+	int32_t B, P, E2, E3;
+	const double* Xw;      /* [3B] initial position of each point                                  */
+	const double* q;       /* [4P] x,y,z,w                                                         */
+	const double* t;       /* [3P]                                                                 */
+	const double* cam;     /* [5P] fx,fy,cx,cy,bf                                                  */
+	const int32_t* ptr2;   /* [B+1]                                                                */
+	const int32_t* iP2;    /* [E2] pose of each monocular edge, in [0, P)                          */
+	const double* meas2;   /* [2*E2]                                                               */
+	const double* omega2;  /* [E2]                                                                 */
+	const int32_t* ptr3;   /* [B+1]                                                                */
+	const int32_t* iP3;    /* [E3]                                                                 */
+	const double* meas3;   /* [3*E3]                                                               */
+	const double* omega3;  /* [E3]                                                                 */
+} cuba_point_batch;
+
+/* Runs the schedule of cuba_pose_round (restart = from the point's input position) on every point: ONE kernel launch (one warp per
+ * point, four points per CTA), one host->device and one device->host copy.  Every edge starts at level 0.  Each point's result is
+ * what the engine computes for the point's sub-problem: set_problem with the point's distinct observing poses as fixed pose vertices,
+ * the point as the only free landmark and its edges; per round set_robust_kernel, set_state to the input Xw on restart,
+ * optimize(iterations), classify_edges.  The LM rules are those of cuba_engine_optimize (lambda from the largest of Hll's 3 diagonal
+ * entries) and the damped solve is the engine's landmark-only arithmetic, so the two agree to rounding.  Always fp64; each point's
+ * result is bit-reproducible and independent of the other points of the batch and of its position in it.  A point without edges
+ * comes back unchanged with no iteration and zero counts; a round with no edge at level 0 writes no iteration.  Runs on the engine's
+ * device and stream, ignores set_comm, and neither reads nor changes the engine's problem, state, levels or solver state.
+ * Outputs: Xw_out [3B]; levels_out [E2+E3] (mono then stereo, 0/1 after the last round); counts [B][nrounds][4] (as classify_edges);
+ * stats [B][sum of iterations] (round r of point b at b * sum + iterations of rounds < r, pcg fields 0); nstats [B][nrounds].
+ * Every output except Xw_out may be NULL.  B = 0 does nothing.
+ * CUBA_ERR_INVALID, with nothing run, for B, P, E2 or E3 < 0, a malformed ptr2 / ptr3, an iP outside [0, P), a non-finite omega or
+ * delta, or a schedule cuba_engine_optimize_poses refuses. */
+int cuba_engine_optimize_points(cuba_engine* e, const cuba_point_batch* batch, int nrounds, const cuba_pose_round* rounds,
+	double* Xw_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats);
+
+/* ---- the same three batches on device-resident data (csrc/cuba_batch_io.cuh) ----
  * Every array pointer of the batch and every output is a DEVICE pointer on the engine's device; the schedule / parameters stay host
  * structs.  The call validates, packs, runs the batch's kernel and unpacks on `stream` (NULL = the engine's stream; the legacy default
  * stream is cudaStreamLegacy): it copies nothing between host and device, never synchronises, allocates nothing and neither reads nor
  * changes any engine state (the engine's buffers, its launch count included), so it can be captured into a CUDA graph, and two calls
  * with two workspaces on two streams are independent.  The results are bit for bit those of cuba_engine_optimize_poses /
- * _optimize_sim3: the same packed records go to the same kernel.  Output layouts are theirs.
+ * _optimize_sim3 / _optimize_points: the same packed records go to the same kernel.  Output layouts are theirs.
  *
  * The workspace is the caller's: at least *_workspace_bytes(...) bytes of device memory, 8-byte aligned, used only during the call's
  * work on `stream`.  The size functions are host-only; they return 0 for B <= 0 and for arguments the call itself refuses.  with_stats:
  * whether `stats` will be non-NULL.
  *
  * Host-side checks (CUBA_ERR_INVALID before any launch, with the messages of the host entry points where they check the same thing,
- * and before the engine is looked at): a NULL batch, B < 0, N < 0 or a negative edge count, the schedule / parameters, NULL pointers
+ * and before the engine is looked at): a NULL batch, B < 0, N < 0, P < 0 or a negative edge count, the schedule / parameters, NULL pointers
  * the host entry points refuse, a NULL status, a workspace that is too small or misaligned.
  * Data-dependent checks run on the device and land in *status (a device int32, written on the stream by every call that returns
  * CUBA_OK, B = 0 included; a call refused on the host writes nothing): 0 when the batch is valid, else the OR of the CUBA_BATCH_* bits of every check that failed.  When *status != 0 no output array is written. */
@@ -377,6 +415,7 @@ int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* batch, cons
 #define CUBA_BATCH_NONFINITE_ITEM 8      /* a non-finite omega (pose batch) or pair value (X1, X2, obs1, obs2, omega) */
 #define CUBA_BATCH_NONFINITE_PROBLEM 16  /* Sim3: a non-finite q, t, s or intrinsic                                   */
 #define CUBA_BATCH_SCALE 32              /* Sim3: a finite s <= 0                                                     */
+#define CUBA_BATCH_INDEX 64              /* points: an iP outside [0, P)                                              */
 size_t cuba_pose_batch_workspace_bytes(int B, int E2, int E3, int nrounds, const cuba_pose_round* rounds, int with_stats);
 int cuba_engine_optimize_poses_device(cuba_engine* e, const cuba_pose_batch* batch_dev, int nrounds, const cuba_pose_round* rounds,
 	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats,
@@ -385,6 +424,10 @@ size_t cuba_sim3_batch_workspace_bytes(int B, int N, const cuba_sim3_params* par
 int cuba_engine_optimize_sim3_device(cuba_engine* e, const cuba_sim3_batch* batch_dev, const cuba_sim3_params* params,
 	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, double* s_out, uint8_t* levels_out, int32_t* ninliers,
 	cuba_iter_stat* stats, int32_t* nstats, int32_t* status, void* stream);
+size_t cuba_point_batch_workspace_bytes(int B, int P, int E2, int E3, int nrounds, const cuba_pose_round* rounds, int with_stats);
+int cuba_engine_optimize_points_device(cuba_engine* e, const cuba_point_batch* batch_dev, int nrounds, const cuba_pose_round* rounds,
+	void* workspace, size_t workspace_bytes, double* Xw_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats,
+	int32_t* nstats, int32_t* status, void* stream);
 
 /* seconds per profile bucket accumulated since set_problem, [CUBA_PROF_NUM] */
 int cuba_engine_get_profile(cuba_engine* e, double* seconds);
