@@ -150,7 +150,7 @@ _lib = None
 _SYMBOLS = [
     "cuba_last_error", "cuba_version", "cuba_engine_create", "cuba_engine_destroy", "cuba_engine_set_robust_kernel",
     "cuba_comm_unique_id", "cuba_engine_set_comm", "cuba_engine_set_problem", "cuba_engine_set_linear_solver", "cuba_engine_set_structure_reuse", "cuba_engine_get_structure_reuses", "cuba_engine_set_state", "cuba_engine_get_sizes", "cuba_engine_reset_state", "cuba_engine_get_stream", "cuba_engine_get_device", "cuba_engine_flush_l2",
-    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_set_problem_device", "cuba_engine_set_state_device", "cuba_engine_get_state_device", "cuba_engine_get_chi2_device", "cuba_engine_set_edge_levels_device", "cuba_engine_get_edge_levels_device", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_pose_batch_workspace_bytes", "cuba_engine_optimize_poses_device", "cuba_sim3_batch_workspace_bytes", "cuba_engine_optimize_sim3_device", "cuba_engine_optimize_points", "cuba_point_batch_workspace_bytes", "cuba_engine_optimize_points_device", "cuba_engine_get_profile",
+    "cuba_engine_optimize", "cuba_engine_get_state", "cuba_engine_get_chi2", "cuba_engine_set_edge_levels", "cuba_engine_get_edge_levels", "cuba_engine_classify_edges", "cuba_engine_set_problem_device", "cuba_engine_set_state_device", "cuba_engine_get_state_device", "cuba_engine_get_chi2_device", "cuba_engine_set_edge_levels_device", "cuba_engine_get_edge_levels_device", "cuba_engine_optimize_poses", "cuba_engine_optimize_sim3", "cuba_pose_batch_workspace_bytes", "cuba_engine_optimize_poses_device", "cuba_sim3_batch_workspace_bytes", "cuba_engine_optimize_sim3_device", "cuba_engine_optimize_points", "cuba_point_batch_workspace_bytes", "cuba_engine_optimize_points_device", "cuba_engine_optimize_landmarks", "cuba_engine_optimize_landmarks_device", "cuba_engine_get_profile",
     "cuba_engine_get_launch_count", "cuba_get_transfer_bytes", "cuba_stage_linearize", "cuba_stage_max_diagonal", "cuba_stage_solve", "cuba_stage_update",
     "cuba_stage_commit", "cuba_stage_chi2", "cuba_debug_get_hpl_structure", "cuba_debug_get_hsc_structure",
     "cuba_debug_get_system", "cuba_debug_get_schur", "cuba_debug_get_delta", "cuba_debug_get_pcg_info", "cuba_debug_get_coarse", "cuba_debug_coarse_inverse", "cuba_debug_dense_solve", "cuba_debug_peer_allreduce", "cuba_debug_pcg5_ranks", "cuba_debug_build_structure_host", "cuba_debug_pcg_partition", "cuba_debug_pcg5_plan", "cuba_debug_pcg5_plan_apc", "cuba_debug_pcg5t_layout", "cuba_debug_dense_layout", "cuba_debug_dropin_problem", "cuba_debug_dropin_levels", "cuba_bench_stage",
@@ -207,6 +207,8 @@ def load_library():
                                              vp, vp],
         "cuba_engine_optimize_points": [vp, C.POINTER(_PointBatch), i, vp, vp, vp, vp, vp, vp],
         "cuba_engine_optimize_points_device": [vp, C.POINTER(_PointBatch), i, vp, vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp],
+        "cuba_engine_optimize_landmarks": [vp, vp, C.c_int32, i, vp, vp, vp, vp],
+        "cuba_engine_optimize_landmarks_device": [vp, vp, C.c_int32, i, vp, vp, vp, vp, vp],
         "cuba_engine_get_profile": [vp, vp],
         "cuba_engine_get_launch_count": [vp, C.POINTER(C.c_longlong)],
         "cuba_get_transfer_bytes": [C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)],
@@ -609,6 +611,53 @@ class Engine:
         return [dict(Xw=r["Xw"][b], counts=r["counts"][b], stats=self._round_stats(r["stats"][b], r["nstats"][b], rounds),
                      levels=np.concatenate([r["levels"][ptr2[b]:ptr2[b + 1]], r["levels"][E2 + ptr3[b]:E2 + ptr3[b + 1]]]))
                 for b in range(batch.B)]
+
+    # --- structure-only refinement of the held problem's landmarks in place (include/cuba_b200.h: cuba_engine_optimize_landmarks) ------
+    def _landmark_count(self, what, landmarks):
+        if self.sizes is None:
+            raise CubaError("%s before initialize / initialize_device" % what)
+        return self.sizes["numL"] if landmarks is None else int(landmarks.shape[0]) if landmarks.ndim == 1 else -1
+
+    def optimize_landmarks(self, rounds, landmarks=None, with_stats=False):
+        """Refines the listed free landmarks of the held problem (int array of iL in [0, numL), no repeats; None = every free landmark)
+        against the current poses, in place, under the round schedule (list of PoseRound; restart = from the landmark's position on
+        entry), starting from the edges' current levels.  Returns a dict of counts [R,4] (included mono, included stereo, newly
+        excluded, re-included over the refined landmarks' edges after each round), nstats [n,R] and, with with_stats, stats [n, sum of
+        iterations] (the structured array of the _flat methods)."""
+        what = "optimize_landmarks"
+        lst = None if landmarks is None else np.ascontiguousarray(np.asarray(landmarks).reshape(-1), dtype=np.int32)
+        n = self._landmark_count(what, lst)
+        R = len(rounds)
+        S = sum(max(int(r.iterations), 0) for r in rounds)
+        out = dict(counts=np.zeros((R, 4), np.int32), nstats=np.zeros((n, R), np.int32))
+        st = (_IterStat * max(n * S, 1))() if with_stats else None
+        _check(self.L.cuba_engine_optimize_landmarks(self.h, _p(lst), n, R, self._rounds_struct(rounds), _p(out["counts"]), st,
+                                                     _p(out["nstats"])))
+        if with_stats:
+            out["stats"] = np.frombuffer(st, dtype=ITER_STAT_DTYPE)[:n * S].reshape(n, S).copy()
+        return out
+
+    def optimize_landmarks_device(self, rounds, landmarks=None, with_stats=True, out=None):
+        """optimize_landmarks with the list (an int32 CUDA tensor [n] of the engine's device, or None) and the per-landmark outputs in
+        device memory, on torch.cuda.current_stream(); one host read-back of the counts.  Returns a dict of counts (numpy [R,4]),
+        nstats (int32 CUDA [n,R]) and stats (float64 CUDA [n, sum of iterations, 4] words holding cuba_iter_stat, for stats_view(); None
+        without with_stats).  out: an earlier result dict to write nstats / stats into; it must fit exactly.  A list entry outside [0,
+        numL) or repeated raises CubaError, with the engine and the outputs unchanged."""
+        what = "optimize_landmarks_device"
+        import torch
+        self._check_tensors(what, [("landmarks", landmarks, torch.int32, None)])
+        if landmarks is not None and landmarks.dim() != 1:
+            raise ValueError("%s: landmarks must be one-dimensional, got shape %s" % (what, tuple(landmarks.shape)))
+        n = self._landmark_count(what, landmarks)
+        R = len(rounds)
+        S = sum(max(int(r.iterations), 0) for r in rounds)
+        spec = dict(nstats=((n, R), torch.int32), stats=((n, S, 4), torch.float64))
+        out, _, torch = self._device_call(what, [("landmarks", landmarks)], spec, with_stats, out, None)
+        counts = np.zeros((R, 4), np.int32)
+        p = lambda a: None if a is None else a.data_ptr()
+        _check(self.L.cuba_engine_optimize_landmarks_device(self.h, p(landmarks), n, R, self._rounds_struct(rounds), _p(counts),
+                                                            p(out.get("stats")), p(out["nstats"]), C.c_void_p(self._torch_stream())))
+        return dict(counts=counts, nstats=out["nstats"], stats=out.get("stats"))
 
     # --- batched Sim(3) alignment (ORB-SLAM2's OptimizeSim3 over many keyframe pairs in one launch) ------------------------------------
     def optimize_sim3_flat(self, ptr, q, t, s, cam1, cam2, fix_scale, X1, X2, obs1, obs2, omega1, omega2, params=None, B=None, N=None):

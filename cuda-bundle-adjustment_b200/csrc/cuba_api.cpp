@@ -448,6 +448,45 @@ public:
 		out.excluded = static_cast<size_t>(c[2]); out.reincluded = static_cast<size_t>(c[3]);
 		return out;
 	}
+	// include/cuba_b200_points.h: the held problem's free landmarks (all of them, or `list`) refined in place on the engine
+	std::vector<OutlierCounts> optimizeLandmarks(const std::vector<cuba_pose_round>& rounds, const std::vector<LandmarkVertex*>* list)
+	{
+		if (!engine_ || !uploaded_) throw std::logic_error("cuba::optimizeLandmarks: no optimize() since the last initialize()");
+		std::vector<int32_t> idx;
+		if (list) {
+			idx.reserve(list->size());
+			for (const LandmarkVertex* v : *list) {
+				// a free landmark of the uploaded graph: its index names it in the flat problem
+				if (!v || v->iL < 0 || v->iL >= numL_ || vL_[static_cast<size_t>(v->iL)] != v)
+					throw std::invalid_argument("cuba::optimizeLandmarks: a vertex that is not a free landmark of the uploaded graph");
+				idx.push_back(v->iL);
+			}
+		}
+		pushLevels();
+		const size_t R = rounds.size();
+		std::vector<int32_t> c(4 * std::max<size_t>(R, 1), 0);
+		const int32_t n = list ? static_cast<int32_t>(idx.size()) : numL_;
+		const int rc = cuba_engine_optimize_landmarks(engine_, list ? idx.data() : nullptr, n, static_cast<int>(R), rounds.data(), c.data(),
+			nullptr, nullptr);
+		if (rc == CUBA_ERR_INVALID) throw std::invalid_argument(std::string("cuba::optimizeLandmarks: ") + cuba_last_error());
+		check(rc);
+		std::vector<OutlierCounts> out(R);
+		for (size_t r = 0; r < R; r++) {
+			out[r].includedMono = static_cast<size_t>(c[4 * r]); out[r].includedStereo = static_cast<size_t>(c[4 * r + 1]);
+			out[r].excluded = static_cast<size_t>(c[4 * r + 2]); out[r].reincluded = static_cast<size_t>(c[4 * r + 3]);
+			if (c[4 * r + 2] + c[4 * r + 3] > 0) levDevNewer_ = true;
+		}
+		// optimize()'s finalize for the refined vertices, and the per-edge chi2 it refreshes
+		check(cuba_engine_get_state(engine_, q_.data(), t_.data(), Xw_.data()));
+		auto put = [this](size_t i) { for (int k = 0; k < 3; k++) vL_[i]->Xw.data()[k] = Xw_[3 * i + k]; };
+		if (list) for (int32_t i : idx) put(static_cast<size_t>(i));
+		else parallel_for(static_cast<size_t>(numL_), [&](size_t b, size_t e) { for (size_t i = b; i < e; i++) put(i); });
+		chi_.resize(om2_.size() + om3_.size());
+		if (chi_.size()) check(cuba_engine_get_chi2(engine_, chi_.data()));
+		chiMono_ = activeMono_; chiStereo_ = activeStereo_;
+		chiIndexValid_ = false;
+		return out;
+	}
 	// the engine optimizePoses() runs on (include/cuba_b200_pose.h): this object's, created on demand
 	cuba_engine* poseEngine()
 	{
@@ -852,6 +891,18 @@ std::vector<PointResult> optimizePoints(CudaBundleAdjustment& ba, const std::vec
 		res.rounds = round_stats(rounds, stats, nstats, b, perPoint);
 	}
 	return out;
+}
+
+std::vector<OutlierCounts> optimizeLandmarks(CudaBundleAdjustment& ba, const std::vector<PoseRound>& schedule)
+{
+	size_t per = 0;
+	return impl_of(ba).optimizeLandmarks(c_rounds(schedule, per), nullptr);
+}
+std::vector<OutlierCounts> optimizeLandmarks(CudaBundleAdjustment& ba, const std::vector<PoseRound>& schedule,
+	const std::vector<LandmarkVertex*>& landmarks)
+{
+	size_t per = 0;
+	return impl_of(ba).optimizeLandmarks(c_rounds(schedule, per), &landmarks);
 }
 
 // include/cuba_b200_sim3.h

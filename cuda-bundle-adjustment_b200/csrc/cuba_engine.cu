@@ -31,6 +31,7 @@
 #include "cuba_pose_batch.cuh"
 #include "cuba_sim3_batch.cuh"
 #include "cuba_point_batch.cuh"
+#include "cuba_landmark_refine.cuh"
 #include "cuba_batch_io.cuh"
 #include "cuba_problem_io.cuh"
 #include "cuba_schur3.cuh"
@@ -372,6 +373,11 @@ struct EngineBase {
 		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats) = 0;
 	virtual int optimize_points(const cuba_point_batch* bt, const pb::Schedule& s, double* XwOut, uint8_t* levelsOut, int32_t* counts,
 		cuba_iter_stat* stats, int32_t* nstats) = 0;
+	// structure-only refinement of the held problem's free landmarks in place; dev: list, stats and nstats are device pointers
+	virtual int optimize_landmarks(const int32_t* list, int n, const pb::Schedule& s, int32_t* counts, cuba_iter_stat* stats,
+		int32_t* nstats, bool dev, cudaStream_t caller) = 0;
+	virtual int num_free_landmarks() const = 0;
+	virtual bool fp32() const = 0;
 };
 
 template <typename T>
@@ -454,6 +460,9 @@ struct Engine : EngineBase {
 	DBuf<unsigned char> lvLevel;   // [E] in edge-id order; a rank reads and writes its own edges only
 	DBuf<int> lvPartial;
 	DBuf<double> lvCount;
+	// optimize_landmarks: per-CTA counts, the per-round totals | status word (one read-back), the device list's marks
+	DBuf<int> lrPartial, lrMark;
+	DBuf<double> lrTotal;
 	// the batched LM kernels (optimize_poses, optimize_sim3, optimize_points, one after the other on the stream): the packed batch
 	// and the packed results, device and page-locked host copies
 	DBuf<double> batchIn, batchOut;
@@ -2688,6 +2697,108 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
+	// ---- structure-only refinement of the held landmarks in place (cuba_landmark_refine.cuh) -----------------------------------
+	int num_free_landmarks() const override { return S.numL; }
+	bool fp32() const override { return sizeof(T) != 8; }
+
+	// One launch of k_refine_landmarks (after k_check_landmarks for a device list), the counts summed per round and all-reduced, one
+	// read-back of the totals and the status word, then the mask scattered once if some level changed.  The list was checked on the
+	// host (host list) or is checked on the device (dev).  Host entry: the list goes up, stats / nstats come down, through the batch
+	// buffers.
+	int optimize_landmarks(const int32_t* list, int n, const pb::Schedule& s, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats,
+		bool dev, cudaStream_t caller) override
+	{
+		if constexpr (sizeof(T) != 8) {
+			return fail(CUBA_ERR_INVALID, "optimize_landmarks: the fp32 engine is not supported (use an fp64 or mixed-precision engine)");
+		} else {
+			if (counts) memset(counts, 0, sizeof(int32_t) * 4 * (size_t)s.n);
+			if (n == 0) return CUBA_OK;
+			return on_caller_stream(dev ? caller : stream, [&] { return refine_landmarks(list, n, s, counts, stats, nstats, dev); });
+		}
+	}
+	int refine_landmarks(const int32_t* list, int n, const pb::Schedule& s, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats, bool dev)
+	{
+		int rc = levels_init(); if (rc) return rc;
+		const size_t R = (size_t)s.n, nb = (size_t)n, nS = (size_t)s.statOff[s.n];
+		const unsigned grid = (unsigned)((nb + ptb::WARPS - 1) / ptb::WARPS);
+		CUDA_TRY(lrPartial.alloc(4 * R * grid)); CUDA_TRY(lrTotal.alloc(4 * pb::MAX_ROUNDS + 1));
+		int* status = (int*)(lrTotal.p + 4 * R);
+		CUDA_TRY(cudaMemsetAsync(lrTotal.p + 4 * R, 0, sizeof(double), stream));
+		ptb::LandmarkArgs a;
+		a.n = n; a.lmBeg = S.lmBeg; a.lmEnd = S.lmEnd;
+		a.pose = pose[cur].p; a.cam = cam.p; a.Xw = Xw[cur].p;
+		a.mx = e_mx.p; a.my = e_my.p; a.mz = e_mz.p; a.om0 = e_om0.p; a.ip = e_ip.p; a.user = e_user.p; a.lmPtr = lmPtr.p;
+		a.level = lvLevel.p; a.partial = lrPartial.p;
+		// per-landmark outputs: the caller's device arrays, or the batch buffers (stats, then nstats) copied down afterwards
+		const size_t oN = 4 * nb * nS, nOut = oN + (nb * R + 1) / 2;
+		if (dev) {
+			a.list = list; a.status = list ? status : nullptr; a.stats = (lm::IterStat*)stats; a.nstats = nstats;
+			if (list) {
+				CUDA_TRY(lrMark.alloc((size_t)std::max(S.numL, 1)));
+				CUDA_TRY(cudaMemsetAsync(lrMark.p, 0, sizeof(int) * (size_t)std::max(S.numL, 1), stream));
+				ptb::k_check_landmarks<<<(unsigned)((nb + 255) / 256), 256, 0, stream>>>(list, n, S.numL, lrMark.p, status);
+				launches++;
+				CUDA_TRY(cudaGetLastError());
+			}
+		} else {
+			a.status = nullptr;
+			CUDA_TRY(batchOut.alloc(std::max<size_t>(nOut, 1))); CUDA_TRY(batchHostOut.grow(sizeof(double) * std::max<size_t>(nOut, 1)));
+			a.stats = stats ? (lm::IterStat*)batchOut.p : nullptr;
+			a.nstats = nstats ? (int*)(batchOut.p + oN) : nullptr;
+			a.list = nullptr;
+			if (list) {
+				const size_t nIn = (nb + 1) / 2;
+				CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchIn.alloc(nIn));
+				memcpy(batchHostIn.p, list, sizeof(int32_t) * nb);
+				CUDA_TRY(cudaMemcpyAsync(batchIn.p, batchHostIn.p, sizeof(int32_t) * nb, cudaMemcpyHostToDevice, stream));
+				g_h2dBytes += (long long)(sizeof(int32_t) * nb);
+				a.list = (const int*)batchIn.p;
+			}
+		}
+		ptb::k_refine_landmarks<<<grid, lm::BLOCK, 0, stream>>>(a, s);
+		launches++;
+		CUDA_TRY(cudaGetLastError());
+		for (size_t r = 0; r < R; r++) {
+			lv::k_sum_counts<<<1, RED_BLOCK, 0, stream>>>(lrPartial.p + 4 * r * grid, (int)grid, lrTotal.p + 4 * r);
+			launches++;
+			CUDA_TRY(cudaGetLastError());
+		}
+		rc = allreduce(lrTotal.p, 4 * R, false); if (rc) return rc;
+		double tot[4 * pb::MAX_ROUNDS + 1];
+		g_d2hBytes += (long long)(sizeof(double) * (4 * R + 1));
+		CUDA_TRY(cudaMemcpyAsync(tot, lrTotal.p, sizeof(double) * (4 * R + 1), cudaMemcpyDeviceToHost, stream));
+		const size_t nBack = (stats ? oN : 0) * sizeof(double) + (nstats ? sizeof(int32_t) * nb * R : 0);
+		if (!dev && nBack) {
+			if (stats) CUDA_TRY(cudaMemcpyAsync(batchHostOut.p, batchOut.p, sizeof(double) * oN, cudaMemcpyDeviceToHost, stream));
+			if (nstats) CUDA_TRY(cudaMemcpyAsync((double*)batchHostOut.p + oN, batchOut.p + oN, sizeof(int32_t) * nb * R, cudaMemcpyDeviceToHost, stream));
+			g_d2hBytes += (long long)nBack;
+		}
+		CUDA_TRY(cudaStreamSynchronize(stream));
+		int st;
+		memcpy(&st, tot + 4 * R, sizeof(st));
+		if (st) {
+			const bool bad = st & ptb::BAD_INDEX;
+			return fail(CUBA_ERR_INVALID, bad ? "optimize_landmarks: a landmark outside [0, numL)" : "optimize_landmarks: a landmark listed twice");
+		}
+		if (!dev) {
+			const double* o = (const double*)batchHostOut.p;
+			if (stats) memcpy(stats, o, sizeof(cuba_iter_stat) * nb * nS);
+			if (nstats) memcpy(nstats, o + oN, sizeof(int32_t) * nb * R);
+		}
+		double changed = 0, delta = 0;
+		for (size_t r = 0; r < R; r++) {
+			changed += tot[4 * r + 2] + tot[4 * r + 3];
+			delta += tot[4 * r + 3] - tot[4 * r + 2];
+			if (counts) for (int k = 0; k < 4; k++) counts[4 * r + k] = (int32_t)tot[4 * r + k];
+		}
+		// some level changed (on some rank): scatter the mask once.  The new positions invalidate whatever a trial or a solve left.
+		if (changed > 0) { rc = levels_scatter(); if (rc) return rc; }
+		lvIncluded += (long long)delta;
+		trialValid = false;
+		forget_solves();
+		return CUBA_OK;
+	}
+
 	int get_profile(double* sec) override
 	{
 		resolveProfile();
@@ -3533,6 +3644,45 @@ int cuba_engine_optimize_points_device(cuba_engine* e, const cuba_point_batch* b
 	bio::k_unpack_points<<<gridIo, bio::BLOCK, 0, st>>>(L, B, s.n, bt->E2, bt->E3, (int)statPer, in, Xw_out, levels_out, counts, stats, nstats, status);
 	CUDA_TRY(cudaGetLastError());
 	return CUBA_OK;
+}
+
+// The checks of optimize_landmarks and optimize_landmarks_device that need no list entry, in the order the header states them
+static int landmark_args(cuba_engine* e, const int32_t* landmarks, int32_t n, int nrounds, const cuba_pose_round* rounds, pb::Schedule& s)
+{
+	int rc = pose_schedule(nrounds, rounds, s, "optimize_points"); if (rc) return rc;
+	if (n < 0) return fail(CUBA_ERR_INVALID, "optimize_landmarks: n < 0");
+	if (!e->impl->haveProblem) return fail(CUBA_ERR_STATE, "optimize_landmarks before set_problem");
+	if (!landmarks && n != e->impl->num_free_landmarks()) return fail(CUBA_ERR_INVALID, "optimize_landmarks: a NULL list needs n = numL");
+	return CUBA_OK;
+}
+
+int cuba_engine_optimize_landmarks(cuba_engine* e, const int32_t* landmarks, int32_t n, int nrounds, const cuba_pose_round* rounds,
+	int32_t* counts, cuba_iter_stat* stats, int32_t* nstats)
+{
+	ENGINE_OR_FAIL(e);
+	pb::Schedule s;
+	int rc = landmark_args(e, landmarks, n, nrounds, rounds, s); if (rc) return rc;
+	if (landmarks) {
+		const int numL = e->impl->num_free_landmarks();
+		std::vector<unsigned char> seen((size_t)std::max(numL, 1), 0);
+		for (int32_t i = 0; i < n; i++) {
+			const int32_t l = landmarks[i];
+			if (l < 0 || l >= numL) return fail(CUBA_ERR_INVALID, "optimize_landmarks: landmarks[" + std::to_string(i) + "] outside [0, numL)");
+			if (seen[(size_t)l]++) return fail(CUBA_ERR_INVALID, "optimize_landmarks: landmarks[" + std::to_string(i) + "] listed twice");
+		}
+	}
+	if (e->impl->fp32()) return fail(CUBA_ERR_INVALID, "optimize_landmarks: the fp32 engine is not supported (use an fp64 or mixed-precision engine)");
+	return e->impl->optimize_landmarks(landmarks, n, s, counts, stats, nstats, false, nullptr);
+}
+
+int cuba_engine_optimize_landmarks_device(cuba_engine* e, const int32_t* landmarks, int32_t n, int nrounds, const cuba_pose_round* rounds,
+	int32_t* counts, cuba_iter_stat* stats, int32_t* nstats, void* stream)
+{
+	ENGINE_OR_FAIL(e);
+	pb::Schedule s;
+	int rc = landmark_args(e, landmarks, n, nrounds, rounds, s); if (rc) return rc;
+	if (e->impl->fp32()) return fail(CUBA_ERR_INVALID, "optimize_landmarks: the fp32 engine is not supported (use an fp64 or mixed-precision engine)");
+	return e->impl->optimize_landmarks(landmarks, n, s, counts, stats, nstats, true, (cudaStream_t)stream);
 }
 
 int cuba_engine_get_profile(cuba_engine* e, double* sec) { ENGINE_OR_FAIL(e); if (!sec) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_profile(sec); }

@@ -13,6 +13,9 @@
 //
 // Edges and their pose records are read from global memory on every pass; levels live in global memory, one byte per edge, and a
 // lane reads and writes only its own edges (k = lane mod 32), so no fence is needed between passes.
+//
+// The per-point problem (Point) reads its edges through an edge source: BatchEdges here, the engine's landmark-major stream in
+// k_refine_landmarks (cuba_landmark_refine.cuh), which runs the same rounds (run_schedule) on the engine's own landmarks.
 #pragma once
 
 #include "cuba_lm_batch.cuh"
@@ -39,25 +42,43 @@ struct Args {
 	lm::IterStat* stats;              // [B][statOff[n]] or null
 };
 
-// one point's LM problem under a round's robust kernels; the state is X(3), the same in every lane
-struct Point {
-	static constexpr int N = 3;
-	const double* pose;               // Args::pose, cam, edge, iP, level; the point's edges are e0 .. e0 + n, mono first
-	const double* cam;
-	const double* edge;
+// The edges of a point of the batch: point b's are e0 .. e0 + n of the packed arrays, its mono edges first
+struct BatchEdges {
+	const double* edge;               // Args::edge, iP, level
 	const int* iP;
-	const unsigned char* level;
-	int e0, n, nMono;
-	RobustParams rk;
+	unsigned char* level;
+	int e0, nMono;
 
-	// edge k's pose, camera-frame point and residual at X, and its weighted squared error om |r|^2
-	__device__ __forceinline__ double residual(int k, const double X[3], double q[4], double c[5], double Xc[3], double r[3], double& om) const
+	// edge k's pose and type
+	__device__ __forceinline__ int pose(int k, bool& stereo) const { stereo = k >= nMono; return iP[e0 + k]; }
+	// edge k's measurement (m[2] = 0 for a mono edge) and omega
+	__device__ __forceinline__ void meas(int k, bool, double m[3], double& om) const
 	{
-		const bool stereo = k >= nMono;
-		double t[3], m[3];
-		load_pose(pose, cam, iP[e0 + k], q, t, c);
 		ld2(edge + 4 * (size_t)(e0 + k), m[0], m[1]);
 		ld2(edge + 4 * (size_t)(e0 + k) + 2, m[2], om);
+	}
+	// edge k's level byte
+	__device__ __forceinline__ unsigned char* slot(int k) const { return level + e0 + k; }
+};
+
+// one point's LM problem under a round's robust kernels, over the edges of an edge source (BatchEdges; StreamEdges of
+// cuba_landmark_refine.cuh); the state is X(3), the same in every lane
+template <class Edges>
+struct Point {
+	static constexpr int N = 3;
+	const double* pose;               // [P][8] q t pad, [P][8] fx fy cx cy bf pad
+	const double* cam;
+	Edges ed;
+	int n;
+	RobustParams rk;
+
+	// edge k's pose, type, camera-frame point and residual at X, and its weighted squared error om |r|^2
+	__device__ __forceinline__ double residual(int k, const double X[3], bool& stereo, double q[4], double c[5], double Xc[3], double r[3],
+		double& om) const
+	{
+		double t[3], m[3];
+		load_pose(pose, cam, ed.pose(k, stereo), q, t, c);
+		ed.meas(k, stereo, m, om);
 		edge_residual(q, t, c, X, m, stereo, Xc, r);
 		return om * (r[0] * r[0] + r[1] * r[1] + r[2] * r[2]);
 	}
@@ -66,10 +87,10 @@ struct Point {
 	__device__ __forceinline__ void linearize(double acc[10], const double* X) const
 	{
 		for (int k = threadIdx.x & 31; k < n; k += 32) {
-			if (level[e0 + k]) continue;
-			const bool stereo = k >= nMono;
+			if (*ed.slot(k)) continue;
+			bool stereo;
 			double q[4], c[5], Xc[3], r[3], om, rho, drho;
-			const double e2 = residual(k, X, q, c, Xc, r, om);
+			const double e2 = residual(k, X, stereo, q, c, Xc, r, om);
 			// constant indices: a run-time index into rk would keep the whole Point in local memory
 			robust<double>(stereo ? rk.type[1] : rk.type[0], stereo ? rk.delta[1] : rk.delta[0], e2, rho, drho);
 			acc[9] += rho;
@@ -100,10 +121,10 @@ struct Point {
 	{
 		double chi = 0;
 		for (int k = threadIdx.x & 31; k < n; k += 32) {
-			if (level[e0 + k]) continue;
-			const bool stereo = k >= nMono;
+			if (*ed.slot(k)) continue;
+			bool stereo;
 			double q[4], c[5], Xc[3], r[3], om, rho, drho;
-			const double e2 = residual(k, X, q, c, Xc, r, om);
+			const double e2 = residual(k, X, stereo, q, c, Xc, r, om);
 			robust<double>(stereo ? rk.type[1] : rk.type[0], stereo ? rk.delta[1] : rk.delta[0], e2, rho, drho);
 			chi += rho;
 		}
@@ -126,7 +147,50 @@ struct Point {
 #pragma unroll
 		for (int i = 0; i < 3; i++) Xt[i] = X[i] + x[i];
 	}
+
+	// the outlier test of lv::k_classify_edges on X: new levels, and the warp's counts (included mono, included stereo, newly
+	// excluded, re-included) in every lane.  A lane reads and writes only its own edges' levels.
+	__device__ __forceinline__ void classify(const double X[3], const pb::Round& R, int c4[4]) const
+	{
+		c4[0] = c4[1] = c4[2] = c4[3] = 0;
+		for (int k = threadIdx.x & 31; k < n; k += 32) {
+			bool stereo;
+			double q[4], c[5], Xc[3], r[3], om;
+			const double chi2 = residual(k, X, stereo, q, c, Xc, r, om);
+			const bool fail = chi2 > (stereo ? R.chi2[1] : R.chi2[0]) || ((R.flags & lv::FAIL_DEPTH) && Xc[2] <= 0);
+			unsigned char* s = ed.slot(k);
+			const int old = *s;
+			const int now = (R.flags & lv::REINCLUDE) ? (fail ? 1 : 0) : (old | (fail ? 1 : 0));
+			if (now != old) *s = (unsigned char)now;
+			c4[0] += !now && !stereo; c4[1] += !now && stereo; c4[2] += !old && now; c4[3] += old && !now;
+		}
+#pragma unroll
+		for (int k = 0; k < 4; k++)
+#pragma unroll
+			for (int o = 16; o > 0; o >>= 1) c4[k] += __shfl_xor_sync(0xffffffffu, c4[k], o);
+	}
 };
+
+// The round schedule on one point, by its warp: per round an optional restart to Xin, lm::optimize_warp from X, then the outlier
+// test on the committed X.  included: the point's edges at level 0 on entry.  stats: the point's first stat slot, or null.  After
+// each round, out(rd, iterations written, c4) with the warp's counts in every lane.
+template <class Edges, class Out>
+__device__ __forceinline__ void run_schedule(const double* pose, const double* cam, const Edges& ed, int n, const pb::Schedule& s,
+	const double Xin[3], double X[3], int included, lm::IterStat* stats, Out&& out)
+{
+	for (int rd = 0; rd < s.n; rd++) {
+		const pb::Round R = s.r[rd];
+		if (R.restart)
+#pragma unroll
+			for (int i = 0; i < 3; i++) X[i] = Xin[i];
+		const Point<Edges> P = { pose, cam, ed, n, s.rk[rd] };
+		const int nIt = lm::optimize_warp(P, X, included, R.iterations, stats ? stats + s.statOff[rd] : nullptr);
+		int c4[4];
+		P.classify(X, R, c4);
+		included = c4[0] + c4[1];
+		out(rd, nIt, c4);
+	}
+}
 
 __global__ void __launch_bounds__(lm::BLOCK) k_point_batch(const Args a, const pb::Schedule s)
 {
@@ -139,35 +203,12 @@ __global__ void __launch_bounds__(lm::BLOCK) k_point_batch(const Args a, const p
 #pragma unroll
 	for (int i = 0; i < 3; i++) X[i] = Xin[i] = a.Xw[4 * (size_t)b + i];
 	for (int k = lane; k < n; k += 32) a.level[e0 + k] = 0;
-	int included = n;
-
-	for (int rd = 0; rd < s.n; rd++) {
-		const pb::Round R = s.r[rd];
-		if (R.restart)
-#pragma unroll
-			for (int i = 0; i < 3; i++) X[i] = Xin[i];
-		const Point P = { a.pose, a.cam, a.edge, a.iP, a.level, e0, n, nMono, s.rk[rd] };
-		const int nIt = lm::optimize_warp(P, X, included, R.iterations, a.stats ? a.stats + (size_t)b * s.statOff[s.n] + s.statOff[rd] : nullptr);
-		// ---- the outlier test on the committed position (lv::k_classify_edges) ----
-		int c4[4] = { 0, 0, 0, 0 };
-		for (int k = lane; k < n; k += 32) {
-			const bool stereo = k >= nMono;
-			double q[4], c[5], Xc[3], r[3], om;
-			const double chi2 = P.residual(k, X, q, c, Xc, r, om);
-			const bool fail = chi2 > (stereo ? R.chi2[1] : R.chi2[0]) || ((R.flags & lv::FAIL_DEPTH) && Xc[2] <= 0);
-			const int old = a.level[e0 + k];
-			const int now = (R.flags & lv::REINCLUDE) ? (fail ? 1 : 0) : (old | (fail ? 1 : 0));
-			if (now != old) a.level[e0 + k] = (unsigned char)now;
-			c4[0] += !now && !stereo; c4[1] += !now && stereo; c4[2] += !old && now; c4[3] += old && !now;
-		}
-#pragma unroll
-		for (int k = 0; k < 4; k++)
-#pragma unroll
-			for (int o = 16; o > 0; o >>= 1) c4[k] += __shfl_xor_sync(0xffffffffu, c4[k], o);
-		included = c4[0] + c4[1];
-		if (lane < 4) a.counts[((size_t)b * s.n + rd) * 4 + lane] = lane == 0 ? c4[0] : lane == 1 ? c4[1] : lane == 2 ? c4[2] : c4[3];
-		if (lane == 0) a.nstats[(size_t)b * s.n + rd] = nIt;
-	}
+	const BatchEdges ed = { a.edge, a.iP, a.level, e0, nMono };
+	run_schedule(a.pose, a.cam, ed, n, s, Xin, X, n, a.stats ? a.stats + (size_t)b * s.statOff[s.n] : nullptr,
+		[&](int rd, int nIt, const int c4[4]) {
+			if (lane < 4) a.counts[((size_t)b * s.n + rd) * 4 + lane] = lane == 0 ? c4[0] : lane == 1 ? c4[1] : lane == 2 ? c4[2] : c4[3];
+			if (lane == 0) a.nstats[(size_t)b * s.n + rd] = nIt;
+		});
 	if (lane < 4) a.XwOut[4 * (size_t)b + lane] = lane == 0 ? X[0] : lane == 1 ? X[1] : lane == 2 ? X[2] : 0.0;
 }
 

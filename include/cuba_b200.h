@@ -429,6 +429,31 @@ int cuba_engine_optimize_points_device(cuba_engine* e, const cuba_point_batch* b
 	void* workspace, size_t workspace_bytes, double* Xw_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats,
 	int32_t* nstats, int32_t* status, void* stream);
 
+/* Structure-only refinement of the held problem's free landmarks, in place (DESIGN.md 4.9).  landmarks: [n] iL in [0, numL), no
+ * repeats, host memory; NULL = every free landmark, b = iL, and n must equal numL.  Per landmark b: nstats[n][nrounds] and stats
+ * [n][sum of the rounds' iterations] (the layout of cuba_engine_optimize_points; either may be NULL); counts[nrounds][4] = included
+ * mono, included stereo, newly excluded, re-included over the refined landmarks' edges (all ranks), host.
+ * Runs the schedule of cuba_pose_round on each listed landmark against the poses of the current estimate, held fixed: per round
+ * restart = back to the landmark's position on entry, optimize(iterations) under the round's kernels, the outlier test of
+ * classify_edges on the result.  Each edge starts at its current level (set_edge_levels / classify_edges), and the test rewrites it.
+ * Each landmark's result is what the engine computes for its sub-problem (its distinct observing poses fixed, the landmark the only
+ * free vertex, its edges at their current levels; per round set_robust_kernel, set_state on restart, optimize, classify_edges), and
+ * afterwards the engine is bit for bit one given set_state with the refined positions and set_edge_levels with the new levels.
+ * Bit-reproducible; a landmark's result depends neither on the other entries nor on its position in the list.  Poses, fixed and
+ * unlisted landmarks, the robust kernel setting and the state reset_state returns to (the last set_problem / set_state) are kept.
+ * Landmark-sharded runs: each rank refines the listed landmarks of its own shard and writes 0 into the per-landmark outputs of the
+ * others; the counts are summed over the ranks (under CUBA_DRY_SHARD they are the rank's own).  One kernel launch, one read-back of
+ * the counts.  n = 0 does nothing and returns zero counts.
+ * CUBA_ERR_INVALID, with the engine untouched: a schedule cuba_engine_optimize_points refuses (its messages), n < 0, a NULL list with
+ * n != numL, an entry outside [0, numL) or repeated, the fp32 engine (use_fp32 = 1).  CUBA_ERR_STATE before set_problem. */
+int cuba_engine_optimize_landmarks(cuba_engine* e, const int32_t* landmarks, int32_t n, int nrounds, const cuba_pose_round* rounds,
+	int32_t* counts, cuba_iter_stat* stats, int32_t* nstats);
+/* The same with landmarks, stats and nstats in device memory, ordered after `stream`'s work (NULL: the engine's stream); one
+ * read-back of the counts (host), as set_edge_levels_device.  The list is checked on the device: an entry outside [0, numL) or
+ * repeated returns CUBA_ERR_INVALID after the read-back, with the state, the levels and every output unchanged. */
+int cuba_engine_optimize_landmarks_device(cuba_engine* e, const int32_t* landmarks, int32_t n, int nrounds,
+	const cuba_pose_round* rounds, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats, void* stream);
+
 /* seconds per profile bucket accumulated since set_problem, [CUBA_PROF_NUM] */
 int cuba_engine_get_profile(cuba_engine* e, double* seconds);
 /* number of kernels this library launched since create (for bench.py's gpu_launches) */

@@ -48,6 +48,18 @@ struct PointResult
 std::vector<PointResult> optimizePoints(CudaBundleAdjustment& ba, const std::vector<PointProblem>& points,
 	const std::vector<PoseRound>& schedule);
 
+/** Structure-only refinement of the optimizer's own landmarks in place: the free landmarks of the graph the last initialize() uploaded
+ *  (every one, or those listed) against its poses as they stand, held fixed, on the GPU that holds the graph, without a new upload.
+ *  Each edge starts at its current level (setEdgeLevel(), classifyEdges()) and each round ends with the outlier test of
+ *  classifyEdges() on the refined landmarks' edges, which writes their levels (edgeLevel() shows them).  The refined Xw goes into
+ *  each vertex, chiSquared() reports the new estimate, and the next optimize() continues from it; poses and the other landmarks are
+ *  not changed.  The fp32 build (USE_FLOAT32) is refused.  Returns the counts of each round over the refined landmarks' edges.
+ *  std::logic_error without an optimize() since the last initialize(); std::invalid_argument for a listed vertex that is not a free
+ *  landmark of the uploaded graph (null, fixed, added since, or listed twice), or a schedule the engine refuses. */
+std::vector<OutlierCounts> optimizeLandmarks(CudaBundleAdjustment& ba, const std::vector<PoseRound>& schedule);
+std::vector<OutlierCounts> optimizeLandmarks(CudaBundleAdjustment& ba, const std::vector<PoseRound>& schedule,
+	const std::vector<LandmarkVertex*>& landmarks);
+
 } // namespace cuba
 
 #endif

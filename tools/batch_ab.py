@@ -3,8 +3,9 @@
 builds of the library can be compared bit for bit (swap the in-tree library between two `dump` runs, as tools/ab_libs.sh does):
 
   dump OUT.npz        Engine.optimize_poses on every frame of ba_kitti_00 (kitti00_shaped when the fixture is absent) under
-                      ORB-SLAM2's schedule, and Engine.optimize_sim3 on the Sim3 workload with fix_scale off and on: q, t, s, levels,
-                      counts / ninliers, nstats and the per-iteration statistics (iteration, trials, chi2, lambda)
+                      ORB-SLAM2's schedule, Engine.optimize_sim3 on the Sim3 workload with fix_scale off and on, and
+                      Engine.optimize_points on every landmark (perturbed) under tools/point_batch_timing.py's schedule: q, t, s, Xw,
+                      levels, counts / ninliers, nstats and the per-iteration statistics (iteration, trials, chi2, lambda)
   compare A.npz B.npz the bytes, dtype and shape of every array; prints the arrays that differ and exits 1 if any does
 
 Usage: python tools/batch_ab.py dump out.npz;  python tools/batch_ab.py compare a.npz b.npz"""
@@ -17,6 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import __graft_entry__ as ge  # noqa: E402
+import point_batch_timing  # noqa: E402
 import sim3_batch_timing  # noqa: E402
 
 
@@ -46,6 +48,9 @@ def dump(path):
         for p in problems:
             p.fix_scale = fix
         arrays.update(flatten("sim3_fix%d_" % fix, eng.optimize_sim3(problems)))
+    pts = prob.copy()
+    pts.Xw = pts.Xw + np.random.default_rng(7).normal(0, 0.1, pts.Xw.shape)
+    arrays.update(flatten("points_", eng.optimize_points(pkg.graphio.point_batch(pts, range(pts.Lall)), point_batch_timing.schedule(pkg))))
     np.savez(path, **arrays)
     print("%s: %d frames, %d Sim3 problems, %d arrays" % (path, prob.Pall, len(problems), len(arrays)))
 
