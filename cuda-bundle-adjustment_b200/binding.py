@@ -262,6 +262,15 @@ def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _dp(a):
+    return None if a is None else a.data_ptr()
+
+
+def _f64(a, w):
+    """a as a contiguous float64 array [n, w] ([n] for w = 1)"""
+    return np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape((-1, w) if w > 1 else (-1,)))
+
+
 def _problem_struct(prob):
     keep = [np.ascontiguousarray(prob.q, dtype=np.float64), np.ascontiguousarray(prob.t, dtype=np.float64),
             np.ascontiguousarray(prob.cam, dtype=np.float64), np.ascontiguousarray(prob.Xw, dtype=np.float64),
@@ -544,9 +553,8 @@ class Engine:
     def optimize_poses_flat(self, q, t, cam, ptr2, X2, meas2, omega2, ptr3, X3, meas3, omega3, rounds, B=None, E2=None, E3=None):
         """cuba_engine_optimize_poses on flat arrays (include/cuba_b200.h); B / E2 / E3 default to the array sizes.  Returns a dict of
         q [B,4], t [B,3], levels [E2+E3] (mono then stereo), counts [B,R,4], stats [B,sum of iterations] (structured) and nstats [B,R]."""
-        f64 = lambda a, w: np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1, w) if w > 1 else np.asarray(a, dtype=np.float64).reshape(-1))
-        q, t, cam = f64(q, 4), f64(t, 3), f64(cam, 5)
-        X2, meas2, omega2, X3, meas3, omega3 = f64(X2, 3), f64(meas2, 2), f64(omega2, 1), f64(X3, 3), f64(meas3, 3), f64(omega3, 1)
+        q, t, cam = _f64(q, 4), _f64(t, 3), _f64(cam, 5)
+        X2, meas2, omega2, X3, meas3, omega3 = _f64(X2, 3), _f64(meas2, 2), _f64(omega2, 1), _f64(X3, 3), _f64(meas3, 3), _f64(omega3, 1)
         ptr2 = np.ascontiguousarray(ptr2, dtype=np.int32); ptr3 = np.ascontiguousarray(ptr3, dtype=np.int32)
         B = len(q) if B is None else int(B)
         E2 = len(omega2) if E2 is None else int(E2)
@@ -558,9 +566,7 @@ class Engine:
         batch = _PoseBatch(B, E2, E3, _p(q), _p(t), _p(cam), _p(ptr2), _p(X2), _p(meas2), _p(omega2), _p(ptr3), _p(X3), _p(meas3), _p(omega3))
         _check(self.L.cuba_engine_optimize_poses(self.h, C.byref(batch), R, self._rounds_struct(rounds), _p(out["q"]), _p(out["t"]),
                                                  _p(out["levels"]), _p(out["counts"]), out["stats"], _p(out["nstats"])))
-        st = np.frombuffer(out["stats"], dtype=np.dtype([("iteration", "<i4"), ("trials", "<i4"), ("chi2", "<f8"), ("lambda_", "<f8"),
-                                                          ("pcg_iters", "<i4"), ("pcg_failed", "<i4")]))
-        out["stats"] = st[:nb * S].reshape(nb, S).copy()
+        out["stats"] = np.frombuffer(out["stats"], dtype=ITER_STAT_DTYPE)[:nb * S].reshape(nb, S).copy()
         return out
 
     def optimize_poses(self, frames, rounds):
@@ -581,10 +587,9 @@ class Engine:
                              E3=None):
         """cuba_engine_optimize_points on flat arrays (include/cuba_b200.h); B / P / E2 / E3 default to the array sizes.  Returns a dict
         of Xw [B,3], levels [E2+E3] (mono then stereo), counts [B,R,4], stats [B,sum of iterations] (structured) and nstats [B,R]."""
-        f64 = lambda a, w: np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1, w) if w > 1 else np.asarray(a, dtype=np.float64).reshape(-1))
         i32 = lambda a: np.ascontiguousarray(np.asarray(a).reshape(-1), dtype=np.int32)
-        Xw, q, t, cam = f64(Xw, 3), f64(q, 4), f64(t, 3), f64(cam, 5)
-        meas2, omega2, meas3, omega3 = f64(meas2, 2), f64(omega2, 1), f64(meas3, 3), f64(omega3, 1)
+        Xw, q, t, cam = _f64(Xw, 3), _f64(q, 4), _f64(t, 3), _f64(cam, 5)
+        meas2, omega2, meas3, omega3 = _f64(meas2, 2), _f64(omega2, 1), _f64(meas3, 3), _f64(omega3, 1)
         ptr2, iP2, ptr3, iP3 = i32(ptr2), i32(iP2), i32(ptr3), i32(iP3)
         B = len(Xw) if B is None else int(B)
         P = len(q) if P is None else int(P)
@@ -654,9 +659,8 @@ class Engine:
         spec = dict(nstats=((n, R), torch.int32), stats=((n, S, 4), torch.float64))
         out, _, torch = self._device_call(what, [("landmarks", landmarks)], spec, with_stats, out, None)
         counts = np.zeros((R, 4), np.int32)
-        p = lambda a: None if a is None else a.data_ptr()
-        _check(self.L.cuba_engine_optimize_landmarks_device(self.h, p(landmarks), n, R, self._rounds_struct(rounds), _p(counts),
-                                                            p(out.get("stats")), p(out["nstats"]), C.c_void_p(self._torch_stream())))
+        _check(self.L.cuba_engine_optimize_landmarks_device(self.h, _dp(landmarks), n, R, self._rounds_struct(rounds), _p(counts),
+                                                            _dp(out.get("stats")), _dp(out["nstats"]), C.c_void_p(self._torch_stream())))
         return dict(counts=counts, nstats=out["nstats"], stats=out.get("stats"))
 
     # --- batched Sim(3) alignment (ORB-SLAM2's OptimizeSim3 over many keyframe pairs in one launch) ------------------------------------
@@ -665,9 +669,8 @@ class Engine:
         Returns a dict of q [B,4], t [B,3], s [B], levels [N], ninliers [B], stats [B, iterations + max(bad, good)] (structured) and
         nstats [B,2]."""
         params = Sim3Params() if params is None else params
-        f64 = lambda a, w: np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1, w) if w > 1 else np.asarray(a, dtype=np.float64).reshape(-1))
-        q, t, s, cam1, cam2 = f64(q, 4), f64(t, 3), f64(s, 1), f64(cam1, 4), f64(cam2, 4)
-        X1, X2, obs1, obs2, omega1, omega2 = f64(X1, 3), f64(X2, 3), f64(obs1, 2), f64(obs2, 2), f64(omega1, 1), f64(omega2, 1)
+        q, t, s, cam1, cam2 = _f64(q, 4), _f64(t, 3), _f64(s, 1), _f64(cam1, 4), _f64(cam2, 4)
+        X1, X2, obs1, obs2, omega1, omega2 = _f64(X1, 3), _f64(X2, 3), _f64(obs1, 2), _f64(obs2, 2), _f64(omega1, 1), _f64(omega2, 1)
         ptr = np.ascontiguousarray(ptr, dtype=np.int32)
         fix = None if fix_scale is None else np.ascontiguousarray(fix_scale, dtype=np.int32)
         B = len(s) if B is None else int(B)
@@ -682,9 +685,7 @@ class Engine:
                           int(params.min_pairs))
         _check(self.L.cuba_engine_optimize_sim3(self.h, C.byref(batch), C.byref(prm), _p(out["q"]), _p(out["t"]), _p(out["s"]),
                                                 _p(out["levels"]), _p(out["ninliers"]), out["stats"], _p(out["nstats"])))
-        st = np.frombuffer(out["stats"], dtype=np.dtype([("iteration", "<i4"), ("trials", "<i4"), ("chi2", "<f8"), ("lambda_", "<f8"),
-                                                          ("pcg_iters", "<i4"), ("pcg_failed", "<i4")]))
-        out["stats"] = st[:nb * S].reshape(nb, S).copy()
+        out["stats"] = np.frombuffer(out["stats"], dtype=ITER_STAT_DTYPE)[:nb * S].reshape(nb, S).copy()
         return out
 
     def optimize_sim3(self, problems, params=None):
@@ -802,12 +803,11 @@ class Engine:
         out, workspace, torch = self._device_call(what, [(n, a) for n, a, _ in inputs], spec, with_stats, out, workspace)
         rs = self._rounds_struct(rounds)
         workspace = self._workspace(torch, workspace, int(self.L.cuba_pose_batch_workspace_bytes(B, E2, E3, R, rs, int(bool(with_stats)))))
-        ptr = lambda a: None if a is None else a.data_ptr()
-        batch = _PoseBatch(B, E2, E3, ptr(q), ptr(t), ptr(cam), ptr(ptr2), ptr(X2), ptr(meas2), ptr(omega2), ptr(ptr3), ptr(X3), ptr(meas3),
-                           ptr(omega3))
-        _check(self.L.cuba_engine_optimize_poses_device(self.h, C.byref(batch), R, rs, ptr(workspace), workspace.numel() * workspace.element_size(),
-                                                        ptr(out["q"]), ptr(out["t"]), ptr(out["levels"]), ptr(out["counts"]),
-                                                        ptr(out["stats"]), ptr(out["nstats"]), ptr(out["status"]), C.c_void_p(self._torch_stream())))
+        batch = _PoseBatch(B, E2, E3, _dp(q), _dp(t), _dp(cam), _dp(ptr2), _dp(X2), _dp(meas2), _dp(omega2), _dp(ptr3), _dp(X3), _dp(meas3),
+                           _dp(omega3))
+        _check(self.L.cuba_engine_optimize_poses_device(self.h, C.byref(batch), R, rs, _dp(workspace), workspace.numel() * workspace.element_size(),
+                                                        _dp(out["q"]), _dp(out["t"]), _dp(out["levels"]), _dp(out["counts"]),
+                                                        _dp(out["stats"]), _dp(out["nstats"]), _dp(out["status"]), C.c_void_p(self._torch_stream())))
         out["workspace"] = workspace
         return out
 
@@ -841,11 +841,10 @@ class Engine:
         prm = _Sim3Params(float(params.chi2), int(params.iterations), int(params.iterations_bad), int(params.iterations_good),
                           int(params.min_pairs))
         workspace = self._workspace(torch, workspace, int(self.L.cuba_sim3_batch_workspace_bytes(B, N, C.byref(prm), int(bool(with_stats)))))
-        p = lambda a: None if a is None else a.data_ptr()
-        batch = _Sim3Batch(B, N, p(ptr), p(q), p(t), p(s), p(cam1), p(cam2), p(fix_scale), p(X1), p(X2), p(obs1), p(obs2), p(omega1), p(omega2))
-        _check(self.L.cuba_engine_optimize_sim3_device(self.h, C.byref(batch), C.byref(prm), p(workspace),
-                                                       workspace.numel() * workspace.element_size(), p(out["q"]), p(out["t"]), p(out["s"]),
-                                                       p(out["levels"]), p(out["ninliers"]), p(out["stats"]), p(out["nstats"]), p(out["status"]),
+        batch = _Sim3Batch(B, N, _dp(ptr), _dp(q), _dp(t), _dp(s), _dp(cam1), _dp(cam2), _dp(fix_scale), _dp(X1), _dp(X2), _dp(obs1), _dp(obs2), _dp(omega1), _dp(omega2))
+        _check(self.L.cuba_engine_optimize_sim3_device(self.h, C.byref(batch), C.byref(prm), _dp(workspace),
+                                                       workspace.numel() * workspace.element_size(), _dp(out["q"]), _dp(out["t"]), _dp(out["s"]),
+                                                       _dp(out["levels"]), _dp(out["ninliers"]), _dp(out["stats"]), _dp(out["nstats"]), _dp(out["status"]),
                                                        C.c_void_p(self._torch_stream())))
         out["workspace"] = workspace
         return out
@@ -879,12 +878,11 @@ class Engine:
         out, workspace, torch = self._device_call(what, [(n, a) for n, a, _ in inputs], spec, with_stats, out, workspace)
         rs = self._rounds_struct(rounds)
         workspace = self._workspace(torch, workspace, int(self.L.cuba_point_batch_workspace_bytes(B, P, E2, E3, R, rs, int(bool(with_stats)))))
-        ptr = lambda a: None if a is None else a.data_ptr()
-        batch = _PointBatch(B, P, E2, E3, ptr(Xw), ptr(q), ptr(t), ptr(cam), ptr(ptr2), ptr(iP2), ptr(meas2), ptr(omega2), ptr(ptr3), ptr(iP3),
-                            ptr(meas3), ptr(omega3))
-        _check(self.L.cuba_engine_optimize_points_device(self.h, C.byref(batch), R, rs, ptr(workspace), workspace.numel() * workspace.element_size(),
-                                                         ptr(out["Xw"]), ptr(out["levels"]), ptr(out["counts"]), ptr(out["stats"]),
-                                                         ptr(out["nstats"]), ptr(out["status"]), C.c_void_p(self._torch_stream())))
+        batch = _PointBatch(B, P, E2, E3, _dp(Xw), _dp(q), _dp(t), _dp(cam), _dp(ptr2), _dp(iP2), _dp(meas2), _dp(omega2), _dp(ptr3), _dp(iP3),
+                            _dp(meas3), _dp(omega3))
+        _check(self.L.cuba_engine_optimize_points_device(self.h, C.byref(batch), R, rs, _dp(workspace), workspace.numel() * workspace.element_size(),
+                                                         _dp(out["Xw"]), _dp(out["levels"]), _dp(out["counts"]), _dp(out["stats"]),
+                                                         _dp(out["nstats"]), _dp(out["status"]), C.c_void_p(self._torch_stream())))
         out["workspace"] = workspace
         return out
 

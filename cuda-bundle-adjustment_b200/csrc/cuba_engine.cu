@@ -325,14 +325,18 @@ struct EngineBase {
 	int devOrdinal = 0;      // CUDA device every call of this engine runs on (set once in init)
 	void* comm = nullptr;
 	bool haveProblem = false;
+	cudaStream_t stream = nullptr;   // the engine's own (init)
 	long long launches = 0;
 	double prof[CUBA_PROF_NUM] = { 0 };
+	// the batched LM kernels' packed batch and packed results, device and page-locked host copies, grown to the largest call; the
+	// host entry of optimize_landmarks moves its list and per-landmark outputs through them too
+	DBuf<double> batchIn, batchOut;
+	PinnedBuf batchHostIn, batchHostOut;
 
 	virtual int set_problem(const cuba_problem* p) = 0;
 	virtual int set_state(const double* q, const double* t, const double* Xw) = 0;
 	virtual int get_sizes(cuba_sizes* out) const = 0;
 	virtual int reset_state() = 0;
-	virtual int get_stream(void** s) = 0;
 	virtual int flush_l2() = 0;
 	virtual int optimize(int niter, cuba_iter_stat* stats, int* nstats) = 0;
 	virtual int get_state(double* q, double* t, double* Xw) = 0;
@@ -367,12 +371,17 @@ struct EngineBase {
 	virtual int get_chi2_device(double* out, cudaStream_t caller) = 0;
 	virtual int set_edge_levels_device(const uint8_t* levels, cudaStream_t caller) = 0;
 	virtual int get_edge_levels_device(uint8_t* levels, cudaStream_t caller) = 0;
-	virtual int optimize_poses(const cuba_pose_batch* bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
-		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) = 0;
-	virtual int optimize_sim3(const cuba_sim3_batch* bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
-		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats) = 0;
-	virtual int optimize_points(const cuba_point_batch* bt, const pb::Schedule& s, double* XwOut, uint8_t* levelsOut, int32_t* counts,
-		cuba_iter_stat* stats, int32_t* nstats) = 0;
+	// the batched LM kernels on host arrays (cuba_batch_io.cuh): always fp64, on the stream; they touch nothing of the engine's
+	// problem.  The batch was validated by the caller and has B > 0.
+	int optimize_poses(const cuba_pose_batch& bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut, int32_t* counts,
+		cuba_iter_stat* stats, int32_t* nstats);
+	int optimize_sim3(const cuba_sim3_batch& bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
+		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats);
+	int optimize_points(const cuba_point_batch& bt, const pb::Schedule& s, double* XwOut, uint8_t* levelsOut, int32_t* counts,
+		cuba_iter_stat* stats, int32_t* nstats);
+	int batch_grow(size_t nIn, size_t nOut);
+	int batch_up(size_t nIn);
+	int batch_down(size_t nOut);
 	// structure-only refinement of the held problem's free landmarks in place; dev: list, stats and nstats are device pointers
 	virtual int optimize_landmarks(const int32_t* list, int n, const pb::Schedule& s, int32_t* counts, cuba_iter_stat* stats,
 		int32_t* nstats, bool dev, cudaStream_t caller) = 0;
@@ -383,7 +392,6 @@ struct EngineBase {
 template <typename T>
 struct Engine : EngineBase {
 	Structure S;
-	cudaStream_t stream = nullptr;
 	int numSMs = 0;
 	int smemMax = 0;        // opt-in dynamic shared memory of one CTA
 	int ntiles = 0, nPoseBlocks = 0, nChiBlocks = 0;
@@ -463,10 +471,6 @@ struct Engine : EngineBase {
 	// optimize_landmarks: per-CTA counts, the per-round totals | status word (one read-back), the device list's marks
 	DBuf<int> lrPartial, lrMark;
 	DBuf<double> lrTotal;
-	// the batched LM kernels (optimize_poses, optimize_sim3, optimize_points, one after the other on the stream): the packed batch
-	// and the packed results, device and page-locked host copies
-	DBuf<double> batchIn, batchOut;
-	PinnedBuf batchHostIn, batchHostOut;
 	DBuf<Scalars> dScal;
 	Scalars* hScal = nullptr;   // pinned
 	DBuf<double> flushBuf;
@@ -1097,7 +1101,6 @@ struct Engine : EngineBase {
 		trialValid = false;
 		return CUBA_OK;
 	}
-	int get_stream(void** s) override { *s = (void*)stream; return CUBA_OK; }
 	int flush_l2() override
 	{
 		const size_t flushN = (size_t)40 << 20;
@@ -2495,208 +2498,6 @@ struct Engine : EngineBase {
 		return CUBA_OK;
 	}
 
-	// ---- the batched LM kernels: each entry point packs its batch into batchHostIn (layouts of cuba_batch_io.cuh) and unpacks its
-	// results from batchHostOut.  Always fp64, on this engine's stream; they touch nothing of the engine's problem.  The batch was validated by the caller.
-	static_assert(sizeof(lm::IterStat) == sizeof(cuba_iter_stat) && sizeof(lm::IterStat) == 32, "cuba_iter_stat layout");
-
-	// one H2D of the packed batch (nIn doubles), the launch of `grid` CTAs of lm::BLOCK threads, one D2H of the packed results (nOut
-	// doubles)
-	template <class Args, class Params>
-	int batch_round_trip(void (*kernel)(Args, Params), unsigned grid, const Args& a, const Params& p, size_t nIn, size_t nOut)
-	{
-		CUDA_TRY(cudaMemcpyAsync(batchIn.p, batchHostIn.p, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
-		g_h2dBytes += (long long)(sizeof(double) * nIn);
-		kernel<<<grid, lm::BLOCK, 0, stream>>>(a, p);
-		launches++;
-		CUDA_TRY(cudaGetLastError());
-		CUDA_TRY(cudaMemcpyAsync(batchHostOut.p, batchOut.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
-		g_d2hBytes += (long long)(sizeof(double) * nOut);
-		CUDA_TRY(cudaStreamSynchronize(stream));
-		return CUBA_OK;
-	}
-
-	// batched pose optimisation (cuba_pose_batch.cuh)
-	int optimize_poses(const cuba_pose_batch* bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
-		int32_t* counts, cuba_iter_stat* stats, int32_t* nstats) override
-	{
-		const size_t B = (size_t)bt->B, R = (size_t)s.n;
-		if (B == 0) return CUBA_OK;
-		const size_t E2 = (size_t)bt->E2, E3 = (size_t)bt->E3, E = E2 + E3;
-		const size_t nStat = stats ? B * (size_t)s.statOff[s.n] : 0;
-		const bio::PoseLayout L(B, E, R, nStat);
-		const size_t oCam = L.oCam, oEdge = L.oEdge, oPtr = L.oPtr, nIn = L.nIn, oStat = L.oStat, oInt = L.oInt, oLev = L.oLev, nOut = L.nOut;
-		CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * nOut));
-		CUDA_TRY(batchIn.alloc(nIn)); CUDA_TRY(batchOut.alloc(nOut));
-		double* h = (double*)batchHostIn.p;
-		for (size_t b = 0; b < B; b++) {
-			double* p = h + 8 * b;
-			for (int k = 0; k < 4; k++) p[k] = bt->q[4 * b + k];
-			for (int k = 0; k < 3; k++) p[4 + k] = bt->t[3 * b + k];
-			p[7] = 0;
-			double* c = h + oCam + 8 * b;
-			for (int k = 0; k < 5; k++) c[k] = bt->cam[5 * b + k];
-			c[5] = c[6] = c[7] = 0;
-			// a frame's edges are contiguous, its mono edges first: mono i at ptr3[b] + i, stereo j at ptr2[b+1] + j
-			for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) {
-				double* d = h + oEdge + 8 * ((size_t)bt->ptr3[b] + i);
-				d[0] = bt->X2[3 * i]; d[1] = bt->X2[3 * i + 1]; d[2] = bt->X2[3 * i + 2];
-				d[3] = bt->meas2[2 * i]; d[4] = bt->meas2[2 * i + 1]; d[5] = 0; d[6] = bt->omega2[i]; d[7] = 0;
-			}
-			for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) {
-				double* d = h + oEdge + 8 * ((size_t)bt->ptr2[b + 1] + j);
-				d[0] = bt->X3[3 * j]; d[1] = bt->X3[3 * j + 1]; d[2] = bt->X3[3 * j + 2];
-				d[3] = bt->meas3[3 * j]; d[4] = bt->meas3[3 * j + 1]; d[5] = bt->meas3[3 * j + 2]; d[6] = bt->omega3[j]; d[7] = 0;
-			}
-		}
-		int32_t* hp = (int32_t*)(h + oPtr);
-		memcpy(hp, bt->ptr2, sizeof(int32_t) * (B + 1));
-		memcpy(hp + B + 1, bt->ptr3, sizeof(int32_t) * (B + 1));
-		pb::Args a;
-		a.B = (int)B;
-		a.pose = batchIn.p; a.cam = batchIn.p + oCam; a.edge = batchIn.p + oEdge;
-		a.ptr2 = (const int*)(batchIn.p + oPtr); a.ptr3 = a.ptr2 + B + 1;
-		a.poseOut = batchOut.p;
-		a.stats = stats ? (lm::IterStat*)(batchOut.p + oStat) : nullptr;
-		a.counts = (int*)(batchOut.p + oInt); a.nstats = a.counts + 4 * B * R;
-		a.level = (unsigned char*)(batchOut.p + oLev);
-		const int rc = batch_round_trip(pb::k_pose_batch, (unsigned)B, a, s, nIn, nOut); if (rc) return rc;
-		const double* o = (const double*)batchHostOut.p;
-		for (size_t b = 0; b < B; b++) {
-			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
-			for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
-		}
-		if (stats && nStat) memcpy(stats, o + oStat, sizeof(cuba_iter_stat) * nStat);
-		const int32_t* oi = (const int32_t*)(o + oInt);
-		if (counts) memcpy(counts, oi, sizeof(int32_t) * 4 * B * R);
-		if (nstats) memcpy(nstats, oi + 4 * B * R, sizeof(int32_t) * B * R);
-		if (levelsOut) {
-			const unsigned char* lv = (const unsigned char*)(o + oLev);
-			for (size_t b = 0; b < B; b++) {
-				for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) levelsOut[i] = lv[(size_t)bt->ptr3[b] + i];
-				for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) levelsOut[E2 + j] = lv[(size_t)bt->ptr2[b + 1] + j];
-			}
-		}
-		return CUBA_OK;
-	}
-
-	// batched Sim(3) alignment (cuba_sim3_batch.cuh)
-	int optimize_sim3(const cuba_sim3_batch* bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
-		int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats) override
-	{
-		const size_t B = (size_t)bt->B, N = (size_t)bt->N;
-		if (B == 0) return CUBA_OK;
-		const size_t nStat = stats ? B * (size_t)p.statPer : 0;
-		const bio::Sim3Layout L(B, N, nStat);
-		const size_t oPair = L.oPair, oPtr = L.oPtr, nIn = L.nIn, oStat = L.oStat, oInt = L.oInt, oLev = L.oLev, nOut = L.nOut;
-		CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * nOut));
-		CUDA_TRY(batchIn.alloc(nIn)); CUDA_TRY(batchOut.alloc(nOut));
-		double* h = (double*)batchHostIn.p;
-		for (size_t b = 0; b < B; b++) {
-			double* d = h + s3::PROB * b;
-			for (int k = 0; k < 4; k++) d[k] = bt->q[4 * b + k];
-			for (int k = 0; k < 3; k++) d[4 + k] = bt->t[3 * b + k];
-			d[7] = bt->s[b];
-			for (int k = 0; k < 4; k++) { d[8 + k] = bt->cam1[4 * b + k]; d[12 + k] = bt->cam2[4 * b + k]; }
-			d[16] = bt->fix_scale && bt->fix_scale[b] ? 1.0 : 0.0;
-			d[17] = d[18] = d[19] = 0;
-		}
-		for (size_t i = 0; i < N; i++) {
-			double* d = h + oPair + s3::PAIR * i;
-			for (int k = 0; k < 3; k++) { d[k] = bt->X1[3 * i + k]; d[3 + k] = bt->X2[3 * i + k]; }
-			d[6] = bt->obs1[2 * i]; d[7] = bt->obs1[2 * i + 1]; d[8] = bt->obs2[2 * i]; d[9] = bt->obs2[2 * i + 1];
-			d[10] = bt->omega1[i]; d[11] = bt->omega2[i];
-		}
-		memcpy(h + oPtr, bt->ptr, sizeof(int32_t) * (B + 1));
-		s3::Args a;
-		a.B = (int)B;
-		a.prob = batchIn.p; a.pair = batchIn.p + oPair; a.ptr = (const int*)(batchIn.p + oPtr);
-		a.Sout = batchOut.p;
-		a.stats = stats ? (lm::IterStat*)(batchOut.p + oStat) : nullptr;
-		a.ninliers = (int*)(batchOut.p + oInt); a.nstats = a.ninliers + B;
-		a.level = (unsigned char*)(batchOut.p + oLev);
-		const int rc = batch_round_trip(s3::k_sim3_batch, (unsigned)B, a, p, nIn, nOut); if (rc) return rc;
-		const double* o = (const double*)batchHostOut.p;
-		for (size_t b = 0; b < B; b++) {
-			for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
-			for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
-			sOut[b] = o[8 * b + 7];
-		}
-		if (stats && nStat) memcpy(stats, o + oStat, sizeof(cuba_iter_stat) * nStat);
-		const int32_t* oi = (const int32_t*)(o + oInt);
-		if (ninliers) memcpy(ninliers, oi, sizeof(int32_t) * B);
-		if (nstats) memcpy(nstats, oi + B, sizeof(int32_t) * 2 * B);
-		if (levelsOut && N) memcpy(levelsOut, (const unsigned char*)(o + oLev), N);
-		return CUBA_OK;
-	}
-
-	// batched structure-only refinement (cuba_point_batch.cuh)
-	int optimize_points(const cuba_point_batch* bt, const pb::Schedule& s, double* XwOut, uint8_t* levelsOut, int32_t* counts,
-		cuba_iter_stat* stats, int32_t* nstats) override
-	{
-		const size_t B = (size_t)bt->B, P = (size_t)bt->P, R = (size_t)s.n;
-		if (B == 0) return CUBA_OK;
-		const size_t E2 = (size_t)bt->E2, E3 = (size_t)bt->E3, E = E2 + E3;
-		const size_t nStat = stats ? B * (size_t)s.statOff[s.n] : 0;
-		const bio::PointLayout L(B, P, E, R, nStat);
-		CUDA_TRY(batchHostIn.grow(sizeof(double) * L.nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * L.nOut));
-		CUDA_TRY(batchIn.alloc(L.nIn)); CUDA_TRY(batchOut.alloc(L.nOut));
-		double* h = (double*)batchHostIn.p;
-		for (size_t p = 0; p < P; p++) {
-			double* d = h + L.oPose + 8 * p;
-			for (int k = 0; k < 4; k++) d[k] = bt->q[4 * p + k];
-			for (int k = 0; k < 3; k++) d[4 + k] = bt->t[3 * p + k];
-			d[7] = 0;
-			double* c = h + L.oCam + 8 * p;
-			for (int k = 0; k < 5; k++) c[k] = bt->cam[5 * p + k];
-			c[5] = c[6] = c[7] = 0;
-		}
-		int32_t* hi = (int32_t*)(h + L.oIdx);
-		for (size_t b = 0; b < B; b++) {
-			double* x = h + 4 * b;
-			for (int k = 0; k < 3; k++) x[k] = bt->Xw[3 * b + k];
-			x[3] = 0;
-			// a point's edges are contiguous, its mono edges first: mono i at ptr3[b] + i, stereo j at ptr2[b+1] + j
-			for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) {
-				const size_t k = (size_t)bt->ptr3[b] + i;
-				double* d = h + L.oEdge + 4 * k;
-				d[0] = bt->meas2[2 * i]; d[1] = bt->meas2[2 * i + 1]; d[2] = 0; d[3] = bt->omega2[i];
-				hi[k] = bt->iP2[i];
-			}
-			for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) {
-				const size_t k = (size_t)bt->ptr2[b + 1] + j;
-				double* d = h + L.oEdge + 4 * k;
-				d[0] = bt->meas3[3 * j]; d[1] = bt->meas3[3 * j + 1]; d[2] = bt->meas3[3 * j + 2]; d[3] = bt->omega3[j];
-				hi[k] = bt->iP3[j];
-			}
-		}
-		memcpy(hi + E, bt->ptr2, sizeof(int32_t) * (B + 1));
-		memcpy(hi + E + B + 1, bt->ptr3, sizeof(int32_t) * (B + 1));
-		ptb::Args a;
-		a.B = (int)B;
-		a.Xw = batchIn.p; a.pose = batchIn.p + L.oPose; a.cam = batchIn.p + L.oCam; a.edge = batchIn.p + L.oEdge;
-		a.iP = (const int*)(batchIn.p + L.oIdx); a.ptr2 = a.iP + E; a.ptr3 = a.ptr2 + B + 1;
-		a.XwOut = batchOut.p;
-		a.stats = stats ? (lm::IterStat*)(batchOut.p + L.oStat) : nullptr;
-		a.counts = (int*)(batchOut.p + L.oInt); a.nstats = a.counts + 4 * B * R;
-		a.level = (unsigned char*)(batchOut.p + L.oLev);
-		const int rc = batch_round_trip(ptb::k_point_batch, (unsigned)((B + ptb::WARPS - 1) / ptb::WARPS), a, s, L.nIn, L.nOut); if (rc) return rc;
-		const double* o = (const double*)batchHostOut.p;
-		for (size_t b = 0; b < B; b++)
-			for (int k = 0; k < 3; k++) XwOut[3 * b + k] = o[4 * b + k];
-		if (stats && nStat) memcpy(stats, o + L.oStat, sizeof(cuba_iter_stat) * nStat);
-		const int32_t* oi = (const int32_t*)(o + L.oInt);
-		if (counts) memcpy(counts, oi, sizeof(int32_t) * 4 * B * R);
-		if (nstats) memcpy(nstats, oi + 4 * B * R, sizeof(int32_t) * B * R);
-		if (levelsOut) {
-			const unsigned char* lv = (const unsigned char*)(o + L.oLev);
-			for (size_t b = 0; b < B; b++) {
-				for (size_t i = (size_t)bt->ptr2[b]; i < (size_t)bt->ptr2[b + 1]; i++) levelsOut[i] = lv[(size_t)bt->ptr3[b] + i];
-				for (size_t j = (size_t)bt->ptr3[b]; j < (size_t)bt->ptr3[b + 1]; j++) levelsOut[E2 + j] = lv[(size_t)bt->ptr2[b + 1] + j];
-			}
-		}
-		return CUBA_OK;
-	}
-
 	// ---- structure-only refinement of the held landmarks in place (cuba_landmark_refine.cuh) -----------------------------------
 	int num_free_landmarks() const override { return S.numL; }
 	bool fp32() const override { return sizeof(T) != 8; }
@@ -3142,6 +2943,99 @@ struct Engine : EngineBase {
 	}
 };
 
+// ---- the batched LM kernels from host arrays: grow the buffers, pack on the host, copy up, launch, copy down, synchronise, unpack on
+// the host
+static_assert(sizeof(lm::IterStat) == sizeof(cuba_iter_stat) && sizeof(lm::IterStat) == 32, "cuba_iter_stat layout");
+
+int EngineBase::batch_grow(size_t nIn, size_t nOut)
+{
+	CUDA_TRY(batchHostIn.grow(sizeof(double) * nIn)); CUDA_TRY(batchHostOut.grow(sizeof(double) * nOut));
+	CUDA_TRY(batchIn.alloc(nIn)); CUDA_TRY(batchOut.alloc(nOut));
+	return CUBA_OK;
+}
+
+// the nIn packed doubles of batchHostIn up to batchIn
+int EngineBase::batch_up(size_t nIn)
+{
+	CUDA_TRY(cudaMemcpyAsync(batchIn.p, batchHostIn.p, sizeof(double) * nIn, cudaMemcpyHostToDevice, stream));
+	g_h2dBytes += (long long)(sizeof(double) * nIn);
+	return CUBA_OK;
+}
+
+// after the one launch on batchIn: the nOut result doubles of batchOut down to batchHostOut, synchronised
+int EngineBase::batch_down(size_t nOut)
+{
+	launches++;
+	CUDA_TRY(cudaGetLastError());
+	CUDA_TRY(cudaMemcpyAsync(batchHostOut.p, batchOut.p, sizeof(double) * nOut, cudaMemcpyDeviceToHost, stream));
+	g_d2hBytes += (long long)(sizeof(double) * nOut);
+	CUDA_TRY(cudaStreamSynchronize(stream));
+	return CUBA_OK;
+}
+
+int EngineBase::optimize_poses(const cuba_pose_batch& bt, const pb::Schedule& s, double* qOut, double* tOut, uint8_t* levelsOut,
+	int32_t* counts, cuba_iter_stat* stats, int32_t* nstats)
+{
+	const size_t B = (size_t)bt.B, nStat = stats ? B * (size_t)s.statOff[s.n] : 0;
+	const bio::PoseLayout L(B, (size_t)bt.E2 + (size_t)bt.E3, (size_t)s.n, nStat);
+	int rc = batch_grow(L.nIn, L.nOut); if (rc) return rc;
+	bio::pack_poses(bt, L, (double*)batchHostIn.p);
+	rc = batch_up(L.nIn); if (rc) return rc;
+	bio::launch_poses(L, bt.B, s, batchIn.p, batchOut.p, stats != nullptr, stream);
+	rc = batch_down(L.nOut); if (rc) return rc;
+	const double* o = (const double*)batchHostOut.p;
+	const int32_t* p2 = (const int32_t*)((const double*)batchHostIn.p + L.oPtr);
+	for (size_t b = 0; b < B; b++) {
+		for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
+		for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
+		bio::unpack_rounds(L, o, p2, (int)b, bt.B, s.n, bt.E2, s.statOff[s.n], 0, 1, levelsOut, counts, stats, nstats);
+	}
+	return CUBA_OK;
+}
+
+int EngineBase::optimize_sim3(const cuba_sim3_batch& bt, const s3::Params& p, double* qOut, double* tOut, double* sOut, uint8_t* levelsOut,
+	int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats)
+{
+	const size_t B = (size_t)bt.B, N = (size_t)bt.N, nStat = stats ? B * (size_t)p.statPer : 0;
+	const bio::Sim3Layout L(B, N, nStat);
+	int rc = batch_grow(L.nIn, L.nOut); if (rc) return rc;
+	bio::pack_sim3(bt, L, (double*)batchHostIn.p);
+	rc = batch_up(L.nIn); if (rc) return rc;
+	bio::launch_sim3(L, bt.B, p, batchIn.p, batchOut.p, stats != nullptr, stream);
+	rc = batch_down(L.nOut); if (rc) return rc;
+	const double* o = (const double*)batchHostOut.p;
+	for (size_t b = 0; b < B; b++) {
+		for (int k = 0; k < 4; k++) qOut[4 * b + k] = o[8 * b + k];
+		for (int k = 0; k < 3; k++) tOut[3 * b + k] = o[8 * b + 4 + k];
+		sOut[b] = o[8 * b + 7];
+	}
+	if (stats && nStat) memcpy(stats, o + L.oStat, sizeof(cuba_iter_stat) * nStat);
+	const int32_t* oi = (const int32_t*)(o + L.oInt);
+	if (ninliers) memcpy(ninliers, oi, sizeof(int32_t) * B);
+	if (nstats) memcpy(nstats, oi + B, sizeof(int32_t) * 2 * B);
+	if (levelsOut && N) memcpy(levelsOut, (const unsigned char*)(o + L.oLev), N);
+	return CUBA_OK;
+}
+
+int EngineBase::optimize_points(const cuba_point_batch& bt, const pb::Schedule& s, double* XwOut, uint8_t* levelsOut, int32_t* counts,
+	cuba_iter_stat* stats, int32_t* nstats)
+{
+	const size_t B = (size_t)bt.B, E = (size_t)bt.E2 + (size_t)bt.E3, nStat = stats ? B * (size_t)s.statOff[s.n] : 0;
+	const bio::PointLayout L(B, (size_t)bt.P, E, (size_t)s.n, nStat);
+	int rc = batch_grow(L.nIn, L.nOut); if (rc) return rc;
+	bio::pack_points(bt, L, (double*)batchHostIn.p);
+	rc = batch_up(L.nIn); if (rc) return rc;
+	bio::launch_points(L, bt.B, E, s, batchIn.p, batchOut.p, stats != nullptr, stream);
+	rc = batch_down(L.nOut); if (rc) return rc;
+	const double* o = (const double*)batchHostOut.p;
+	const int32_t* p2 = (const int32_t*)((const double*)batchHostIn.p + L.oIdx) + E;
+	for (size_t b = 0; b < B; b++) {
+		for (int k = 0; k < 3; k++) XwOut[3 * b + k] = o[4 * b + k];
+		bio::unpack_rounds(L, o, p2, (int)b, bt.B, s.n, bt.E2, s.statOff[s.n], 0, 1, levelsOut, counts, stats, nstats);
+	}
+	return CUBA_OK;
+}
+
 }  // namespace cuba_b200
 
 // ======================================================================================================
@@ -3239,7 +3133,7 @@ int cuba_engine_set_state(cuba_engine* e, const double* q, const double* t, cons
 }
 int cuba_engine_reset_state(cuba_engine* e) { ENGINE_OR_FAIL(e); return e->impl->reset_state(); }
 int cuba_engine_get_device(const cuba_engine* e, int* device) { ENGINE_OR_FAIL(e); if (!device) return fail(CUBA_ERR_INVALID, "null out"); *device = e->impl->devOrdinal; return CUBA_OK; }
-int cuba_engine_get_stream(cuba_engine* e, void** s) { ENGINE_OR_FAIL(e); if (!s) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_stream(s); }
+int cuba_engine_get_stream(cuba_engine* e, void** s) { ENGINE_OR_FAIL(e); if (!s) return fail(CUBA_ERR_INVALID, "null out"); *s = (void*)e->impl->stream; return CUBA_OK; }
 int cuba_engine_flush_l2(cuba_engine* e) { ENGINE_OR_FAIL(e); return e->impl->flush_l2(); }
 int cuba_engine_get_sizes(const cuba_engine* e, cuba_sizes* out) { ENGINE_OR_FAIL(e); if (!out) return fail(CUBA_ERR_INVALID, "null out"); return e->impl->get_sizes(out); }
 int cuba_engine_optimize(cuba_engine* e, int niter, cuba_iter_stat* stats, int* nstats) { ENGINE_OR_FAIL(e); return e->impl->optimize(niter, stats, nstats); }
@@ -3343,22 +3237,35 @@ static int pose_schedule(int nrounds, const cuba_pose_round* rounds, pb::Schedul
 	return CUBA_OK;
 }
 
+// the checks of optimize_poses and optimize_poses_device that need no element of the batch's arrays
+static int pose_batch_args(const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds, pb::Schedule& s)
+{
+	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_poses: null batch");
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: B < 0");
+	return pose_schedule(nrounds, rounds, s);
+}
+
+// pose_batch_args' checks of the pointers, for B > 0
+static int pose_batch_pointers(const cuba_pose_batch* bt, const double* qOut, const double* tOut)
+{
+	if (!bt->q || !bt->t || !bt->cam || !qOut || !tOut) return fail(CUBA_ERR_INVALID, "optimize_poses: null pose array");
+	if ((long long)bt->E2 + bt->E3 > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many edges");
+	return CUBA_OK;
+}
+
 int cuba_engine_optimize_poses(cuba_engine* e, const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds,
 	double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats, int32_t* nstats)
 {
 	ENGINE_OR_FAIL(e);
-	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_poses: null batch");
-	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: B < 0");
 	pb::Schedule s;
-	{ const int rc0 = pose_schedule(nrounds, rounds, s); if (rc0) return rc0; }
+	int rc = pose_batch_args(bt, nrounds, rounds, s); if (rc) return rc;
 	const int B = bt->B;
 	if (B == 0) return CUBA_OK;
-	if (!bt->q || !bt->t || !bt->cam || !q_out || !t_out) return fail(CUBA_ERR_INVALID, "optimize_poses: null pose array");
-	if ((long long)bt->E2 + bt->E3 > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many edges");
-	int rc = csr_ok("optimize_poses: ptr2", B, bt->E2, bt->ptr2, { bt->X2, bt->meas2, bt->omega2 }); if (rc) return rc;
+	rc = pose_batch_pointers(bt, q_out, t_out); if (rc) return rc;
+	rc = csr_ok("optimize_poses: ptr2", B, bt->E2, bt->ptr2, { bt->X2, bt->meas2, bt->omega2 }); if (rc) return rc;
 	rc = csr_ok("optimize_poses: ptr3", B, bt->E3, bt->ptr3, { bt->X3, bt->meas3, bt->omega3 }); if (rc) return rc;
 	if (!all_finite(bt->omega2, bt->E2) || !all_finite(bt->omega3, bt->E3)) return fail(CUBA_ERR_INVALID, "optimize_poses: non-finite omega");
-	return e->impl->optimize_poses(bt, s, q_out, t_out, levels_out, counts, stats, nstats);
+	return e->impl->optimize_poses(*bt, s, q_out, t_out, levels_out, counts, stats, nstats);
 }
 
 // host arrays of a point batch: a pose index outside [0, P)
@@ -3394,16 +3301,16 @@ int cuba_engine_optimize_points(cuba_engine* e, const cuba_point_batch* bt, int 
 {
 	ENGINE_OR_FAIL(e);
 	pb::Schedule s;
-	{ const int rc0 = point_batch_args(bt, nrounds, rounds, s); if (rc0) return rc0; }
+	int rc = point_batch_args(bt, nrounds, rounds, s); if (rc) return rc;
 	const int B = bt->B;
 	if (B == 0) return CUBA_OK;
-	int rc = point_batch_pointers(bt, Xw_out); if (rc) return rc;
+	rc = point_batch_pointers(bt, Xw_out); if (rc) return rc;
 	rc = csr_ok("optimize_points: ptr2", B, bt->E2, bt->ptr2, { bt->iP2, bt->meas2, bt->omega2 }); if (rc) return rc;
 	rc = csr_ok("optimize_points: ptr3", B, bt->E3, bt->ptr3, { bt->iP3, bt->meas3, bt->omega3 }); if (rc) return rc;
 	if (!poses_in_range(bt->iP2, bt->E2, bt->P)) return fail(CUBA_ERR_INVALID, "optimize_points: iP2 outside [0, P)");
 	if (!poses_in_range(bt->iP3, bt->E3, bt->P)) return fail(CUBA_ERR_INVALID, "optimize_points: iP3 outside [0, P)");
 	if (!all_finite(bt->omega2, bt->E2) || !all_finite(bt->omega3, bt->E3)) return fail(CUBA_ERR_INVALID, "optimize_points: non-finite omega");
-	return e->impl->optimize_points(bt, s, Xw_out, levels_out, counts, stats, nstats);
+	return e->impl->optimize_points(*bt, s, Xw_out, levels_out, counts, stats, nstats);
 }
 
 // the parameters of optimize_sim3, checked
@@ -3420,21 +3327,35 @@ static int sim3_params(const cuba_sim3_params& P, s3::Params& p)
 	return CUBA_OK;
 }
 
+// the checks of optimize_sim3 and optimize_sim3_device that need no element of the batch's arrays
+static int sim3_batch_args(const cuba_sim3_batch* bt, const cuba_sim3_params* params, s3::Params& p)
+{
+	if (!bt || !params) return fail(CUBA_ERR_INVALID, "optimize_sim3: null batch or params");
+	const int rc = sim3_params(*params, p); if (rc) return rc;
+	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: B < 0");
+	if (bt->N < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: N < 0");
+	return CUBA_OK;
+}
+
+// sim3_batch_args' checks of the problem pointers, for B > 0
+static int sim3_batch_pointers(const cuba_sim3_batch* bt, const double* qOut, const double* tOut, const double* sOut)
+{
+	if (!bt->q || !bt->t || !bt->s || !bt->cam1 || !bt->cam2 || !qOut || !tOut || !sOut)
+		return fail(CUBA_ERR_INVALID, "optimize_sim3: null problem array");
+	return CUBA_OK;
+}
+
 int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const cuba_sim3_params* params, double* q_out, double* t_out,
 	double* s_out, uint8_t* levels_out, int32_t* ninliers, cuba_iter_stat* stats, int32_t* nstats)
 {
 	ENGINE_OR_FAIL(e);
-	if (!bt || !params) return fail(CUBA_ERR_INVALID, "optimize_sim3: null batch or params");
 	s3::Params p;
-	{ const int rc0 = sim3_params(*params, p); if (rc0) return rc0; }
-	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: B < 0");
-	if (bt->N < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: N < 0");
+	int rc = sim3_batch_args(bt, params, p); if (rc) return rc;
 	const int B = bt->B;
 	if (B == 0) return CUBA_OK;
 	const size_t nb = (size_t)B, N = (size_t)bt->N;
-	const int rc = csr_ok("optimize_sim3: ptr", B, bt->N, bt->ptr, { bt->X1, bt->X2, bt->obs1, bt->obs2, bt->omega1, bt->omega2 }); if (rc) return rc;
-	if (!bt->q || !bt->t || !bt->s || !bt->cam1 || !bt->cam2 || !q_out || !t_out || !s_out)
-		return fail(CUBA_ERR_INVALID, "optimize_sim3: null problem array");
+	rc = csr_ok("optimize_sim3: ptr", B, bt->N, bt->ptr, { bt->X1, bt->X2, bt->obs1, bt->obs2, bt->omega1, bt->omega2 }); if (rc) return rc;
+	rc = sim3_batch_pointers(bt, q_out, t_out, s_out); if (rc) return rc;
 	if (!all_finite(bt->q, 4 * nb) || !all_finite(bt->t, 3 * nb) || !all_finite(bt->s, nb) || !all_finite(bt->cam1, 4 * nb) ||
 		!all_finite(bt->cam2, 4 * nb))
 		return fail(CUBA_ERR_INVALID, "optimize_sim3: non-finite S12 or intrinsics");
@@ -3443,7 +3364,7 @@ int cuba_engine_optimize_sim3(cuba_engine* e, const cuba_sim3_batch* bt, const c
 	if (!all_finite(bt->X1, 3 * N) || !all_finite(bt->X2, 3 * N) || !all_finite(bt->obs1, 2 * N) || !all_finite(bt->obs2, 2 * N) ||
 		!all_finite(bt->omega1, N) || !all_finite(bt->omega2, N))
 		return fail(CUBA_ERR_INVALID, "optimize_sim3: non-finite pair");
-	return e->impl->optimize_sim3(bt, p, q_out, t_out, s_out, levels_out, ninliers, stats, nstats);
+	return e->impl->optimize_sim3(*bt, p, q_out, t_out, s_out, levels_out, ninliers, stats, nstats);
 }
 
 // ---- the batches on device-resident data (cuba_batch_io.cuh).  Host-side checks come first and touch neither the engine nor a
@@ -3467,13 +3388,13 @@ static int workspace_ok(const char* what, const void* ws, size_t bytes, size_t n
 	return CUBA_OK;
 }
 
-static cudaStream_t batch_stream(cuba_engine* e, void* stream)
-{
-	if (stream) return (cudaStream_t)stream;
-	void* s = nullptr;
-	e->impl->get_stream(&s);
-	return (cudaStream_t)s;
-}
+// keeps the last error as it was over its scope: a size query leaves it alone
+struct KeepLastError {
+	const std::string saved = g_err;
+	~KeepLastError() { g_err = saved; }
+};
+
+static cudaStream_t batch_stream(cuba_engine* e, void* stream) { return stream ? (cudaStream_t)stream : e->impl->stream; }
 
 static size_t pose_workspace(int B, int E2, int E3, const pb::Schedule& s, bool withStats)
 {
@@ -3486,26 +3407,21 @@ size_t cuba_pose_batch_workspace_bytes(int B, int E2, int E3, int nrounds, const
 {
 	pb::Schedule s;
 	if (B <= 0 || E2 < 0 || E3 < 0 || (long long)E2 + E3 > INT32_MAX) return 0;
-	const std::string err = g_err;
-	const int rc = pose_schedule(nrounds, rounds, s);
-	g_err = err;       // a size query leaves the last error alone
-	return rc ? 0 : pose_workspace(B, E2, E3, s, with_stats != 0);
+	KeepLastError keep;
+	return pose_schedule(nrounds, rounds, s) ? 0 : pose_workspace(B, E2, E3, s, with_stats != 0);
 }
 
 int cuba_engine_optimize_poses_device(cuba_engine* e, const cuba_pose_batch* bt, int nrounds, const cuba_pose_round* rounds,
 	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, uint8_t* levels_out, int32_t* counts, cuba_iter_stat* stats,
 	int32_t* nstats, int32_t* status, void* stream)
 {
-	if (!bt) return fail(CUBA_ERR_INVALID, "optimize_poses: null batch");
-	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_poses: B < 0");
 	pb::Schedule s;
-	{ const int rc0 = pose_schedule(nrounds, rounds, s); if (rc0) return rc0; }
+	int rc = pose_batch_args(bt, nrounds, rounds, s); if (rc) return rc;
 	if (!status) return fail(CUBA_ERR_INVALID, "optimize_poses_device: null status");
 	const int B = bt->B;
 	if (B > 0) {
-		if (!bt->q || !bt->t || !bt->cam || !q_out || !t_out) return fail(CUBA_ERR_INVALID, "optimize_poses: null pose array");
-		if ((long long)bt->E2 + bt->E3 > INT32_MAX) return fail(CUBA_ERR_INVALID, "optimize_poses: too many edges");
-		int rc = csr_present("optimize_poses: ptr2", bt->E2, bt->ptr2, { bt->X2, bt->meas2, bt->omega2 }); if (rc) return rc;
+		rc = pose_batch_pointers(bt, q_out, t_out); if (rc) return rc;
+		rc = csr_present("optimize_poses: ptr2", bt->E2, bt->ptr2, { bt->X2, bt->meas2, bt->omega2 }); if (rc) return rc;
 		rc = csr_present("optimize_poses: ptr3", bt->E3, bt->ptr3, { bt->X3, bt->meas3, bt->omega3 }); if (rc) return rc;
 		rc = workspace_ok("optimize_poses_device", workspace, workspace_bytes, pose_workspace(B, bt->E2, bt->E3, s, stats != nullptr)); if (rc) return rc;
 	}
@@ -3518,16 +3434,7 @@ int cuba_engine_optimize_poses_device(cuba_engine* e, const cuba_pose_batch* bt,
 	double* in = (double*)workspace;
 	bio::k_validate_poses<<<bio::grid_for(std::max(nb + 1, E)), bio::BLOCK, 0, st>>>(*bt, status);
 	bio::k_pack_poses<<<(unsigned)B, bio::BLOCK, 0, st>>>(*bt, L, in, status);
-	pb::Args a;
-	a.B = B;
-	a.pose = in; a.cam = in + L.oCam; a.edge = in + L.oEdge;
-	a.ptr2 = (const int*)(in + L.oPtr); a.ptr3 = a.ptr2 + nb + 1;
-	double* o = in + L.nIn;
-	a.poseOut = o;
-	a.stats = stats ? (lm::IterStat*)(o + L.oStat) : nullptr;
-	a.counts = (int*)(o + L.oInt); a.nstats = a.counts + 4 * nb * (size_t)s.n;
-	a.level = (unsigned char*)(o + L.oLev);
-	pb::k_pose_batch<<<(unsigned)B, lm::BLOCK, 0, st>>>(a, s);
+	bio::launch_poses(L, B, s, in, in + L.nIn, stats != nullptr, st);
 	bio::k_unpack_poses<<<(unsigned)B, bio::BLOCK, 0, st>>>(L, B, s.n, bt->E2, (int)statPer, in, q_out, t_out, levels_out, counts, stats, nstats, status);
 	CUDA_TRY(cudaGetLastError());
 	return CUBA_OK;
@@ -3543,27 +3450,21 @@ size_t cuba_sim3_batch_workspace_bytes(int B, int N, const cuba_sim3_params* par
 {
 	s3::Params p;
 	if (B <= 0 || N < 0 || !params) return 0;
-	const std::string err = g_err;
-	const int rc = sim3_params(*params, p);
-	g_err = err;
-	return rc ? 0 : sim3_workspace(B, N, p, with_stats != 0);
+	KeepLastError keep;
+	return sim3_params(*params, p) ? 0 : sim3_workspace(B, N, p, with_stats != 0);
 }
 
 int cuba_engine_optimize_sim3_device(cuba_engine* e, const cuba_sim3_batch* bt, const cuba_sim3_params* params,
 	void* workspace, size_t workspace_bytes, double* q_out, double* t_out, double* s_out, uint8_t* levels_out, int32_t* ninliers,
 	cuba_iter_stat* stats, int32_t* nstats, int32_t* status, void* stream)
 {
-	if (!bt || !params) return fail(CUBA_ERR_INVALID, "optimize_sim3: null batch or params");
 	s3::Params p;
-	{ const int rc0 = sim3_params(*params, p); if (rc0) return rc0; }
-	if (bt->B < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: B < 0");
-	if (bt->N < 0) return fail(CUBA_ERR_INVALID, "optimize_sim3: N < 0");
+	int rc = sim3_batch_args(bt, params, p); if (rc) return rc;
 	if (!status) return fail(CUBA_ERR_INVALID, "optimize_sim3_device: null status");
 	const int B = bt->B;
 	if (B > 0) {
-		int rc = csr_present("optimize_sim3: ptr", bt->N, bt->ptr, { bt->X1, bt->X2, bt->obs1, bt->obs2, bt->omega1, bt->omega2 }); if (rc) return rc;
-		if (!bt->q || !bt->t || !bt->s || !bt->cam1 || !bt->cam2 || !q_out || !t_out || !s_out)
-			return fail(CUBA_ERR_INVALID, "optimize_sim3: null problem array");
+		rc = csr_present("optimize_sim3: ptr", bt->N, bt->ptr, { bt->X1, bt->X2, bt->obs1, bt->obs2, bt->omega1, bt->omega2 }); if (rc) return rc;
+		rc = sim3_batch_pointers(bt, q_out, t_out, s_out); if (rc) return rc;
 		rc = workspace_ok("optimize_sim3_device", workspace, workspace_bytes, sim3_workspace(B, bt->N, p, stats != nullptr)); if (rc) return rc;
 	}
 	ENGINE_OR_FAIL(e);
@@ -3575,15 +3476,7 @@ int cuba_engine_optimize_sim3_device(cuba_engine* e, const cuba_sim3_batch* bt, 
 	double* in = (double*)workspace;
 	bio::k_validate_sim3<<<bio::grid_for(std::max(4 * nb + 1, 3 * N)), bio::BLOCK, 0, st>>>(*bt, status);
 	bio::k_pack_sim3<<<bio::grid_for(s3::PROB * nb + s3::PAIR * N + nb + 1), bio::BLOCK, 0, st>>>(*bt, L, in, status);
-	s3::Args a;
-	a.B = B;
-	a.prob = in; a.pair = in + L.oPair; a.ptr = (const int*)(in + L.oPtr);
-	double* o = in + L.nIn;
-	a.Sout = o;
-	a.stats = stats ? (lm::IterStat*)(o + L.oStat) : nullptr;
-	a.ninliers = (int*)(o + L.oInt); a.nstats = a.ninliers + nb;
-	a.level = (unsigned char*)(o + L.oLev);
-	s3::k_sim3_batch<<<(unsigned)B, lm::BLOCK, 0, st>>>(a, p);
+	bio::launch_sim3(L, B, p, in, in + L.nIn, stats != nullptr, st);
 	bio::k_unpack_sim3<<<bio::grid_for(std::max(8 * nb, std::max(4 * nStat, N))), bio::BLOCK, 0, st>>>(L, B, bt->N, nStat, in, q_out, t_out,
 		s_out, levels_out, ninliers, stats, nstats, status);
 	CUDA_TRY(cudaGetLastError());
@@ -3601,10 +3494,8 @@ size_t cuba_point_batch_workspace_bytes(int B, int P, int E2, int E3, int nround
 {
 	pb::Schedule s;
 	if (B <= 0 || P < 0 || E2 < 0 || E3 < 0 || (long long)E2 + E3 > INT32_MAX) return 0;
-	const std::string err = g_err;
-	const int rc = pose_schedule(nrounds, rounds, s);
-	g_err = err;       // a size query leaves the last error alone
-	return rc ? 0 : point_workspace(B, P, E2, E3, s, with_stats != 0);
+	KeepLastError keep;
+	return pose_schedule(nrounds, rounds, s) ? 0 : point_workspace(B, P, E2, E3, s, with_stats != 0);
 }
 
 int cuba_engine_optimize_points_device(cuba_engine* e, const cuba_point_batch* bt, int nrounds, const cuba_pose_round* rounds,
@@ -3612,11 +3503,11 @@ int cuba_engine_optimize_points_device(cuba_engine* e, const cuba_point_batch* b
 	int32_t* nstats, int32_t* status, void* stream)
 {
 	pb::Schedule s;
-	{ const int rc0 = point_batch_args(bt, nrounds, rounds, s); if (rc0) return rc0; }
+	int rc = point_batch_args(bt, nrounds, rounds, s); if (rc) return rc;
 	if (!status) return fail(CUBA_ERR_INVALID, "optimize_points_device: null status");
 	const int B = bt->B;
 	if (B > 0) {
-		int rc = point_batch_pointers(bt, Xw_out); if (rc) return rc;
+		rc = point_batch_pointers(bt, Xw_out); if (rc) return rc;
 		rc = csr_present("optimize_points: ptr2", bt->E2, bt->ptr2, { bt->iP2, bt->meas2, bt->omega2 }); if (rc) return rc;
 		rc = csr_present("optimize_points: ptr3", bt->E3, bt->ptr3, { bt->iP3, bt->meas3, bt->omega3 }); if (rc) return rc;
 		rc = workspace_ok("optimize_points_device", workspace, workspace_bytes, point_workspace(B, bt->P, bt->E2, bt->E3, s, stats != nullptr)); if (rc) return rc;
@@ -3631,16 +3522,7 @@ int cuba_engine_optimize_points_device(cuba_engine* e, const cuba_point_batch* b
 	const unsigned gridIo = (unsigned)((nb + bio::POINTS_PER_BLOCK - 1) / bio::POINTS_PER_BLOCK);
 	bio::k_validate_points<<<bio::grid_for(std::max(nb + 1, E)), bio::BLOCK, 0, st>>>(*bt, status);
 	bio::k_pack_points<<<gridIo, bio::BLOCK, 0, st>>>(*bt, L, in, status);
-	ptb::Args a;
-	a.B = B;
-	a.Xw = in; a.pose = in + L.oPose; a.cam = in + L.oCam; a.edge = in + L.oEdge;
-	a.iP = (const int*)(in + L.oIdx); a.ptr2 = a.iP + E; a.ptr3 = a.ptr2 + nb + 1;
-	double* o = in + L.nIn;
-	a.XwOut = o;
-	a.stats = stats ? (lm::IterStat*)(o + L.oStat) : nullptr;
-	a.counts = (int*)(o + L.oInt); a.nstats = a.counts + 4 * nb * (size_t)s.n;
-	a.level = (unsigned char*)(o + L.oLev);
-	ptb::k_point_batch<<<(unsigned)((nb + ptb::WARPS - 1) / ptb::WARPS), lm::BLOCK, 0, st>>>(a, s);
+	bio::launch_points(L, B, E, s, in, in + L.nIn, stats != nullptr, st);
 	bio::k_unpack_points<<<gridIo, bio::BLOCK, 0, st>>>(L, B, s.n, bt->E2, bt->E3, (int)statPer, in, Xw_out, levels_out, counts, stats, nstats, status);
 	CUDA_TRY(cudaGetLastError());
 	return CUBA_OK;
